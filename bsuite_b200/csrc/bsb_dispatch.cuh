@@ -163,8 +163,9 @@ int device_launch(bsb_env* e, LaunchArgs a, cudaStream_t stream) {
   }
   size_t per_warp = smem_floats_per_warp<F>(K, a.emit_bulk != 0, a.group_lanes, a.stage_rows) * sizeof(float);
   if ((EmitKind<F>::value == EMIT_ROWS || EmitKind<F>::value == EMIT_TWOHOT) && per_warp > 96 * 1024) {
-    // rows / boards too long for a per-warp stage (catch boards beyond ~19 x 20 cells, umbrella_chain with more than
-    // ~380 distractors): boards fall back to shuffle-rendered vector stores, rows are rendered in place
+    // rows / boards too long for a per-warp stage: long rows always get ONE stage (above), so the limit is
+    // 32 * K * 4 bytes > 96 KB, i.e. K > 768 (catch boards of more than 768 cells such as 28 x 28, umbrella_chain
+    // with more than 765 distractors): boards fall back to shuffle-rendered vector stores, rows are rendered in place
     a.emit_bulk = 0; a.stage_rows = 0; per_warp = 0;
   }
   const size_t cta_extra = (size_t)a.cta_extra_floats * sizeof(float);
