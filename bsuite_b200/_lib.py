@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BSB_LIBRARY points the binding at another build of the SAME library (tools/host_sanitize.sh: ASan/UBSan build)
 LIB_PATH = os.environ.get('BSB_LIBRARY') or os.path.join(_HERE, 'libbsuite_b200.so')
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 DEVICE_HOST = -1
 MAX_INFO = 4
 COMM_ID_BYTES = 128
@@ -51,6 +51,21 @@ class Config(ctypes.Structure):
       ('table', ctypes.c_void_p), ('table_bytes', ctypes.c_int64),
       ('table2', ctypes.c_void_p), ('table2_bytes', ctypes.c_int64),
       ('log_schedule', ctypes.c_void_p), ('log_schedule_len', ctypes.c_int64),
+  ]
+
+
+class ImageDesc(ctypes.Structure):
+  """struct bsb_image_desc."""
+  _fields_ = [
+      ('in_rows', ctypes.c_int32), ('in_cols', ctypes.c_int32), ('out_rows', ctypes.c_int32), ('out_cols', ctypes.c_int32),
+      ('channels', ctypes.c_int32), ('row_radius', ctypes.c_int32), ('col_radius', ctypes.c_int32),
+      ('reserved0', ctypes.c_int32),
+      ('row_index', ctypes.c_void_p), ('row_index_len', ctypes.c_int64),
+      ('row_weight', ctypes.c_void_p), ('row_weight_len', ctypes.c_int64),
+      ('col_index', ctypes.c_void_p), ('col_index_len', ctypes.c_int64),
+      ('col_weight', ctypes.c_void_p), ('col_weight_len', ctypes.c_int64),
+      ('row_taps', ctypes.c_void_p), ('row_taps_len', ctypes.c_int64),
+      ('col_taps', ctypes.c_void_p), ('col_taps_len', ctypes.c_int64),
   ]
 
 
@@ -105,6 +120,9 @@ EXPORTS = {
                                        ctypes.c_void_p, ctypes.c_void_p]),
     'bsb_comm_wait': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p]),
     'bsb_launch_count': (ctypes.c_int64, []),
+    'bsb_image_plan_create': (ctypes.c_int32, [ctypes.POINTER(ImageDesc), ctypes.c_int32, ctypes.POINTER(ctypes.c_void_p)]),
+    'bsb_image_plan_destroy': (ctypes.c_int32, [ctypes.c_void_p]),
+    'bsb_to_image': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
 }
 
 _lib = None

@@ -8,8 +8,10 @@
   * `ImageObservation` / `to_image` -- `bsuite/utils/wrappers.py:150-247`: small observations (size <= 4) are
                       tiled into an image of the requested shape.  Works on numpy arrays (B = 1 face) and on torch
                       tensors with leading batch axes (the batched engine: tiling happens on the device).  Larger
-                      observations need `skimage.transform.resize` in the reference (`:207-219`); that branch is
-                      host-side and only available when scikit-image is installed.
+                      observations are resized as `skimage.transform.resize(..., preserve_range=True)` does in the
+                      reference (`:207-219`): for torch tensors by the engine (`bsuite_b200.imaging`: a batched
+                      kernel on the GPU, the host path on the CPU), for numpy arrays by scikit-image when it is
+                      installed.  `ImageObservation` uses the engine on both faces.
 """
 
 from typing import Any, Dict, Sequence, Tuple
@@ -153,13 +155,16 @@ def to_image(shape: Sequence[int], observation, batch_dims: int = 0):
       empty = np.empty(lead_shape + shape, dtype=observation.dtype)
     return _tile_small(shape, flat, empty, batch_dims)
   if len(observation.shape) - batch_dims <= 2:
+    if is_torch:
+      from bsuite_b200 import imaging  # pylint: disable=import-outside-toplevel
+      return imaging.resize(observation, shape, batch_dims)
     try:
       from skimage import transform  # type: ignore  # pylint: disable=import-outside-toplevel
     except ImportError as error:
       raise NotImplementedError('interpolating observations larger than 4 values needs scikit-image '
                                 '(skimage.transform.resize), as in the reference (wrappers.py:207-219)') from error
-    if is_torch or batch_dims:
-      raise NotImplementedError('the interpolation branch is host-side and per observation')
+    if batch_dims:
+      raise NotImplementedError('numpy observations are interpolated one at a time; pass a torch tensor for a batch')
     plane = observation if observation.ndim > 1 else observation[None]
     image = transform.resize(plane, shape[:2], preserve_range=True)
     while image.ndim < len(shape):
@@ -174,7 +179,8 @@ class ImageObservation(dm_env.Environment):
   """Environment wrapper converting observations to an image-like format (wrappers.py:150-176).
 
   Wraps either face: a B = 1 environment (numpy observations) or a `BatchedEnvironment` (the observation tensor
-  [B, ...] is tiled on its device into [B, *shape])."""
+  [B, ...] is converted on its device into [B, *shape]).  Observations of more than 4 values are resized by the
+  engine on both faces (`bsuite_b200.imaging`; a B = 1 float32 observation takes the host path)."""
 
   def __init__(self, env, shape: Sequence[int]):
     self._env, self._shape = env, tuple(shape)
@@ -188,7 +194,12 @@ class ImageObservation(dm_env.Environment):
     return self._env.action_spec()
 
   def _convert(self, timestep):
-    return timestep._replace(observation=to_image(self._shape, timestep.observation, self._batch_dims))
+    observation = timestep.observation
+    if isinstance(observation, np.ndarray) and observation.dtype == np.float32 and observation.size > 4 \
+        and observation.ndim <= 2:
+      import torch  # pylint: disable=import-outside-toplevel
+      return timestep._replace(observation=to_image(self._shape, torch.from_numpy(observation)).numpy())
+    return timestep._replace(observation=to_image(self._shape, observation, self._batch_dims))
 
   def reset(self):
     return self._convert(self._env.reset())

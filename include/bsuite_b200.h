@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define BSB_ABI_VERSION 6
+#define BSB_ABI_VERSION 7
 #define BSB_DEVICE_HOST (-1)
 #define BSB_MAX_INFO 4
 
@@ -404,6 +404,69 @@ int32_t bsb_comm_wait(bsb_comm* comm, void* stream);
 
 /* Number of kernels this library has launched in this process (bench evidence). */
 int64_t bsb_launch_count(void);
+
+/*
+ * Interpolating branch of ImageObservation / to_image (utils/wrappers.py:207-219):
+ * skimage.transform.resize(plane, (out_rows, out_cols), preserve_range=True)
+ * on each [in_rows, in_cols] float32 plane, broadcast over `channels` trailing
+ * floats.  skimage (>= 0.19) computes
+ *   1. only when out_rows < in_rows or out_cols < in_cols: a Gaussian
+ *      anti-aliasing pass per axis (scipy.ndimage.gaussian_filter, mode
+ *      'mirror'), rows first, each pass accumulated in float64 and rounded to
+ *      float32;
+ *   2. scipy.ndimage.zoom(order=1, mode='mirror', grid_mode=True): per output
+ *      pixel sum over the 2 x 2 neighbourhood (row-major, from 0.0) of
+ *      value * row_weight * col_weight in float64, rounded to float32;
+ *   3. a clip to [min, max] of the unfiltered input plane.
+ * The plan does not depend on any environment handle.  The caller builds the
+ * tables with numpy, with the operations scipy uses, so they are equal by
+ * construction (like the deep_sea mapping tables of bsb_config):
+ *   row_index / row_weight  [out_rows][2]  mirrored source rows (i0, i1) and
+ *                                          weights (w0, w1) of each output row
+ *   col_index / col_weight  [out_cols][2]  the same per output column
+ *   row_taps                [row_radius + 1] Gaussian taps of the row pass:
+ *                                          centre, then distance 1 .. radius
+ *                                          (radius 0 / NULL: no pass)
+ *   col_taps                [col_radius + 1] the same for the column pass
+ * Every *_len is the number of elements of its table.  Tables are HOST
+ * pointers; bsb_image_plan_create copies them (synchronously, to `device`).
+ */
+typedef struct bsb_image_desc {
+  int32_t in_rows, in_cols;       /* h, w of every input plane */
+  int32_t out_rows, out_cols;     /* H, W of every output image */
+  int32_t channels;               /* C: each output pixel is repeated over C consecutive floats */
+  int32_t row_radius, col_radius; /* Gaussian radius per axis; 0 = no pass on that axis */
+  int32_t reserved0;
+  const int32_t* row_index; int64_t row_index_len;
+  const double* row_weight; int64_t row_weight_len;
+  const int32_t* col_index; int64_t col_index_len;
+  const double* col_weight; int64_t col_weight_len;
+  const double* row_taps;   int64_t row_taps_len;
+  const double* col_taps;   int64_t col_taps_len;
+} bsb_image_desc;
+
+typedef struct bsb_image_plan bsb_image_plan; /* opaque handle */
+
+/* device >= 0: CUDA device ordinal; BSB_DEVICE_HOST: explicit host path. */
+int32_t bsb_image_plan_create(const bsb_image_desc* desc, int32_t device,
+                              bsb_image_plan** out);
+int32_t bsb_image_plan_destroy(bsb_image_plan* plan);
+
+/*
+ * in: float32 [batch, in_rows, in_cols], out: float32 [batch, out_rows,
+ * out_cols, channels], both dense and caller-owned, in the plan's memory space.
+ * A device plan enqueues one kernel on `stream` and neither synchronises nor
+ * allocates, so the call may be captured into a CUDA graph; a host plan is
+ * synchronous.  batch 0 does nothing.  A device plan with a Gaussian pass
+ * whose planes do not fit the kernel's shared-memory stage (in_rows *
+ * in_cols above 6 144 values) filters through scratch memory the plan owns:
+ * launches of such a plan must not overlap, so issue them on one stream (or
+ * order the streams with events).  Other plans hold read-only tables only
+ * and may run concurrently.  NaN values are skipped by the clip's
+ * [min, max] (np.nanmin / np.nanmax, as skimage does when a plane holds NaN).
+ */
+int32_t bsb_to_image(bsb_image_plan* plan, const float* in, int64_t batch,
+                     float* out, void* stream);
 
 #ifdef __cplusplus
 }

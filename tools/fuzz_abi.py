@@ -22,6 +22,50 @@ INT_VALUES = [-5, -1, 0, 1, 2, 3, 5, 10, 28, 64, 65, 255, 256, 1000, 1534, 1 << 
 FLOAT_VALUES = [0.0, 1.0, -1.0, 0.01, 3.0, 1e300, float('nan'), float('inf')]
 
 
+def fuzz_image(lib, rng, iterations):
+  """bsb_image_plan_create / bsb_to_image / bsb_image_plan_destroy with hostile descriptors and arguments."""
+  from bsuite_b200 import imaging  # pylint: disable=import-outside-toplevel
+  created = 0
+  for _ in range(iterations):
+    h, w, H, W = (rng.choice([1, 2, 3, 10, 28]) for _ in range(4))
+    (ri, rw, rt), (ci, cw, ct) = imaging.tables((h, w), (H, W))
+    tables = {'row_index': ri, 'row_weight': rw, 'col_index': ci, 'col_weight': cw, 'row_taps': rt, 'col_taps': ct}
+    desc = _lib.ImageDesc()
+    desc.in_rows, desc.in_cols, desc.out_rows, desc.out_cols = h, w, H, W
+    desc.channels = rng.choice([1, 3, 4])
+    for name, array in tables.items():
+      if array is not None:
+        setattr(desc, name, array.ctypes.data)
+        setattr(desc, name + '_len', array.size)
+    desc.row_radius = 0 if rt is None else rt.size - 1
+    desc.col_radius = 0 if ct is None else ct.size - 1
+    if rng.random() < 0.6:                   # one hostile field
+      field = rng.choice(['in_rows', 'in_cols', 'out_rows', 'out_cols', 'channels', 'row_radius', 'col_radius',
+                          'row_index_len', 'col_weight_len', 'row_taps_len', 'col_taps_len', 'row_index', 'col_taps'])
+      value = None if field in ('row_index', 'col_taps') else rng.choice([-5, -1, 0, 1, 7, 1 << 20, (1 << 31) - 1])
+      setattr(desc, field, value)
+      if rng.random() < 0.3:
+        ri[...] = rng.choice([-1, h, 1 << 30])       # indices outside the plane
+    plan = ctypes.c_void_p()
+    status = lib.bsb_image_plan_create(ctypes.byref(desc), _lib.DEVICE_HOST, ctypes.byref(plan))
+    if status != 0:
+      assert lib.bsb_last_error() and not plan.value
+      continue
+    created += 1
+    if max(desc.in_rows * desc.in_cols, desc.out_rows * desc.out_cols * desc.channels) > 5_000_000:
+      assert lib.bsb_image_plan_destroy(plan) == 0
+      continue
+    batch = rng.choice([0, 1, 3])          # buffers sized from the descriptor the plan accepted
+    src = np.random.RandomState(rng.getrandbits(31)).randn(max(batch, 1), desc.in_rows, desc.in_cols).astype(np.float32)
+    dst = np.zeros(max(batch, 1) * desc.out_rows * desc.out_cols * desc.channels, np.float32)
+    assert lib.bsb_to_image(plan, src.ctypes.data, batch, dst.ctypes.data, None) == 0
+    assert lib.bsb_to_image(plan, src.ctypes.data, rng.choice([-1, -(1 << 40)]), dst.ctypes.data, None) != 0
+    assert lib.bsb_to_image(plan, None if rng.random() < 0.5 else src.ctypes.data + 2, 1, dst.ctypes.data, None) != 0
+    assert lib.bsb_image_plan_destroy(plan) == 0
+  assert lib.bsb_to_image(None, None, 1, None, None) != 0 and lib.bsb_image_plan_destroy(None) == 0
+  print(f'fuzz_abi: {created} image plans created, {iterations - created} descriptors rejected')
+
+
 def main():
   iterations = int(sys.argv[1]) if len(sys.argv) > 1 else 3000
   rng = random.Random(int(sys.argv[2]) if len(sys.argv) > 2 else 0)
@@ -123,6 +167,7 @@ def main():
       assert lib.bsb_set_state(handle, ctypes.c_void_p(blob.ctypes.data), nbytes.value + 8, None) != 0
       assert lib.bsb_set_state(handle, ctypes.c_void_p(blob.ctypes.data), nbytes.value, None) == 0
     lib.bsb_destroy(handle)
+  fuzz_image(lib, rng, max(iterations // 10, 20))
   print(f'fuzz_abi: {created} handles created, {rejected} configurations rejected, no crash')
 
 

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """A workload for compute-sanitizer that exercises the PERSISTENT deep_sea path (dynamic chunk counter, grouped
-TMA bulk stores with L2 hints, PDL) plus the catch / row bulk emitters at a size the sanitizer finishes quickly.
+TMA bulk stores with L2 hints, PDL) plus the catch / row bulk emitters and the to_image kernel at a size the
+sanitizer finishes quickly.
 
     compute-sanitizer --tool memcheck  python tools/sanitize_check.py
     compute-sanitizer --tool racecheck python tools/sanitize_check.py
@@ -115,4 +116,18 @@ for _ in range(3):
 assert torch.equal(a.gather_returns(), b.local_returns().unsqueeze(0))
 print('sweep graph == eager, one-launch reduction == per-id reductions: True', flush=True)
 a.close(); b.close()
+# bsb_to_image: staged and unstaged planes, bulk stores and the unaligned streaming-store fallback.
+from bsuite_b200 import adapters
+for plane, target, offset in (((10, 5), (84, 84, 4), 0), ((28, 28), (16, 16), 1), ((130, 100), (90, 70, 3), 1)):
+  planes = torch.randn((300,) + plane, device='cuda')
+  want = adapters.to_image(target, planes.cpu(), batch_dims=1)
+  got = adapters.to_image(target, planes, batch_dims=1)
+  buf = torch.empty(want.numel() + offset, device='cuda')
+  import ctypes
+  from bsuite_b200 import imaging
+  imaging.plan_for(plane, target[:2], (target[2] if len(target) > 2 else 1), planes.device)(
+      planes, buf[offset:], ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+  torch.cuda.synchronize()
+  assert torch.equal(got.cpu(), want) and torch.equal(buf[offset:].cpu().view(want.shape), want)
+  print(plane, '->', target, 'offset', offset, 'CUDA to_image == host path: True', flush=True)
 print('sanitize workload finished')
