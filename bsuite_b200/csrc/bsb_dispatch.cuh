@@ -1,5 +1,7 @@
 // Host path and kernel launch, instantiated once per family (fam_<name>.cu).
 #pragma once
+#include <type_traits>
+
 #include "bsb_env.h"
 
 namespace bsb {
@@ -36,25 +38,17 @@ void host_run(const EnvParams& p, const LaunchArgs& a) {
   typedef typename RngOf<RK>::type R;
   const int64_t B = p.batch;
   const int K = p.obs_numel;
-  const bool noise = p.wrapper == BSB_WRAP_REWARD_NOISE;
-  const bool has_rng = p.rng_pos != nullptr;
-  const bool track = p.ep != nullptr;
+  const bool noise = p.wrapper == BSB_WRAP_REWARD_NOISE && a.mode != MODE_INIT;
+  const bool track = p.ep != nullptr && a.mode != MODE_INIT;
+  const MailFields out = {a.actions, a.obs, a.reward, a.reward_f64, a.discount, a.step_type, 0, 0};
   for (int64_t lane = 0; lane < B; ++lane) {
     typename F::Lane L;
     R rng, wrng;
     EpisodeStats ep;
     ActionStream action_stream;
     action_stream.open();
-    if (a.mode == MODE_INIT) F::init(p, L); else F::load(p, lane, L);
-    if (has_rng) rng_open(rng, p, lane, false);
-    if (noise) rng_open(wrng, p, lane, true);
-    if (track) ep.load(p, lane);
-    if (a.mode == MODE_INIT) {
-      F::ctor_draws(p, L, rng);
-      F::store(p, lane, L);
-      if (has_rng) rng_close(rng, p, lane, false);
-      continue;
-    }
+    lane_open<F>(p, lane, L, rng, wrng, ep, a.mode, noise, track);
+    if (a.mode == MODE_INIT) F::ctor_draws(p, L, rng);
     for (int64_t t = 0; t < a.T; ++t) {
       const int64_t off = t * B + lane;
       int32_t action = 0;
@@ -63,31 +57,25 @@ void host_run(const EnvParams& p, const LaunchArgs& a) {
                            : action_stream.sample(a.action_seed, p.lane_offset + (uint64_t)lane, (uint64_t)(a.step0 + t), p.num_actions);
         if (a.actions_out) a.actions_out[off] = action;
       }
-      const bool after_last = L.nr != 0;
-      const StepOut o = lane_transition<F, R, R>(p, lane, L, rng, wrng, action, a.mode, noise);
-      if (track) {
-        ep.track(p, lane, o, a.step0 + t, after_last);
-        if (p.log_rows && o.step_type == LAST && log_row_due(p, lane)) {
-          F::store(p, lane, L); ep.store(p, lane);
-          log_row_write(p, lane, a.step0 + t + 1);
-        }
-      }
-      if (a.reward) a.reward[off] = (float)o.reward;
-      if (a.reward_f64) a.reward_f64[off] = o.reward;
-      if (a.discount) a.discount[off] = o.discount;
-      if (a.step_type) a.step_type[off] = o.step_type;
+      lane_step<F>(p, lane, L, rng, wrng, ep, action, a.mode, noise, track, a.step0 + t, out, off);
       HostEmit<F>::run(p, L, rng, a.obs + off * (int64_t)K);
     }
-    F::store(p, lane, L);
-    if (has_rng) rng_close(rng, p, lane, false);
-    if (noise) rng_close(wrng, p, lane, true);
-    if (track) ep.store(p, lane);
+    lane_close<F>(p, lane, L, rng, wrng, ep, noise, track);
   }
 }
 
 // --------------------------- device dispatch --------------------------------
-template <class F, int RK, bool kNoise, bool kTrack>
-int device_launch(bsb_env* e, LaunchArgs a, cudaStream_t stream) {
+// Launch geometry, shared by the launchers of both kernels.
+struct Geometry { int threads = 0; size_t smem = 0; int64_t n_chunks = 0, grid = 0; int extra_blocks = 0; };
+
+// Chunk lanes, emitter plan (group lanes, stage rows), CTA size, shared memory and grid of a launch; fills a's
+// emitter fields and, for a persistent grid, its chunk counter.  The rest is for two-phase host steps: `group` > 0
+// sets the lanes per deep_sea bulk store; `no_obs`: no observation (no shared memory: co-resident with another
+// handle's observation stream), one chunk per warp; `extra_threads` > 0 puts g.extra_blocks blocks of that many
+// threads in all (at least one) in front of the chunk owners; `ctas_per_sm` > 0 caps a persistent grid per SM.
+template <class F>
+int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int group = 0, bool no_obs = false, int extra_threads = 0,
+                int ctas_per_sm = 0) {
   const int K = e->p.obs_numel;
   const bool is_onehot = EmitKind<F>::value == EMIT_ONEHOT;
   const bool is_image = EmitKind<F>::value == EMIT_IMAGE;
@@ -116,7 +104,7 @@ int device_launch(bsb_env* e, LaunchArgs a, cudaStream_t stream) {
     while (chunk > 8 && (B + chunk - 1) / chunk < 4 * (int64_t)e->num_sms) chunk >>= 1;
   if (e->chunk_lanes > 0) chunk = e->chunk_lanes;
   a.chunk_lanes = chunk;
-  const int64_t n_chunks = (B + chunk - 1) / chunk;
+  g.n_chunks = (B + chunk - 1) / chunk;
   int threads = e->block_threads;
   bool persistent = false;
   const size_t tile = (size_t)K * 4;
@@ -126,7 +114,7 @@ int device_launch(bsb_env* e, LaunchArgs a, cudaStream_t stream) {
     int m = 1;
     while (m < 16 && (size_t)(2 * m) * tile <= 40 * 1024) m <<= 1;
     if (e->deep_sea_group > 0) m = e->deep_sea_group;
-    if (a.phase == 2 && e->split_group > 0) m = e->split_group;      // observation-only launch of a split host step
+    if (group > 0) m = group;
     if (m > chunk) m = chunk;               // a group never spans chunks
     if (((size_t)m * tile) % 16 != 0 || (size_t)TILE_STAGES * m * tile > 100 * 1024) {
       a.emit_bulk = 0;                      // tiles too large (or misaligned) for the staged path: vector stores
@@ -152,15 +140,11 @@ int device_launch(bsb_env* e, LaunchArgs a, cudaStream_t stream) {
       a.emit_bulk = 0;
     } else {
       a.group_lanes = m; a.stage_rows = stages; threads = 128; a.cta_extra_floats = mz * K; persistent = e->deep_sea_persistent != 0;
-      if (n_chunks < 2 * (int64_t)e->num_sms) threads = 64;      // small batches: more, smaller CTAs
+      if (g.n_chunks < 2 * (int64_t)e->num_sms) threads = 64;      // small batches: more, smaller CTAs
     }
   }
   a.use_pdl = (e->use_pdl && !a.no_pdl && a.mode == MODE_STEP && a.T == 1) ? 1 : 0;
-  if (a.phase == 1) {
-    // transitions-only launch of a split host step: no emitter, no shared memory (so that it is co-resident with the
-    // observation stream of ANOTHER handle), one chunk per warp
-    a.emit_bulk = 0; a.stage_rows = 0; a.cta_extra_floats = 0; a.group_lanes = 1; threads = 128; persistent = false;
-  }
+  if (no_obs) { a.emit_bulk = 0; a.stage_rows = 0; a.cta_extra_floats = 0; a.group_lanes = 1; threads = 128; persistent = false; }
   size_t per_warp = smem_floats_per_warp<F>(K, a.emit_bulk != 0, a.group_lanes, a.stage_rows) * sizeof(float);
   if ((EmitKind<F>::value == EMIT_ROWS || EmitKind<F>::value == EMIT_TWOHOT) && per_warp > 96 * 1024) {
     // rows / boards too long for a per-warp stage: long rows always get ONE stage (above), so the limit is
@@ -172,36 +156,34 @@ int device_launch(bsb_env* e, LaunchArgs a, cudaStream_t stream) {
   size_t smem = per_warp * (size_t)(threads / 32) + cta_extra;
   while (smem > 96 * 1024 && threads > 32) { threads >>= 1; smem = per_warp * (size_t)(threads / 32) + cta_extra; }
   if (smem > 200 * 1024) return fail(BSB_UNSUPPORTED, "observation too large for the staged emitter");
-  auto kernel = transition_kernel<F, RK, kNoise, kTrack>;
-  if (smem > 48 * 1024) BSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int64_t grid = (n_chunks + threads / 32 - 1) / (threads / 32);
-  // Two-phase host step: the first blocks are COPIERS (they ship the staged scalars to the host, then join phase 2):
-  // enough of them for ~512 threads, i.e. ~64 KB of 16-byte loads in flight.
-  const bool two_phase = a.early_scalars != 0 && a.mailbox != nullptr;
-  const int copiers = two_phase ? (512 / threads > 1 ? 512 / threads : 1) : 0;
-  a.early_scalars = copiers;
-  grid += copiers;
+  g.threads = threads;
+  g.smem = smem;
+  g.extra_blocks = extra_threads > 0 ? (extra_threads / threads > 1 ? extra_threads / threads : 1) : 0;
+  g.grid = (g.n_chunks + threads / 32 - 1) / (threads / 32) + g.extra_blocks;
   if (persistent) {
     // As many CTAs as are co-resident (shared-memory bound; 1 KB per CTA is reserved by the driver); their warps
     // draw chunks from the environment's global counter.
     int64_t per_sm = (int64_t)((227 * 1024) / (smem + 1024));
     per_sm = per_sm < 1 ? 1 : (per_sm > 16 ? 16 : per_sm);
-    // observation-only launch of a split host step: leave room for ANOTHER handle's observation stream on every SM
-    if (a.phase == 2 && e->split_ctas_per_sm > 0 && per_sm > e->split_ctas_per_sm) per_sm = e->split_ctas_per_sm;
+    if (ctas_per_sm > 0 && per_sm > ctas_per_sm) per_sm = ctas_per_sm;
     const int64_t resident = (int64_t)e->num_sms * per_sm;
-    if (grid > resident) {
-      grid = resident;
+    if (g.grid > resident) {      // else everything is resident anyway: one chunk per warp
+      g.grid = resident;
       a.work_counter = a.clock ? a.clock + CLOCK_CHUNK : e->work_counter;
       a.work_base = a.clock ? 0ull : e->work_base;
-    } else {
-      persistent = false;      // everything is resident anyway: one chunk per warp
     }
   }
+  return BSB_OK;
+}
+
+template <class Kernel, class... Args>
+int launch(bsb_env* e, const LaunchArgs& a, const Geometry& g, cudaStream_t stream, Kernel kernel, const Args&... args) {
+  if (g.smem > 48 * 1024) BSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3((unsigned)threads);
-  cfg.dynamicSmemBytes = smem;
+  cfg.gridDim = dim3((unsigned)g.grid);
+  cfg.blockDim = dim3((unsigned)g.threads);
+  cfg.dynamicSmemBytes = g.smem;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   if (a.use_pdl) {
@@ -210,30 +192,61 @@ int device_launch(bsb_env* e, LaunchArgs a, cudaStream_t stream) {
     cfg.attrs = attr;
     cfg.numAttrs = 1;
   }
-  BSB_CUDA(cudaLaunchKernelEx(&cfg, kernel, e->p, a));
+  BSB_CUDA(cudaLaunchKernelEx(&cfg, kernel, args...));
   // chunks [warps, n_chunks) are fetched once each and every warp makes exactly one failing fetch
   // (graph-safe mode: the last CTA zeroes the counter instead)
-  if (a.work_counter && !a.clock) e->work_base += (unsigned long long)n_chunks + (unsigned long long)(copiers * (threads / 32));
+  if (a.work_counter && !a.clock) e->work_base += (unsigned long long)g.n_chunks + (unsigned long long)(g.extra_blocks * (g.threads / 32));
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return BSB_OK;
 }
 
-template <class F, int RK>
-int device_launch_flags(bsb_env* e, const LaunchArgs& a, cudaStream_t stream) {
+template <class F, int RK, bool kNoise, bool kTrack>
+int device_launch(bsb_env* e, LaunchArgs a, cudaStream_t stream) {
+  Geometry g;
+  const int rc = plan_launch<F>(e, a, g);
+  return rc != BSB_OK ? rc : launch(e, a, g, stream, transition_kernel<F, RK, kNoise, kTrack>, e->p, a);
+}
+
+// Two-phase host step (DeepSea, Catch): one launch (h.phase 0) or one of the two launches of a split step.
+template <class F, int RK, bool kNoise, bool kTrack>
+int two_phase_launch(bsb_env* e, LaunchArgs a, TwoPhaseArgs h, cudaStream_t stream) {
+  if (a.clock) return fail(BSB_INTERNAL, "a host step reached graph-safe mode, which turns the mailbox path off");
+  // Copiers: enough of them for ~512 threads, i.e. ~64 KB of 16-byte loads in flight.  The observation-only launch
+  // of a split step has none and may take its own group size (BSB_SPLIT_GROUP) and leave room for ANOTHER handle's
+  // observation stream on every SM (BSB_SPLIT_CTAS_PER_SM).
+  Geometry g;
+  const bool obs_only = h.phase == 2;
+  const int rc = plan_launch<F>(e, a, g, obs_only ? e->split_group : 0, h.phase == 1, obs_only ? 0 : 512,
+                                obs_only ? e->split_ctas_per_sm : 0);
+  if (rc != BSB_OK) return rc;
+  h.copiers = g.extra_blocks;
+  return launch(e, a, g, stream, two_phase_host_kernel<F, RK, kNoise, kTrack>, e->p, a, h);
+}
+
+// Runs `launch(noise, track)` with the template flags of the launch's wrappers (none for the constructor).
+template <class Launch>
+int with_flags(const bsb_env* e, const LaunchArgs& a, Launch launch) {
   const bool noise = e->p.wrapper == BSB_WRAP_REWARD_NOISE && a.mode != MODE_INIT;
   const bool track = e->p.ep != nullptr && a.mode != MODE_INIT;
-  if (noise) return track ? device_launch<F, RK, true, true>(e, a, stream) : device_launch<F, RK, true, false>(e, a, stream);
-  return track ? device_launch<F, RK, false, true>(e, a, stream) : device_launch<F, RK, false, false>(e, a, stream);
+  if (noise) return track ? launch(std::true_type(), std::true_type()) : launch(std::true_type(), std::false_type());
+  return track ? launch(std::false_type(), std::true_type()) : launch(std::false_type(), std::false_type());
 }
 
 template <class F>
-int run_family(bsb_env* e, const LaunchArgs& a, cudaStream_t stream) {
+int run_family(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr) {
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
   if (e->device < 0) {
     if (mt) host_run<F, 1>(e->p, a); else host_run<F, 0>(e->p, a);
     return BSB_OK;
   }
-  return mt ? device_launch_flags<F, 1>(e, a, stream) : device_launch_flags<F, 0>(e, a, stream);
+  return with_flags(e, a, [&](auto noise, auto track) {
+    constexpr bool kNoise = decltype(noise)::value, kTrack = decltype(track)::value;
+    if constexpr (ObsFromState<F>::value) {
+      if (two_phase) return mt ? two_phase_launch<F, 1, kNoise, kTrack>(e, a, *two_phase, stream)
+                               : two_phase_launch<F, 0, kNoise, kTrack>(e, a, *two_phase, stream);
+    }
+    return mt ? device_launch<F, 1, kNoise, kTrack>(e, a, stream) : device_launch<F, 0, kNoise, kTrack>(e, a, stream);
+  });
 }
 
 }  // namespace bsb

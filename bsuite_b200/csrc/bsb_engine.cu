@@ -82,7 +82,8 @@ template <class T> int env_alloc_t(bsb_env* e, T** out, size_t count, bool snaps
   return rc;
 }
 
-int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream) {
+// `two_phase`: a two-phase host step (mailbox_launch; deep_sea and catch only).
+int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr) {
   DeviceGuard guard(e->device);
   LaunchArgs a = args;
   if (e->device >= 0) {
@@ -92,8 +93,8 @@ int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream) {
     if (e->graph_safe) a.clock = e->clock;      // a.step0 == e->steps_done, which no longer moves
   }
   switch (e->p.family) {
-    case BSB_DEEP_SEA: return run_deep_sea(e, a, stream);
-    case BSB_CATCH: return run_catch(e, a, stream);
+    case BSB_DEEP_SEA: return run_deep_sea(e, a, stream, two_phase);
+    case BSB_CATCH: return run_catch(e, a, stream, two_phase);
     case BSB_CARTPOLE: return run_cartpole(e, a, stream);
     case BSB_CARTPOLE_SWINGUP: return run_cartpole_swingup(e, a, stream);
     case BSB_MOUNTAIN_CAR: return run_mountain_car(e, a, stream);
@@ -229,40 +230,37 @@ bool family_obs_from_state(const bsb_env* e) {
 }
 
 int mailbox_launch(bsb_env* e, unsigned long long ticket, int64_t step0, const MailFields* fields, bool wait_doorbell, bool split = false) {
-  LaunchArgs a;
-  memset(&a, 0, sizeof(a));
-  if (fields) {
-    a.actions = fields->actions; a.obs = fields->obs; a.reward = fields->reward; a.reward_f64 = fields->reward_f64;
-    a.discount = fields->discount; a.step_type = fields->step_type; a.obs_vec_ok = fields->obs_vec_ok;
-  }
-  a.T = 1; a.step0 = step0; a.mode = MODE_STEP;
+  const bsb_outputs out = fields ? bsb_outputs{fields->obs, fields->reward, fields->reward_f64, fields->discount, fields->step_type}
+                                : bsb_outputs{};
+  LaunchArgs a = make_args(e, fields ? &out : nullptr, fields ? fields->actions : nullptr, 1, MODE_STEP);
+  a.step0 = step0;
   a.mailbox = e->mailbox_dev; a.mail = e->mail; a.ticket = ticket; a.wait_doorbell = wait_doorbell ? 1 : 0;
   a.doorbell_timeout_ns = e->doorbell_timeout_ns;
   { static const int timing = getenv("BSB_HOST_TIMING") ? atoi(getenv("BSB_HOST_TIMING")) : 0; a.timing = timing; }
-  a.early_scalars = (e->host_early && family_obs_from_state(e)) ? 1 : 0;      // device_launch turns it into the copier count
-  if (a.early_scalars) {
-    // device staging of the scalars: reward | discount | step_type in one block (as the staged-copy path keeps them)
-    const size_t B = (size_t)e->p.batch;
-    if (!e->d_reward) {
-      BSB_CUDA(cudaMalloc(&e->d_reward, 3 * B * 4));
-      e->d_discount = e->d_reward + B;
-      e->d_step_type = reinterpret_cast<int32_t*>(e->d_reward + 2 * B);
-    }
-    if (!e->d_reward64) BSB_CUDA(cudaMalloc(&e->d_reward64, B * 8));
-    a.stage.reward = e->d_reward; a.stage.reward_f64 = e->d_reward64; a.stage.discount = e->d_discount; a.stage.step_type = e->d_step_type;
-    e->early_inflight = true;
-    if (split && e->host_split && !wait_doorbell) {
-      // BSB_HOST_NO_WAIT: the caller alternates between handles.  Two launches instead of one -- transitions + copiers
-      // (no shared memory), then the observation stream -- so that THIS handle's transitions and PCIe traffic run
-      // while the OTHER handle's observations have the SMs' shared memory and the HBM.
-      LaunchArgs first = a, second = a;
-      first.phase = 1;
-      second.phase = 2; second.mailbox = nullptr; second.early_scalars = 0;
-      int rc = run(e, first, e->copy_stream);
-      return rc != BSB_OK ? rc : run(e, second, e->copy_stream);
-    }
+  if (!e->host_early || !family_obs_from_state(e)) return run(e, a, e->copy_stream);
+  // device staging of the scalars: reward | discount | step_type in one block (as the staged-copy path keeps them)
+  const size_t B = (size_t)e->p.batch;
+  if (!e->d_reward) {
+    BSB_CUDA(cudaMalloc(&e->d_reward, 3 * B * 4));
+    e->d_discount = e->d_reward + B;
+    e->d_step_type = reinterpret_cast<int32_t*>(e->d_reward + 2 * B);
   }
-  return run(e, a, e->copy_stream);
+  if (!e->d_reward64) BSB_CUDA(cudaMalloc(&e->d_reward64, B * 8));
+  TwoPhaseArgs h;
+  memset(&h, 0, sizeof(h));
+  h.stage.reward = e->d_reward; h.stage.reward_f64 = e->d_reward64; h.stage.discount = e->d_discount; h.stage.step_type = e->d_step_type;
+  e->early_inflight = true;
+  if (split && e->host_split && !wait_doorbell) {
+    // BSB_HOST_NO_WAIT: the caller alternates between handles.  Two launches instead of one -- transitions + copiers
+    // (no shared memory), then the observation stream -- so that THIS handle's transitions and PCIe traffic run
+    // while the OTHER handle's observations have the SMs' shared memory and the HBM.
+    h.phase = 1;
+    int rc = run(e, a, e->copy_stream, &h);
+    if (rc != BSB_OK) return rc;
+    a.mailbox = nullptr;
+    h.phase = 2;
+  }
+  return run(e, a, e->copy_stream, &h);
 }
 
 // Spins on the mailbox until `ticket` is done (the kernel's last CTA stores it after a system-scope fence).
@@ -354,49 +352,12 @@ __global__ void episode_stat_kernel(const EnvParams p, int field, int64_t calls,
   if (i < p.batch) dst[i] = episode_stat(p, i, field, calls);
 }
 
-// Sums of the five Logging columns over the lanes.  Deterministic: a fixed grid (a function of the batch only) of
-// block-strided partial sums lands in scratch[block][5]; the block that finishes last adds the partials in block
-// order and re-arms the ticket.  (No floating-point atomics: the result must not depend on scheduling -- a graph
-// replay and an eager call must agree to the bit.)
-constexpr int kSumBlocks = 64, kSumThreads = 256;
-__global__ void episode_sum_kernel(const EnvParams p, int64_t calls, const unsigned long long* clock,
-                                   double* scratch, unsigned long long* ticket, double* dst5) {
-  if (clock) calls += (int64_t)*clock;
-  __shared__ double partial[5][kSumThreads / 32];
-  __shared__ bool is_last;
-  double v[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.batch; i += (int64_t)gridDim.x * blockDim.x)
-#pragma unroll
-    for (int f = 0; f < 5; ++f) v[f] += episode_stat(p, i, f, calls);
-#pragma unroll
-  for (int f = 0; f < 5; ++f)
-    for (int o = 16; o > 0; o >>= 1) v[f] += __shfl_down_sync(0xffffffffu, v[f], o);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) for (int f = 0; f < 5; ++f) partial[f][warp] = v[f];
-  __syncthreads();
-  if (threadIdx.x < 5) {
-    double s = 0.0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += partial[threadIdx.x][w];
-    scratch[blockIdx.x * 5 + threadIdx.x] = s;
-    __threadfence();
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) is_last = atomicAdd(ticket, 1ull) == (unsigned long long)gridDim.x - 1ull;
-  __syncthreads();
-  if (!is_last) return;
-  __threadfence();
-  if (threadIdx.x < 5) {
-    double s = 0.0;
-    for (unsigned b = 0; b < gridDim.x; ++b) s += __ldcg(scratch + b * 5 + threadIdx.x);
-    dst5[threadIdx.x] = s;
-  }
-  if (threadIdx.x == 0) *ticket = 0ull;
-}
-
-// The same reduction for up to kSumManyMax environments in ONE launch (blockIdx.y = environment): a log point of
-// the 23-experiment sweep is one kernel instead of 23.  Each environment keeps its own scratch and ticket, and
-// its sums are combined in block order, so the result equals episode_sum_kernel's bit for bit.
-constexpr int kSumManyMax = 64;
+// Sums of the five Logging columns over the lanes of up to kSumManyMax environments in ONE launch (blockIdx.y =
+// environment: a log point of the 23-experiment sweep is one kernel instead of 23).  Deterministic: a fixed grid (a
+// function of the batch only) of block-strided partial sums lands in the environment's scratch[block][5]; the block
+// that finishes last adds the partials in block order and re-arms the ticket.  (No floating-point atomics: the result
+// must not depend on scheduling -- a graph replay and an eager call must agree to the bit.)
+constexpr int kSumBlocks = 64, kSumThreads = 256, kSumManyMax = 64;
 struct SumJob { const double* ep; int64_t batch; int64_t calls; const unsigned long long* clock; double* scratch; };
 struct SumJobs { SumJob job[kSumManyMax]; };
 __global__ void episode_sum_many_kernel(const SumJobs jobs, double* dst) {
@@ -404,7 +365,7 @@ __global__ void episode_sum_many_kernel(const SumJobs jobs, double* dst) {
   EnvParams p;
   p.ep = const_cast<double*>(j.ep); p.batch = j.batch;
   int64_t calls = j.calls;
-  if (j.clock) calls += (int64_t)*j.clock;
+  if (j.clock) calls += (int64_t)*j.clock;      // graph-safe mode: steps since the switch are counted on the device
   __shared__ double partial[5][kSumThreads / 32];
   __shared__ bool is_last;
   double v[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
@@ -418,7 +379,7 @@ __global__ void episode_sum_many_kernel(const SumJobs jobs, double* dst) {
   if (lane == 0) for (int f = 0; f < 5; ++f) partial[f][warp] = v[f];
   __syncthreads();
   // blocks that own no lanes of this environment contribute exact zeros, so the block-order sum below equals the
-  // one episode_sum_kernel forms over min(blocks, ceil(batch / threads)) blocks
+  // one a grid of min(blocks, ceil(batch / threads)) blocks forms (bsb_sum_episode_stats launches that many)
   if (threadIdx.x < 5) {
     double s = 0.0;
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += partial[threadIdx.x][w];
@@ -749,9 +710,11 @@ int32_t bsb_sum_episode_stats(bsb_env* env, double* dst5, void* stream) {
     DeviceGuard guard(env->device);
     int64_t blocks = (B + kSumThreads - 1) / kSumThreads;
     if (blocks > kSumBlocks) blocks = kSumBlocks;
-    episode_sum_kernel<<<(unsigned)blocks, kSumThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        env->p, env->steps_done, env->graph_safe ? env->clock : nullptr, env->sum_scratch,
-        reinterpret_cast<unsigned long long*>(env->sum_scratch + kSumBlocks * 5), dst5);
+    SumJobs jobs;
+    memset(&jobs, 0, sizeof(jobs));
+    jobs.job[0].ep = env->p.ep; jobs.job[0].batch = B; jobs.job[0].calls = env->steps_done;
+    jobs.job[0].clock = env->graph_safe ? env->clock : nullptr; jobs.job[0].scratch = env->sum_scratch;
+    episode_sum_many_kernel<<<dim3((unsigned)blocks, 1), kSumThreads, 0, static_cast<cudaStream_t>(stream)>>>(jobs, dst5);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     BSB_CUDA(cudaGetLastError());
   } else {

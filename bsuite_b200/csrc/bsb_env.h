@@ -86,8 +86,9 @@ struct bsb_env {
 
 namespace bsb {
 // One entry per family, each defined in its own translation unit (fam_<name>.cu).
-int run_deep_sea(bsb_env*, const LaunchArgs&, cudaStream_t);
-int run_catch(bsb_env*, const LaunchArgs&, cudaStream_t);
+// deep_sea and catch also run the two-phase host step (`two_phase`: its arguments).
+int run_deep_sea(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs* two_phase = nullptr);
+int run_catch(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs* two_phase = nullptr);
 int run_cartpole(bsb_env*, const LaunchArgs&, cudaStream_t);
 int run_cartpole_swingup(bsb_env*, const LaunchArgs&, cudaStream_t);
 int run_mountain_car(bsb_env*, const LaunchArgs&, cudaStream_t);

@@ -25,13 +25,14 @@
 //   * mnist: groups of 4 gathered int8 images -> float32 tiles in shared memory -> one bulk store; the all-zero
 //     LAST frames of a group leave as one bulk store from zero tiles the CTA's warps share.
 //
-// A launch covers T consecutive steps with lane state held in registers (T = 1
-// for bsb_step); actions come from the caller or from the on-device Philox
-// action stream.  Host-driven steps (bsb_step_host) signal completion through a
-// pinned mailbox and, for deep_sea, run in two phases (all transitions first, the
-// scalars shipped to the host by a few copier blocks, then the observations).  With use_pdl the kernel is launched with programmatic stream
-// serialization: everything before griddepcontrol.wait (index math, zeroing the
-// shared-memory stages) overlaps the tail of the previous step's kernel.
+// A launch of transition_kernel covers T consecutive steps with lane state held in registers (T = 1 for bsb_step);
+// actions come from the caller or from the on-device Philox action stream.  Host-driven steps (bsb_step_host) signal
+// completion through a pinned mailbox.  For deep_sea and catch with observations of 1 KB or more they run in two
+// phases in a kernel of their own, two_phase_host_kernel (all transitions first, the scalars shipped to the host by a
+// few copier blocks, then the observations).  Both kernels share the emitters, the lane open / step / close sequence
+// (which the host path runs too) and the mailbox protocol.  With use_pdl a kernel is launched with programmatic
+// stream serialization: everything before griddepcontrol.wait (index math, zeroing the shared-memory stages)
+// overlaps the tail of the previous step's kernel.
 #pragma once
 #include "bsb_families.cuh"
 
@@ -79,16 +80,19 @@ struct LaunchArgs {
                                      // paying a stream synchronise.
   struct DeviceMail* mail;           // device memory: doorbell relay + finished-CTA counter
   unsigned long long ticket;
-  int32_t early_scalars;             // > 0: two-phase host step; the value is the number of COPIER blocks (blocks
-                                     // [0, n) own no chunks at first: they ship the scalars to the host, see below)
-  MailFields stage;                  // two-phase: device staging of reward / reward_f64 / discount / step_type
   int32_t timing;                    // BSB_HOST_TIMING: leave %globaltimer stamps in the mailbox
   int32_t wait_doorbell;             // 1: pre-launched -- poll the doorbell for `ticket`, then take the buffers from the mailbox
   unsigned long long doorbell_timeout_ns;
   int32_t* bad_action;      // pinned host flag (device alias): set to 1 when an action is outside [0, num_actions)
-  int32_t phase;            // two-phase host step split over TWO launches (BSB_HOST_NO_WAIT): 1 = transitions + copiers
-                            // only (no shared memory: co-resident with another handle's observation stream),
-                            // 2 = observations only (waits for mail->phase1 == ticket, not for launch 1 to END); 0 = one launch
+};
+
+// The arguments only two_phase_host_kernel takes.
+struct TwoPhaseArgs {
+  int32_t copiers;          // blocks [0, copiers) own no chunks at first: they ship the scalars to the host (see the kernel)
+  int32_t phase;            // step split over TWO launches (BSB_HOST_NO_WAIT): 1 = transitions + copiers only (no shared
+                            // memory: co-resident with another handle's observation stream), 2 = observations only
+                            // (waits for mail->phase1 == ticket, not for launch 1 to END); 0 = one launch
+  MailFields stage;         // device staging of reward / reward_f64 / discount / step_type
 };
 
 // Host <-> device mailbox of the doorbell mode.  The host fills `in` and then stores `doorbell = ticket` (release
@@ -169,6 +173,48 @@ BSB_HD StepOut lane_transition(const EnvParams& p, int64_t i, typename F::Lane& 
     else if (p.wrapper == 2) { o.reward = o.reward * p.reward_scale; }
   }
   return o;
+}
+
+// ----- one lane over a run of steps: open, one lane_step per step, close ------------------------------------------
+// The kernels and the host path (host_run) all go through these three.  Reading and checking the action stays with
+// each caller: the host path rejects bad actions up front, the kernels clamp them and raise `bad_action`.
+// Opens the lane's state (F::init for the constructor), both RNG streams and the Logging accumulators.
+// `state_loaded`: the caller has read L and ep already (phase 1 of the two-phase host step batches those loads).
+template <class F, class R>
+BSB_HD void lane_open(const EnvParams& p, int64_t lane, typename F::Lane& L, R& rng, R& wrng, EpisodeStats& ep,
+                      int32_t mode, bool noise, bool track, bool state_loaded = false) {
+  if (!state_loaded) { if (mode == MODE_INIT) F::init(p, L); else F::load(p, lane, L); }
+  if (p.rng_pos) rng_open(rng, p, lane, false);
+  if (noise) rng_open(wrng, p, lane, true);
+  if (track && !state_loaded) ep.load(p, lane);
+}
+template <class F, class R>
+BSB_HD void lane_close(const EnvParams& p, int64_t lane, const typename F::Lane& L, const R& rng, const R& wrng,
+                       const EpisodeStats& ep, bool noise, bool track) {
+  F::store(p, lane, L);
+  if (p.rng_pos) rng_close(rng, p, lane, false);
+  if (noise) rng_close(wrng, p, lane, true);
+  if (track) ep.store(p, lane);
+}
+// One step of an open lane: the transition, the Logging accumulators with their log row, and the four scalar outputs
+// at index `off` of `out` (null outputs are skipped).  `step`: global index of this step.
+template <class F, class R>
+BSB_HD void lane_step(const EnvParams& p, int64_t lane, typename F::Lane& L, R& rng, R& wrng, EpisodeStats& ep,
+                      int32_t action, int32_t mode, bool noise, bool track, int64_t step, const MailFields& out,
+                      int64_t off) {
+  const bool after_last = L.nr != 0;
+  const StepOut o = lane_transition<F, R, R>(p, lane, L, rng, wrng, action, mode, noise);
+  if (track) {
+    ep.track(p, lane, o, step, after_last);
+    if (p.log_rows && o.step_type == LAST && log_row_due(p, lane)) {      // <= 49 times per 10 000 episodes
+      F::store(p, lane, L); ep.store(p, lane);                          // the row reads them from memory
+      log_row_write(p, lane, step + 1);
+    }
+  }
+  if (out.reward) out.reward[off] = (float)o.reward;
+  if (out.reward_f64) out.reward_f64[off] = o.reward;
+  if (out.discount) out.discount[off] = o.discount;
+  if (out.step_type) out.step_type[off] = o.step_type;
 }
 
 // Observation emitter of each family.
@@ -523,443 +569,269 @@ __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wa
 static const int CLOCK_GROUPS = 32, CLOCK_CHUNK = 16 * CLOCK_GROUPS, CLOCK_TOP = CLOCK_CHUNK + 16,
                  CLOCK_SUB0 = CLOCK_TOP + 16, CLOCK_WORDS = CLOCK_SUB0 + 16 * CLOCK_GROUPS;
 
-template <class F, int RK, bool kNoise, bool kTrack>
-__global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kernel(const EnvParams p, const LaunchArgs a) {
-  typedef typename RngOf<RK>::type R;
-  constexpr int kEmit = EmitKind<F>::value;
-  extern __shared__ float4 smem_raw[];
-  __shared__ MailFields mail_in;
-  __shared__ int mail_cancel;
-  const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
-  const int64_t B = p.batch;
-  const int K = p.obs_numel;
-  const size_t stage_floats = smem_floats_per_warp<F>(K, a.emit_bulk != 0, a.group_lanes, a.stage_rows);
-  const unsigned row_mask = a.stage_rows == 2 ? 1u : 0u;      // row / board stage of store number n: n & row_mask
-  float* stage = reinterpret_cast<float*>(smem_raw) + (size_t)warp * stage_floats;
-  // mnist bulk path: all-zero tiles shared by the CTA's warps (source of the LAST-frame stores), after the stages
-  float* cta_zero = reinterpret_cast<float*>(smem_raw) + (size_t)warps_per_cta * stage_floats;
+// ----- pieces both kernels share ----------------------------------------------------------------------------------
+// Per-warp staging state of the observation emitters; it persists across the chunks and steps of a launch.
+struct WarpStage {
+  float* stage;            // this warp's shared-memory stages
+  float* cta_zero;         // mnist bulk path: all-zero tiles shared by the CTA's warps (source of the LAST-frame stores)
+  unsigned row_mask;       // row / board stage of store number n: n & row_mask
+  unsigned emitted = 0;    // bulk stores issued by this warp so far (double-buffer parity)
+  int poked_a0 = -1, poked_b0 = -1, poked_a1 = -1, poked_b1 = -1;   // catch: cells poked into stage buffer 0 / 1
+  int tile_poked0 = -1, tile_poked1 = -1;      // deep_sea bulk path: cell this thread poked into group buffer 0 / 1
+  bool any_bulk = false;   // a chunk went through the TMA unit
+};
 
-  // Stages that rely on staying zero between steps are cleared once, before the dependency wait.
+// Carves the warp's stages out of dynamic shared memory and clears those that rely on staying zero between steps
+// (before the dependency wait).  Every thread of the CTA calls it.
+template <class F>
+__device__ __forceinline__ WarpStage clear_stages(const EnvParams& p, const LaunchArgs& a) {
+  extern __shared__ float4 smem_raw[];
+  constexpr int kEmit = EmitKind<F>::value;
+  const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
+  const size_t stage_floats = smem_floats_per_warp<F>(p.obs_numel, a.emit_bulk != 0, a.group_lanes, a.stage_rows);
+  WarpStage ws;
+  ws.stage = reinterpret_cast<float*>(smem_raw) + (size_t)warp * stage_floats;
+  ws.cta_zero = reinterpret_cast<float*>(smem_raw) + (size_t)warps_per_cta * stage_floats;
+  ws.row_mask = a.stage_rows == 2 ? 1u : 0u;
   if (kEmit == EMIT_TWOHOT || (kEmit == EMIT_ONEHOT && a.emit_bulk)) {
-    float4* s4 = reinterpret_cast<float4*>(stage);
+    float4* s4 = reinterpret_cast<float4*>(ws.stage);
     const int total4 = (int)(stage_floats >> 2);
     for (int q = tid; q < total4; q += 32) s4[q] = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int e = (total4 << 2) + tid; e < (int)stage_floats; e += 32) stage[e] = 0.f;
+    for (int e = (total4 << 2) + tid; e < (int)stage_floats; e += 32) ws.stage[e] = 0.f;
     __syncwarp();
   }
   if (kEmit == EMIT_IMAGE) {      // pixel table: image.astype(float32) / 255 for every int8 value (mnist.py:64)
-    for (int i = tid; i < 256; i += 32) stage[i] = Mnist::pixel((int8_t)(uint8_t)i);
-    for (int i = threadIdx.x; i < a.cta_extra_floats; i += blockDim.x) cta_zero[i] = 0.f;
+    for (int i = tid; i < 256; i += 32) ws.stage[i] = Mnist::pixel((int8_t)(uint8_t)i);
+    for (int i = threadIdx.x; i < a.cta_extra_floats; i += blockDim.x) ws.cta_zero[i] = 0.f;
     fence_proxy_async_smem();
     __syncthreads();
   }
+  return ws;
+}
+
+// Caller-owned buffers of the launch: its arguments or -- pre-launched (doorbell) mode -- whatever the host wrote
+// into the mailbox before it rang this launch's ticket.  `cancelled`: the host stood the launch down, or nobody rang
+// before the timeout.  Every thread of the CTA calls it.
+__device__ __forceinline__ MailFields receive_doorbell(const LaunchArgs& a, bool& cancelled) {
+  __shared__ MailFields mail_in;
+  __shared__ int mail_cancel;
+  MailFields io = {a.actions, a.obs, a.reward, a.reward_f64, a.discount, a.step_type, a.obs_vec_ok, 0};
+  cancelled = false;
+  if (!a.mailbox || !a.wait_doorbell) return io;
+  const int tid = threadIdx.x & 31;
+  if (blockIdx.x == 0 && (threadIdx.x >> 5) == 0) {
+    // The one poller of host memory: lanes 0..7 read the mailbox's first 64-byte line (doorbell + fields) with ONE
+    // coalesced request per poll; when the ring shows, the line is read once more (the host wrote the fields
+    // before the doorbell, so this second read cannot be stale), parked in device memory, and the ticket is
+    // relayed to the other blocks through L2.
+    const volatile unsigned long long* line = &a.mailbox->doorbell;
+    const unsigned long long deadline = global_timer_ns() + a.doorbell_timeout_ns;
+    unsigned long long word = 0, seen;
+    do {
+      if (tid < 8) word = ld_sys_u64(line + tid);
+      seen = __shfl_sync(0xffffffffu, word, 0);
+    } while ((seen & ~MAIL_CANCEL) < a.ticket && global_timer_ns() < deadline);
+    if ((seen & ~MAIL_CANCEL) < a.ticket) seen = a.ticket | MAIL_CANCEL;        // nobody rang: stand down
+    __threadfence_system();
+    if (tid < 8) word = ld_sys_u64(line + tid);
+    if (tid >= 1 && tid < 8) reinterpret_cast<unsigned long long*>(&a.mail->in)[tid - 1] = word;
+    __threadfence();
+    __syncwarp();
+    if (tid == 0) a.mail->relay = seen;
+  }
+  if (threadIdx.x == 0) {
+    unsigned long long seen;
+    do { seen = a.mail->relay; } while ((seen & ~MAIL_CANCEL) < a.ticket);
+    __threadfence();
+    mail_cancel = (seen & MAIL_CANCEL) ? 1 : 0;
+    const volatile unsigned long long* src = reinterpret_cast<const volatile unsigned long long*>(&a.mail->in);
+    unsigned long long* dst = reinterpret_cast<unsigned long long*>(&mail_in);
+    for (int k = 0; k < (int)(sizeof(MailFields) / 8); ++k) dst[k] = src[k];
+  }
+  __syncthreads();
+  io = mail_in;
+  cancelled = mail_cancel != 0;
+  return io;
+}
+
+// The elected lane draws chunk indices [total_warps, n_chunks) from the global counter and broadcasts them with a
+// shuffle (chunk = global warp index is taken without asking).
+__device__ __forceinline__ int64_t fetch_chunk(const LaunchArgs& a, int64_t total_warps) {
+  unsigned long long v = 0;
+  if ((threadIdx.x & 31) == 0) v = atomicAdd(a.work_counter, 1ull) - a.work_base;      // graph-safe mode: clock + 1, base 0
+  return total_warps + (int64_t)__shfl_sync(0xffffffffu, v, 0);
+}
+
+// Which chunks leave through the TMA unit (16-byte aligned spans); warp-uniform per chunk.
+template <class F>
+__device__ __forceinline__ bool chunk_is_bulk(const EnvParams& p, const LaunchArgs& a, bool vec, int n_lanes) {
+  constexpr int kEmit = EmitKind<F>::value;
+  const int K = p.obs_numel;
+  bool bulk = a.emit_bulk && vec;
+  if (kEmit == EMIT_ROWS) bulk = bulk && K >= 3 && ((n_lanes * K) & 3) == 0;
+  if (kEmit == EMIT_TWOHOT) bulk = bulk && ((n_lanes * K) & 3) == 0;
+  if (kEmit == EMIT_ONEHOT) bulk = bulk && ((K & 3) == 0 || ((n_lanes % a.group_lanes) == 0 && ((a.group_lanes * K) & 3) == 0));
+  if (kEmit == EMIT_IMAGE) bulk = bulk && (K & 3) == 0;
+  return bulk;
+}
+
+// Observation emitter of the warp for one chunk and step.
+template <class F, class R>
+__device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a, WarpStage& ws, const typename F::Lane& L,
+                                         R& rng, float* obs_t, int64_t warp_base, int n_lanes, int64_t lane, bool active,
+                                         bool bulk, bool vec) {
+  constexpr int kEmit = EmitKind<F>::value;
+  const int tid = threadIdx.x & 31;
+  const int K = p.obs_numel;
+  if (kEmit == EMIT_ONEHOT) {
+    const int hot = Descriptor<F>::a(L);
+    if (bulk) {
+      // Groups of m consecutive lanes share one staging buffer (m tiles, contiguous in global memory too) and
+      // leave as ONE bulk store of up to m * 4K bytes: large stores amortise the per-operation cost of the
+      // TMA unit.
+      const int m = a.group_lanes;
+      for (int g0 = 0; g0 < n_lanes; g0 += m) {
+        const int in_group = (n_lanes - g0) < m ? (n_lanes - g0) : m;
+        const int s = (int)(ws.emitted & 1u);
+        float* group = ws.stage + (size_t)s * m * K;
+        if (tid == 0) bulk_wait_read<TILE_STAGES - 1>();    // the store two back, last reader of `group`, is done
+        __syncwarp();
+        if (s == 0) { if (ws.tile_poked0 >= 0) { group[ws.tile_poked0] = 0.f; ws.tile_poked0 = -1; } }
+        else        { if (ws.tile_poked1 >= 0) { group[ws.tile_poked1] = 0.f; ws.tile_poked1 = -1; } }
+        __syncwarp();     // a thread of an earlier group may clear the very cell another thread sets now
+        if (tid >= g0 && tid < g0 + in_group && hot >= 0) {
+          const int cell = (tid - g0) * K + hot;
+          group[cell] = 1.f;
+          if (s == 0) ws.tile_poked0 = cell; else ws.tile_poked1 = cell;
+        }
+        fence_proxy_async_smem();
+        __syncwarp();
+        if (tid == 0) {
+          float* tile_dst = obs_t + (warp_base + g0) * (int64_t)K;
+          const uint32_t tile_bytes = (uint32_t)in_group * (uint32_t)K * 4u;
+          bulk_store_obs(tile_dst, group, tile_bytes, a.l2_hint);
+          bulk_commit();
+        }
+        ++ws.emitted;
+      }
+    } else {
+      emit_onehot_vec(obs_t, warp_base, n_lanes, K, hot, vec && (K & 3) == 0);
+    }
+  } else if (kEmit == EMIT_TWOHOT) {
+    const int hot_a = Descriptor<F>::a(L), hot_b = Descriptor<F>::b(L);
+    if (bulk) {
+      const int buf = (int)(ws.emitted & ws.row_mask);
+      float* boards = ws.stage + (size_t)buf * 32 * K;
+      if (tid == 0) { if (ws.row_mask) bulk_wait_read<1>(); else bulk_wait_read<0>(); }   // the store that last read `boards` is done with it
+      __syncwarp();
+      float* mine = boards + tid * K;
+      const int old_a = buf ? ws.poked_a1 : ws.poked_a0, old_b = buf ? ws.poked_b1 : ws.poked_b0;
+      if (old_a >= 0) mine[old_a] = 0.f;
+      if (old_b >= 0) mine[old_b] = 0.f;
+      int new_a = -1, new_b = -1;
+      if (active) { mine[hot_a] = 1.f; mine[hot_b] = 1.f; new_a = hot_a; new_b = hot_b; }
+      if (buf) { ws.poked_a1 = new_a; ws.poked_b1 = new_b; } else { ws.poked_a0 = new_a; ws.poked_b0 = new_b; }
+      fence_proxy_async_smem();
+      __syncwarp();
+      if (tid == 0) { bulk_store_obs(obs_t + warp_base * (int64_t)K, boards, (uint32_t)n_lanes * (uint32_t)K * 4u, a.l2_hint); bulk_commit(); }
+      ++ws.emitted;
+    } else {
+      emit_twohot_vec(obs_t, warp_base, n_lanes, K, hot_a, hot_b, vec);
+    }
+  } else if (kEmit == EMIT_IMAGE) {
+    const int image = Descriptor<F>::a(L);
+    if (bulk) emit_image_bulk(p, ws.stage, ws.cta_zero, obs_t, warp_base, n_lanes, K, active ? image : -1, a.group_lanes,
+                              a.cta_extra_floats / K, a.l2_hint, a.stage_rows, ws.emitted);
+    else emit_image(p, ws.stage, obs_t, warp_base, n_lanes, K, image, vec && (K & 3) == 0);
+  } else if (!a.stage_rows) {
+    // observation rows too long for a shared-memory stage: every thread renders its row in place
+    if (active) RowRenderer<F, R>::run(p, L, rng, obs_t + lane * (int64_t)K);
+  } else {
+    float* rows = ws.stage + (size_t)(ws.emitted & ws.row_mask) * 32 * K;
+    if (bulk) { if (tid == 0) { if (ws.row_mask) bulk_wait_read<1>(); else bulk_wait_read<0>(); } }
+    __syncwarp();
+    if (active) RowRenderer<F, R>::run(p, L, rng, rows + tid * K);
+    if (bulk) {
+      fence_proxy_async_smem();
+      __syncwarp();
+      if (tid == 0) { bulk_store_obs(obs_t + warp_base * (int64_t)K, rows, (uint32_t)n_lanes * (uint32_t)K * 4u, a.l2_hint); bulk_commit(); }
+    } else {
+      __syncwarp();
+      flush_rows_vec(rows, obs_t, warp_base, n_lanes, K, vec);
+    }
+    ++ws.emitted;
+  }
+}
+
+// The warp is done: shared memory must outlive its last bulk read.  `drain`: the stores themselves must have
+// completed (a single-phase host step's `done` tells the host that the observations are in device memory).
+__device__ __forceinline__ void retire_warp(const LaunchArgs& a, const WarpStage& ws, bool drain) {
+  if (ws.any_bulk && (threadIdx.x & 31) == 0) { if (drain) bulk_wait_all(); else bulk_wait_read<0>(); }
+  if (a.timing && a.mail && threadIdx.x == 0) atomicMax(&a.mail->last_exit, global_timer_ns());
+}
+
+// Completion of a host step: every CTA counts itself finished once its zero-copy outputs are visible to the host;
+// the last one stores `word` (the ticket, with MAIL_CANCEL if the launch stood down) into the mailbox.
+__device__ __forceinline__ void signal_done(const LaunchArgs& a, unsigned long long word) {
+  __threadfence_system();                  // every thread: its zero-copy outputs are visible to the host ...
+  __syncthreads();                         // ... before the CTA counts itself finished
+  if (threadIdx.x == 0 && atomicAdd(&a.mail->finished, 1ull) == (unsigned long long)gridDim.x - 1ull) {
+    a.mail->finished = 0ull;
+    __threadfence_system();
+    st_sys_u64(&a.mailbox->done, word);
+  }
+}
+
+// The fused transition kernel: ordinary launches (constructor, reset, step, rollout), graph-safe mode and the
+// single-phase host step.
+template <class F, int RK, bool kNoise, bool kTrack>
+__global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kernel(const EnvParams p, const LaunchArgs a) {
+  typedef typename RngOf<RK>::type R;
+  const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
+  const int64_t B = p.batch;
+  const int K = p.obs_numel;
+  WarpStage ws = clear_stages<F>(p, a);
   // Wait for the previous step's kernel (it wrote the lane state read below), THEN allow the next step's kernel
   // to become resident: its CTAs park at their own wait, so at most one dependent grid is ever pending.
-  // (The observation-only launch of a split host step must not wait for its predecessor -- the transitions launch,
-  // whose copiers are still shipping scalars over PCIe -- to END: it waits for that launch's phase-1 flag below.)
-  if (a.use_pdl) { if (a.phase != 2) pdl_wait(); pdl_launch_dependents(); }
+  if (a.use_pdl) { pdl_wait(); pdl_launch_dependents(); }
   int64_t step0 = a.step0;
   if (a.clock) step0 += (int64_t)*reinterpret_cast<volatile unsigned long long*>(a.clock + 16 * (blockIdx.x % CLOCK_GROUPS));
-
-  // Caller-owned buffers: launch arguments, or -- doorbell mode -- whatever the host wrote into the mailbox
-  // before it rang this launch's ticket.
-  MailFields io;
-  io.actions = a.actions; io.obs = a.obs; io.reward = a.reward; io.reward_f64 = a.reward_f64;
-  io.discount = a.discount; io.step_type = a.step_type; io.obs_vec_ok = a.obs_vec_ok; io.pad = 0;
-  bool cancelled = false;
-  if (a.mailbox && a.wait_doorbell) {
-    if (blockIdx.x == 0 && warp == 0) {
-      // The one poller of host memory: lanes 0..7 read the mailbox's first 64-byte line (doorbell + fields) with ONE
-      // coalesced request per poll; when the ring shows, the line is read once more (the host wrote the fields
-      // before the doorbell, so this second read cannot be stale), parked in device memory, and the ticket is
-      // relayed to the other blocks through L2.
-      const volatile unsigned long long* line = &a.mailbox->doorbell;
-      const unsigned long long deadline = global_timer_ns() + a.doorbell_timeout_ns;
-      unsigned long long word = 0, seen;
-      do {
-        if (tid < 8) word = ld_sys_u64(line + tid);
-        seen = __shfl_sync(0xffffffffu, word, 0);
-      } while ((seen & ~MAIL_CANCEL) < a.ticket && global_timer_ns() < deadline);
-      if ((seen & ~MAIL_CANCEL) < a.ticket) seen = a.ticket | MAIL_CANCEL;        // nobody rang: stand down
-      __threadfence_system();
-      if (tid < 8) word = ld_sys_u64(line + tid);
-      if (tid >= 1 && tid < 8) reinterpret_cast<unsigned long long*>(&a.mail->in)[tid - 1] = word;
-      __threadfence();
-      __syncwarp();
-      if (tid == 0) a.mail->relay = seen;
-    }
-    if (threadIdx.x == 0) {
-      unsigned long long seen;
-      do { seen = a.mail->relay; } while ((seen & ~MAIL_CANCEL) < a.ticket);
-      __threadfence();
-      mail_cancel = (seen & MAIL_CANCEL) ? 1 : 0;
-      const volatile unsigned long long* src = reinterpret_cast<const volatile unsigned long long*>(&a.mail->in);
-      unsigned long long* dst = reinterpret_cast<unsigned long long*>(&mail_in);
-      for (int k = 0; k < (int)(sizeof(MailFields) / 8); ++k) dst[k] = src[k];
-    }
-    __syncthreads();
-    io = mail_in;
-    cancelled = mail_cancel != 0;
-  }
+  bool cancelled;
+  const MailFields io = receive_doorbell(a, cancelled);
   const bool vec = io.obs_vec_ok != 0;
 
   const int cl = a.chunk_lanes;
   const int64_t n_chunks = (B + cl - 1) / cl;
   const bool dynamic = a.work_counter != nullptr;
   const bool lazy = a.lazy_fetch != 0;
-  // The elected lane draws chunk indices [total_warps, n_chunks) from the global counter and broadcasts them
-  // with a shuffle; chunk (global warp index) is taken without asking.
-  // Two-phase host steps set the first blocks aside as COPIERS (see below): they own no chunks at first.
-  const bool two_phase = ObsFromState<F>::value && a.early_scalars > 0 && a.mailbox && !cancelled;
-  const unsigned copier_blocks = two_phase ? (unsigned)a.early_scalars : 0u;
-  const unsigned worker_blocks = gridDim.x - copier_blocks;
-  const unsigned worker_block = blockIdx.x - copier_blocks;
-  const int64_t total_warps = (int64_t)worker_blocks * warps_per_cta;
-  auto fetch_chunk = [&]() -> int64_t {
-    unsigned long long v = 0;
-    if (tid == 0) v = atomicAdd(a.work_counter, 1ull) - a.work_base;      // graph-safe mode: clock + 1, base 0
-    return total_warps + (int64_t)__shfl_sync(0xffffffffu, v, 0);
-  };
-  int64_t cur_chunk = (int64_t)worker_block * warps_per_cta + warp;
+  const int64_t total_warps = (int64_t)gridDim.x * warps_per_cta;
   if (cancelled) {
     // A stood-down launch still owes the chunk counter its share: a launch over C chunks advances it by exactly C.
-    // (a two-phase launch also owes one failing fetch per copier warp, which the host's arithmetic counts too)
-    if (dynamic && blockIdx.x == 0 && threadIdx.x == 0)
-      atomicAdd(a.work_counter, (unsigned long long)n_chunks + (unsigned long long)(a.early_scalars > 0 ? a.early_scalars * warps_per_cta : 0));
-    cur_chunk = n_chunks;
+    if (dynamic && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(a.work_counter, (unsigned long long)n_chunks);
+    retire_warp(a, ws, false);
+    signal_done(a, a.ticket | MAIL_CANCEL);
+    return;                                  // host steps never carry the device clock
   }
-
-  const bool has_rng = p.rng_pos != nullptr;
-  // catch: cells this thread poked into stage buffer 0 / 1 (cleared when that buffer is reused)
-  int poked_a0 = -1, poked_b0 = -1, poked_a1 = -1, poked_b1 = -1;
-  // deep_sea bulk path: offset of the cell this thread poked into group buffer 0 / 1 (cleared on reuse)
-  int tile_poked0 = -1, tile_poked1 = -1;
-  unsigned emitted = 0;          // bulk stores issued by this warp so far (double-buffer parity)
-  bool any_bulk = false;
-
-  // Observation emitter of this warp for one chunk and step (shared by the ordinary loop and by the two-phase
-  // host-step path below); the staging state above persists across calls.
-  auto emit_obs = [&](const typename F::Lane& L, R& rng, float* obs_t, int64_t warp_base, int n_lanes, int64_t lane,
-                      bool active, bool bulk) {
-    if (kEmit == EMIT_ONEHOT) {
-      const int hot = Descriptor<F>::a(L);
-      if (bulk) {
-        // Groups of m consecutive lanes share one staging buffer (m tiles, contiguous in global memory too) and
-        // leave as ONE bulk store of up to m * 4K bytes: large stores amortise the per-operation cost of the
-        // TMA unit.
-        const int m = a.group_lanes;
-        for (int g0 = 0; g0 < n_lanes; g0 += m) {
-          const int in_group = (n_lanes - g0) < m ? (n_lanes - g0) : m;
-          const int s = (int)(emitted & 1u);
-          float* group = stage + (size_t)s * m * K;
-          if (tid == 0) bulk_wait_read<TILE_STAGES - 1>();    // the store two back, last reader of `group`, is done
-          __syncwarp();
-          if (s == 0) { if (tile_poked0 >= 0) { group[tile_poked0] = 0.f; tile_poked0 = -1; } }
-          else        { if (tile_poked1 >= 0) { group[tile_poked1] = 0.f; tile_poked1 = -1; } }
-          __syncwarp();     // a thread of an earlier group may clear the very cell another thread sets now
-          if (tid >= g0 && tid < g0 + in_group && hot >= 0) {
-            const int cell = (tid - g0) * K + hot;
-            group[cell] = 1.f;
-            if (s == 0) tile_poked0 = cell; else tile_poked1 = cell;
-          }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (tid == 0) {
-            float* tile_dst = obs_t + (warp_base + g0) * (int64_t)K;
-            const uint32_t tile_bytes = (uint32_t)in_group * (uint32_t)K * 4u;
-            bulk_store_obs(tile_dst, group, tile_bytes, a.l2_hint);
-            bulk_commit();
-          }
-          ++emitted;
-        }
-      } else {
-        emit_onehot_vec(obs_t, warp_base, n_lanes, K, hot, vec && (K & 3) == 0);
-      }
-    } else if (kEmit == EMIT_TWOHOT) {
-      const int hot_a = Descriptor<F>::a(L), hot_b = Descriptor<F>::b(L);
-      if (bulk) {
-        const int buf = (int)(emitted & row_mask);
-        float* boards = stage + (size_t)buf * 32 * K;
-        if (tid == 0) { if (row_mask) bulk_wait_read<1>(); else bulk_wait_read<0>(); }   // the store that last read `boards` is done with it
-        __syncwarp();
-        float* mine = boards + tid * K;
-        const int old_a = buf ? poked_a1 : poked_a0, old_b = buf ? poked_b1 : poked_b0;
-        if (old_a >= 0) mine[old_a] = 0.f;
-        if (old_b >= 0) mine[old_b] = 0.f;
-        int new_a = -1, new_b = -1;
-        if (active) { mine[hot_a] = 1.f; mine[hot_b] = 1.f; new_a = hot_a; new_b = hot_b; }
-        if (buf) { poked_a1 = new_a; poked_b1 = new_b; } else { poked_a0 = new_a; poked_b0 = new_b; }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (tid == 0) { bulk_store_obs(obs_t + warp_base * (int64_t)K, boards, (uint32_t)n_lanes * (uint32_t)K * 4u, a.l2_hint); bulk_commit(); }
-        ++emitted;
-      } else {
-        emit_twohot_vec(obs_t, warp_base, n_lanes, K, hot_a, hot_b, vec);
-      }
-    } else if (kEmit == EMIT_IMAGE) {
-      const int image = Descriptor<F>::a(L);
-      if (bulk) emit_image_bulk(p, stage, cta_zero, obs_t, warp_base, n_lanes, K, active ? image : -1, a.group_lanes,
-                                a.cta_extra_floats / K, a.l2_hint, a.stage_rows, emitted);
-      else emit_image(p, stage, obs_t, warp_base, n_lanes, K, image, vec && (K & 3) == 0);
-    } else if (!a.stage_rows) {
-      // observation rows too long for a shared-memory stage: every thread renders its row in place
-      if (active) RowRenderer<F, R>::run(p, L, rng, obs_t + lane * (int64_t)K);
-    } else {
-      float* rows = stage + (size_t)(emitted & row_mask) * 32 * K;
-      if (bulk) { if (tid == 0) { if (row_mask) bulk_wait_read<1>(); else bulk_wait_read<0>(); } }
-      __syncwarp();
-      if (active) RowRenderer<F, R>::run(p, L, rng, rows + tid * K);
-      if (bulk) {
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (tid == 0) { bulk_store_obs(obs_t + warp_base * (int64_t)K, rows, (uint32_t)n_lanes * (uint32_t)K * 4u, a.l2_hint); bulk_commit(); }
-      } else {
-        __syncwarp();
-        flush_rows_vec(rows, obs_t, warp_base, n_lanes, K, vec);
-      }
-      ++emitted;
-    }
-  };
-  // Which chunks leave through the TMA unit (16-byte aligned spans); warp-uniform per chunk.
-  auto chunk_is_bulk = [&](int n_lanes) -> bool {
-    bool bulk = a.emit_bulk && vec;
-    if (kEmit == EMIT_ROWS) bulk = bulk && K >= 3 && ((n_lanes * K) & 3) == 0;
-    if (kEmit == EMIT_TWOHOT) bulk = bulk && ((n_lanes * K) & 3) == 0;
-    if (kEmit == EMIT_ONEHOT) bulk = bulk && ((K & 3) == 0 || ((n_lanes % a.group_lanes) == 0 && ((a.group_lanes * K) & 3) == 0));
-    if (kEmit == EMIT_IMAGE) bulk = bulk && (K & 3) == 0;
-    return bulk;
-  };
-
-  // ---- two-phase host step (a.early_scalars; families whose observation is a function of the stored state) ----
-  // A host-driven step (bsb_step_host) returns when reward / discount / step_type are in host memory; the
-  // observation stays on the device.  So the transitions of ALL chunks run first (phase 1: statically dealt; the
-  // actions of a warp's chunks are fetched over PCIe in one round trip), and the observations are streamed
-  // afterwards (phase 2, dynamically dealt as usual) while the host already decides the next action.  Phase 2
-  // re-reads the lane state phase 1 stored (L2-resident) and renders from it; a warp's first chunk stays in
-  // registers.
-  // Who ships the scalars to the host?  Not the workers: 768 KB of posted PCIe writes per step back-pressure the
-  // warps that issue them (tools/e2e_timeline.py shows it: a phase 1 that writes to host memory takes several times
-  // longer), and they have 268 MB of observations to issue.  The workers write reward / discount / step_type to a DEVICE staging block, fence at GPU scope and
-  // count themselves out.  The first `early_scalars` blocks, the COPIERS, own no chunks at first: they wait for
-  // that count, copy the staging block to the host's pinned buffers with 16-byte stores (16 per thread in flight:
-  // ~128 KB across the copiers, enough for the link), issue the system fence, and the last one stores the completion
-  // word; then they join phase 2 through the chunk counter like everybody else.
-  // (PTX memory model: workers release / copiers acquire at gpu scope; the copiers' own stores, fence.sc.sys and the
-  // completion word are program-ordered; the host's acquire load of the word therefore sees every scalar.)
-  if constexpr (ObsFromState<F>::value) {
-    if (two_phase && blockIdx.x < copier_blocks) {
-      if (threadIdx.x == 0) {
-        const unsigned long long t_start = a.timing ? global_timer_ns() : 0ull;
-        while (*reinterpret_cast<volatile unsigned long long*>(&a.mail->finished) < (unsigned long long)worker_blocks) {}
-        if (blockIdx.x == 0) {
-          a.mail->phase1 = a.ticket;         // every chunk's state is stored: phase 2 may read any lane's state
-          if (a.timing) {
-            st_sys_u64(&a.mailbox->stamp[0], t_start);
-            st_sys_u64(&a.mailbox->stamp[1], global_timer_ns());
-            st_sys_u64(&a.mailbox->stamp[3], a.mail->last_exit);
-          }
-        }
-      }
-      __syncthreads();
-      __threadfence();                       // acquire: the staging block is read below
-      const int64_t n_thr = (int64_t)copier_blocks * blockDim.x, me = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-      auto ship = [&](const void* from, void* to, int64_t bytes) {
-        if (!from || !to) return;
-        if ((reinterpret_cast<uintptr_t>(from) | reinterpret_cast<uintptr_t>(to)) & 15) {      // odd batch sizes: words
-          const uint32_t* s32 = reinterpret_cast<const uint32_t*>(from);
-          uint32_t* d32 = reinterpret_cast<uint32_t*>(to);
-          for (int64_t i = me; i < (bytes >> 2); i += n_thr) d32[i] = __ldcg(s32 + i);
-          return;
-        }
-        const uint4* src = reinterpret_cast<const uint4*>(from);
-        uint4* dst = reinterpret_cast<uint4*>(to);
-        const int64_t n16 = bytes >> 4;
-        constexpr int U = 16;     // 16 x 16 B per thread in flight: ~128 KB across the copiers, enough for the PCIe link
-        for (int64_t i0 = me; i0 < n16; i0 += U * n_thr) {
-          uint4 v[U];
-#pragma unroll
-          for (int u = 0; u < U; ++u) { const int64_t i = i0 + u * n_thr; if (i < n16) v[u] = __ldcg(src + i); }
-#pragma unroll
-          for (int u = 0; u < U; ++u) { const int64_t i = i0 + u * n_thr; if (i < n16) dst[i] = v[u]; }
-        }
-        const char* tail_src = reinterpret_cast<const char*>(from) + (n16 << 4);
-        char* tail_dst = reinterpret_cast<char*>(to) + (n16 << 4);
-        for (int64_t i = me; i < (bytes & 15); i += n_thr) tail_dst[i] = tail_src[i];
-      };
-      ship(a.stage.reward, io.reward, B * 4);
-      ship(a.stage.reward_f64, io.reward_f64, B * 8);
-      ship(a.stage.discount, io.discount, B * 4);
-      ship(a.stage.step_type, io.step_type, B * 4);
-      __threadfence_system();
-      __syncthreads();
-      if (threadIdx.x == 0 && atomicAdd(&a.mail->copied, 1ull) == (unsigned long long)copier_blocks - 1ull) {
-        a.mail->finished = 0ull;             // every copier is past its wait: re-arm both counts for the next launch
-        a.mail->copied = 0ull;
-        __threadfence_system();
-        if (a.timing) st_sys_u64(&a.mailbox->stamp[2], global_timer_ns());
-        st_sys_u64(&a.mailbox->done, a.ticket);      // the host may read its scalars
-      }
-      // join phase 2: the copiers own no chunk of their own, the counter deals them the rest
-      cur_chunk = n_chunks;
-      if (dynamic) {
-        typename F::Lane L;
-        int64_t c = fetch_chunk();
-        while (c < n_chunks) {
-          const int64_t warp_base = c * cl;
-          const int n_lanes = (B - warp_base) < cl ? (int)(B - warp_base) : cl;
-          const int64_t lane = warp_base + tid;
-          const bool active = tid < n_lanes;
-          F::init(p, L);
-          if (active) { F::load(p, lane, L); F::describe(p, L); }
-          const bool bulk = chunk_is_bulk(n_lanes);
-          any_bulk = any_bulk || bulk;
-          R unused_rng;
-          emit_obs(L, unused_rng, io.obs, warp_base, n_lanes, lane, active, bulk);
-          c = fetch_chunk();
-        }
-      }
-    } else if (two_phase) {
-      const int64_t own = cur_chunk;
-      typename F::Lane keep;
-      F::init(p, keep);
-      constexpr int kAhead = 4;              // chunks whose loads (action, lane state, accumulators) are in flight together
-      for (int64_t c0 = own; c0 < n_chunks; c0 += kAhead * total_warps) {
-        // every independent load of up to kAhead chunks first: one round trip to L2 (or over PCIe, when the actions
-        // were not staged on the device) instead of one per chunk -- a warp owns 4-5 chunks of a 65 536-lane batch
-        int32_t fetched[kAhead];
-        typename F::Lane lanes[kAhead];
-        EpisodeStats eps[kAhead];
-#pragma unroll
-        for (int k = 0; k < kAhead; ++k) {
-          const int64_t c = c0 + k * total_warps;
-          const int64_t lane = c * cl + tid;
-          const bool live = c < n_chunks && tid < cl && lane < B;
-          fetched[k] = 0;
-          F::init(p, lanes[k]);
-          if (live) {
-            fetched[k] = __ldcv(io.actions + lane);
-            F::load(p, lane, lanes[k]);
-            if (kTrack) eps[k].load(p, lane);
-          }
-        }
-#pragma unroll
-        for (int k = 0; k < kAhead; ++k) {
-          const int64_t c = c0 + k * total_warps;
-          if (c >= n_chunks) break;
-          const int64_t lane = c * cl + tid;
-          typename F::Lane& L = lanes[k];
-          if (tid < cl && lane < B) {
-            R rng, wrng;
-            if (has_rng) rng_open(rng, p, lane, false);
-            if (kNoise) rng_open(wrng, p, lane, true);
-            int32_t action = fetched[k];
-            if ((uint32_t)action >= (uint32_t)p.num_actions) {
-              if (a.bad_action) *a.bad_action = 1;
-              action = action < 0 ? 0 : p.num_actions - 1;
-            }
-            const bool after_last = L.nr != 0;
-            const StepOut o = lane_transition<F, R, R>(p, lane, L, rng, wrng, action, MODE_STEP, kNoise);
-            F::store(p, lane, L);
-            if (has_rng) rng_close(rng, p, lane, false);
-            if (kNoise) rng_close(wrng, p, lane, true);
-            if (kTrack) {
-              eps[k].track(p, lane, o, step0, after_last);
-              eps[k].store(p, lane);
-              if (p.log_rows && o.step_type == LAST && log_row_due(p, lane)) log_row_write(p, lane, step0 + 1);
-            }
-            if (a.stage.reward) a.stage.reward[lane] = (float)o.reward;
-            if (a.stage.reward_f64) a.stage.reward_f64[lane] = o.reward;
-            if (a.stage.discount) a.stage.discount[lane] = o.discount;
-            if (a.stage.step_type) a.stage.step_type[lane] = o.step_type;
-          }
-          if (c == own) keep = L;
-        }
-      }
-      __threadfence();                       // gpu scope (device memory only): the copiers do the system-scope one
-      __syncthreads();
-      if (threadIdx.x == 0) atomicAdd(&a.mail->finished, 1ull);
-      bool mine = true;
-      int64_t c = a.phase == 1 ? n_chunks : own;      // split step: the observations are the next launch's
-      while (c < n_chunks) {
-        const int64_t warp_base = c * cl;
-        const int n_lanes = (B - warp_base) < cl ? (int)(B - warp_base) : cl;
-        const int64_t lane = warp_base + tid;
-        const bool active = tid < n_lanes;
-        typename F::Lane L = keep;
-        if (!mine) {
-          // a dynamically dealt chunk: some other warp ran its phase 1 -- long ago in practice, but wait for it
-          if (tid == 0) while (a.mail->phase1 != a.ticket) {}
-          __syncwarp();
-          __threadfence();                   // acquire: the loads below must not be served from a stale L1 line
-          F::init(p, L);
-          if (active) { F::load(p, lane, L); F::describe(p, L); }
-        }
-        const bool bulk = chunk_is_bulk(n_lanes);
-        any_bulk = any_bulk || bulk;
-        R unused_rng;
-        emit_obs(L, unused_rng, io.obs, warp_base, n_lanes, lane, active, bulk);
-        mine = false;
-        c = dynamic ? fetch_chunk() : n_chunks;
-      }
-      cur_chunk = n_chunks;                  // nothing left for the ordinary loop
-    } else if (a.phase == 2) {
-      // Observation-only launch of a split host step: the transitions launch ahead of it in the stream stored every
-      // lane's state and raised mail->phase1; render from the stored state, chunks dealt as usual.
-      if (tid == 0) while (a.mail->phase1 != a.ticket) {}
-      __syncwarp();
-      __threadfence();                       // acquire
-      int64_t c = cur_chunk;
-      while (c < n_chunks) {
-        const int64_t warp_base = c * cl;
-        const int n_lanes = (B - warp_base) < cl ? (int)(B - warp_base) : cl;
-        const int64_t lane = warp_base + tid;
-        const bool active = tid < n_lanes;
-        typename F::Lane L;
-        F::init(p, L);
-        if (active) { F::load(p, lane, L); F::describe(p, L); }
-        const bool bulk = chunk_is_bulk(n_lanes);
-        any_bulk = any_bulk || bulk;
-        R unused_rng;
-        emit_obs(L, unused_rng, io.obs, warp_base, n_lanes, lane, active, bulk);
-        c = dynamic ? fetch_chunk() : n_chunks;
-      }
-      cur_chunk = n_chunks;
-    }
-  }
+  int64_t cur_chunk = (int64_t)blockIdx.x * warps_per_cta + warp;
 
   while (cur_chunk < n_chunks) {
     const int64_t warp_base = cur_chunk * cl;
     // eager policy: reserve the next chunk now; lazy (default): only after this chunk's stores are issued
-    cur_chunk = (dynamic && !lazy) ? fetch_chunk() : n_chunks;
+    cur_chunk = (dynamic && !lazy) ? fetch_chunk(a, total_warps) : n_chunks;
     const int n_lanes = (B - warp_base) < cl ? (int)(B - warp_base) : cl;
     const int64_t lane = warp_base + tid;
     const bool active = tid < n_lanes;
-    const bool bulk = chunk_is_bulk(n_lanes);
-    any_bulk = any_bulk || bulk;
+    const bool bulk = chunk_is_bulk<F>(p, a, vec, n_lanes);
+    ws.any_bulk = ws.any_bulk || bulk;
 
     typename F::Lane L;
     R rng, wrng;
     EpisodeStats ep;
     ActionStream action_stream;
     action_stream.open();
-    if (active) {
-      if (a.mode == MODE_INIT) F::init(p, L); else F::load(p, lane, L);
-      if (has_rng) rng_open(rng, p, lane, false);
-      if (kNoise) rng_open(wrng, p, lane, true);
-      if (kTrack) ep.load(p, lane);
-    } else {
-      F::init(p, L);
-    }
-
-    if (a.mode == MODE_INIT) {
-      if (active) {
-        F::ctor_draws(p, L, rng);
-        F::store(p, lane, L);
-        if (has_rng) rng_close(rng, p, lane, false);
-      }
-      if (dynamic && lazy) cur_chunk = fetch_chunk();
-      continue;
-    }
+    if (active) lane_open<F>(p, lane, L, rng, wrng, ep, a.mode, kNoise, kTrack);
+    else F::init(p, L);
+    if (a.mode == MODE_INIT && active) F::ctor_draws(p, L, rng);      // the constructor runs no step (T = 0)
 
     for (int64_t t = 0; t < a.T; ++t) {
       const int64_t off = t * B + lane;
@@ -978,50 +850,16 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
           }
           if (a.actions_out) a.actions_out[off] = action;
         }
-        const bool after_last = L.nr != 0;
-        const StepOut o = lane_transition<F, R, R>(p, lane, L, rng, wrng, action, a.mode, kNoise);
-        if (kTrack) {
-          ep.track(p, lane, o, step0 + t, after_last);
-          if (p.log_rows && o.step_type == LAST && log_row_due(p, lane)) {      // <= 49 times per 10 000 episodes
-            F::store(p, lane, L); ep.store(p, lane);
-            log_row_write(p, lane, step0 + t + 1);
-          }
-        }
-        if (io.reward) io.reward[off] = (float)o.reward;
-        if (io.reward_f64) io.reward_f64[off] = o.reward;
-        if (io.discount) io.discount[off] = o.discount;
-        if (io.step_type) io.step_type[off] = o.step_type;
+        lane_step<F>(p, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, io, off);
       }
-      float* obs_t = io.obs + t * B * (int64_t)K;
-
-      emit_obs(L, rng, obs_t, warp_base, n_lanes, lane, active, bulk);
+      emit_obs<F>(p, a, ws, L, rng, io.obs + t * B * (int64_t)K, warp_base, n_lanes, lane, active, bulk, vec);
     }
 
-    if (active) {
-      F::store(p, lane, L);
-      if (has_rng) rng_close(rng, p, lane, false);
-      if (kNoise) rng_close(wrng, p, lane, true);
-      if (kTrack) ep.store(p, lane);
-    }
-    if (dynamic && lazy) cur_chunk = fetch_chunk();        // lazy: nothing was reserved while working
+    if (active) lane_close<F>(p, lane, L, rng, wrng, ep, kNoise, kTrack);
+    if (dynamic && lazy) cur_chunk = fetch_chunk(a, total_warps);        // lazy: nothing was reserved while working
   }
-  if (any_bulk && tid == 0) {
-    // shared memory must outlive the last bulk read; in doorbell mode the host takes `done` to mean that the
-    // observations are in device memory, so there the stores themselves must have completed
-    if (a.mailbox && !a.early_scalars) bulk_wait_all(); else bulk_wait_read<0>();
-  }
-  if (a.timing && a.mail && threadIdx.x == 0) atomicMax(&a.mail->last_exit, global_timer_ns());
-  if (a.mailbox && !two_phase) {
-    __threadfence_system();                  // every thread: its zero-copy outputs are visible to the host ...
-    __syncthreads();                         // ... before the CTA counts itself finished
-    if (threadIdx.x == 0) {
-      if (atomicAdd(&a.mail->finished, 1ull) == (unsigned long long)gridDim.x - 1ull) {
-        a.mail->finished = 0ull;
-        __threadfence_system();
-        st_sys_u64(&a.mailbox->done, a.ticket | (cancelled ? MAIL_CANCEL : 0ull));
-      }
-    }
-  }
+  retire_warp(a, ws, a.mailbox != nullptr);
+  if (a.mailbox) signal_done(a, a.ticket);
   if (a.clock) {
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -1043,6 +881,191 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
       }
     }
   }
+}
+
+// ----- the two-phase host step ------------------------------------------------------------------------------------
+// Families whose observation is a function of the STORED lane state (ObsFromState: deep_sea, catch), host-driven
+// steps (bsb_step_host) on pinned buffers.  Such a step returns when reward / discount / step_type are in host
+// memory; the observation stays on the device.  So the transitions of ALL chunks run first (phase 1: statically
+// dealt; the actions of a warp's chunks are fetched in one round trip), and the observations are streamed
+// afterwards (phase 2, dynamically dealt as usual) while the host already decides the next action.  Phase 2
+// re-reads the lane state phase 1 stored (L2-resident) and renders from it; a warp's first chunk stays in
+// registers.
+// Who ships the scalars to the host?  Not the workers: 768 KB of posted PCIe writes per step back-pressure the
+// warps that issue them (tools/e2e_timeline.py shows it: a phase 1 that writes to host memory takes several times
+// longer), and they have 268 MB of observations to issue.  The workers write reward / discount / step_type to a
+// DEVICE staging block, fence at GPU scope and count themselves out.  The first `h.copiers` blocks, the COPIERS, own
+// no chunks at first: they wait for that count, copy the staging block to the host's pinned buffers with 16-byte
+// stores (16 per thread in flight: ~128 KB across the copiers, enough for the link), issue the system fence, and
+// the last one stores the completion word; then they join phase 2 through the chunk counter like everybody else.
+// (PTX memory model: workers release / copiers acquire at gpu scope; the copiers' own stores, fence.sc.sys and the
+// completion word are program-ordered; the host's acquire load of the word therefore sees every scalar.)
+// A step split over two launches (h.phase 1 / 2, BSB_HOST_NO_WAIT) runs phase 1 with the copiers in the first and
+// phase 2 in the second, which waits for mail->phase1 instead of for the first launch to end.  Host steps never
+// run in graph-safe mode (the launcher checks): there is no device clock here.
+template <class F, int RK, bool kNoise, bool kTrack>
+__global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F))
+two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs h) {
+  static_assert(ObsFromState<F>::value, "the two-phase host step renders observations from the stored lane state");
+  typedef typename RngOf<RK>::type R;
+  const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
+  const int64_t B = p.batch;
+  WarpStage ws = clear_stages<F>(p, a);
+  // The observation-only launch must not wait for its predecessor -- the transitions launch, whose copiers are
+  // still shipping scalars over PCIe -- to END: it waits for that launch's phase-1 flag instead.
+  if (a.use_pdl) { if (h.phase != 2) pdl_wait(); pdl_launch_dependents(); }
+  bool cancelled;
+  const MailFields io = receive_doorbell(a, cancelled);
+  const bool vec = io.obs_vec_ok != 0;
+
+  const int cl = a.chunk_lanes;
+  const int64_t n_chunks = (B + cl - 1) / cl;
+  const bool dynamic = a.work_counter != nullptr;
+  if (cancelled) {
+    // A stood-down launch still owes the chunk counter its share: C chunks plus one failing fetch per copier warp.
+    if (dynamic && blockIdx.x == 0 && threadIdx.x == 0)
+      atomicAdd(a.work_counter, (unsigned long long)n_chunks + (unsigned long long)h.copiers * warps_per_cta);
+    retire_warp(a, ws, false);
+    signal_done(a, a.ticket | MAIL_CANCEL);
+    return;
+  }
+  const unsigned copier_blocks = (unsigned)h.copiers;
+  const unsigned worker_blocks = gridDim.x - copier_blocks;
+  const int64_t total_warps = (int64_t)worker_blocks * warps_per_cta;
+  const int64_t own = (int64_t)(blockIdx.x - copier_blocks) * warps_per_cta + warp;      // workers only
+
+  // Phase 2: streams the observations of chunk c and of every chunk the counter deals after it, rendered from the
+  // stored lane state.  `kept`: chunk c is the warp's own, its state `first` still in registers from phase 1.
+  auto render_stored = [&](int64_t c, bool kept, const typename F::Lane& first) {
+    while (c < n_chunks) {
+      const int64_t warp_base = c * cl;
+      const int n_lanes = (B - warp_base) < cl ? (int)(B - warp_base) : cl;
+      const int64_t lane = warp_base + tid;
+      const bool active = tid < n_lanes;
+      typename F::Lane L = first;
+      if (!kept) {
+        // some other warp ran this chunk's phase 1 -- long ago in practice, but wait for every chunk's
+        if (tid == 0) while (a.mail->phase1 != a.ticket) {}
+        __syncwarp();
+        __threadfence();                   // acquire: the loads below must not be served from a stale L1 line
+        F::init(p, L);
+        if (active) { F::load(p, lane, L); F::describe(p, L); }
+      }
+      const bool bulk = chunk_is_bulk<F>(p, a, vec, n_lanes);
+      ws.any_bulk = ws.any_bulk || bulk;
+      R unused_rng;
+      emit_obs<F>(p, a, ws, L, unused_rng, io.obs, warp_base, n_lanes, lane, active, bulk, vec);
+      kept = false;
+      c = dynamic ? fetch_chunk(a, total_warps) : n_chunks;
+    }
+  };
+  typename F::Lane keep;
+  F::init(p, keep);
+
+  if (blockIdx.x < copier_blocks) {
+    if (threadIdx.x == 0) {
+      const unsigned long long t_start = a.timing ? global_timer_ns() : 0ull;
+      while (*reinterpret_cast<volatile unsigned long long*>(&a.mail->finished) < (unsigned long long)worker_blocks) {}
+      if (blockIdx.x == 0) {
+        a.mail->phase1 = a.ticket;         // every chunk's state is stored: phase 2 may read any lane's state
+        if (a.timing) {
+          st_sys_u64(&a.mailbox->stamp[0], t_start);
+          st_sys_u64(&a.mailbox->stamp[1], global_timer_ns());
+          st_sys_u64(&a.mailbox->stamp[3], a.mail->last_exit);
+        }
+      }
+    }
+    __syncthreads();
+    __threadfence();                       // acquire: the staging block is read below
+    const int64_t n_thr = (int64_t)copier_blocks * blockDim.x, me = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    auto ship = [&](const void* from, void* to, int64_t bytes) {
+      if (!from || !to) return;
+      if ((reinterpret_cast<uintptr_t>(from) | reinterpret_cast<uintptr_t>(to)) & 15) {      // odd batch sizes: words
+        const uint32_t* s32 = reinterpret_cast<const uint32_t*>(from);
+        uint32_t* d32 = reinterpret_cast<uint32_t*>(to);
+        for (int64_t i = me; i < (bytes >> 2); i += n_thr) d32[i] = __ldcg(s32 + i);
+        return;
+      }
+      const uint4* src = reinterpret_cast<const uint4*>(from);
+      uint4* dst = reinterpret_cast<uint4*>(to);
+      const int64_t n16 = bytes >> 4;
+      constexpr int U = 16;     // 16 x 16 B per thread in flight: ~128 KB across the copiers, enough for the PCIe link
+      for (int64_t i0 = me; i0 < n16; i0 += U * n_thr) {
+        uint4 v[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) { const int64_t i = i0 + u * n_thr; if (i < n16) v[u] = __ldcg(src + i); }
+#pragma unroll
+        for (int u = 0; u < U; ++u) { const int64_t i = i0 + u * n_thr; if (i < n16) dst[i] = v[u]; }
+      }
+      const char* tail_src = reinterpret_cast<const char*>(from) + (n16 << 4);
+      char* tail_dst = reinterpret_cast<char*>(to) + (n16 << 4);
+      for (int64_t i = me; i < (bytes & 15); i += n_thr) tail_dst[i] = tail_src[i];
+    };
+    ship(h.stage.reward, io.reward, B * 4);
+    ship(h.stage.reward_f64, io.reward_f64, B * 8);
+    ship(h.stage.discount, io.discount, B * 4);
+    ship(h.stage.step_type, io.step_type, B * 4);
+    __threadfence_system();
+    __syncthreads();
+    if (threadIdx.x == 0 && atomicAdd(&a.mail->copied, 1ull) == (unsigned long long)copier_blocks - 1ull) {
+      a.mail->finished = 0ull;             // every copier is past its wait: re-arm both counts for the next launch
+      a.mail->copied = 0ull;
+      __threadfence_system();
+      if (a.timing) st_sys_u64(&a.mailbox->stamp[2], global_timer_ns());
+      st_sys_u64(&a.mailbox->done, a.ticket);      // the host may read its scalars
+    }
+    // join phase 2: the copiers own no chunk of their own, the counter deals them the rest
+    render_stored(dynamic ? fetch_chunk(a, total_warps) : n_chunks, false, keep);
+  } else if (h.phase == 2) {
+    // observation-only launch: the transitions launch ahead of it in the stream stored every lane's state
+    render_stored(own, false, keep);
+  } else {
+    constexpr int kAhead = 4;              // chunks whose loads (action, lane state, accumulators) are in flight together
+    for (int64_t c0 = own; c0 < n_chunks; c0 += kAhead * total_warps) {
+      // every independent load of up to kAhead chunks first: one round trip to L2 (or over PCIe, when the actions
+      // were not staged on the device) instead of one per chunk -- a warp owns 4-5 chunks of a 65 536-lane batch
+      int32_t fetched[kAhead];
+      typename F::Lane lanes[kAhead];
+      EpisodeStats eps[kAhead];
+#pragma unroll
+      for (int k = 0; k < kAhead; ++k) {
+        const int64_t c = c0 + k * total_warps;
+        const int64_t lane = c * cl + tid;
+        const bool live = c < n_chunks && tid < cl && lane < B;
+        fetched[k] = 0;
+        F::init(p, lanes[k]);
+        if (live) {
+          fetched[k] = __ldcv(io.actions + lane);
+          F::load(p, lane, lanes[k]);
+          if (kTrack) eps[k].load(p, lane);
+        }
+      }
+#pragma unroll
+      for (int k = 0; k < kAhead; ++k) {
+        const int64_t c = c0 + k * total_warps;
+        if (c >= n_chunks) break;
+        const int64_t lane = c * cl + tid;
+        typename F::Lane& L = lanes[k];
+        if (tid < cl && lane < B) {
+          R rng, wrng;
+          lane_open<F>(p, lane, L, rng, wrng, eps[k], MODE_STEP, kNoise, kTrack, /*state_loaded=*/true);
+          int32_t action = fetched[k];
+          if ((uint32_t)action >= (uint32_t)p.num_actions) {
+            if (a.bad_action) *a.bad_action = 1;
+            action = action < 0 ? 0 : p.num_actions - 1;
+          }
+          lane_step<F>(p, lane, L, rng, wrng, eps[k], action, MODE_STEP, kNoise, kTrack, a.step0, h.stage, lane);
+          lane_close<F>(p, lane, L, rng, wrng, eps[k], kNoise, kTrack);
+        }
+        if (c == own) keep = L;
+      }
+    }
+    __threadfence();                       // gpu scope (device memory only): the copiers do the system-scope one
+    __syncthreads();
+    if (threadIdx.x == 0) atomicAdd(&a.mail->finished, 1ull);
+    render_stored(h.phase == 1 ? n_chunks : own, true, keep);      // split step: the observations are the next launch's
+  }
+  retire_warp(a, ws, false);
 }
 
 #endif  // __CUDACC__

@@ -1,8 +1,10 @@
-// catch: kernel instantiations (Philox / MT19937 x RewardNoise x Logging accumulators) and host path.
+// catch: instantiations of both kernels (Philox / MT19937 x RewardNoise x Logging accumulators) and host path.
 #include <cstring>
 
 #include "bsb_dispatch.cuh"
 
 namespace bsb {
-int run_catch(bsb_env* e, const LaunchArgs& a, cudaStream_t stream) { return run_family<Catch>(e, a, stream); }
+int run_catch(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoPhaseArgs* two_phase) {
+  return run_family<Catch>(e, a, stream, two_phase);
+}
 }  // namespace bsb

@@ -18,7 +18,10 @@ also go through oracle.run_lanes, which anchors the comparison outside the engin
   group A  every instantiation transition_kernel<family, Philox | MT19937, noise, track> once (80 kernels);
   group B  the paths the default dispatch selects, at batch sizes derived from its rules (margins quoted for the
            132 SMs of an H100 SXM);
-  group C  every non-default value of the A/B tuning knobs, read from the environment when a handle is created.
+  group C  every non-default value of the A/B tuning knobs, read from the environment when a handle is created;
+  group H  every instantiation two_phase_host_kernel<deep_sea | catch, Philox | MT19937, noise, track> (16 kernels),
+           driven by host steps (bsb_step_host on pinned buffers): waited for, pre-launched, and BSB_HOST_NO_WAIT
+           (which splits the step over two launches).
 
 Exactness follows tests/conftest.py: integer / grid families bit for bit (step_type, discount, reward, observation,
 bsuite_info, episode_stats, log rows, state blob); float dynamics, the reward-noise wrapper and stochastic deep_sea
@@ -162,6 +165,16 @@ GROUP_B = [
     _case('umbrella_chain', 1000, dict(UMB, n_distractor=20), lane_offset=2**33 - 40),
     _case('deep_sea', 2000, dict(DS, size=12, deterministic=False), lane_offset=2**32 + 1),
 ]
+
+# group H: observations of >= 1 KB take the two-phase host step (deep_sea N = 16, catch 16 x 16)
+H_KWARGS = dict(deep_sea=dict(DS, size=16), catch=dict(rows=16, columns=16))
+HOST_MODES = ('wait', 'prelaunch', 'no_wait')
+GROUP_H = [(_case(f, 97, H_KWARGS[f], rng=r, noise=0.1 if n else None, track=t,
+                  reward_dtype='float64' if t else 'float32'), mode)
+           for f, r, n, t in itertools.product(('deep_sea', 'catch'), RNGS, (False, True), (False, True))
+           for mode in HOST_MODES]
+# deep_sea N = 16 at 30 001 lanes: 938 chunks over a persistent grid of 792 CTAs (6 per SM), copiers in front
+GROUP_H += [(_case('deep_sea', 30001, H_KWARGS['deep_sea'], track=True), mode) for mode in HOST_MODES]
 
 
 def _knob(family, batch, kwargs=None, **knobs):
@@ -351,6 +364,21 @@ class Twins:
     self.reset_at.append(self.t)
     self.check_call('reset()', outs, 0)
 
+  def step_host(self, mode):
+    """One bsb_step_host call per twin: pinned actions and scalars, the observation left on the device."""
+    acts = self.rng.randint(self.envs[0].num_actions, size=self.case['batch']).astype(np.int32)
+    outs = []
+    for env in self.envs:
+      host, out = env.make_host_buffers(), env.make_buffers()
+      actions = torch.from_numpy(acts)
+      env.step_host(actions.pin_memory() if env.device.type == 'cuda' else actions, host, out=out,
+                    prelaunch=mode == 'prelaunch', wait=mode != 'no_wait')
+      if mode == 'no_wait':
+        env.host_wait()
+      outs.append(type(out)(observation=out.observation, reward=host.reward, discount=host.discount,
+                            step_type=host.step_type))
+    self.check_call(f'step_host({mode})', outs, 0, acts[None])
+
   def run_script(self):
     case = self.case
     self.check_state('constructor')
@@ -427,18 +455,30 @@ def image_dirs(tmp_path_factory):
 
 # ------------------------------------------------------------------ CPU: the driver and the case lists
 def test_group_a_covers_every_kernel_instantiation():
-  """A new family, bit source or template flag of transition_kernel cannot appear without a group A case."""
+  """A new family, bit source or template flag of transition_kernel or two_phase_host_kernel cannot appear without a
+  group A or group H case."""
   csrc = bsb_build.CSRC
   with open(os.path.join(csrc, 'bsb_kernels.cuh')) as fh:
     kernels = fh.read()
   assert re.search(r'template <class F, int RK, bool kNoise, bool kTrack>\s*__global__ void[^\n]*\btransition_kernel\(', kernels)
+  assert re.search(r'template <class F, int RK, bool kNoise, bool kTrack>\s*__global__ void[^\n]*\n?'
+                   r'two_phase_host_kernel\(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs h\)', kernels)
+  # the two-phase kernel is instantiated for the families of ObsFromState, each in all four flag combinations
+  two_phase = sorted(re.findall(r'template <> struct ObsFromState<(\w+)> \{ static const bool value = true; \};', kernels))
+  assert two_phase == ['Catch', 'DeepSea']
+  got = sorted((c['family'], c['rng'], c['noise'] is not None, c['track'], mode) for c, mode in GROUP_H if c['batch'] == 97)
+  assert got == sorted(itertools.product(('catch', 'deep_sea'), RNGS, (False, True), (False, True), HOST_MODES))
   assert sorted(int(k) for k in re.findall(r'template <> struct RngOf<(\d+)>', kernels)) == list(range(len(RNGS)))
   compiled = sorted(f[4:-3] for f in os.listdir(csrc) if f.startswith('fam_') and f.endswith('.cu'))
   assert sorted(FAMILIES) == compiled == sorted(experiments.ENVIRONMENT_CLASSES)
   got = sorted((c['family'], c['rng'], c['noise'] is not None, c['track']) for c in GROUP_A)
   assert got == sorted(itertools.product(FAMILIES, RNGS, (False, True), (False, True)))
-  ids = [_case_id(c) for c in GROUP_A + GROUP_B + GROUP_C]
+  ids = [_case_id(c) for c in GROUP_A + GROUP_B + GROUP_C] + [_h_id(h) for h in GROUP_H]
   assert len(ids) == len(set(ids))
+
+
+def _h_id(case_mode):
+  return f'{_case_id(case_mode[0])}-{case_mode[1]}'
 
 
 HOST_SELF_CHECK = [_case(f, 5, A_KWARGS[f], noise=0.1 if k % 2 else None, track=k % 3 == 0,
@@ -497,6 +537,26 @@ def test_default_dispatch_paths_match_the_host_path(case, image_dirs):
 @pytest.mark.parametrize('case', GROUP_C, ids=_case_id)
 def test_tuning_knobs_match_the_host_path(case, image_dirs, monkeypatch):
   drive(case, image_dirs, monkeypatch=monkeypatch)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('case_mode', GROUP_H, ids=_h_id)
+def test_two_phase_host_kernel_matches_the_host_path(case_mode, image_dirs):
+  """Host steps around an ordinary step: every call compared with the host twin, then the state (which stands a
+  pre-launched kernel down: the cancelled case)."""
+  case, mode = case_mode
+  twins = Twins(case, ('cuda', 'cpu'), image_dirs)
+  try:
+    twins.check_state('constructor')
+    for _ in range(4):
+      twins.step_host(mode)
+    twins.step()
+    for _ in range(3):
+      twins.step_host(mode)
+    twins.check_state('end of script')
+    twins.anchor()
+  finally:
+    twins.close()
 
 
 @pytest.mark.gpu
