@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BSB_LIBRARY points the binding at another build of the SAME library (tools/host_sanitize.sh: ASan/UBSan build)
 LIB_PATH = os.environ.get('BSB_LIBRARY') or os.path.join(_HERE, 'libbsuite_b200.so')
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 DEVICE_HOST = -1
 MAX_INFO = 4
 COMM_ID_BYTES = 128
@@ -28,6 +28,8 @@ WRAP_NONE, WRAP_REWARD_NOISE, WRAP_REWARD_SCALE = range(3)
 # enum bsb_rng_kind
 RNG_PHILOX, RNG_MT19937 = range(2)
 FLAG_TRACK_EPISODES = 1
+# enum bsb_obs_dtype
+OBS_FLOAT32, OBS_BFLOAT16, OBS_UINT8 = range(3)
 HOST_ORDER_AFTER_STREAM, HOST_PRELAUNCH, HOST_FENCE_CALLER, HOST_NO_WAIT = 1, 2, 4, 8      # bsb_step_host flags
 EPISODE_STAT_FIELDS = ('steps', 'episode', 'total_return', 'episode_len', 'episode_return')
 
@@ -42,7 +44,7 @@ class Config(ctypes.Structure):
       ('chain_length', ctypes.c_int32), ('n_distractor', ctypes.c_int32),
       ('num_actions', ctypes.c_int32), ('max_steps', ctypes.c_int32),
       ('num_data', ctypes.c_int32), ('image_rows', ctypes.c_int32), ('image_cols', ctypes.c_int32),
-      ('reserved0', ctypes.c_int32),
+      ('obs_dtype', ctypes.c_int32),
       ('unscaled_move_cost', ctypes.c_double),
       ('height_threshold', ctypes.c_double), ('x_threshold', ctypes.c_double), ('timescale', ctypes.c_double),
       ('max_time', ctypes.c_double), ('init_range', ctypes.c_double),

@@ -1,6 +1,7 @@
 // Host path and kernel launch, instantiated once per family (fam_<name>.cu).
 #pragma once
 #include <type_traits>
+#include <vector>
 
 #include "bsb_env.h"
 
@@ -33,11 +34,15 @@ template <> struct HostEmit<Mnist> {
   }
 };
 
-template <class F, int RK>
+// Observations of type O other than float32: each lane's float32 observation is rendered into `f32` and converted
+// element by element with obs_cast, the function the kernels use.
+template <class F, int RK, class O>
 void host_run(const EnvParams& p, const LaunchArgs& a) {
   typedef typename RngOf<RK>::type R;
   const int64_t B = p.batch;
   const int K = p.obs_numel;
+  O* const obs = reinterpret_cast<O*>(a.obs);
+  std::vector<float> f32(std::is_same<O, float>::value ? 0 : (size_t)K);
   const bool noise = p.wrapper == BSB_WRAP_REWARD_NOISE && a.mode != MODE_INIT;
   const bool track = p.ep != nullptr && a.mode != MODE_INIT;
   const MailFields out = {a.actions, a.obs, a.reward, a.reward_f64, a.discount, a.step_type, 0, 0};
@@ -58,7 +63,12 @@ void host_run(const EnvParams& p, const LaunchArgs& a) {
         if (a.actions_out) a.actions_out[off] = action;
       }
       lane_step<F>(p, lane, L, rng, wrng, ep, action, a.mode, noise, track, a.step0 + t, out, off);
-      HostEmit<F>::run(p, L, rng, a.obs + off * (int64_t)K);
+      if constexpr (std::is_same<O, float>::value) {
+        HostEmit<F>::run(p, L, rng, obs + off * (int64_t)K);
+      } else {
+        HostEmit<F>::run(p, L, rng, f32.data());
+        for (int e = 0; e < K; ++e) obs[off * (int64_t)K + e] = obs_cast<O>(f32[(size_t)e]);
+      }
     }
     lane_close<F>(p, lane, L, rng, wrng, ep, noise, track);
   }
@@ -73,7 +83,7 @@ struct Geometry { int threads = 0; size_t smem = 0; int64_t n_chunks = 0, grid =
 // sets the lanes per deep_sea bulk store; `no_obs`: no observation (no shared memory: co-resident with another
 // handle's observation stream), one chunk per warp; `extra_threads` > 0 puts g.extra_blocks blocks of that many
 // threads in all (at least one) in front of the chunk owners; `ctas_per_sm` > 0 caps a persistent grid per SM.
-template <class F>
+template <class F, class O>
 int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int group = 0, bool no_obs = false, int extra_threads = 0,
                 int ctas_per_sm = 0) {
   const int K = e->p.obs_numel;
@@ -90,11 +100,12 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int group = 0, bool no_o
   // one) unless that costs resident warps -- 16 warps per SM fit the register budget, so a warp can afford
   // ~14 KB of shared memory.  umbrella_distract (103-float rows, 13 KB per stage) would hold 8 warps per SM
   // with two stages and is bound by integer-multiply latency, not by the store.
-  a.stage_rows = ((size_t)2 * 32 * (size_t)K * sizeof(float) <= 14 * 1024) ? 2 : 1;
+  const size_t elem = sizeof(O);                     // bytes per observation element (obs_dtype)
+  a.stage_rows = ((size_t)2 * 32 * (size_t)K * elem <= 14 * 1024) ? 2 : 1;
   // A single-step launch gives every warp exactly one row block to emit: the second stage would only be zeroed
   // (catch) and hold shared memory that another CTA could use.
   if (a.T == 1 && (EmitKind<F>::value == EMIT_ROWS || EmitKind<F>::value == EMIT_TWOHOT)) a.stage_rows = 1;
-  a.cta_extra_floats = 0;
+  a.cta_extra_elems = 0;
   a.bad_action = e->bad_action_dev;
   // Lanes per chunk.  The image emitter walks the chunk's lanes a few 3 KB tiles at a time, so it is bound by how
   // many warps share the batch: keep >= 4 warps per SM by halving the chunk (down to 8 lanes) when 32-lane chunks
@@ -107,10 +118,11 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int group = 0, bool no_o
   g.n_chunks = (B + chunk - 1) / chunk;
   int threads = e->block_threads;
   bool persistent = false;
-  const size_t tile = (size_t)K * 4;
+  const size_t tile = (size_t)K * elem;
   if (is_onehot && a.emit_bulk) {
     // Lanes per bulk store: the largest power of two <= 16 with one store <= 40 KB (BSB_DEEP_SEA_GROUP overrides).
     // N = 32 -> 8 lanes (32 KB stores), N = 50 -> 4 lanes (40 KB); tools/bench_variants.py compares group sizes.
+    // Narrow tiles reach the 16-lane cap first: N = 32 in bfloat16 -> 16 lanes (32 KB), in uint8 -> 16 lanes (16 KB).
     int m = 1;
     while (m < 16 && (size_t)(2 * m) * tile <= 40 * 1024) m <<= 1;
     if (e->deep_sea_group > 0) m = e->deep_sea_group;
@@ -139,20 +151,21 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int group = 0, bool no_o
     if ((K & 15) != 0 || (size_t)stages * m * tile > 64 * 1024) {
       a.emit_bulk = 0;
     } else {
-      a.group_lanes = m; a.stage_rows = stages; threads = 128; a.cta_extra_floats = mz * K; persistent = e->deep_sea_persistent != 0;
+      a.group_lanes = m; a.stage_rows = stages; threads = 128; a.cta_extra_elems = mz * K; persistent = e->deep_sea_persistent != 0;
       if (g.n_chunks < 2 * (int64_t)e->num_sms) threads = 64;      // small batches: more, smaller CTAs
     }
   }
   a.use_pdl = (e->use_pdl && !a.no_pdl && a.mode == MODE_STEP && a.T == 1) ? 1 : 0;
-  if (no_obs) { a.emit_bulk = 0; a.stage_rows = 0; a.cta_extra_floats = 0; a.group_lanes = 1; threads = 128; persistent = false; }
-  size_t per_warp = smem_floats_per_warp<F>(K, a.emit_bulk != 0, a.group_lanes, a.stage_rows) * sizeof(float);
+  if (no_obs) { a.emit_bulk = 0; a.stage_rows = 0; a.cta_extra_elems = 0; a.group_lanes = 1; threads = 128; persistent = false; }
+  size_t per_warp = smem_elems_per_warp<F, O>(K, a.emit_bulk != 0, a.group_lanes, a.stage_rows) * elem;
   if ((EmitKind<F>::value == EMIT_ROWS || EmitKind<F>::value == EMIT_TWOHOT) && per_warp > 96 * 1024) {
     // rows / boards too long for a per-warp stage: long rows always get ONE stage (above), so the limit is
-    // 32 * K * 4 bytes > 96 KB, i.e. K > 768 (catch boards of more than 768 cells such as 28 x 28, umbrella_chain
-    // with more than 765 distractors): boards fall back to shuffle-rendered vector stores, rows are rendered in place
+    // 32 * K * 4 bytes > 96 KB, i.e. K > 768 in float32 (catch boards of more than 768 cells such as 28 x 28,
+    // umbrella_chain with more than 765 distractors), K > 1 536 in bfloat16, K > 3 072 in uint8: boards fall back to
+    // shuffle-rendered vector stores, rows are rendered in place
     a.emit_bulk = 0; a.stage_rows = 0; per_warp = 0;
   }
-  const size_t cta_extra = (size_t)a.cta_extra_floats * sizeof(float);
+  const size_t cta_extra = (size_t)a.cta_extra_elems * elem;
   size_t smem = per_warp * (size_t)(threads / 32) + cta_extra;
   while (smem > 96 * 1024 && threads > 32) { threads >>= 1; smem = per_warp * (size_t)(threads / 32) + cta_extra; }
   if (smem > 200 * 1024) return fail(BSB_UNSUPPORTED, "observation too large for the staged emitter");
@@ -200,15 +213,15 @@ int launch(bsb_env* e, const LaunchArgs& a, const Geometry& g, cudaStream_t stre
   return BSB_OK;
 }
 
-template <class F, int RK, bool kNoise, bool kTrack>
+template <class F, int RK, bool kNoise, bool kTrack, class O>
 int device_launch(bsb_env* e, LaunchArgs a, cudaStream_t stream) {
   Geometry g;
-  const int rc = plan_launch<F>(e, a, g);
-  return rc != BSB_OK ? rc : launch(e, a, g, stream, transition_kernel<F, RK, kNoise, kTrack>, e->p, a);
+  const int rc = plan_launch<F, O>(e, a, g);
+  return rc != BSB_OK ? rc : launch(e, a, g, stream, transition_kernel<typename KernelFamily<F, O>::type, RK, kNoise, kTrack>, e->p, a);
 }
 
 // Two-phase host step (DeepSea, Catch): one launch (h.phase 0) or one of the two launches of a split step.
-template <class F, int RK, bool kNoise, bool kTrack>
+template <class F, int RK, bool kNoise, bool kTrack, class O>
 int two_phase_launch(bsb_env* e, LaunchArgs a, TwoPhaseArgs h, cudaStream_t stream) {
   if (a.clock) return fail(BSB_INTERNAL, "a host step reached graph-safe mode, which turns the mailbox path off");
   // Copiers: enough of them for ~512 threads, i.e. ~64 KB of 16-byte loads in flight.  The observation-only launch
@@ -216,11 +229,11 @@ int two_phase_launch(bsb_env* e, LaunchArgs a, TwoPhaseArgs h, cudaStream_t stre
   // observation stream on every SM (BSB_SPLIT_CTAS_PER_SM).
   Geometry g;
   const bool obs_only = h.phase == 2;
-  const int rc = plan_launch<F>(e, a, g, obs_only ? e->split_group : 0, h.phase == 1, obs_only ? 0 : 512,
+  const int rc = plan_launch<F, O>(e, a, g, obs_only ? e->split_group : 0, h.phase == 1, obs_only ? 0 : 512,
                                 obs_only ? e->split_ctas_per_sm : 0);
   if (rc != BSB_OK) return rc;
   h.copiers = g.extra_blocks;
-  return launch(e, a, g, stream, two_phase_host_kernel<F, RK, kNoise, kTrack>, e->p, a, h);
+  return launch(e, a, g, stream, two_phase_host_kernel<typename KernelFamily<F, O>::type, RK, kNoise, kTrack>, e->p, a, h);
 }
 
 // Runs `launch(noise, track)` with the template flags of the launch's wrappers (none for the constructor).
@@ -232,21 +245,56 @@ int with_flags(const bsb_env* e, const LaunchArgs& a, Launch launch) {
   return track ? launch(std::false_type(), std::true_type()) : launch(std::false_type(), std::false_type());
 }
 
-template <class F>
-int run_family(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr) {
+// Float32 observations: both bit sources.  Reduced dtypes: Philox only (bsb_create refuses MT19937 with them).
+template <class F, class O>
+int run_family_as(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoPhaseArgs* two_phase) {
+  constexpr bool kF32 = std::is_same<O, float>::value;
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
+  if (!kF32 && mt) return fail(BSB_INTERNAL, "reduced obs_dtype with MT19937");
   if (e->device < 0) {
-    if (mt) host_run<F, 1>(e->p, a); else host_run<F, 0>(e->p, a);
+    if constexpr (kF32) { if (mt) { host_run<F, 1, O>(e->p, a); return BSB_OK; } }
+    host_run<F, 0, O>(e->p, a);
     return BSB_OK;
   }
   return with_flags(e, a, [&](auto noise, auto track) {
     constexpr bool kNoise = decltype(noise)::value, kTrack = decltype(track)::value;
     if constexpr (ObsFromState<F>::value) {
-      if (two_phase) return mt ? two_phase_launch<F, 1, kNoise, kTrack>(e, a, *two_phase, stream)
-                               : two_phase_launch<F, 0, kNoise, kTrack>(e, a, *two_phase, stream);
+      if constexpr (kF32) {
+        if (two_phase) return mt ? two_phase_launch<F, 1, kNoise, kTrack, O>(e, a, *two_phase, stream)
+                                 : two_phase_launch<F, 0, kNoise, kTrack, O>(e, a, *two_phase, stream);
+      } else {
+        if (two_phase) return two_phase_launch<F, 0, kNoise, kTrack, O>(e, a, *two_phase, stream);
+      }
     }
-    return mt ? device_launch<F, 1, kNoise, kTrack>(e, a, stream) : device_launch<F, 0, kNoise, kTrack>(e, a, stream);
+    if constexpr (kF32) {
+      if (mt) return device_launch<F, 1, kNoise, kTrack, O>(e, a, stream);
+    }
+    return device_launch<F, 0, kNoise, kTrack, O>(e, a, stream);
   });
+}
+
+// bfloat16 for every family, uint8 for the 0 / 1 observations of deep_sea and catch (BinaryObs).  Instantiated in
+// translation units of their own (obs_<family>.cu): a float32 handle never loads their modules.
+template <class F>
+int run_reduced(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoPhaseArgs* two_phase) {
+  switch (e->obs_dtype) {
+    case BSB_OBS_BFLOAT16: return run_family_as<F, Bf16>(e, a, stream, two_phase);
+    case BSB_OBS_UINT8:
+      if constexpr (BinaryObs<F>::value) return run_family_as<F, uint8_t>(e, a, stream, two_phase);
+      break;
+  }
+  return fail(BSB_INTERNAL, "obs_dtype not compiled for this family");
+}
+#define BSB_REDUCED(F) extern template int run_reduced<F>(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs*);
+BSB_REDUCED(DeepSea) BSB_REDUCED(Catch) BSB_REDUCED(Cartpole) BSB_REDUCED(CartpoleSwingup) BSB_REDUCED(MountainCar)
+BSB_REDUCED(MemoryChain) BSB_REDUCED(Bandit) BSB_REDUCED(UmbrellaChain) BSB_REDUCED(DiscountingChain) BSB_REDUCED(Mnist)
+#undef BSB_REDUCED
+
+// Kernels and host path of the handle's observation dtype.
+template <class F>
+int run_family(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr) {
+  if (e->obs_dtype != BSB_OBS_FLOAT32) return run_reduced<F>(e, a, stream, two_phase);
+  return run_family_as<F, float>(e, a, stream, two_phase);
 }
 
 }  // namespace bsb

@@ -113,7 +113,7 @@ LaunchArgs make_args(const bsb_env* e, const bsb_outputs* out, const int32_t* ac
   a.actions = actions;
   if (out) { a.obs = out->observation; a.reward = out->reward; a.reward_f64 = out->reward_f64; a.discount = out->discount; a.step_type = out->step_type; }
   a.T = T; a.step0 = e->steps_done; a.mode = mode;
-  const size_t step_bytes = (size_t)e->p.batch * (size_t)e->p.obs_numel * sizeof(float);
+  const size_t step_bytes = (size_t)e->p.batch * (size_t)e->p.obs_numel * (size_t)e->obs_elem_bytes;
   a.obs_vec_ok = (out && (reinterpret_cast<uintptr_t>(out->observation) % 16 == 0) && (T == 1 || step_bytes % 16 == 0)) ? 1 : 0;
   return a;
 }
@@ -158,6 +158,11 @@ int validate(const bsb_config& c, int64_t batch, int* obs_rows, int* obs_cols, i
       *obs_rows = c.image_rows; *obs_cols = c.image_cols; *n_actions = 10; break;
     default: return fail(BSB_INVALID_ARGUMENT, "unknown family");
   }
+  if (c.obs_dtype < BSB_OBS_FLOAT32 || c.obs_dtype > BSB_OBS_UINT8) return fail(BSB_INVALID_ARGUMENT, "unknown obs_dtype");
+  if (c.obs_dtype == BSB_OBS_UINT8 && c.family != BSB_DEEP_SEA && c.family != BSB_CATCH)
+    return fail(BSB_UNSUPPORTED, "obs_dtype uint8 is only available for deep_sea and catch, whose observations are 0 / 1");
+  if (c.obs_dtype != BSB_OBS_FLOAT32 && c.rng_kind == BSB_RNG_MT19937)
+    return fail(BSB_UNSUPPORTED, "a bfloat16 or uint8 obs_dtype needs rng_kind BSB_RNG_PHILOX");
   if (c.log_schedule_len < 0 || c.log_schedule_len > 4096) return fail(BSB_INVALID_ARGUMENT, "log_schedule_len must be in [0, 4096]");
   if (c.log_schedule_len > 0) {
     if (!c.log_schedule) return fail(BSB_INVALID_ARGUMENT, "log_schedule_len > 0 needs a log_schedule");
@@ -224,7 +229,8 @@ int mailbox_open(bsb_env* e) {
 // buffers from the mailbox once the host rings `ticket` (pre-launch); otherwise from `fields` right away.
 // Two-phase host steps pay off where the observation stream is long next to the scalar traffic over PCIe (12 B per
 // lane out, 4 B in): deep_sea from N = 16 up (>= 1 KB of observation per lane).  catch (200 B per lane) is bound
-// by the 2 MB of scalars per step either way and keeps the single-phase kernel.
+// by the 2 MB of scalars per step either way and keeps the single-phase kernel.  The rule counts float32 bytes
+// whatever the handle's obs_dtype, so a reduced-dtype handle takes the same path as its float32 twin.
 bool family_obs_from_state(const bsb_env* e) {
   return (e->p.family == BSB_DEEP_SEA || e->p.family == BSB_CATCH) && (size_t)e->p.obs_numel * sizeof(float) >= 1024;
 }
@@ -427,7 +433,8 @@ int32_t bsb_create(const bsb_config* config, int64_t batch, int32_t device, uint
 
   bsb_env* e = new bsb_env();
   memset(&e->p, 0, sizeof(e->p));
-  e->device = device; e->steps_done = 0; e->graph_safe = false; e->clock = nullptr; e->sum_scratch = nullptr; e->names = info_names(c.family);
+  e->device = device; e->steps_done = 0;
+  e->obs_dtype = c.obs_dtype; e->obs_elem_bytes = c.obs_dtype == BSB_OBS_BFLOAT16 ? 2 : c.obs_dtype == BSB_OBS_UINT8 ? 1 : 4; e->graph_safe = false; e->clock = nullptr; e->sum_scratch = nullptr; e->names = info_names(c.family);
   {  // tuning knobs (environment variables, read once per handle)
     auto flag = [](const char* name, int dflt) { const char* v = getenv(name); return v ? (atoi(v) != 0 ? 1 : 0) : dflt; };
     const char* bt = getenv("BSB_BLOCK_THREADS");
@@ -874,6 +881,7 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
   DeviceGuard guard(env->device);
   { int arc = finish_awaited(env); if (arc != BSB_OK) return arc; }      // one step in flight per handle
   const size_t B = (size_t)env->p.batch, K = (size_t)env->p.obs_numel;
+  const size_t obs_bytes = B * K * (size_t)env->obs_elem_bytes;
   if (!env->copy_stream) BSB_CUDA(cudaStreamCreateWithFlags(&env->copy_stream, cudaStreamNonBlocking));
   if (flags & BSB_HOST_ORDER_AFTER_STREAM) {
     // Work the caller enqueued earlier on ITS stream (bsb_reset / bsb_step / bsb_rollout of this handle) must have
@@ -905,7 +913,7 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
     const bool all_mapped = d_actions && (!host_out->reward || d_reward) && (!host_out->reward_f64 || d_reward64) &&
                             (!host_out->discount || d_discount) && (!host_out->step_type || d_step_type);
     if (all_mapped) {
-      if (!device_obs && !env->d_obs) BSB_CUDA(cudaMalloc(&env->d_obs, B * K * 4));
+      if (!device_obs && !env->d_obs) BSB_CUDA(cudaMalloc(&env->d_obs, obs_bytes));
       MailFields f;
       memset(&f, 0, sizeof(f));
       f.actions = static_cast<const int32_t*>(d_actions);
@@ -927,7 +935,7 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
         dev.observation = f.obs; dev.reward = f.reward; dev.reward_f64 = f.reward_f64; dev.discount = f.discount; dev.step_type = f.step_type;
         int zrc = bsb_step(env, f.actions, &dev, zs);
         if (zrc != BSB_OK) return zrc;
-        if (host_out->observation) BSB_CUDA(cudaMemcpyAsync(host_out->observation, dev.observation, B * K * 4, cudaMemcpyDeviceToHost, zs));
+        if (host_out->observation) BSB_CUDA(cudaMemcpyAsync(host_out->observation, dev.observation, obs_bytes, cudaMemcpyDeviceToHost, zs));
         BSB_CUDA(cudaStreamSynchronize(zs));
         return report_bad_actions(env);
       }
@@ -1006,7 +1014,7 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
     env->d_step_type = reinterpret_cast<int32_t*>(env->d_reward + 2 * B);
   }
   if (host_out->reward_f64 && !env->d_reward64) BSB_CUDA(cudaMalloc(&env->d_reward64, B * 8));
-  if (!device_obs && !env->d_obs) BSB_CUDA(cudaMalloc(&env->d_obs, B * K * 4));
+  if (!device_obs && !env->d_obs) BSB_CUDA(cudaMalloc(&env->d_obs, obs_bytes));
   { int vrc = check_host_actions(env, actions, (int64_t)B); if (vrc != BSB_OK) return vrc; }
   cudaStream_t s = env->copy_stream;
   BSB_CUDA(cudaMemcpyAsync(env->h2d_actions, actions, B * 4, cudaMemcpyHostToDevice, s));
@@ -1029,7 +1037,7 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
     if (host_out->step_type) BSB_CUDA(cudaMemcpyAsync(host_out->step_type, dev.step_type, B * 4, cudaMemcpyDeviceToHost, s));
   }
   if (host_out->reward_f64) BSB_CUDA(cudaMemcpyAsync(host_out->reward_f64, dev.reward_f64, B * 8, cudaMemcpyDeviceToHost, s));
-  if (host_out->observation) BSB_CUDA(cudaMemcpyAsync(host_out->observation, dev.observation, B * K * 4, cudaMemcpyDeviceToHost, s));
+  if (host_out->observation) BSB_CUDA(cudaMemcpyAsync(host_out->observation, dev.observation, obs_bytes, cudaMemcpyDeviceToHost, s));
   BSB_CUDA(cudaStreamSynchronize(s));
   return BSB_OK;
 }

@@ -31,6 +31,8 @@ extern std::atomic<int64_t> g_launches;                // kernels launched by th
 struct bsb_env {
   bsb::EnvParams p;
   int device;             // BSB_DEVICE_HOST or CUDA ordinal
+  int obs_dtype;          // bsb_obs_dtype of the observations this handle writes
+  int obs_elem_bytes;     // ... and their size: 4, 2 or 1
   int64_t steps_done;     // step() calls so far (host counter; frozen at the switch to graph-safe mode)
   // Graph-safe mode: entered for good when a launch of this handle is first captured into a CUDA graph.  From
   // then on the device clock counts the steps (kernel comment in bsb_kernels.cuh) and steps = steps_done + clock[0].

@@ -6,6 +6,7 @@
 // rendering is described by small per-lane descriptors so that the kernels can
 // emit dense tensors warp-cooperatively.
 #pragma once
+#include "bsb_obs_dtype.h"
 #include "bsb_rng.cuh"
 
 namespace bsb {
@@ -303,17 +304,17 @@ struct CartpoleT {
     }
     return make_mid(reward);
   }
-  // Observation row; dst[k * stride].
-  static BSB_HD void row(const EnvParams& p, const Lane& L, float* dst, int64_t stride) {
-    dst[0 * stride] = (float)(L.s.x / p.x_threshold);
-    dst[1 * stride] = (float)(L.s.x_dot / p.x_threshold);
-    dst[2 * stride] = (float)L.trig.sn;
-    dst[3 * stride] = (float)L.trig.cs;
-    dst[4 * stride] = (float)L.s.theta_dot;
-    dst[5 * stride] = (float)(L.s.t / p.max_time);
+  // Observation row; dst[k * stride].  Every row is computed in float32 and written as O (obs_cast).
+  template <class O> static BSB_HD void row(const EnvParams& p, const Lane& L, O* dst, int64_t stride) {
+    dst[0 * stride] = obs_cast<O>((float)(L.s.x / p.x_threshold));
+    dst[1 * stride] = obs_cast<O>((float)(L.s.x_dot / p.x_threshold));
+    dst[2 * stride] = obs_cast<O>((float)L.trig.sn);
+    dst[3 * stride] = obs_cast<O>((float)L.trig.cs);
+    dst[4 * stride] = obs_cast<O>((float)L.s.theta_dot);
+    dst[5 * stride] = obs_cast<O>((float)(L.s.t / p.max_time));
     if (kSwingup) {
-      dst[6 * stride] = fabs(L.s.x) < p.x_reward_threshold ? 1.0f : -1.0f;
-      dst[7 * stride] = fabs(L.s.theta_dot) < p.theta_dot_threshold ? 1.0f : -1.0f;
+      dst[6 * stride] = obs_cast<O>(fabs(L.s.x) < p.x_reward_threshold ? 1.0f : -1.0f);
+      dst[7 * stride] = obs_cast<O>(fabs(L.s.theta_dot) < p.theta_dot_threshold ? 1.0f : -1.0f);
     }
   }
 };
@@ -356,9 +357,9 @@ struct MountainCar {
     if (L.pos >= 0.5 || L.t >= (uint32_t)p.max_steps) return make_last(reward);  // :88-90
     return make_mid(reward);
   }
-  static BSB_HD void row(const EnvParams& p, const Lane& L, float* dst, int64_t stride) {
-    dst[0] = (float)L.pos; dst[stride] = (float)L.vel;       // mountain_car.py:62-64
-    dst[2 * stride] = (float)((double)L.t / (double)p.max_steps);
+  template <class O> static BSB_HD void row(const EnvParams& p, const Lane& L, O* dst, int64_t stride) {
+    dst[0] = obs_cast<O>((float)L.pos); dst[stride] = obs_cast<O>((float)L.vel);       // mountain_car.py:62-64
+    dst[2 * stride] = obs_cast<O>((float)((double)L.t / (double)p.max_steps));
   }
 };
 
@@ -402,11 +403,11 @@ struct MemoryChain {
     p.info[p.batch + i] += 2.0;
     return make_last(-1.0);
   }
-  static BSB_HD void row(const EnvParams& p, const Lane& L, float* dst, int64_t stride) {  // :60-71
-    dst[0] = (float)(1.0 - (double)L.obs_t / (double)p.memory_length);
-    dst[stride] = (L.obs_t == (uint32_t)(p.memory_length - 1)) ? (float)L.query : 0.0f;
+  template <class O> static BSB_HD void row(const EnvParams& p, const Lane& L, O* dst, int64_t stride) {  // :60-71
+    dst[0] = obs_cast<O>((float)(1.0 - (double)L.obs_t / (double)p.memory_length));
+    dst[stride] = obs_cast<O>((L.obs_t == (uint32_t)(p.memory_length - 1)) ? (float)L.query : 0.0f);
     for (int b = 0; b < p.num_bits; ++b)
-      dst[(2 + b) * stride] = (L.obs_t == 0) ? (float)(2 * (int32_t)((L.ctx >> b) & 1ull) - 1) : 0.0f;
+      dst[(2 + b) * stride] = obs_cast<O>((L.obs_t == 0) ? (float)(2 * (int32_t)((L.ctx >> b) & 1ull) - 1) : 0.0f);
   }
 };
 
@@ -427,7 +428,7 @@ struct Bandit {
     p.info[i] += 1.0 - reward;                               // _optimal_return = 1.
     return make_last(reward);
   }
-  static BSB_HD void row(const EnvParams&, const Lane&, float* dst, int64_t) { dst[0] = 1.0f; }  // bandit.py:53-54
+  template <class O> static BSB_HD void row(const EnvParams&, const Lane&, O* dst, int64_t) { dst[0] = obs_cast<O>(1.0f); }  // bandit.py:53-54
 };
 
 // ===========================================================================
@@ -463,13 +464,13 @@ struct UmbrellaChain {
     return make_mid(reward);
   }
   // The observation draws n_distractor fresh Bernoullis on EVERY call (:60-66).
-  template <class R> static BSB_HD void row(const EnvParams& p, const Lane& L, R& rng, float* dst, int64_t stride) {
-    dst[0] = (float)L.need; dst[stride] = (float)L.has;
-    dst[2 * stride] = (float)(1.0 - (double)L.t / (double)p.chain_length);
+  template <class R, class O> static BSB_HD void row(const EnvParams& p, const Lane& L, R& rng, O* dst, int64_t stride) {
+    dst[0] = obs_cast<O>((float)L.need); dst[stride] = obs_cast<O>((float)L.has);
+    dst[2 * stride] = obs_cast<O>((float)(1.0 - (double)L.t / (double)p.chain_length));
     for (int k0 = 0; k0 < p.n_distractor; k0 += 64) {
       const int n = (p.n_distractor - k0) < 64 ? (p.n_distractor - k0) : 64;
       const uint64_t bits = rng.binomial_half_bits(n);
-      for (int k = 0; k < n; ++k) dst[(3 + k0 + k) * stride] = (float)((bits >> k) & 1ull);
+      for (int k = 0; k < n; ++k) dst[(3 + k0 + k) * stride] = obs_cast<O>((float)((bits >> k) & 1ull));
     }
   }
 };
@@ -503,8 +504,8 @@ struct DiscountingChain {
     if (L.t == 100u) return make_last(reward);               // _episode_len = 100
     return make_mid(reward);
   }
-  static BSB_HD void row(const EnvParams&, const Lane& L, float* dst, int64_t stride) {  // :63-67
-    dst[0] = (float)L.context; dst[stride] = (float)((double)L.t / 100.0);
+  template <class O> static BSB_HD void row(const EnvParams&, const Lane& L, O* dst, int64_t stride) {  // :63-67
+    dst[0] = obs_cast<O>((float)L.context); dst[stride] = obs_cast<O>((float)((double)L.t / 100.0));
   }
 };
 

@@ -33,6 +33,8 @@
 // (which the host path runs too) and the mailbox protocol.  With use_pdl a kernel is launched with programmatic
 // stream serialization: everything before griddepcontrol.wait (index math, zeroing the shared-memory stages)
 // overlaps the tail of the previous step's kernel.
+// Observations may be written as bfloat16 or uint8 instead (bsb_config.obs_dtype; ObsAs below): the emitters stage and
+// store elements of that type, each the float32 value converted by obs_cast (bsb_obs_dtype.h).
 #pragma once
 #include "bsb_families.cuh"
 
@@ -71,7 +73,8 @@ struct LaunchArgs {
   int32_t chunk_lanes;      // lanes per chunk (= per warp pass): 32, or 16 / 8 when the batch would under-fill the SMs
   int32_t stage_rows;       // row / board emitters: number of [32, K] shared-memory stages per warp (2: double buffered;
                             // 1: long rows, where a second stage would cost resident warps; 0: straight to global memory)
-  int32_t cta_extra_floats; // shared memory after the per-warp stages (mnist bulk path: the CTA's all-zero tiles)
+  int32_t cta_extra_elems;  // observation elements of shared memory after the per-warp stages (mnist bulk path: the
+                            // CTA's all-zero tiles)
   // Host-driven steps (bsb_step_host, pinned buffers): completion is signalled through a pinned mailbox; with
   // BSB_HOST_PRELAUNCH the launch is even enqueued BEFORE its inputs exist and waits for the host to ring
   // `ticket`, taking pointers and actions from the mailbox.
@@ -121,6 +124,20 @@ struct DeviceMail {
 };
 
 enum { MODE_STEP = 0, MODE_RESET = 1, MODE_INIT = 2 };
+
+// Observation element type of a kernel (bsb_config.obs_dtype).  The first template argument of both kernels is the
+// family F itself for float32 observations, or ObsAs<F, O> for observations written as O (Bf16, uint8_t): the
+// float32 kernels keep their template arguments, their names and their code.
+template <class Family, class O> struct ObsAs {};
+template <class F> struct FamilyOf { typedef F type; };
+template <class Family, class O> struct FamilyOf<ObsAs<Family, O> > { typedef Family type; };
+template <class F> struct ObsElemOf { typedef float type; };
+template <class Family, class O> struct ObsElemOf<ObsAs<Family, O> > { typedef O type; };
+// Kernel argument F for observations of type O.
+template <class Family, class O> struct KernelFamily { typedef ObsAs<Family, O> type; };
+template <class Family> struct KernelFamily<Family, float> { typedef Family type; };
+// log2 of the observation elements per 16-byte vector store.
+template <class O> struct Vec16 { static const int shift = sizeof(O) == 4 ? 2 : sizeof(O) == 2 ? 3 : 4; };
 
 // ----- RNG plumbing ---------------------------------------------------------
 template <int RK> struct RngOf;
@@ -231,16 +248,21 @@ template <> struct EmitKind<Mnist> { static const int value = EMIT_IMAGE; };
 static const int ROW_STAGES = 2;      // at most: double-buffered [32, K] stage per warp (LaunchArgs::stage_rows)
 static const int TILE_STAGES = 2;     // deep_sea bulk path: double-buffered groups of `group_lanes` tiles per warp
 
-// Dynamic shared memory per warp, in floats.
-template <class F> inline
+// Families whose observations hold only 0 and 1, so that uint8 represents them exactly (obs_dtype uint8).
+template <class F> struct BinaryObs {
+  static const bool value = EmitKind<F>::value == EMIT_ONEHOT || EmitKind<F>::value == EMIT_TWOHOT;
+};
+
+// Dynamic shared memory per warp, in observation elements of type O (times sizeof(O): bytes).
+template <class F, class O> inline
 #if defined(__CUDACC__)
 __host__ __device__
 #endif
-size_t smem_floats_per_warp(int K, bool emit_bulk, int group_lanes, int row_stages) {
+size_t smem_elems_per_warp(int K, bool emit_bulk, int group_lanes, int row_stages) {
   if (EmitKind<F>::value == EMIT_ROWS || EmitKind<F>::value == EMIT_TWOHOT) return (size_t)row_stages * 32 * (size_t)K;
   if (EmitKind<F>::value == EMIT_ONEHOT && emit_bulk) return (size_t)TILE_STAGES * (size_t)group_lanes * (size_t)K;
   if (EmitKind<F>::value == EMIT_IMAGE)                    // int8 pixel -> float32 table (+ two staging buffers of m tiles)
-    return 256 + (emit_bulk ? (size_t)row_stages * (size_t)group_lanes * (size_t)K : 0);
+    return 256 * sizeof(float) / sizeof(O) + (emit_bulk ? (size_t)row_stages * (size_t)group_lanes * (size_t)K : 0);
   return 0;
 }
 
@@ -248,6 +270,31 @@ size_t smem_floats_per_warp(int K, bool emit_bulk, int group_lanes, int row_stag
 
 __device__ __forceinline__ void st_stream(float4* dst, float4 v) { __stcs(dst, v); }
 __device__ __forceinline__ void st_stream(float* dst, float v) { __stcs(dst, v); }
+__device__ __forceinline__ void st_stream(Bf16* dst, Bf16 v) { __stcs(reinterpret_cast<unsigned short*>(dst), v.bits); }
+__device__ __forceinline__ void st_stream(uint8_t* dst, uint8_t v) { __stcs(dst, v); }
+// Bits of the observation element O for 1.0 (the hot cells of deep_sea and catch).
+template <class O> __device__ __forceinline__ uint32_t one_bits() {
+  return sizeof(O) == 2 ? 0x3f80u : 1u;       // bfloat16 1.0, uint8 1
+}
+// Four consecutive observation elements (one 16-, 8- or 4-byte word) from four float32 values.
+template <class O> struct Quad;
+template <> struct Quad<float> { typedef float4 type; static __device__ __forceinline__ float4 of(float4 v) { return v; } };
+template <> struct Quad<Bf16> {
+  typedef uint2 type;
+  static __device__ __forceinline__ uint2 of(float4 v) {
+    return make_uint2((uint32_t)f32_to_bf16_bits(v.x) | ((uint32_t)f32_to_bf16_bits(v.y) << 16),
+                      (uint32_t)f32_to_bf16_bits(v.z) | ((uint32_t)f32_to_bf16_bits(v.w) << 16));
+  }
+};
+template <> struct Quad<uint8_t> {
+  typedef unsigned int type;
+  static __device__ __forceinline__ unsigned int of(float4 v) {
+    return (uint32_t)f32_to_u8(v.x) | ((uint32_t)f32_to_u8(v.y) << 8) | ((uint32_t)f32_to_u8(v.z) << 16) |
+           ((uint32_t)f32_to_u8(v.w) << 24);
+  }
+};
+__device__ __forceinline__ void st_stream(uint2* dst, uint2 v) { __stcs(dst, v); }
+__device__ __forceinline__ void st_stream(unsigned int* dst, unsigned int v) { __stcs(dst, v); }
 
 // ----- TMA bulk store (shared::cta -> global) and PDL primitives --------------
 __device__ __forceinline__ void bulk_store_s2g(void* gdst, const void* ssrc, uint32_t bytes) {
@@ -279,10 +326,29 @@ __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepc
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // ----- vector-store emitters ---------------------------------------------------
-// One-hot tiles: `hot` is the flat index of the single 1.0 (or -1: all zeros).
-__device__ __forceinline__ void emit_onehot_vec(float* obs_t, int64_t warp_base, int n_lanes, int K, int hot, bool vec) {
+// One-hot tiles: `hot` is the flat index of the single 1.0 (or -1: all zeros).  `vec`: 16-byte stores (every tile
+// is a whole number of them).
+template <class O>
+__device__ __forceinline__ void emit_onehot_vec(O* obs_t, int64_t warp_base, int n_lanes, int K, int hot, bool vec) {
   const int tid = threadIdx.x & 31;
-  if (vec) {
+  if (vec && sizeof(O) != 4) {
+    // 8 bfloat16 or 16 uint8 per store: the hot element is one word of the store's four, shifted into place
+    constexpr int S = Vec16<O>::shift;
+    const int KV = K >> S;
+    for (int j = 0; j < n_lanes; ++j) {
+      const int h = __shfl_sync(0xffffffffu, hot, j);
+      const int hq = h < 0 ? -1 : (h >> S), hb = (h & ((1 << S) - 1)) * (int)sizeof(O);
+      const int word = hb >> 2;
+      const uint32_t bits = one_bits<O>() << ((hb & 3) * 8);
+      uint4* dst = reinterpret_cast<uint4*>(obs_t + (warp_base + j) * (int64_t)K);
+#pragma unroll 8
+      for (int q = tid; q < KV; q += 32) {
+        uint4 v = make_uint4(0u, 0u, 0u, 0u);
+        if (q == hq) { if (word == 0) v.x = bits; else if (word == 1) v.y = bits; else if (word == 2) v.z = bits; else v.w = bits; }
+        __stcs(dst + q, v);
+      }
+    }
+  } else if (vec) {
     const int K4 = K >> 2;
     for (int j = 0; j < n_lanes; ++j) {
       const int h = __shfl_sync(0xffffffffu, hot, j);
@@ -298,18 +364,40 @@ __device__ __forceinline__ void emit_onehot_vec(float* obs_t, int64_t warp_base,
   } else {
     for (int j = 0; j < n_lanes; ++j) {
       const int h = __shfl_sync(0xffffffffu, hot, j);
-      float* dst = obs_t + (warp_base + j) * (int64_t)K;
-      for (int e = tid; e < K; e += 32) st_stream(dst + e, e == h ? 1.f : 0.f);
+      O* dst = obs_t + (warp_base + j) * (int64_t)K;
+      for (int e = tid; e < K; e += 32) st_stream(dst + e, obs_cast<O>(e == h ? 1.f : 0.f));
     }
   }
 }
 
-// Boards with up to two hot cells; the warp's boards form one contiguous span.
-__device__ __forceinline__ void emit_twohot_vec(float* obs_t, int64_t warp_base, int n_lanes, int K, int hot_a, int hot_b, bool vec) {
+// Boards with up to two hot cells; the warp's boards form one contiguous span.  Its start is 16-byte aligned
+// whenever its length is a whole number of 16-byte stores: a full chunk of 8, 16 or 32 boards of K elements of s
+// bytes starts at a multiple of 8 * K * s bytes, which is a multiple of 16 unless s = 1 and K is odd -- and then no
+// span of fewer than 16 boards is a multiple of 16 bytes long.
+template <class O>
+__device__ __forceinline__ void emit_twohot_vec(O* obs_t, int64_t warp_base, int n_lanes, int K, int hot_a, int hot_b, bool vec) {
   const int tid = threadIdx.x & 31;
   const int total = n_lanes * K;
-  float* dst = obs_t + warp_base * (int64_t)K;
-  if (vec && (total & 3) == 0) {
+  O* dst = obs_t + warp_base * (int64_t)K;
+  constexpr int S = Vec16<O>::shift;
+  if (vec && sizeof(O) != 4 && (total & ((1 << S) - 1)) == 0) {
+    const int totalV = total >> S;
+    for (int q0 = 0; q0 < totalV; q0 += 32) {
+      const int q = q0 + tid;
+      const int e0 = (q < totalV ? q : 0) << S;
+      int j = e0 / K, c = e0 - j * K;
+      uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+      for (int k = 0; k < (1 << S); ++k) {
+        const int jj = j < 32 ? j : 31;
+        const int a = __shfl_sync(0xffffffffu, hot_a, jj);
+        const int b = __shfl_sync(0xffffffffu, hot_b, jj);
+        if (c == a || c == b) w[(k * (int)sizeof(O)) >> 2] |= one_bits<O>() << (((k * (int)sizeof(O)) & 3) * 8);
+        if (++c >= K) { c = 0; ++j; }
+      }
+      if (q < totalV) __stcs(reinterpret_cast<uint4*>(dst) + q, make_uint4(w[0], w[1], w[2], w[3]));
+    }
+  } else if (vec && (total & ((1 << S) - 1)) == 0) {
     const int total4 = total >> 2;
     for (int q0 = 0; q0 < total4; q0 += 32) {
       const int q = q0 + tid;
@@ -333,7 +421,7 @@ __device__ __forceinline__ void emit_twohot_vec(float* obs_t, int64_t warp_base,
       const int j = ee / K, c = ee - j * K;
       const int a = __shfl_sync(0xffffffffu, hot_a, j);
       const int b = __shfl_sync(0xffffffffu, hot_b, j);
-      if (e < total) st_stream(dst + e, (c == a || c == b) ? 1.f : 0.f);
+      if (e < total) st_stream(dst + e, obs_cast<O>((c == a || c == b) ? 1.f : 0.f));
     }
   }
 }
@@ -342,19 +430,21 @@ __device__ __forceinline__ void emit_twohot_vec(float* obs_t, int64_t warp_base,
 // (float)(int8)i / 255 in shared memory: IEEE float division costs ~10 instructions and takes a slow path for zero
 // numerators (most MNIST pixels), a table lookup costs one LDS.  The gather is latency-bound if each load ->
 // convert -> store chain runs serially, so all loads of a pass (8 x 32 char4 = 1 024 pixels) are issued first.
-__device__ __forceinline__ void emit_image(const EnvParams& p, const float* lut, float* obs_t, int64_t warp_base, int n_lanes, int K, int image, bool vec) {
+// Observations of type O other than float32 convert each looked-up float32 (4 pixels: one 8-byte bfloat16 store).
+template <class O>
+__device__ __forceinline__ void emit_image(const EnvParams& p, const float* lut, O* obs_t, int64_t warp_base, int n_lanes, int K, int image, bool vec) {
   const int tid = threadIdx.x & 31;
   constexpr int U = 8;
   for (int j = 0; j < n_lanes; ++j) {
     const int img = __shfl_sync(0xffffffffu, image, j);
-    float* dst = obs_t + (warp_base + j) * (int64_t)K;
+    O* dst = obs_t + (warp_base + j) * (int64_t)K;
     const int8_t* src = p.images + (int64_t)(img < 0 ? 0 : img) * K;
     if (vec) {
       const int K4 = K >> 2;
       const uchar4* src4 = reinterpret_cast<const uchar4*>(src);
-      float4* dst4 = reinterpret_cast<float4*>(dst);
+      typename Quad<O>::type* dst4 = reinterpret_cast<typename Quad<O>::type*>(dst);
       if (img < 0) {
-        for (int q = tid; q < K4; q += 32) st_stream(dst4 + q, make_float4(0.f, 0.f, 0.f, 0.f));
+        for (int q = tid; q < K4; q += 32) st_stream(dst4 + q, Quad<O>::of(make_float4(0.f, 0.f, 0.f, 0.f)));
         continue;
       }
       for (int q0 = 0; q0 < K4; q0 += 32 * U) {
@@ -368,11 +458,11 @@ __device__ __forceinline__ void emit_image(const EnvParams& p, const float* lut,
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           const int q = q0 + u * 32 + tid;
-          if (q < K4) st_stream(dst4 + q, make_float4(lut[c[u].x], lut[c[u].y], lut[c[u].z], lut[c[u].w]));
+          if (q < K4) st_stream(dst4 + q, Quad<O>::of(make_float4(lut[c[u].x], lut[c[u].y], lut[c[u].z], lut[c[u].w])));
         }
       }
     } else {
-      for (int e = tid; e < K; e += 32) st_stream(dst + e, img >= 0 ? lut[(uint8_t)src[e]] : 0.f);
+      for (int e = tid; e < K; e += 32) st_stream(dst + e, obs_cast<O>(img >= 0 ? lut[(uint8_t)src[e]] : 0.f));
     }
   }
 }
@@ -404,16 +494,18 @@ __device__ __forceinline__ float4 pixels4(uint32_t w) {
 //   * otherwise the block goes in groups of `m` (<= 4) lanes: all 16-byte loads of the group's int8 images (49 per
 //     28 x 28 tile) are issued before the first conversion, the float32 tiles land in a staging buffer and leave
 //     as one bulk store of m * 4K bytes.
-// stage = [256 floats: table of the vector path][stages x m x K floats]; `emitted` counts staged stores (buffer
+// stage = [256 floats: table of the vector path][stages x m x K elements of O; a bfloat16 tile is converted after
+// pixel_div255]; `emitted` counts staged stores (buffer
 // parity).  Small staging buffers (m = 2, one stage: 6 KB per warp) keep 16 warps per SM resident -- the conversion
 // is issue-bound, so resident warps matter -- while the
 // zero frames, which are pure bandwidth, still leave in 25 KB stores.
-__device__ __forceinline__ void emit_image_bulk(const EnvParams& p, float* stage, const float* cta_zero, float* obs_t,
+template <class O>
+__device__ __forceinline__ void emit_image_bulk(const EnvParams& p, O* stage, const O* cta_zero, O* obs_t,
                                                 int64_t warp_base, int n_lanes, int K, int image, int m, int mz,
                                                 int l2_hint, int stages, unsigned& emitted) {
   constexpr int MAXM = 4;
   const int tid = threadIdx.x & 31;
-  float* tiles = stage + 256;
+  O* tiles = reinterpret_cast<O*>(reinterpret_cast<float*>(stage) + 256);
   const int K16 = K >> 4;
   const unsigned showing = __ballot_sync(0xffffffffu, image >= 0);
   for (int z0 = 0; z0 < n_lanes; z0 += mz) {
@@ -421,16 +513,16 @@ __device__ __forceinline__ void emit_image_bulk(const EnvParams& p, float* stage
     const unsigned block_mask = (in_block >= 32 ? 0xffffffffu : ((1u << in_block) - 1u));
     if (((showing >> z0) & block_mask) == 0u) {
       if (tid == 0) {
-        bulk_store_obs(obs_t + (warp_base + z0) * (int64_t)K, cta_zero, (uint32_t)in_block * (uint32_t)K * 4u, l2_hint);
+        bulk_store_obs(obs_t + (warp_base + z0) * (int64_t)K, cta_zero, (uint32_t)in_block * (uint32_t)K * (uint32_t)sizeof(O), l2_hint);
         bulk_commit();
       }
       continue;
     }
     for (int g0 = z0; g0 < z0 + in_block; g0 += m) {
       const int in_group = (z0 + in_block - g0) < m ? (z0 + in_block - g0) : m;
-      float* dst = obs_t + (warp_base + g0) * (int64_t)K;
-      const uint32_t bytes = (uint32_t)in_group * (uint32_t)K * 4u;
-      float* buf = tiles + (size_t)(stages == 2 ? (emitted & 1u) : 0u) * m * K;
+      O* dst = obs_t + (warp_base + g0) * (int64_t)K;
+      const uint32_t bytes = (uint32_t)in_group * (uint32_t)K * (uint32_t)sizeof(O);
+      O* buf = tiles + (size_t)(stages == 2 ? (emitted & 1u) : 0u) * m * K;
       // two staging buffers: at most the newest store may still be reading, never this buffer; one: none may
       if (tid == 0) { if (stages == 2) bulk_wait_read<1>(); else bulk_wait_read<0>(); }
       __syncwarp();
@@ -454,9 +546,9 @@ __device__ __forceinline__ void emit_image_bulk(const EnvParams& p, float* stage
           for (int r = 0; r < 2; ++r) {
             const int q = q0 + r * 32 + tid;
             if (j < in_group && q < K16) {
-              float4* out = reinterpret_cast<float4*>(buf + (size_t)j * K) + 4 * q;
-              out[0] = pixels4(c[j][r].x); out[1] = pixels4(c[j][r].y);
-              out[2] = pixels4(c[j][r].z); out[3] = pixels4(c[j][r].w);
+              typename Quad<O>::type* out = reinterpret_cast<typename Quad<O>::type*>(buf + (size_t)j * K) + 4 * q;
+              out[0] = Quad<O>::of(pixels4(c[j][r].x)); out[1] = Quad<O>::of(pixels4(c[j][r].y));
+              out[2] = Quad<O>::of(pixels4(c[j][r].z)); out[3] = Quad<O>::of(pixels4(c[j][r].w));
             }
           }
       }
@@ -469,13 +561,16 @@ __device__ __forceinline__ void emit_image_bulk(const EnvParams& p, float* stage
 }
 
 // Stream the warp's staged [n_lanes, K] block with ordinary stores (ragged tail warps, unaligned buffers).
-__device__ __forceinline__ void flush_rows_vec(const float* stage, float* obs_t, int64_t warp_base, int n_lanes, int K, bool vec) {
+// (16-byte moves whatever the element type; the alignment argument of emit_twohot_vec holds for rows too.)
+template <class O>
+__device__ __forceinline__ void flush_rows_vec(const O* stage, O* obs_t, int64_t warp_base, int n_lanes, int K, bool vec) {
   const int tid = threadIdx.x & 31;
   const int total = n_lanes * K;
-  float* dst = obs_t + warp_base * (int64_t)K;
-  if (vec && (total & 3) == 0) {
+  O* dst = obs_t + warp_base * (int64_t)K;
+  constexpr int S = Vec16<O>::shift;
+  if (vec && (total & ((1 << S) - 1)) == 0) {
     const float4* s4 = reinterpret_cast<const float4*>(stage);
-    for (int q = tid; q < (total >> 2); q += 32) st_stream(reinterpret_cast<float4*>(dst) + q, s4[q]);
+    for (int q = tid; q < (total >> S); q += 32) st_stream(reinterpret_cast<float4*>(dst) + q, s4[q]);
   } else {
     for (int e = tid; e < total; e += 32) st_stream(dst + e, stage[e]);
   }
@@ -483,14 +578,14 @@ __device__ __forceinline__ void flush_rows_vec(const float* stage, float* obs_t,
 
 // ----- per-family glue ------------------------------------------------------------
 template <class F, class R> struct RowRenderer {
-  static __device__ __forceinline__ void run(const EnvParams& p, const typename F::Lane& L, R&, float* dst) { F::row(p, L, dst, 1); }
+  template <class O> static __device__ __forceinline__ void run(const EnvParams& p, const typename F::Lane& L, R&, O* dst) { F::row(p, L, dst, 1); }
 };
 template <class R> struct RowRenderer<UmbrellaChain, R> {   // the observation itself draws from the stream
-  static __device__ __forceinline__ void run(const EnvParams& p, const UmbrellaChain::Lane& L, R& r, float* dst) { UmbrellaChain::row(p, L, r, dst, 1); }
+  template <class O> static __device__ __forceinline__ void run(const EnvParams& p, const UmbrellaChain::Lane& L, R& r, O* dst) { UmbrellaChain::row(p, L, r, dst, 1); }
 };
-template <class R> struct RowRenderer<DeepSea, R> { static __device__ __forceinline__ void run(const EnvParams&, const DeepSea::Lane&, R&, float*) {} };
-template <class R> struct RowRenderer<Catch, R> { static __device__ __forceinline__ void run(const EnvParams&, const Catch::Lane&, R&, float*) {} };
-template <class R> struct RowRenderer<Mnist, R> { static __device__ __forceinline__ void run(const EnvParams&, const Mnist::Lane&, R&, float*) {} };
+template <class R> struct RowRenderer<DeepSea, R> { template <class O> static __device__ __forceinline__ void run(const EnvParams&, const DeepSea::Lane&, R&, O*) {} };
+template <class R> struct RowRenderer<Catch, R> { template <class O> static __device__ __forceinline__ void run(const EnvParams&, const Catch::Lane&, R&, O*) {} };
+template <class R> struct RowRenderer<Mnist, R> { template <class O> static __device__ __forceinline__ void run(const EnvParams&, const Mnist::Lane&, R&, O*) {} };
 
 template <class F> struct Descriptor {
   static __device__ __forceinline__ int a(const typename F::Lane&) { return -1; }
@@ -543,7 +638,7 @@ template <> struct MinBlocksPerSM<DiscountingChain> { static const int value = 8
 #ifdef BSB_MIN_BLOCKS_PER_SM   // build-time override for tuning experiments
 #define BSB_LAUNCH_MIN_BLOCKS(F) BSB_MIN_BLOCKS_PER_SM
 #else
-#define BSB_LAUNCH_MIN_BLOCKS(F) MinBlocksPerSM<F>::value
+#define BSB_LAUNCH_MIN_BLOCKS(F) MinBlocksPerSM<typename FamilyOf<F>::type>::value
 #endif
 // System-scope accesses to the pinned mailbox (host memory over PCIe) and volatile accesses to its L2 relay.
 __device__ __forceinline__ unsigned long long ld_sys_u64(const volatile unsigned long long* ptr) {
@@ -570,10 +665,12 @@ static const int CLOCK_GROUPS = 32, CLOCK_CHUNK = 16 * CLOCK_GROUPS, CLOCK_TOP =
                  CLOCK_SUB0 = CLOCK_TOP + 16, CLOCK_WORDS = CLOCK_SUB0 + 16 * CLOCK_GROUPS;
 
 // ----- pieces both kernels share ----------------------------------------------------------------------------------
-// Per-warp staging state of the observation emitters; it persists across the chunks and steps of a launch.
+// Per-warp staging state of the observation emitters; it persists across the chunks and steps of a launch.  The
+// stages hold observation elements of type O (the mnist table in front of them is float32).
+template <class O>
 struct WarpStage {
-  float* stage;            // this warp's shared-memory stages
-  float* cta_zero;         // mnist bulk path: all-zero tiles shared by the CTA's warps (source of the LAST-frame stores)
+  O* stage;                // this warp's shared-memory stages
+  O* cta_zero;             // mnist bulk path: all-zero tiles shared by the CTA's warps (source of the LAST-frame stores)
   unsigned row_mask;       // row / board stage of store number n: n & row_mask
   unsigned emitted = 0;    // bulk stores issued by this warp so far (double-buffer parity)
   int poked_a0 = -1, poked_b0 = -1, poked_a1 = -1, poked_b1 = -1;   // catch: cells poked into stage buffer 0 / 1
@@ -583,26 +680,27 @@ struct WarpStage {
 
 // Carves the warp's stages out of dynamic shared memory and clears those that rely on staying zero between steps
 // (before the dependency wait).  Every thread of the CTA calls it.
-template <class F>
-__device__ __forceinline__ WarpStage clear_stages(const EnvParams& p, const LaunchArgs& a) {
+template <class F, class O>
+__device__ __forceinline__ WarpStage<O> clear_stages(const EnvParams& p, const LaunchArgs& a) {
   extern __shared__ float4 smem_raw[];
   constexpr int kEmit = EmitKind<F>::value;
   const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
-  const size_t stage_floats = smem_floats_per_warp<F>(p.obs_numel, a.emit_bulk != 0, a.group_lanes, a.stage_rows);
-  WarpStage ws;
-  ws.stage = reinterpret_cast<float*>(smem_raw) + (size_t)warp * stage_floats;
-  ws.cta_zero = reinterpret_cast<float*>(smem_raw) + (size_t)warps_per_cta * stage_floats;
+  constexpr int S = Vec16<O>::shift;
+  const size_t stage_elems = smem_elems_per_warp<F, O>(p.obs_numel, a.emit_bulk != 0, a.group_lanes, a.stage_rows);
+  WarpStage<O> ws;
+  ws.stage = reinterpret_cast<O*>(smem_raw) + (size_t)warp * stage_elems;
+  ws.cta_zero = reinterpret_cast<O*>(smem_raw) + (size_t)warps_per_cta * stage_elems;
   ws.row_mask = a.stage_rows == 2 ? 1u : 0u;
   if (kEmit == EMIT_TWOHOT || (kEmit == EMIT_ONEHOT && a.emit_bulk)) {
     float4* s4 = reinterpret_cast<float4*>(ws.stage);
-    const int total4 = (int)(stage_floats >> 2);
+    const int total4 = (int)(stage_elems >> S);
     for (int q = tid; q < total4; q += 32) s4[q] = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int e = (total4 << 2) + tid; e < (int)stage_floats; e += 32) ws.stage[e] = 0.f;
+    for (int e = (total4 << S) + tid; e < (int)stage_elems; e += 32) ws.stage[e] = obs_cast<O>(0.f);
     __syncwarp();
   }
   if (kEmit == EMIT_IMAGE) {      // pixel table: image.astype(float32) / 255 for every int8 value (mnist.py:64)
-    for (int i = tid; i < 256; i += 32) ws.stage[i] = Mnist::pixel((int8_t)(uint8_t)i);
-    for (int i = threadIdx.x; i < a.cta_extra_floats; i += blockDim.x) ws.cta_zero[i] = 0.f;
+    for (int i = tid; i < 256; i += 32) reinterpret_cast<float*>(ws.stage)[i] = Mnist::pixel((int8_t)(uint8_t)i);
+    for (int i = threadIdx.x; i < a.cta_extra_elems; i += blockDim.x) ws.cta_zero[i] = obs_cast<O>(0.f);
     fence_proxy_async_smem();
     __syncthreads();
   }
@@ -662,25 +760,29 @@ __device__ __forceinline__ int64_t fetch_chunk(const LaunchArgs& a, int64_t tota
   return total_warps + (int64_t)__shfl_sync(0xffffffffu, v, 0);
 }
 
-// Which chunks leave through the TMA unit (16-byte aligned spans); warp-uniform per chunk.
-template <class F>
+// Which chunks leave through the TMA unit (spans that are whole multiples of 16 bytes, from 16-byte aligned starts:
+// see emit_twohot_vec); warp-uniform per chunk.
+template <class F, class O>
 __device__ __forceinline__ bool chunk_is_bulk(const EnvParams& p, const LaunchArgs& a, bool vec, int n_lanes) {
   constexpr int kEmit = EmitKind<F>::value;
+  constexpr int V1 = (1 << Vec16<O>::shift) - 1;     // elements per 16 bytes, minus one
   const int K = p.obs_numel;
   bool bulk = a.emit_bulk && vec;
-  if (kEmit == EMIT_ROWS) bulk = bulk && K >= 3 && ((n_lanes * K) & 3) == 0;
-  if (kEmit == EMIT_TWOHOT) bulk = bulk && ((n_lanes * K) & 3) == 0;
-  if (kEmit == EMIT_ONEHOT) bulk = bulk && ((K & 3) == 0 || ((n_lanes % a.group_lanes) == 0 && ((a.group_lanes * K) & 3) == 0));
+  if (kEmit == EMIT_ROWS) bulk = bulk && K >= 3 && ((n_lanes * K) & V1) == 0;
+  if (kEmit == EMIT_TWOHOT) bulk = bulk && ((n_lanes * K) & V1) == 0;
+  if (kEmit == EMIT_ONEHOT) bulk = bulk && ((K & V1) == 0 || ((n_lanes % a.group_lanes) == 0 && ((a.group_lanes * K) & V1) == 0));
   if (kEmit == EMIT_IMAGE) bulk = bulk && (K & 3) == 0;
   return bulk;
 }
 
-// Observation emitter of the warp for one chunk and step.
-template <class F, class R>
-__device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a, WarpStage& ws, const typename F::Lane& L,
-                                         R& rng, float* obs_t, int64_t warp_base, int n_lanes, int64_t lane, bool active,
+// Observation emitter of the warp for one chunk and step.  Every element is converted where it is written to the
+// stage or to global memory (obs_cast).
+template <class F, class O, class R>
+__device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a, WarpStage<O>& ws, const typename F::Lane& L,
+                                         R& rng, O* obs_t, int64_t warp_base, int n_lanes, int64_t lane, bool active,
                                          bool bulk, bool vec) {
   constexpr int kEmit = EmitKind<F>::value;
+  constexpr int V1 = (1 << Vec16<O>::shift) - 1;
   const int tid = threadIdx.x & 31;
   const int K = p.obs_numel;
   if (kEmit == EMIT_ONEHOT) {
@@ -693,47 +795,47 @@ __device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a
       for (int g0 = 0; g0 < n_lanes; g0 += m) {
         const int in_group = (n_lanes - g0) < m ? (n_lanes - g0) : m;
         const int s = (int)(ws.emitted & 1u);
-        float* group = ws.stage + (size_t)s * m * K;
+        O* group = ws.stage + (size_t)s * m * K;
         if (tid == 0) bulk_wait_read<TILE_STAGES - 1>();    // the store two back, last reader of `group`, is done
         __syncwarp();
-        if (s == 0) { if (ws.tile_poked0 >= 0) { group[ws.tile_poked0] = 0.f; ws.tile_poked0 = -1; } }
-        else        { if (ws.tile_poked1 >= 0) { group[ws.tile_poked1] = 0.f; ws.tile_poked1 = -1; } }
+        if (s == 0) { if (ws.tile_poked0 >= 0) { group[ws.tile_poked0] = obs_cast<O>(0.f); ws.tile_poked0 = -1; } }
+        else        { if (ws.tile_poked1 >= 0) { group[ws.tile_poked1] = obs_cast<O>(0.f); ws.tile_poked1 = -1; } }
         __syncwarp();     // a thread of an earlier group may clear the very cell another thread sets now
         if (tid >= g0 && tid < g0 + in_group && hot >= 0) {
           const int cell = (tid - g0) * K + hot;
-          group[cell] = 1.f;
+          group[cell] = obs_cast<O>(1.f);
           if (s == 0) ws.tile_poked0 = cell; else ws.tile_poked1 = cell;
         }
         fence_proxy_async_smem();
         __syncwarp();
         if (tid == 0) {
-          float* tile_dst = obs_t + (warp_base + g0) * (int64_t)K;
-          const uint32_t tile_bytes = (uint32_t)in_group * (uint32_t)K * 4u;
+          O* tile_dst = obs_t + (warp_base + g0) * (int64_t)K;
+          const uint32_t tile_bytes = (uint32_t)in_group * (uint32_t)K * (uint32_t)sizeof(O);
           bulk_store_obs(tile_dst, group, tile_bytes, a.l2_hint);
           bulk_commit();
         }
         ++ws.emitted;
       }
     } else {
-      emit_onehot_vec(obs_t, warp_base, n_lanes, K, hot, vec && (K & 3) == 0);
+      emit_onehot_vec(obs_t, warp_base, n_lanes, K, hot, vec && (K & V1) == 0);
     }
   } else if (kEmit == EMIT_TWOHOT) {
     const int hot_a = Descriptor<F>::a(L), hot_b = Descriptor<F>::b(L);
     if (bulk) {
       const int buf = (int)(ws.emitted & ws.row_mask);
-      float* boards = ws.stage + (size_t)buf * 32 * K;
+      O* boards = ws.stage + (size_t)buf * 32 * K;
       if (tid == 0) { if (ws.row_mask) bulk_wait_read<1>(); else bulk_wait_read<0>(); }   // the store that last read `boards` is done with it
       __syncwarp();
-      float* mine = boards + tid * K;
+      O* mine = boards + tid * K;
       const int old_a = buf ? ws.poked_a1 : ws.poked_a0, old_b = buf ? ws.poked_b1 : ws.poked_b0;
-      if (old_a >= 0) mine[old_a] = 0.f;
-      if (old_b >= 0) mine[old_b] = 0.f;
+      if (old_a >= 0) mine[old_a] = obs_cast<O>(0.f);
+      if (old_b >= 0) mine[old_b] = obs_cast<O>(0.f);
       int new_a = -1, new_b = -1;
-      if (active) { mine[hot_a] = 1.f; mine[hot_b] = 1.f; new_a = hot_a; new_b = hot_b; }
+      if (active) { mine[hot_a] = obs_cast<O>(1.f); mine[hot_b] = obs_cast<O>(1.f); new_a = hot_a; new_b = hot_b; }
       if (buf) { ws.poked_a1 = new_a; ws.poked_b1 = new_b; } else { ws.poked_a0 = new_a; ws.poked_b0 = new_b; }
       fence_proxy_async_smem();
       __syncwarp();
-      if (tid == 0) { bulk_store_obs(obs_t + warp_base * (int64_t)K, boards, (uint32_t)n_lanes * (uint32_t)K * 4u, a.l2_hint); bulk_commit(); }
+      if (tid == 0) { bulk_store_obs(obs_t + warp_base * (int64_t)K, boards, (uint32_t)n_lanes * (uint32_t)K * (uint32_t)sizeof(O), a.l2_hint); bulk_commit(); }
       ++ws.emitted;
     } else {
       emit_twohot_vec(obs_t, warp_base, n_lanes, K, hot_a, hot_b, vec);
@@ -741,20 +843,21 @@ __device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a
   } else if (kEmit == EMIT_IMAGE) {
     const int image = Descriptor<F>::a(L);
     if (bulk) emit_image_bulk(p, ws.stage, ws.cta_zero, obs_t, warp_base, n_lanes, K, active ? image : -1, a.group_lanes,
-                              a.cta_extra_floats / K, a.l2_hint, a.stage_rows, ws.emitted);
-    else emit_image(p, ws.stage, obs_t, warp_base, n_lanes, K, image, vec && (K & 3) == 0);
+                              a.cta_extra_elems / K, a.l2_hint, a.stage_rows, ws.emitted);
+    else emit_image(p, reinterpret_cast<const float*>(ws.stage), obs_t, warp_base, n_lanes, K, image, vec && (K & 3) == 0);
   } else if (!a.stage_rows) {
-    // observation rows too long for a shared-memory stage: every thread renders its row in place
+    // observation rows too long for a shared-memory stage: every thread renders its row in place.  Never taken by
+    // bfloat16 rows: a stage of 32 rows of K <= 1 536 elements (umbrella_chain's longest) always fits.
     if (active) RowRenderer<F, R>::run(p, L, rng, obs_t + lane * (int64_t)K);
   } else {
-    float* rows = ws.stage + (size_t)(ws.emitted & ws.row_mask) * 32 * K;
+    O* rows = ws.stage + (size_t)(ws.emitted & ws.row_mask) * 32 * K;
     if (bulk) { if (tid == 0) { if (ws.row_mask) bulk_wait_read<1>(); else bulk_wait_read<0>(); } }
     __syncwarp();
     if (active) RowRenderer<F, R>::run(p, L, rng, rows + tid * K);
     if (bulk) {
       fence_proxy_async_smem();
       __syncwarp();
-      if (tid == 0) { bulk_store_obs(obs_t + warp_base * (int64_t)K, rows, (uint32_t)n_lanes * (uint32_t)K * 4u, a.l2_hint); bulk_commit(); }
+      if (tid == 0) { bulk_store_obs(obs_t + warp_base * (int64_t)K, rows, (uint32_t)n_lanes * (uint32_t)K * (uint32_t)sizeof(O), a.l2_hint); bulk_commit(); }
     } else {
       __syncwarp();
       flush_rows_vec(rows, obs_t, warp_base, n_lanes, K, vec);
@@ -765,7 +868,8 @@ __device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a
 
 // The warp is done: shared memory must outlive its last bulk read.  `drain`: the stores themselves must have
 // completed (a single-phase host step's `done` tells the host that the observations are in device memory).
-__device__ __forceinline__ void retire_warp(const LaunchArgs& a, const WarpStage& ws, bool drain) {
+template <class O>
+__device__ __forceinline__ void retire_warp(const LaunchArgs& a, const WarpStage<O>& ws, bool drain) {
   if (ws.any_bulk && (threadIdx.x & 31) == 0) { if (drain) bulk_wait_all(); else bulk_wait_read<0>(); }
   if (a.timing && a.mail && threadIdx.x == 0) atomicMax(&a.mail->last_exit, global_timer_ns());
 }
@@ -786,11 +890,13 @@ __device__ __forceinline__ void signal_done(const LaunchArgs& a, unsigned long l
 // single-phase host step.
 template <class F, int RK, bool kNoise, bool kTrack>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kernel(const EnvParams p, const LaunchArgs a) {
+  typedef typename FamilyOf<F>::type Fam;          // F is the family, or ObsAs<family, O> (observations of type O)
+  typedef typename ObsElemOf<F>::type O;
   typedef typename RngOf<RK>::type R;
   const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
   const int64_t B = p.batch;
   const int K = p.obs_numel;
-  WarpStage ws = clear_stages<F>(p, a);
+  WarpStage<O> ws = clear_stages<Fam, O>(p, a);
   // Wait for the previous step's kernel (it wrote the lane state read below), THEN allow the next step's kernel
   // to become resident: its CTAs park at their own wait, so at most one dependent grid is ever pending.
   if (a.use_pdl) { pdl_wait(); pdl_launch_dependents(); }
@@ -799,6 +905,7 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
   bool cancelled;
   const MailFields io = receive_doorbell(a, cancelled);
   const bool vec = io.obs_vec_ok != 0;
+  O* const obs = reinterpret_cast<O*>(io.obs);      // the ABI's float* addresses elements of type O
 
   const int cl = a.chunk_lanes;
   const int64_t n_chunks = (B + cl - 1) / cl;
@@ -821,17 +928,17 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
     const int n_lanes = (B - warp_base) < cl ? (int)(B - warp_base) : cl;
     const int64_t lane = warp_base + tid;
     const bool active = tid < n_lanes;
-    const bool bulk = chunk_is_bulk<F>(p, a, vec, n_lanes);
+    const bool bulk = chunk_is_bulk<Fam, O>(p, a, vec, n_lanes);
     ws.any_bulk = ws.any_bulk || bulk;
 
-    typename F::Lane L;
+    typename Fam::Lane L;
     R rng, wrng;
     EpisodeStats ep;
     ActionStream action_stream;
     action_stream.open();
-    if (active) lane_open<F>(p, lane, L, rng, wrng, ep, a.mode, kNoise, kTrack);
-    else F::init(p, L);
-    if (a.mode == MODE_INIT && active) F::ctor_draws(p, L, rng);      // the constructor runs no step (T = 0)
+    if (active) lane_open<Fam>(p, lane, L, rng, wrng, ep, a.mode, kNoise, kTrack);
+    else Fam::init(p, L);
+    if (a.mode == MODE_INIT && active) Fam::ctor_draws(p, L, rng);      // the constructor runs no step (T = 0)
 
     for (int64_t t = 0; t < a.T; ++t) {
       const int64_t off = t * B + lane;
@@ -850,12 +957,12 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
           }
           if (a.actions_out) a.actions_out[off] = action;
         }
-        lane_step<F>(p, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, io, off);
+        lane_step<Fam>(p, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, io, off);
       }
-      emit_obs<F>(p, a, ws, L, rng, io.obs + t * B * (int64_t)K, warp_base, n_lanes, lane, active, bulk, vec);
+      emit_obs<Fam>(p, a, ws, L, rng, obs + t * B * (int64_t)K, warp_base, n_lanes, lane, active, bulk, vec);
     }
 
-    if (active) lane_close<F>(p, lane, L, rng, wrng, ep, kNoise, kTrack);
+    if (active) lane_close<Fam>(p, lane, L, rng, wrng, ep, kNoise, kTrack);
     if (dynamic && lazy) cur_chunk = fetch_chunk(a, total_warps);        // lazy: nothing was reserved while working
   }
   retire_warp(a, ws, a.mailbox != nullptr);
@@ -906,17 +1013,20 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
 template <class F, int RK, bool kNoise, bool kTrack>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F))
 two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs h) {
-  static_assert(ObsFromState<F>::value, "the two-phase host step renders observations from the stored lane state");
+  typedef typename FamilyOf<F>::type Fam;          // F is the family, or ObsAs<family, O> (observations of type O)
+  typedef typename ObsElemOf<F>::type O;
+  static_assert(ObsFromState<Fam>::value, "the two-phase host step renders observations from the stored lane state");
   typedef typename RngOf<RK>::type R;
   const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
   const int64_t B = p.batch;
-  WarpStage ws = clear_stages<F>(p, a);
+  WarpStage<O> ws = clear_stages<Fam, O>(p, a);
   // The observation-only launch must not wait for its predecessor -- the transitions launch, whose copiers are
   // still shipping scalars over PCIe -- to END: it waits for that launch's phase-1 flag instead.
   if (a.use_pdl) { if (h.phase != 2) pdl_wait(); pdl_launch_dependents(); }
   bool cancelled;
   const MailFields io = receive_doorbell(a, cancelled);
   const bool vec = io.obs_vec_ok != 0;
+  O* const obs = reinterpret_cast<O*>(io.obs);      // the ABI's float* addresses elements of type O
 
   const int cl = a.chunk_lanes;
   const int64_t n_chunks = (B + cl - 1) / cl;
@@ -936,31 +1046,31 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
 
   // Phase 2: streams the observations of chunk c and of every chunk the counter deals after it, rendered from the
   // stored lane state.  `kept`: chunk c is the warp's own, its state `first` still in registers from phase 1.
-  auto render_stored = [&](int64_t c, bool kept, const typename F::Lane& first) {
+  auto render_stored = [&](int64_t c, bool kept, const typename Fam::Lane& first) {
     while (c < n_chunks) {
       const int64_t warp_base = c * cl;
       const int n_lanes = (B - warp_base) < cl ? (int)(B - warp_base) : cl;
       const int64_t lane = warp_base + tid;
       const bool active = tid < n_lanes;
-      typename F::Lane L = first;
+      typename Fam::Lane L = first;
       if (!kept) {
         // some other warp ran this chunk's phase 1 -- long ago in practice, but wait for every chunk's
         if (tid == 0) while (a.mail->phase1 != a.ticket) {}
         __syncwarp();
         __threadfence();                   // acquire: the loads below must not be served from a stale L1 line
-        F::init(p, L);
-        if (active) { F::load(p, lane, L); F::describe(p, L); }
+        Fam::init(p, L);
+        if (active) { Fam::load(p, lane, L); Fam::describe(p, L); }
       }
-      const bool bulk = chunk_is_bulk<F>(p, a, vec, n_lanes);
+      const bool bulk = chunk_is_bulk<Fam, O>(p, a, vec, n_lanes);
       ws.any_bulk = ws.any_bulk || bulk;
       R unused_rng;
-      emit_obs<F>(p, a, ws, L, unused_rng, io.obs, warp_base, n_lanes, lane, active, bulk, vec);
+      emit_obs<Fam>(p, a, ws, L, unused_rng, obs, warp_base, n_lanes, lane, active, bulk, vec);
       kept = false;
       c = dynamic ? fetch_chunk(a, total_warps) : n_chunks;
     }
   };
-  typename F::Lane keep;
-  F::init(p, keep);
+  typename Fam::Lane keep;
+  Fam::init(p, keep);
 
   if (blockIdx.x < copier_blocks) {
     if (threadIdx.x == 0) {
@@ -1025,7 +1135,7 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
       // every independent load of up to kAhead chunks first: one round trip to L2 (or over PCIe, when the actions
       // were not staged on the device) instead of one per chunk -- a warp owns 4-5 chunks of a 65 536-lane batch
       int32_t fetched[kAhead];
-      typename F::Lane lanes[kAhead];
+      typename Fam::Lane lanes[kAhead];
       EpisodeStats eps[kAhead];
 #pragma unroll
       for (int k = 0; k < kAhead; ++k) {
@@ -1033,10 +1143,10 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
         const int64_t lane = c * cl + tid;
         const bool live = c < n_chunks && tid < cl && lane < B;
         fetched[k] = 0;
-        F::init(p, lanes[k]);
+        Fam::init(p, lanes[k]);
         if (live) {
           fetched[k] = __ldcv(io.actions + lane);
-          F::load(p, lane, lanes[k]);
+          Fam::load(p, lane, lanes[k]);
           if (kTrack) eps[k].load(p, lane);
         }
       }
@@ -1045,17 +1155,17 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
         const int64_t c = c0 + k * total_warps;
         if (c >= n_chunks) break;
         const int64_t lane = c * cl + tid;
-        typename F::Lane& L = lanes[k];
+        typename Fam::Lane& L = lanes[k];
         if (tid < cl && lane < B) {
           R rng, wrng;
-          lane_open<F>(p, lane, L, rng, wrng, eps[k], MODE_STEP, kNoise, kTrack, /*state_loaded=*/true);
+          lane_open<Fam>(p, lane, L, rng, wrng, eps[k], MODE_STEP, kNoise, kTrack, /*state_loaded=*/true);
           int32_t action = fetched[k];
           if ((uint32_t)action >= (uint32_t)p.num_actions) {
             if (a.bad_action) *a.bad_action = 1;
             action = action < 0 ? 0 : p.num_actions - 1;
           }
-          lane_step<F>(p, lane, L, rng, wrng, eps[k], action, MODE_STEP, kNoise, kTrack, a.step0, h.stage, lane);
-          lane_close<F>(p, lane, L, rng, wrng, eps[k], kNoise, kTrack);
+          lane_step<Fam>(p, lane, L, rng, wrng, eps[k], action, MODE_STEP, kNoise, kTrack, a.step0, h.stage, lane);
+          lane_close<Fam>(p, lane, L, rng, wrng, eps[k], kNoise, kTrack);
         }
         if (c == own) keep = L;
       }

@@ -50,12 +50,24 @@ def _resolve_device(device) -> int:
   return dev.index if dev.index is not None else torch.cuda.current_device()
 
 
-def _make_config(spec: EnvSpec, rng_kind: int, flags: int, log_schedule=None):
+def _obs_dtype(value):
+  """(torch dtype, bsb_obs_dtype) of an `obs_dtype` argument: a name or a torch dtype."""
+  import torch
+  codes = {torch.float32: _lib.OBS_FLOAT32, torch.bfloat16: _lib.OBS_BFLOAT16, torch.uint8: _lib.OBS_UINT8}
+  names = {'float32': torch.float32, 'bfloat16': torch.bfloat16, 'uint8': torch.uint8}
+  dtype = names.get(value, value) if isinstance(value, str) else value
+  if dtype not in codes:
+    raise ValueError(f"obs_dtype must be 'float32', 'bfloat16', 'uint8' or the torch dtype, got {value!r}")
+  return dtype, codes[dtype]
+
+
+def _make_config(spec: EnvSpec, rng_kind: int, flags: int, log_schedule=None, obs_dtype: int = 0):
   cfg = _lib.Config()
   cfg.family = spec.family
   cfg.wrapper = spec.wrapper
   cfg.rng_kind = rng_kind
   cfg.flags = flags
+  cfg.obs_dtype = obs_dtype
   cfg.deterministic = 1
   cfg.reward_scale = 1.0
   for key, value in spec.fields.items():
@@ -83,9 +95,9 @@ class _Handle:
   """Owns one bsb_env*."""
 
   def __init__(self, spec: EnvSpec, batch: int, device_ordinal: int, seed: int, lane_offset: int,
-               rng_kind: int, flags: int, log_schedule=None):
+               rng_kind: int, flags: int, log_schedule=None, obs_dtype: int = 0):
     self.lib = _lib.load()
-    cfg, keep = _make_config(spec, rng_kind, flags, log_schedule)
+    cfg, keep = _make_config(spec, rng_kind, flags, log_schedule, obs_dtype)
     ptr = ctypes.c_void_p()
     _lib.check(self.lib.bsb_create(ctypes.byref(cfg), batch, device_ordinal, seed & _MASK64,
                                    lane_offset & _MASK64, ctypes.byref(ptr)))
@@ -114,12 +126,25 @@ class StepBuffers:
     self.step_type = step_type
     self.actions = actions
     self._outputs = None      # struct bsb_outputs over these tensors, built once (the tensors are never swapped)
+    self._bound = None        # observation dtype the struct was last checked against (bind)
     self._timestep = None
 
   def as_outputs(self) -> _lib.Outputs:
     if self._outputs is None:
       self._outputs = self._build_outputs()
     return self._outputs
+
+  def bind(self, obs_dtype) -> _lib.Outputs:
+    """`as_outputs()` for an environment whose observations are `obs_dtype`.  The dtype is checked when the buffers
+    first meet an environment of that dtype; callers on the per-step path write
+    `out._outputs if out._bound is dtype else out.bind(dtype)`, so buffers passed to environments of another dtype
+    are checked again (a kernel would otherwise write past a narrower observation)."""
+    if self._bound is not obs_dtype:
+      if self.observation is not None and self.observation.dtype != obs_dtype:
+        raise ValueError(f'out.observation is {self.observation.dtype}, but this environment writes {obs_dtype} '
+                         'observations (obs_dtype)')
+      self._bound = obs_dtype
+    return self.as_outputs()
 
   def _build_outputs(self) -> _lib.Outputs:
     import torch
@@ -164,11 +189,16 @@ class GraphedSteps:
 
 
 class BatchedEnvironment:
-  """`batch` independent lanes of one environment on one device."""
+  """`batch` independent lanes of one environment on one device.
+
+  `obs_dtype` ('float32', 'bfloat16' or 'uint8', or the torch dtype; fixed for the life of the environment) is the
+  element type of the observations the kernels write: exactly the float32 observation `.to(obs_dtype)`, without a
+  second pass over it.  'uint8' is available for deep_sea and catch (0 / 1 cells); reduced dtypes need
+  rng='philox'.  Rewards, discounts, step types, info, episode statistics and `state_dict()` do not depend on it."""
 
   def __init__(self, spec: EnvSpec, batch: int, device='cuda', seed: Optional[int] = None,
                rng: str = 'philox', lane_offset: int = 0, track_episodes: bool = False,
-               reward_dtype='float32', record_rows: bool = False):
+               reward_dtype='float32', record_rows: bool = False, obs_dtype='float32'):
     import torch
     self._torch = torch
     self._spec = spec
@@ -196,8 +226,9 @@ class BatchedEnvironment:
       from bsuite_b200 import recording  # pylint: disable=import-outside-toplevel
       self._log_schedule = recording.log_schedule(spec.bsuite_num_episodes)
     self._reward_dtype = torch.float64 if str(reward_dtype).endswith('64') else torch.float32
+    self._obs_dtype, obs_code = _obs_dtype(obs_dtype)
     self._handle = _Handle(spec, self._batch, self._ordinal, self._seed, self._lane_offset, self._rng_kind, flags,
-                           self._log_schedule)
+                           self._log_schedule, obs_code)
     self._lib = self._handle.lib
     n = ctypes.c_int32()
     _lib.check(self._lib.bsb_info_count(self._handle.ptr, ctypes.byref(n)))
@@ -213,9 +244,11 @@ class BatchedEnvironment:
   family = property(lambda self: self._spec.family)
   num_actions = property(lambda self: self._spec.num_actions)
   info_names = property(lambda self: self._info_names)
+  obs_dtype = property(lambda self: self._obs_dtype)      # torch dtype of the observation tensors
 
   def observation_spec(self):
-    """Per-lane spec, identical to the reference environment's."""
+    """Per-lane spec, identical to the reference environment's (float32 values).  The observation tensors this
+    environment returns carry `obs_dtype`."""
     if self._spec.obs_bounds is not None:
       lo, hi = self._spec.obs_bounds
       return specs.BoundedArray(shape=self._spec.obs_shape, dtype=np.float32, name=self._spec.obs_spec_name,
@@ -231,7 +264,7 @@ class BatchedEnvironment:
     lead = (self._batch,) if num_steps is None else (int(num_steps), self._batch)
     kw = dict(device=self._device)
     return StepBuffers(
-        observation=torch.empty(lead + tuple(self._spec.obs_shape), dtype=torch.float32, **kw),
+        observation=torch.empty(lead + tuple(self._spec.obs_shape), dtype=self._obs_dtype, **kw),
         reward=torch.empty(lead, dtype=self._reward_dtype, **kw),
         discount=torch.empty(lead, dtype=torch.float32, **kw),
         step_type=torch.empty(lead, dtype=torch.int32, **kw),
@@ -259,7 +292,7 @@ class BatchedEnvironment:
   def reset(self, out: Optional[StepBuffers] = None):
     """base.Environment.reset for every lane (base.py:54-57)."""
     out = out or self.make_buffers()
-    outputs = out.as_outputs()
+    outputs = out.bind(self._obs_dtype)
     self._async_work = True
     _lib.check(self._lib.bsb_reset(self._handle.ptr, ctypes.byref(outputs), self._stream()))
     return out.timestep()
@@ -277,7 +310,9 @@ class BatchedEnvironment:
     if out is None:
       out = self.make_buffers()
     self._async_work = True
-    status = self._lib.bsb_step(self._handle.ptr, actions.data_ptr(), ctypes.byref(out.as_outputs()), self._stream())
+    # bind() (the dtype check) runs when these buffers first meet an environment of this dtype
+    outputs = out._outputs if out._bound is self._obs_dtype else out.bind(self._obs_dtype)
+    status = self._lib.bsb_step(self._handle.ptr, actions.data_ptr(), ctypes.byref(outputs), self._stream())
     if status:
       _lib.check(status)
     return out.timestep()
@@ -290,7 +325,7 @@ class BatchedEnvironment:
     if self._ordinal < 0:
       return self.make_buffers()
     host = self.make_host_buffers()
-    return StepBuffers(observation=torch.empty((self._batch,) + tuple(self._spec.obs_shape), dtype=torch.float32,
+    return StepBuffers(observation=torch.empty((self._batch,) + tuple(self._spec.obs_shape), dtype=self._obs_dtype,
                                                device=self._device),
                        reward=host.reward, discount=host.discount, step_type=host.step_type)
 
@@ -309,7 +344,7 @@ class BatchedEnvironment:
       reward = torch.empty(B, dtype=torch.float64, pin_memory=pin)
       discount = torch.empty(B, dtype=torch.float32, pin_memory=pin)
       step_type = torch.empty(B, dtype=torch.int32, pin_memory=pin)
-    observation = (torch.empty((B,) + tuple(self._spec.obs_shape), dtype=torch.float32, pin_memory=pin)
+    observation = (torch.empty((B,) + tuple(self._spec.obs_shape), dtype=self._obs_dtype, pin_memory=pin)
                    if with_observation else None)
     return StepBuffers(observation=observation, reward=reward, discount=discount, step_type=step_type)
 
@@ -345,7 +380,9 @@ class BatchedEnvironment:
       actions = actions.contiguous()
     if out is None:
       out = self.make_buffers()
-    houts = host.as_outputs()          # struct bsb_outputs over the host tensors, built once per StepBuffers
+    houts = host._outputs if host._bound is self._obs_dtype else host.bind(self._obs_dtype)   # built once
+    if out._bound is not self._obs_dtype:
+      out.bind(self._obs_dtype)          # the device observation's dtype
     dev_obs = None if self._ordinal < 0 else out.observation.data_ptr()
     if self._ordinal < 0:        # host environment: one memory space; `out.observation` is the observation
       houts = _lib.Outputs.from_buffer_copy(houts)
@@ -398,7 +435,7 @@ class BatchedEnvironment:
     if actions is not None:
       actions = self._device_actions(actions, (num_steps, self._batch))
       act_ptr = ctypes.c_void_p(actions.data_ptr())
-    outputs = out.as_outputs()
+    outputs = out.bind(self._obs_dtype)
     act_out = ctypes.c_void_p(out.actions.data_ptr()) if out.actions is not None else None
     self._async_work = True
     _lib.check(self._lib.bsb_rollout(self._handle.ptr, num_steps, act_ptr, int(action_seed) & _MASK64,

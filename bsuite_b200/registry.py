@@ -23,6 +23,9 @@ def unpack_bsuite_id(bsuite_id: str) -> Tuple[str, int]:
 
 def _instantiate(spec, batch, device, seed, rng, **engine_kwargs):
   if batch is None:
+    if 'obs_dtype' in engine_kwargs:
+      raise ValueError('obs_dtype applies to batched environments only (pass batch=...); the B = 1 face writes float32 '
+                       'numpy observations like the reference')
     if engine_kwargs:
       raise TypeError(f'{sorted(engine_kwargs)} only apply to batched environments (pass batch=...)')
     return DmEnvAdapter(spec, device=device, seed=seed, rng=rng)

@@ -24,7 +24,7 @@ class Config(ctypes.Structure):           # struct bsb_config, field for field (
   _fields_ = ([(name, I32) for name in (
       'family', 'wrapper', 'rng_kind', 'flags', 'size', 'deterministic', 'rows', 'columns', 'memory_length',
       'num_bits', 'chain_length', 'n_distractor', 'num_actions', 'max_steps', 'num_data', 'image_rows',
-      'image_cols', 'reserved0')] + [(name, F64) for name in (
+      'image_cols', 'obs_dtype')] + [(name, F64) for name in (
           'unscaled_move_cost', 'height_threshold', 'x_threshold', 'timescale', 'max_time', 'init_range',
           'theta_dot_threshold', 'x_reward_threshold', 'move_cost', 'noise_scale', 'reward_scale')] + [
               ('table', ctypes.c_void_p), ('table_bytes', ctypes.c_int64),

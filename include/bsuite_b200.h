@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define BSB_ABI_VERSION 7
+#define BSB_ABI_VERSION 8
 #define BSB_DEVICE_HOST (-1)
 #define BSB_MAX_INFO 4
 
@@ -87,6 +87,22 @@ typedef enum bsb_rng_kind {
 } bsb_rng_kind;
 
 /*
+ * Element type of the observations a handle writes (bsb_config.obs_dtype),
+ * fixed at bsb_create.  What is written is exactly the float32 observation
+ * converted: bfloat16 rounds to nearest even (as torch.Tensor.to(bfloat16)
+ * does; a NaN, which no observation holds, is written as 0x7fc0), uint8
+ * holds the 0 / 1 cells of deep_sea and catch.  Reduced dtypes
+ * need BSB_RNG_PHILOX; uint8 is for deep_sea and catch only (other
+ * combinations return BSB_UNSUPPORTED).  Rewards, discounts, step types, info,
+ * episode statistics, log rows and the state snapshot do not depend on it.
+ */
+typedef enum bsb_obs_dtype {
+  BSB_OBS_FLOAT32 = 0,
+  BSB_OBS_BFLOAT16 = 1,
+  BSB_OBS_UINT8 = 2
+} bsb_obs_dtype;
+
+/*
  * Environment configuration: the keyword arguments of the reference
  * constructors, flattened into one POD.  Fields that do not apply to `family`
  * are ignored.  Tables are HOST pointers; bsb_create copies them.
@@ -112,7 +128,7 @@ typedef struct bsb_config {
   int32_t max_steps;
   /* mnist.py:36 (num_data = int(fraction * len(labels)), 28x28 images) */
   int32_t num_data, image_rows, image_cols;
-  int32_t reserved0;
+  int32_t obs_dtype;     /* bsb_obs_dtype; 0 = float32 */
 
   double unscaled_move_cost;                         /* deep_sea.py:54 */
   double height_threshold, x_threshold, timescale,   /* cartpole.py:82-87 */
@@ -153,6 +169,11 @@ typedef struct bsb_config {
  * array carries a leading T axis.  Any pointer except `observation` may be
  * NULL (that output is then not written).
  *   observation : float32 [B, obs_numel]   fresh dense tensor every step
+ *                 (a handle created with a reduced obs_dtype writes obs_numel
+ *                 elements of THAT type per lane here: the pointer keeps its
+ *                 declared type and the caller casts, e.g. (float*)bf16_buffer;
+ *                 the same holds for bsb_step_host's device_obs and
+ *                 host_out->observation)
  *   reward      : float32 [B]   (float32 rounding of the float64 reward)
  *   reward_f64  : float64 [B]   (the reference's double-precision reward)
  *   discount    : float32 [B]   1 (MID) / 0 (LAST) / 0 (FIRST = None)
@@ -454,7 +475,8 @@ int32_t bsb_image_plan_destroy(bsb_image_plan* plan);
 
 /*
  * in: float32 [batch, in_rows, in_cols], out: float32 [batch, out_rows,
- * out_cols, channels], both dense and caller-owned, in the plan's memory space.
+ * out_cols, channels], both dense and caller-owned, in the plan's memory space
+ * (float32 only: convert a reduced-dtype observation before resizing it).
  * A device plan enqueues one kernel on `stream` and neither synchronises nor
  * allocates, so the call may be captured into a CUDA graph; a host plan is
  * synchronous.  batch 0 does nothing.  A device plan with a Gaussian pass

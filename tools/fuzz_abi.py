@@ -72,6 +72,7 @@ def main():
   lib = _lib.load()
   table = np.zeros(1 << 16, np.uint8)
   created = rejected = 0
+  by_dtype = [0, 0, 0]                      # handles created per bsb_obs_dtype
   for _ in range(iterations):
     cfg = _lib.Config()
     plausible = rng.random() < 0.5          # half the time start from something a real caller might send
@@ -79,6 +80,10 @@ def main():
     cfg.wrapper = rng.choice([0, 1, 2]) if plausible else rng.choice([-1, 0, 1, 2, 3])
     cfg.rng_kind = rng.choice([0, 1]) if plausible else rng.choice([-1, 0, 1, 2])
     cfg.flags = rng.choice([0, 1, 2, 3])
+    # observation element type: float32 / bfloat16 / uint8, or a value that is no bsb_obs_dtype at all
+    cfg.obs_dtype = rng.choice([0, 0, 1, 2]) if plausible else rng.choice([-1, 0, 1, 2, 3, 1 << 20])
+    if plausible and cfg.obs_dtype == 2 and rng.random() < 0.8:
+      cfg.family = rng.choice([_lib.DEEP_SEA, _lib.CATCH])       # mostly the families uint8 is for
     for field in INT_FIELDS:
       setattr(cfg, field, rng.choice([1, 2, 3, 5, 10]) if plausible else rng.choice(INT_VALUES))
     for field in ('unscaled_move_cost', 'height_threshold', 'x_threshold', 'timescale', 'max_time', 'init_range',
@@ -103,17 +108,25 @@ def main():
     handle = ctypes.c_void_p()
     status = lib.bsb_create(ctypes.byref(cfg), batch, _lib.DEVICE_HOST, rng.choice([0, 5, 2**32, 2**63]),
                             rng.choice([0, 7, 2**40]), ctypes.byref(handle))
+    # reduced observation dtypes: bfloat16 for every family, uint8 for deep_sea / catch, Philox only
+    bad_dtype = cfg.obs_dtype not in (0, 1, 2)
+    unsupported_dtype = (cfg.obs_dtype == 2 and cfg.family not in (_lib.DEEP_SEA, _lib.CATCH)) or \
+        (cfg.obs_dtype in (1, 2) and cfg.rng_kind == _lib.RNG_MT19937)
     if status != 0:
       rejected += 1
       assert lib.bsb_last_error()
+      assert status in (1, 2), status          # BSB_INVALID_ARGUMENT / BSB_UNSUPPORTED, never a crash-shaped code
       continue
+    assert not bad_dtype and not unsupported_dtype, (cfg.obs_dtype, cfg.family, cfg.rng_kind)
     created += 1
+    by_dtype[cfg.obs_dtype] += 1
     numel, n_act = ctypes.c_int64(), ctypes.c_int32()
     lib.bsb_obs_numel(handle, ctypes.byref(numel))
     lib.bsb_num_actions(handle, ctypes.byref(n_act))
     T = rng.choice([1, 2, 5])
     if batch * numel.value * T < 5_000_000:
-      obs = np.zeros(T * batch * numel.value, np.float32)
+      elem = {0: 4, 1: 2, 2: 1}[cfg.obs_dtype]           # the buffer is exactly as large as the dtype needs
+      obs = np.zeros(T * batch * numel.value * elem, np.uint8)
       reward, reward64 = np.zeros(T * batch, np.float32), np.zeros(T * batch, np.float64)
       discount, step_type = np.zeros(T * batch, np.float32), np.zeros(T * batch, np.int32)
       out = _lib.Outputs()
@@ -168,7 +181,8 @@ def main():
       assert lib.bsb_set_state(handle, ctypes.c_void_p(blob.ctypes.data), nbytes.value, None) == 0
     lib.bsb_destroy(handle)
   fuzz_image(lib, rng, max(iterations // 10, 20))
-  print(f'fuzz_abi: {created} handles created, {rejected} configurations rejected, no crash')
+  print(f'fuzz_abi: {created} handles created (float32 / bfloat16 / uint8: {by_dtype[0]} / {by_dtype[1]} / '
+        f'{by_dtype[2]}), {rejected} configurations rejected, no crash')
 
 
 if __name__ == '__main__':

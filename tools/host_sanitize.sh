@@ -9,7 +9,7 @@ OUT=/tmp/bsb_asan
 LOG=${1:-/tmp/bsb_asan/run.log}
 mkdir -p $OUT
 cd "$(dirname "$0")/../bsuite_b200/csrc"
-ls bsb_engine.cu bsb_comm.cu fam_*.cu | xargs -P 16 -I{} sh -c "nvcc -gencode arch=compute_90a,code=sm_90a -O1 -std=c++17 --fmad=false \
+ls bsb_engine.cu bsb_comm.cu bsb_image.cu fam_*.cu obs_*.cu | xargs -P 16 -I{} sh -c "nvcc -gencode arch=compute_90a,code=sm_90a -O1 -std=c++17 --fmad=false \
   -Xcompiler -fPIC,-ffp-contract=off,-O1,-g,-fsanitize=address,-fsanitize=undefined,-fno-omit-frame-pointer -c {} -o $OUT/\$(basename {} .cu).o"
 nvcc -shared -o $OUT/libbsuite_b200.so $OUT/*.o -cudart static -ldl -Xcompiler -fsanitize=address,-fsanitize=undefined 2>/dev/null
 cd ../..

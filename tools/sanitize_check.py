@@ -71,6 +71,16 @@ for bsuite_id, batch in (('deep_sea/11', 20000), ('deep_sea_stochastic/3', 40001
   same = all(torch.equal(a, b) for a, b in zip(*results))
   print(bsuite_id, batch, 'bulk == vector:', same, flush=True)
   assert same
+# Reduced observation dtypes: uint8 deep_sea tiles (16-lane groups) and bfloat16 catch boards, against float32 twins.
+for bsuite_id, batch, dtype in (('deep_sea/11', 20000, torch.uint8), ('catch/0', 5001, torch.bfloat16)):
+  env = bsuite_b200.load_from_id(bsuite_id, batch=batch, device='cuda', seed=3, obs_dtype=dtype)
+  twin = bsuite_b200.load_from_id(bsuite_id, batch=batch, device='cuda', seed=3)
+  acts = torch.as_tensor(env.random_actions(4, action_seed=1, first_step=0)).cuda()
+  for i in range(4):
+    assert torch.equal(env.step(acts[i]).observation, twin.step(acts[i]).observation.to(dtype))
+  assert torch.equal(env.rollout(3, action_seed=2).observation, twin.rollout(3, action_seed=2).observation.to(dtype))
+  print(bsuite_id, batch, dtype, '== float32 twin converted: True', flush=True)
+  env.close(); twin.close()
 # Graph-safe mode: device clock, chunk counter re-armed by the last CTA, the deterministic two-stage reduction.
 for bsuite_id, batch in (('deep_sea/11', 20000), ('catch/0', 5000)):
   env = bsuite_b200.load_from_id(bsuite_id, batch=batch, device='cuda', seed=3, track_episodes=True)
