@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BSB_LIBRARY points the binding at another build of the SAME library (tools/host_sanitize.sh: ASan/UBSan build)
 LIB_PATH = os.environ.get('BSB_LIBRARY') or os.path.join(_HERE, 'libbsuite_b200.so')
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 DEVICE_HOST = -1
 MAX_INFO = 4
 COMM_ID_BYTES = 128
@@ -28,6 +28,7 @@ WRAP_NONE, WRAP_REWARD_NOISE, WRAP_REWARD_SCALE = range(3)
 # enum bsb_rng_kind
 RNG_PHILOX, RNG_MT19937 = range(2)
 FLAG_TRACK_EPISODES = 1
+FLAG_SAME_STEP_RESET = 2
 # enum bsb_obs_dtype
 OBS_FLOAT32, OBS_BFLOAT16, OBS_UINT8 = range(3)
 HOST_ORDER_AFTER_STREAM, HOST_PRELAUNCH, HOST_FENCE_CALLER, HOST_NO_WAIT = 1, 2, 4, 8      # bsb_step_host flags
@@ -74,7 +75,7 @@ class ImageDesc(ctypes.Structure):
 class Outputs(ctypes.Structure):
   """struct bsb_outputs."""
   _fields_ = [('observation', ctypes.c_void_p), ('reward', ctypes.c_void_p), ('reward_f64', ctypes.c_void_p),
-              ('discount', ctypes.c_void_p), ('step_type', ctypes.c_void_p)]
+              ('discount', ctypes.c_void_p), ('step_type', ctypes.c_void_p), ('final_observation', ctypes.c_void_p)]
 
 
 EXPORTS = {

@@ -35,17 +35,27 @@ template <> struct HostEmit<Mnist> {
 };
 
 // Observations of type O other than float32: each lane's float32 observation is rendered into `f32` and converted
-// element by element with obs_cast, the function the kernels use.
-template <class F, int RK, class O>
+// element by element with obs_cast, the function the kernels use.  kSameStep: a lane whose step returned LAST is reset
+// in the same call, and its final observation goes to a.final_obs when that is given.
+template <class F, int RK, class O, bool kSameStep = false>
 void host_run(const EnvParams& p, const LaunchArgs& a) {
   typedef typename RngOf<RK>::type R;
   const int64_t B = p.batch;
   const int K = p.obs_numel;
   O* const obs = reinterpret_cast<O*>(a.obs);
+  O* const fin = reinterpret_cast<O*>(a.final_obs);
   std::vector<float> f32(std::is_same<O, float>::value ? 0 : (size_t)K);
   const bool noise = p.wrapper == BSB_WRAP_REWARD_NOISE && a.mode != MODE_INIT;
   const bool track = p.ep != nullptr && a.mode != MODE_INIT;
   const MailFields out = {a.actions, a.obs, a.reward, a.reward_f64, a.discount, a.step_type, 0, 0};
+  auto render = [&](const typename F::Lane& L, R& rng, O* dst) {
+    if constexpr (std::is_same<O, float>::value) {
+      HostEmit<F>::run(p, L, rng, dst);
+    } else {
+      HostEmit<F>::run(p, L, rng, f32.data());
+      for (int e = 0; e < K; ++e) dst[e] = obs_cast<O>(f32[(size_t)e]);
+    }
+  };
   for (int64_t lane = 0; lane < B; ++lane) {
     typename F::Lane L;
     R rng, wrng;
@@ -54,6 +64,9 @@ void host_run(const EnvParams& p, const LaunchArgs& a) {
     action_stream.open();
     lane_open<F>(p, lane, L, rng, wrng, ep, a.mode, noise, track);
     if (a.mode == MODE_INIT) F::ctor_draws(p, L, rng);
+    MergedReset<F, R> merged;
+    F::init(p, merged.last);
+    merged.done = false;
     for (int64_t t = 0; t < a.T; ++t) {
       const int64_t off = t * B + lane;
       int32_t action = 0;
@@ -62,13 +75,9 @@ void host_run(const EnvParams& p, const LaunchArgs& a) {
                            : action_stream.sample(a.action_seed, p.lane_offset + (uint64_t)lane, (uint64_t)(a.step0 + t), p.num_actions);
         if (a.actions_out) a.actions_out[off] = action;
       }
-      lane_step<F>(p, lane, L, rng, wrng, ep, action, a.mode, noise, track, a.step0 + t, out, off);
-      if constexpr (std::is_same<O, float>::value) {
-        HostEmit<F>::run(p, L, rng, obs + off * (int64_t)K);
-      } else {
-        HostEmit<F>::run(p, L, rng, f32.data());
-        for (int e = 0; e < K; ++e) obs[off * (int64_t)K + e] = obs_cast<O>(f32[(size_t)e]);
-      }
+      lane_step<F, R, kSameStep>(p, lane, L, rng, wrng, ep, action, a.mode, noise, track, a.step0 + t, out, off, &merged);
+      if constexpr (kSameStep) { if (merged.done && fin) render(merged.last, merged.rng, fin + off * (int64_t)K); }
+      render(L, rng, obs + off * (int64_t)K);
     }
     lane_close<F>(p, lane, L, rng, wrng, ep, noise, track);
   }
@@ -213,11 +222,11 @@ int launch(bsb_env* e, const LaunchArgs& a, const Geometry& g, cudaStream_t stre
   return BSB_OK;
 }
 
-template <class F, int RK, bool kNoise, bool kTrack, class O>
+template <class F, int RK, bool kNoise, bool kTrack, class O, bool kSameStep = false>
 int device_launch(bsb_env* e, LaunchArgs a, cudaStream_t stream) {
   Geometry g;
   const int rc = plan_launch<F, O>(e, a, g);
-  return rc != BSB_OK ? rc : launch(e, a, g, stream, transition_kernel<typename KernelFamily<F, O>::type, RK, kNoise, kTrack>, e->p, a);
+  return rc != BSB_OK ? rc : launch(e, a, g, stream, transition_kernel<typename KernelTag<F, O, kSameStep>::type, RK, kNoise, kTrack>, e->p, a);
 }
 
 // Two-phase host step (DeepSea, Catch): one launch (h.phase 0) or one of the two launches of a split step.
@@ -245,20 +254,24 @@ int with_flags(const bsb_env* e, const LaunchArgs& a, Launch launch) {
   return track ? launch(std::false_type(), std::true_type()) : launch(std::false_type(), std::false_type());
 }
 
-// Float32 observations: both bit sources.  Reduced dtypes: Philox only (bsb_create refuses MT19937 with them).
-template <class F, class O>
+// Float32 observations: both bit sources.  Reduced dtypes and same-step handles: Philox only (bsb_create refuses
+// MT19937 with them).  Same-step handles never take the two-phase host step.
+template <class F, class O, bool kSameStep = false>
 int run_family_as(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoPhaseArgs* two_phase) {
-  constexpr bool kF32 = std::is_same<O, float>::value;
+  constexpr bool kF32 = std::is_same<O, float>::value && !kSameStep;
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
-  if (!kF32 && mt) return fail(BSB_INTERNAL, "reduced obs_dtype with MT19937");
+  if (!kF32 && mt) return fail(BSB_INTERNAL, "reduced obs_dtype or same-step auto-reset with MT19937");
+  if (kSameStep && two_phase) return fail(BSB_INTERNAL, "a two-phase host step on a same-step handle");
+  // LaunchArgs::final_obs shares its word with doorbell_timeout_ns: a launch without a mailbox must carry a pointer
+  if (kSameStep && !a.mailbox && a.wait_doorbell) return fail(BSB_INTERNAL, "a doorbell launch without a mailbox");
   if (e->device < 0) {
     if constexpr (kF32) { if (mt) { host_run<F, 1, O>(e->p, a); return BSB_OK; } }
-    host_run<F, 0, O>(e->p, a);
+    host_run<F, 0, O, kSameStep>(e->p, a);
     return BSB_OK;
   }
   return with_flags(e, a, [&](auto noise, auto track) {
     constexpr bool kNoise = decltype(noise)::value, kTrack = decltype(track)::value;
-    if constexpr (ObsFromState<F>::value) {
+    if constexpr (ObsFromState<F>::value && !kSameStep) {
       if constexpr (kF32) {
         if (two_phase) return mt ? two_phase_launch<F, 1, kNoise, kTrack, O>(e, a, *two_phase, stream)
                                  : two_phase_launch<F, 0, kNoise, kTrack, O>(e, a, *two_phase, stream);
@@ -269,7 +282,7 @@ int run_family_as(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const Tw
     if constexpr (kF32) {
       if (mt) return device_launch<F, 1, kNoise, kTrack, O>(e, a, stream);
     }
-    return device_launch<F, 0, kNoise, kTrack, O>(e, a, stream);
+    return device_launch<F, 0, kNoise, kTrack, O, kSameStep>(e, a, stream);
   });
 }
 
@@ -290,9 +303,28 @@ BSB_REDUCED(DeepSea) BSB_REDUCED(Catch) BSB_REDUCED(Cartpole) BSB_REDUCED(Cartpo
 BSB_REDUCED(MemoryChain) BSB_REDUCED(Bandit) BSB_REDUCED(UmbrellaChain) BSB_REDUCED(DiscountingChain) BSB_REDUCED(Mnist)
 #undef BSB_REDUCED
 
-// Kernels and host path of the handle's observation dtype.
+// Same-step auto-reset (BSB_FLAG_SAME_STEP_RESET), every obs_dtype, Philox.  Instantiated in translation units of
+// their own (ss_<family>.cu): a next-step handle never loads their modules.
+template <class F>
+int run_same_step(bsb_env* e, const LaunchArgs& a, cudaStream_t stream) {
+  switch (e->obs_dtype) {
+    case BSB_OBS_FLOAT32: return run_family_as<F, float, true>(e, a, stream, nullptr);
+    case BSB_OBS_BFLOAT16: return run_family_as<F, Bf16, true>(e, a, stream, nullptr);
+    case BSB_OBS_UINT8:
+      if constexpr (BinaryObs<F>::value) return run_family_as<F, uint8_t, true>(e, a, stream, nullptr);
+      break;
+  }
+  return fail(BSB_INTERNAL, "obs_dtype not compiled for this family");
+}
+#define BSB_SAME_STEP(F) extern template int run_same_step<F>(bsb_env*, const LaunchArgs&, cudaStream_t);
+BSB_SAME_STEP(DeepSea) BSB_SAME_STEP(Catch) BSB_SAME_STEP(Cartpole) BSB_SAME_STEP(CartpoleSwingup) BSB_SAME_STEP(MountainCar)
+BSB_SAME_STEP(MemoryChain) BSB_SAME_STEP(Bandit) BSB_SAME_STEP(UmbrellaChain) BSB_SAME_STEP(DiscountingChain) BSB_SAME_STEP(Mnist)
+#undef BSB_SAME_STEP
+
+// Kernels and host path of the handle's auto-reset mode and observation dtype.
 template <class F>
 int run_family(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr) {
+  if (e->same_step) return run_same_step<F>(e, a, stream);
   if (e->obs_dtype != BSB_OBS_FLOAT32) return run_reduced<F>(e, a, stream, two_phase);
   return run_family_as<F, float>(e, a, stream, two_phase);
 }

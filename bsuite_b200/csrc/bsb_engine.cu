@@ -111,10 +111,11 @@ LaunchArgs make_args(const bsb_env* e, const bsb_outputs* out, const int32_t* ac
   LaunchArgs a;
   memset(&a, 0, sizeof(a));
   a.actions = actions;
-  if (out) { a.obs = out->observation; a.reward = out->reward; a.reward_f64 = out->reward_f64; a.discount = out->discount; a.step_type = out->step_type; }
+  if (out) { a.obs = out->observation; a.reward = out->reward; a.reward_f64 = out->reward_f64; a.discount = out->discount; a.step_type = out->step_type; a.final_obs = out->final_observation; }
   a.T = T; a.step0 = e->steps_done; a.mode = mode;
   const size_t step_bytes = (size_t)e->p.batch * (size_t)e->p.obs_numel * (size_t)e->obs_elem_bytes;
   a.obs_vec_ok = (out && (reinterpret_cast<uintptr_t>(out->observation) % 16 == 0) && (T == 1 || step_bytes % 16 == 0)) ? 1 : 0;
+  a.final_vec_ok = (a.final_obs && (reinterpret_cast<uintptr_t>(a.final_obs) % 16 == 0) && (T == 1 || step_bytes % 16 == 0)) ? 1 : 0;
   return a;
 }
 
@@ -163,6 +164,8 @@ int validate(const bsb_config& c, int64_t batch, int* obs_rows, int* obs_cols, i
     return fail(BSB_UNSUPPORTED, "obs_dtype uint8 is only available for deep_sea and catch, whose observations are 0 / 1");
   if (c.obs_dtype != BSB_OBS_FLOAT32 && c.rng_kind == BSB_RNG_MT19937)
     return fail(BSB_UNSUPPORTED, "a bfloat16 or uint8 obs_dtype needs rng_kind BSB_RNG_PHILOX");
+  if ((c.flags & BSB_FLAG_SAME_STEP_RESET) && c.rng_kind == BSB_RNG_MT19937)
+    return fail(BSB_UNSUPPORTED, "BSB_FLAG_SAME_STEP_RESET needs rng_kind BSB_RNG_PHILOX");
   if (c.log_schedule_len < 0 || c.log_schedule_len > 4096) return fail(BSB_INVALID_ARGUMENT, "log_schedule_len must be in [0, 4096]");
   if (c.log_schedule_len > 0) {
     if (!c.log_schedule) return fail(BSB_INVALID_ARGUMENT, "log_schedule_len > 0 needs a log_schedule");
@@ -231,12 +234,13 @@ int mailbox_open(bsb_env* e) {
 // lane out, 4 B in): deep_sea from N = 16 up (>= 1 KB of observation per lane).  catch (200 B per lane) is bound
 // by the 2 MB of scalars per step either way and keeps the single-phase kernel.  The rule counts float32 bytes
 // whatever the handle's obs_dtype, so a reduced-dtype handle takes the same path as its float32 twin.
+// Same-step handles always take the single-phase kernel.
 bool family_obs_from_state(const bsb_env* e) {
-  return (e->p.family == BSB_DEEP_SEA || e->p.family == BSB_CATCH) && (size_t)e->p.obs_numel * sizeof(float) >= 1024;
+  return !e->same_step && (e->p.family == BSB_DEEP_SEA || e->p.family == BSB_CATCH) && (size_t)e->p.obs_numel * sizeof(float) >= 1024;
 }
 
 int mailbox_launch(bsb_env* e, unsigned long long ticket, int64_t step0, const MailFields* fields, bool wait_doorbell, bool split = false) {
-  const bsb_outputs out = fields ? bsb_outputs{fields->obs, fields->reward, fields->reward_f64, fields->discount, fields->step_type}
+  const bsb_outputs out = fields ? bsb_outputs{fields->obs, fields->reward, fields->reward_f64, fields->discount, fields->step_type, nullptr}
                                 : bsb_outputs{};
   LaunchArgs a = make_args(e, fields ? &out : nullptr, fields ? fields->actions : nullptr, 1, MODE_STEP);
   a.step0 = step0;
@@ -264,6 +268,7 @@ int mailbox_launch(bsb_env* e, unsigned long long ticket, int64_t step0, const M
     int rc = run(e, a, e->copy_stream, &h);
     if (rc != BSB_OK) return rc;
     a.mailbox = nullptr;
+    a.final_obs = nullptr;        // the word held the doorbell timeout: a launch without a mailbox reads it as final_obs
     h.phase = 2;
   }
   return run(e, a, e->copy_stream, &h);
@@ -434,7 +439,8 @@ int32_t bsb_create(const bsb_config* config, int64_t batch, int32_t device, uint
   bsb_env* e = new bsb_env();
   memset(&e->p, 0, sizeof(e->p));
   e->device = device; e->steps_done = 0;
-  e->obs_dtype = c.obs_dtype; e->obs_elem_bytes = c.obs_dtype == BSB_OBS_BFLOAT16 ? 2 : c.obs_dtype == BSB_OBS_UINT8 ? 1 : 4; e->graph_safe = false; e->clock = nullptr; e->sum_scratch = nullptr; e->names = info_names(c.family);
+  e->obs_dtype = c.obs_dtype; e->obs_elem_bytes = c.obs_dtype == BSB_OBS_BFLOAT16 ? 2 : c.obs_dtype == BSB_OBS_UINT8 ? 1 : 4;
+  e->same_step = (c.flags & BSB_FLAG_SAME_STEP_RESET) != 0; e->graph_safe = false; e->clock = nullptr; e->sum_scratch = nullptr; e->names = info_names(c.family);
   {  // tuning knobs (environment variables, read once per handle)
     auto flag = [](const char* name, int dflt) { const char* v = getenv(name); return v ? (atoi(v) != 0 ? 1 : 0) : dflt; };
     const char* bt = getenv("BSB_BLOCK_THREADS");
@@ -536,7 +542,8 @@ int32_t bsb_create(const bsb_config* config, int64_t batch, int32_t device, uint
   if (c.family == BSB_CARTPOLE || c.family == BSB_CARTPOLE_SWINGUP) BSB_TRY(env_alloc_t(e, &p.st_f64, 6 * B, true));
   if (c.family == BSB_MOUNTAIN_CAR) BSB_TRY(env_alloc_t(e, &p.st_f64, 2 * B, true));
   BSB_TRY(env_alloc_t(e, &p.info, (size_t)BSB_MAX_INFO * B, true));
-  if (c.flags & BSB_FLAG_TRACK_EPISODES) BSB_TRY(env_alloc_t(e, &p.ep, 5 * B, true));
+  // same-step handles: a sixth column, the marker that restarts episode_len / episode_return (lane_step)
+  if (c.flags & BSB_FLAG_TRACK_EPISODES) BSB_TRY(env_alloc_t(e, &p.ep, (e->same_step ? 6 : 5) * B, true));
   if (c.log_schedule_len > 0) {      // per-lane rows at the Logging wrapper's log-spaced episodes (wrappers.py:140-147)
     int64_t* sched = nullptr;
     BSB_TRY(env_alloc_t(e, &sched, (size_t)c.log_schedule_len, false));
@@ -623,8 +630,16 @@ int32_t bsb_steps_done(const bsb_env* env, int64_t* steps) {
   return rc;
 }
 
+// bsb_outputs.final_observation is for same-step handles only.
+static int check_final_observation(const bsb_env* env, const bsb_outputs* out) {
+  if (out->final_observation && !env->same_step)
+    return fail(BSB_INVALID_ARGUMENT, "final_observation needs a handle created with BSB_FLAG_SAME_STEP_RESET");
+  return BSB_OK;
+}
+
 int32_t bsb_reset(bsb_env* env, const bsb_outputs* out, void* stream) {
   if (!env || !out || !out->observation) return fail(BSB_INVALID_ARGUMENT, "bsb_reset needs outputs with an observation buffer");
+  { int crc = check_final_observation(env, out); if (crc != BSB_OK) return crc; }
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
   LaunchArgs a = make_args(env, out, nullptr, 1, MODE_RESET);
   int rc = run(env, a, static_cast<cudaStream_t>(stream));
@@ -634,6 +649,7 @@ int32_t bsb_reset(bsb_env* env, const bsb_outputs* out, void* stream) {
 
 int32_t bsb_step(bsb_env* env, const int32_t* actions, const bsb_outputs* out, void* stream) {
   if (!env || !actions || !out || !out->observation) return fail(BSB_INVALID_ARGUMENT, "bsb_step needs actions and outputs with an observation buffer");
+  { int crc = check_final_observation(env, out); if (crc != BSB_OK) return crc; }
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
   if (env->device < 0) { int vrc = check_host_actions(env, actions, env->p.batch); if (vrc != BSB_OK) return vrc; }
   LaunchArgs a = make_args(env, out, actions, 1, MODE_STEP);
@@ -646,6 +662,7 @@ int32_t bsb_rollout(bsb_env* env, int64_t num_steps, const int32_t* actions, uin
                     const bsb_outputs* out, int32_t* actions_out, void* stream) {
   if (!env || !out || !out->observation) return fail(BSB_INVALID_ARGUMENT, "bsb_rollout needs outputs with an observation buffer");
   if (num_steps <= 0) return fail(BSB_INVALID_ARGUMENT, "num_steps must be positive");
+  { int crc = check_final_observation(env, out); if (crc != BSB_OK) return crc; }
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
   if (env->device < 0 && actions) { int vrc = check_host_actions(env, actions, num_steps * env->p.batch); if (vrc != BSB_OK) return vrc; }
   LaunchArgs a = make_args(env, out, actions, num_steps, MODE_STEP);
@@ -872,6 +889,7 @@ static int report_bad_actions(bsb_env* env) {
 int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* host_out, float* device_obs,
                       void* caller_stream, uint32_t flags) {
   if (!env || !actions || !host_out) return fail(BSB_INVALID_ARGUMENT, "null argument");
+  if (host_out->final_observation) return fail(BSB_UNSUPPORTED, "bsb_step_host does not deliver final_observation");
   if (env->device < 0) {
     if (!host_out->observation) return fail(BSB_INVALID_ARGUMENT, "a host environment writes observations to host_out->observation");
     return bsb_step(env, actions, host_out, nullptr);
@@ -932,6 +950,7 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
       if (!spin) {
         { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
         bsb_outputs dev;
+        dev.final_observation = nullptr;
         dev.observation = f.obs; dev.reward = f.reward; dev.reward_f64 = f.reward_f64; dev.discount = f.discount; dev.step_type = f.step_type;
         int zrc = bsb_step(env, f.actions, &dev, zs);
         if (zrc != BSB_OK) return zrc;
@@ -1019,6 +1038,7 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
   cudaStream_t s = env->copy_stream;
   BSB_CUDA(cudaMemcpyAsync(env->h2d_actions, actions, B * 4, cudaMemcpyHostToDevice, s));
   bsb_outputs dev;
+  dev.final_observation = nullptr;
   dev.observation = device_obs ? device_obs : env->d_obs;
   dev.reward = host_out->reward ? env->d_reward : nullptr;
   dev.reward_f64 = host_out->reward_f64 ? env->d_reward64 : nullptr;

@@ -35,6 +35,8 @@
 // overlaps the tail of the previous step's kernel.
 // Observations may be written as bfloat16 or uint8 instead (bsb_config.obs_dtype; ObsAs below): the emitters stage and
 // store elements of that type, each the float32 value converted by obs_cast (bsb_obs_dtype.h).
+// Same-step handles (BSB_FLAG_SAME_STEP_RESET; SameStep below) reset a lane in the call whose step returned LAST
+// (lane_step) and can emit that LAST's observation as well (emit_final).
 #pragma once
 #include "bsb_families.cuh"
 
@@ -64,6 +66,7 @@ struct LaunchArgs {
   int32_t group_lanes;      // deep_sea bulk path: lanes per bulk store (power of two, 1..32)
   int32_t lazy_fetch;       // persistent launches: 1 = fetch the next chunk only when the current one is issued
   int32_t l2_hint;          // L2 policy of the observation bulk stores: 0 none, 1 evict_first (default), 2 evict_last
+  int32_t final_vec_ok;     // same-step handles: final_obs base and per-step stride are 16-byte aligned
   unsigned long long* work_counter;  // persistent launches: monotonically increasing chunk counter (device)
   unsigned long long work_base;      // value of *work_counter at which this launch's chunk 0 starts
   // Device clock (graph-safe mode, see the kernel): {steps advanced in this mode, chunk counter, finished CTAs}.
@@ -85,7 +88,12 @@ struct LaunchArgs {
   unsigned long long ticket;
   int32_t timing;                    // BSB_HOST_TIMING: leave %globaltimer stamps in the mailbox
   int32_t wait_doorbell;             // 1: pre-launched -- poll the doorbell for `ticket`, then take the buffers from the mailbox
-  unsigned long long doorbell_timeout_ns;
+  // Host steps never deliver final observations, ordinary launches never wait for a doorbell: the two share a word,
+  // so that the kernels' argument layout is that of the next-step kernels.
+  union {
+    unsigned long long doorbell_timeout_ns;   // host steps (a.mailbox set)
+    float* final_obs;       // same-step handles, ordinary launches: [T,B,K] observations of the LAST timesteps
+  };                        // (bsb_outputs.final_observation), or null
   int32_t* bad_action;      // pinned host flag (device alias): set to 1 when an action is outside [0, num_actions)
 };
 
@@ -138,6 +146,16 @@ template <class Family, class O> struct KernelFamily { typedef ObsAs<Family, O> 
 template <class Family> struct KernelFamily<Family, float> { typedef Family type; };
 // log2 of the observation elements per 16-byte vector store.
 template <class O> struct Vec16 { static const int shift = sizeof(O) == 4 ? 2 : sizeof(O) == 2 ? 3 : 4; };
+// Same-step auto-reset (BSB_FLAG_SAME_STEP_RESET): the first template argument of transition_kernel is
+// SameStep<family, O> for every observation type, float32 included, so the next-step kernels above keep theirs.
+template <class Family, class O> struct SameStep {};
+template <class Family, class O> struct FamilyOf<SameStep<Family, O> > { typedef Family type; };
+template <class Family, class O> struct ObsElemOf<SameStep<Family, O> > { typedef O type; };
+template <class F> struct IsSameStep { static const bool value = false; };
+template <class Family, class O> struct IsSameStep<SameStep<Family, O> > { static const bool value = true; };
+// Kernel argument F for observations of type O in either auto-reset mode.
+template <class Family, class O, bool kSameStep> struct KernelTag { typedef typename KernelFamily<Family, O>::type type; };
+template <class Family, class O> struct KernelTag<Family, O, true> { typedef SameStep<Family, O> type; };
 
 // ----- RNG plumbing ---------------------------------------------------------
 template <int RK> struct RngOf;
@@ -213,15 +231,43 @@ BSB_HD void lane_close(const EnvParams& p, int64_t lane, const typename F::Lane&
   if (noise) rng_close(wrng, p, lane, true);
   if (track) ep.store(p, lane);
 }
+// Random draws an observation makes while it is rendered: umbrella_chain's distractors (umbrella_chain.py:60-66),
+// drawn exactly as UmbrellaChain::row draws them.  Every other observation is a function of the lane state.
+template <class F> struct ObsDraws { template <class R> static BSB_HD void skip(const EnvParams&, R&) {} };
+template <> struct ObsDraws<UmbrellaChain> {
+  template <class R> static BSB_HD void skip(const EnvParams& p, R& rng) {
+    for (int k0 = 0; k0 < p.n_distractor; k0 += 64) rng.binomial_half_bits((p.n_distractor - k0) < 64 ? (p.n_distractor - k0) : 64);
+  }
+};
+// Same-step auto-reset: a step that returns LAST runs the family's reset in the same call.  The reference's order of
+// draws for the two calls folded together is kept: the step's, the LAST observation's (skipped here, replayed from
+// `rng` when the final observation is rendered), the reset's, the FIRST observation's.
+template <class F, class R> struct MergedReset {
+  typename F::Lane last;   // the lane at the LAST, before the reset: the final observation is rendered from it
+  R rng;                   // the env stream before the LAST observation's draws
+  bool done;               // this call returned LAST and reset the lane
+};
+
 // One step of an open lane: the transition, the Logging accumulators with their log row, and the four scalar outputs
 // at index `off` of `out` (null outputs are skipped).  `step`: global index of this step.
-template <class F, class R>
+// kSameStep: `merged` receives the lane as it was at a LAST, and the lane is reset in the same call.  The Logging
+// columns episode_len / episode_return restart at the NEXT call, which the marker ep[5] (same-step handles only)
+// announces: the lane's _reset_next_step bit, which next-step handles use, is clear again after a merged reset.
+template <class F, class R, bool kSameStep = false>
 BSB_HD void lane_step(const EnvParams& p, int64_t lane, typename F::Lane& L, R& rng, R& wrng, EpisodeStats& ep,
                       int32_t action, int32_t mode, bool noise, bool track, int64_t step, const MailFields& out,
-                      int64_t off) {
-  const bool after_last = L.nr != 0;
+                      int64_t off, MergedReset<F, R>* merged = nullptr) {
+  bool after_last = L.nr != 0;
   const StepOut o = lane_transition<F, R, R>(p, lane, L, rng, wrng, action, mode, noise);
   if (track) {
+    if constexpr (kSameStep) {
+      double* restart = p.ep + 5 * p.batch + lane;
+      if (*restart != 0.0) {                 // the first call since a merged reset
+        *restart = 0.0;
+        if (o.step_type == FIRST) after_last = true;          // an explicit reset: as after a LAST
+        else { ep.episode_return = 0.0; p.ep[4 * p.batch + lane] = (double)(step - 1); }   // the episode began at the merged call
+      }
+    }
     ep.track(p, lane, o, step, after_last);
     if (p.log_rows && o.step_type == LAST && log_row_due(p, lane)) {      // <= 49 times per 10 000 episodes
       F::store(p, lane, L); ep.store(p, lane);                          // the row reads them from memory
@@ -232,6 +278,17 @@ BSB_HD void lane_step(const EnvParams& p, int64_t lane, typename F::Lane& L, R& 
   if (out.reward_f64) out.reward_f64[off] = o.reward;
   if (out.discount) out.discount[off] = o.discount;
   if (out.step_type) out.step_type[off] = o.step_type;
+  if constexpr (kSameStep) {
+    merged->done = o.step_type == LAST;
+    if (merged->done) {
+      merged->last = L;
+      merged->rng = rng;
+      ObsDraws<F>::skip(p, rng);
+      F::reset(p, lane, L, rng);
+      L.nr = 0;
+      if (track) p.ep[5 * p.batch + lane] = 1.0;
+    }
+  }
 }
 
 // Observation emitter of each family.
@@ -866,6 +923,50 @@ __device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a
   }
 }
 
+// Same-step handles: the final observation of every lane whose step returned LAST, rendered from the lane as it was
+// before the merged reset; the rows of other lanes are left untouched.  Lanes step in lock-step and most episodes
+// have a fixed length, so usually the whole chunk finishes together: then its rows leave through the observation's
+// own emitter (bulk, vector or scalar stores, by the same rules).  Otherwise only the finished lanes' rows are
+// written, each by the whole warp with streaming stores (rows: by the lane's own thread).
+// Rows are the exception to "the same rules": their stages serve bulk and non-bulk emits alike, and a non-bulk emit
+// neither waits for the TMA unit's reads of a stage nor keeps the stage parity in step with the committed groups.
+// Within a chunk every row emit must therefore take the same path; when the final observation's buffer and the
+// observation's (`obs_bulk`: that chunk's decision) would take different ones, the final rows are rendered straight
+// to global memory by their own threads.  Tiles, boards and images only stage their bulk stores, so any mix is safe.
+template <class F, class O, class R>
+__device__ __forceinline__ void emit_final(const EnvParams& p, const LaunchArgs& a, WarpStage<O>& ws, MergedReset<F, R>& m,
+                                           O* fin_t, int64_t warp_base, int n_lanes, int64_t lane, bool active, bool vec,
+                                           bool obs_bulk) {
+  constexpr int kEmit = EmitKind<F>::value;
+  const int tid = threadIdx.x & 31;
+  const int K = p.obs_numel;
+  const unsigned done = __ballot_sync(0xffffffffu, active && m.done);
+  if (done == 0u) return;
+  const bool bulk = chunk_is_bulk<F, O>(p, a, vec, n_lanes);
+  if (done == (n_lanes >= 32 ? 0xffffffffu : ((1u << n_lanes) - 1u)) && (kEmit != EMIT_ROWS || bulk == obs_bulk)) {
+    ws.any_bulk = ws.any_bulk || bulk;
+    emit_obs<F>(p, a, ws, m.last, m.rng, fin_t, warp_base, n_lanes, lane, active, bulk, vec);
+    return;
+  }
+  if (kEmit == EMIT_ROWS) {
+    if (m.done && active) RowRenderer<F, R>::run(p, m.last, m.rng, fin_t + lane * (int64_t)K);
+    return;
+  }
+  const int da = Descriptor<F>::a(m.last), db = Descriptor<F>::b(m.last);
+  for (unsigned rest = done; rest != 0u; rest &= rest - 1u) {
+    const int j = __ffs(rest) - 1;
+    const int a0 = __shfl_sync(0xffffffffu, da, j), b0 = __shfl_sync(0xffffffffu, db, j);
+    O* dst = fin_t + (warp_base + j) * (int64_t)K;
+    if (kEmit == EMIT_IMAGE) {        // mnist's LAST frame is the all-zero tile (mnist.py:74)
+      const float* lut = reinterpret_cast<const float*>(ws.stage);
+      const int8_t* src = p.images + (int64_t)(a0 < 0 ? 0 : a0) * K;
+      for (int e = tid; e < K; e += 32) st_stream(dst + e, obs_cast<O>(a0 >= 0 ? lut[(uint8_t)src[e]] : 0.f));
+    } else {                          // one-hot (b0 = -1) and two-hot boards
+      for (int e = tid; e < K; e += 32) st_stream(dst + e, obs_cast<O>((e == a0 || e == b0) ? 1.f : 0.f));
+    }
+  }
+}
+
 // The warp is done: shared memory must outlive its last bulk read.  `drain`: the stores themselves must have
 // completed (a single-phase host step's `done` tells the host that the observations are in device memory).
 template <class O>
@@ -890,9 +991,10 @@ __device__ __forceinline__ void signal_done(const LaunchArgs& a, unsigned long l
 // single-phase host step.
 template <class F, int RK, bool kNoise, bool kTrack>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kernel(const EnvParams p, const LaunchArgs a) {
-  typedef typename FamilyOf<F>::type Fam;          // F is the family, or ObsAs<family, O> (observations of type O)
-  typedef typename ObsElemOf<F>::type O;
+  typedef typename FamilyOf<F>::type Fam;          // F is the family, ObsAs<family, O> (observations of type O) or
+  typedef typename ObsElemOf<F>::type O;           // SameStep<family, O> (same-step auto-reset)
   typedef typename RngOf<RK>::type R;
+  constexpr bool kSameStep = IsSameStep<F>::value;
   const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
   const int64_t B = p.batch;
   const int K = p.obs_numel;
@@ -939,6 +1041,8 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
     if (active) lane_open<Fam>(p, lane, L, rng, wrng, ep, a.mode, kNoise, kTrack);
     else Fam::init(p, L);
     if (a.mode == MODE_INIT && active) Fam::ctor_draws(p, L, rng);      // the constructor runs no step (T = 0)
+    MergedReset<Fam, R> merged;            // same-step kernels only
+    if constexpr (kSameStep) { Fam::init(p, merged.last); merged.done = false; }
 
     for (int64_t t = 0; t < a.T; ++t) {
       const int64_t off = t * B + lane;
@@ -957,7 +1061,13 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
           }
           if (a.actions_out) a.actions_out[off] = action;
         }
-        lane_step<Fam>(p, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, io, off);
+        if constexpr (kSameStep) lane_step<Fam, R, true>(p, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, io, off, &merged);
+        else lane_step<Fam>(p, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, io, off);
+      }
+      if constexpr (kSameStep) {
+        if (!a.mailbox && a.final_obs)
+          emit_final<Fam>(p, a, ws, merged, reinterpret_cast<O*>(a.final_obs) + t * B * (int64_t)K, warp_base, n_lanes,
+                          lane, active, a.final_vec_ok != 0, bulk);
       }
       emit_obs<Fam>(p, a, ws, L, rng, obs + t * B * (int64_t)K, warp_base, n_lanes, lane, active, bulk, vec);
     }

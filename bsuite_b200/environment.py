@@ -119,12 +119,14 @@ class _Handle:
 class StepBuffers:
   """Caller-owned output tensors for one step (or T fused steps)."""
 
-  def __init__(self, observation, reward, discount, step_type, actions=None):
+  def __init__(self, observation, reward, discount, step_type, actions=None, final_observation=None):
     self.observation = observation
     self.reward = reward
     self.discount = discount
     self.step_type = step_type
     self.actions = actions
+    # same-step environments: the observation each LAST lane showed before its merged reset (other rows untouched)
+    self.final_observation = final_observation
     self._outputs = None      # struct bsb_outputs over these tensors, built once (the tensors are never swapped)
     self._bound = None        # observation dtype the struct was last checked against (bind)
     self._timestep = None
@@ -140,9 +142,11 @@ class StepBuffers:
     `out._outputs if out._bound is dtype else out.bind(dtype)`, so buffers passed to environments of another dtype
     are checked again (a kernel would otherwise write past a narrower observation)."""
     if self._bound is not obs_dtype:
-      if self.observation is not None and self.observation.dtype != obs_dtype:
-        raise ValueError(f'out.observation is {self.observation.dtype}, but this environment writes {obs_dtype} '
-                         'observations (obs_dtype)')
+      for name in ('observation', 'final_observation'):
+        tensor = getattr(self, name)
+        if tensor is not None and tensor.dtype != obs_dtype:
+          raise ValueError(f'out.{name} is {tensor.dtype}, but this environment writes {obs_dtype} '
+                           'observations (obs_dtype)')
       self._bound = obs_dtype
     return self.as_outputs()
 
@@ -160,6 +164,8 @@ class StepBuffers:
       out.discount = self.discount.data_ptr()
     if self.step_type is not None:
       out.step_type = self.step_type.data_ptr()
+    if self.final_observation is not None:
+      out.final_observation = self.final_observation.data_ptr()
     return out
 
   def timestep(self) -> 'dm_env.TimeStep':
@@ -194,11 +200,20 @@ class BatchedEnvironment:
   `obs_dtype` ('float32', 'bfloat16' or 'uint8', or the torch dtype; fixed for the life of the environment) is the
   element type of the observations the kernels write: exactly the float32 observation `.to(obs_dtype)`, without a
   second pass over it.  'uint8' is available for deep_sea and catch (0 / 1 cells); reduced dtypes need
-  rng='philox'.  Rewards, discounts, step types, info, episode statistics and `state_dict()` do not depend on it."""
+  rng='philox'.  Rewards, discounts, step types, info, episode statistics and `state_dict()` do not depend on it.
+
+  `autoreset` (fixed for the life of the environment): 'next_step' (default) is the reference's dm_env convention,
+  where the call after a LAST timestep ignores its action and returns FIRST.  'same_step' (rng='philox') resets a
+  lane in the call that ends its episode, as EnvPool, Brax, gymnax and gymnasium's SAME_STEP mode do: that call
+  returns LAST with the transition's reward and discount and the NEXT episode's first observation, and every later
+  call is a transition.  The observation that came with the LAST goes to `final_observation` of buffers made with
+  `make_buffers(..., final_observation=True)`.  Per lane, the outputs are the reference's own trace with each LAST
+  merged into the reset that follows it (same random draws, same order), and info, episode statistics and log rows
+  are the reference's on that trace."""
 
   def __init__(self, spec: EnvSpec, batch: int, device='cuda', seed: Optional[int] = None,
                rng: str = 'philox', lane_offset: int = 0, track_episodes: bool = False,
-               reward_dtype='float32', record_rows: bool = False, obs_dtype='float32'):
+               reward_dtype='float32', record_rows: bool = False, obs_dtype='float32', autoreset: str = 'next_step'):
     import torch
     self._torch = torch
     self._spec = spec
@@ -219,7 +234,12 @@ class BatchedEnvironment:
     # record_rows: every lane keeps the rows the reference's Logging wrapper would have written for it, at the
     # log-spaced episode counts of utils/wrappers.py:140-147 (recording.write_lane_csvs turns them into files)
     track_episodes = bool(track_episodes or record_rows)
+    if autoreset not in ('next_step', 'same_step'):
+      raise ValueError(f"autoreset must be 'next_step' or 'same_step', got {autoreset!r}")
+    self._autoreset = autoreset
     flags = _lib.FLAG_TRACK_EPISODES if track_episodes else 0
+    if autoreset == 'same_step':
+      flags |= _lib.FLAG_SAME_STEP_RESET
     self._track = bool(track_episodes)
     self._log_schedule = None
     if record_rows:
@@ -245,6 +265,7 @@ class BatchedEnvironment:
   num_actions = property(lambda self: self._spec.num_actions)
   info_names = property(lambda self: self._info_names)
   obs_dtype = property(lambda self: self._obs_dtype)      # torch dtype of the observation tensors
+  autoreset = property(lambda self: self._autoreset)      # 'next_step' or 'same_step'
 
   def observation_spec(self):
     """Per-lane spec, identical to the reference environment's (float32 values).  The observation tensors this
@@ -259,16 +280,24 @@ class BatchedEnvironment:
     return specs.DiscreteArray(self._spec.num_actions, dtype=self._spec.action_dtype, name='action')
 
   # ---- buffers -------------------------------------------------------------
-  def make_buffers(self, num_steps: Optional[int] = None, with_actions: bool = False) -> StepBuffers:
+  def make_buffers(self, num_steps: Optional[int] = None, with_actions: bool = False,
+                   final_observation: bool = False) -> StepBuffers:
+    """Output tensors for `step` / `reset` (num_steps None) or `rollout`.  `final_observation` (same-step
+    environments): also a tensor shaped like `observation` for the observations of LAST timesteps; rows of lanes
+    that did not finish keep whatever they held (it starts zeroed)."""
     torch = self._torch
+    if final_observation and self._autoreset != 'same_step':
+      raise ValueError("final_observation needs autoreset='same_step'")
     lead = (self._batch,) if num_steps is None else (int(num_steps), self._batch)
     kw = dict(device=self._device)
+    obs_shape = lead + tuple(self._spec.obs_shape)
     return StepBuffers(
-        observation=torch.empty(lead + tuple(self._spec.obs_shape), dtype=self._obs_dtype, **kw),
+        observation=torch.empty(obs_shape, dtype=self._obs_dtype, **kw),
         reward=torch.empty(lead, dtype=self._reward_dtype, **kw),
         discount=torch.empty(lead, dtype=torch.float32, **kw),
         step_type=torch.empty(lead, dtype=torch.int32, **kw),
-        actions=torch.empty(lead, dtype=torch.int32, **kw) if with_actions else None)
+        actions=torch.empty(lead, dtype=torch.int32, **kw) if with_actions else None,
+        final_observation=torch.zeros(obs_shape, dtype=self._obs_dtype, **kw) if final_observation else None)
 
   def _stream(self):
     if self._ordinal < 0:
@@ -380,6 +409,8 @@ class BatchedEnvironment:
       actions = actions.contiguous()
     if out is None:
       out = self.make_buffers()
+    if host.final_observation is not None:
+      raise ValueError('step_host does not deliver final observations')
     houts = host._outputs if host._bound is self._obs_dtype else host.bind(self._obs_dtype)   # built once
     if out._bound is not self._obs_dtype:
       out.bind(self._obs_dtype)          # the device observation's dtype
@@ -443,20 +474,22 @@ class BatchedEnvironment:
     return out.timestep()
 
   def capture(self, num_steps: int = 1, sample_actions: bool = False, fused: bool = False,
-              action_seed: int = 0) -> GraphedSteps:
+              action_seed: int = 0, final_observation: bool = False) -> GraphedSteps:
     """Records `num_steps` steps into a CUDA graph: one launch per step (`fused=False`, the reference's call
     pattern, baselines/experiment.py:45-57) or one fused rollout launch.  Launch arguments are frozen in a graph,
     so the library moves this handle's step counter and chunk scheduler to device memory when it sees the capture
     (include/bsuite_b200.h, "CUDA graphs").  One eager pass is made first on a snapshot of the lane state (module
-    loading and function attributes must not happen inside a capture); the state is restored before recording."""
+    loading and function attributes must not happen inside a capture); the state is restored before recording.
+    `final_observation` (same-step environments): the buffers also receive the final observations."""
     torch = self._torch
     if self._ordinal < 0:
       raise RuntimeError('CUDA graphs need a CUDA environment')
     T = int(num_steps)
-    buffers = self.make_buffers(T, with_actions=sample_actions)
+    buffers = self.make_buffers(T, with_actions=sample_actions, final_observation=final_observation)
     actions = None if sample_actions else torch.zeros((T, self._batch), dtype=torch.int32, device=self._device)
     slices = [StepBuffers(buffers.observation[t:t + 1], buffers.reward[t:t + 1], buffers.discount[t:t + 1],
-                          buffers.step_type[t:t + 1], None if buffers.actions is None else buffers.actions[t:t + 1])
+                          buffers.step_type[t:t + 1], None if buffers.actions is None else buffers.actions[t:t + 1],
+                          None if buffers.final_observation is None else buffers.final_observation[t:t + 1])
               for t in range(T)]
 
     def record():
@@ -569,6 +602,8 @@ class BatchedEnvironment:
     h = hashlib.sha256()
     h.update(repr((sorted(self._spec.fields.items()), self._spec.wrapper, self._rng_kind, self._track,
                    tuple(self._spec.obs_shape), self._spec.num_actions)).encode())
+    if self._autoreset != 'next_step':      # only then: snapshots taken before the mode existed still load
+      h.update(repr(('autoreset', self._autoreset)).encode())
     for table in (self._spec.table, self._spec.table2):
       if table is not None:
         h.update(np.ascontiguousarray(table).tobytes())

@@ -26,6 +26,9 @@ def _instantiate(spec, batch, device, seed, rng, **engine_kwargs):
     if 'obs_dtype' in engine_kwargs:
       raise ValueError('obs_dtype applies to batched environments only (pass batch=...); the B = 1 face writes float32 '
                        'numpy observations like the reference')
+    if 'autoreset' in engine_kwargs:
+      raise ValueError('autoreset applies to batched environments only (pass batch=...); the B = 1 face keeps the '
+                       "reference's dm_env convention (a LAST timestep is followed by a FIRST one)")
     if engine_kwargs:
       raise TypeError(f'{sorted(engine_kwargs)} only apply to batched environments (pass batch=...)')
     return DmEnvAdapter(spec, device=device, seed=seed, rng=rng)

@@ -27,19 +27,23 @@ class Trajectory(NamedTuple):
   step_types: Any     # [T, B] int32
 
 
-def collect(environment, num_steps: int, action_seed: int = 0, last_observation=None) -> Trajectory:
+def collect(environment, num_steps: int, action_seed: int = 0, last_observation=None, final_observations: bool = False):
   """One fused rollout of `num_steps` steps with on-device random actions, returned in Trajectory layout.
 
   `last_observation` [B, ...] is the observation the lanes showed before this call (the previous trajectory's
   `observations[-1]`); on a fresh environment it is not needed: the first call of every lane returns FIRST.
+  `final_observations` (autoreset='same_step'): returns `(Trajectory, finals)`, where `finals[t]` [T, B, ...] holds
+  the observation of every lane whose `step_types[t]` is LAST (`observations[t + 1]` is then the next episode's
+  first observation); pass `finals` to `Replay.add_transitions`.
   """
   import torch
-  out = environment.make_buffers(num_steps, with_actions=True)
+  out = environment.make_buffers(num_steps, with_actions=True, final_observation=final_observations)
   ts = environment.rollout(num_steps, action_seed=action_seed, out=out)
   if last_observation is None:
     last_observation = torch.zeros_like(ts.observation[0])
   observations = torch.cat([last_observation.unsqueeze(0), ts.observation], dim=0)
-  return Trajectory(observations, out.actions, ts.reward, ts.discount, ts.step_type)
+  trajectory = Trajectory(observations, out.actions, ts.reward, ts.discount, ts.step_type)
+  return (trajectory, out.final_observation) if final_observations else trajectory
 
 
 class RandomAgent:
@@ -118,11 +122,17 @@ class Replay:
       slot[slots] = item.to(slot.dtype)
     self._num_added += n
 
-  def add_transitions(self, trajectory: Trajectory) -> int:
-    """Adds every real transition of a `Trajectory` as `(o_tm1, a_tm1, r_t, d_t, o_t)`; returns how many."""
+  def add_transitions(self, trajectory: Trajectory, final_observations=None) -> int:
+    """Adds every real transition of a `Trajectory` as `(o_tm1, a_tm1, r_t, d_t, o_t)`; returns how many.
+
+    `final_observations` [T, B, ...] (same-step environments, `collect(..., final_observations=True)`): `o_t` of a
+    LAST transition is the final observation, not the next episode's first one that `observations` holds."""
     keep = (trajectory.step_types != 0).reshape(-1)
     flat = lambda x: x.reshape((-1,) + tuple(x.shape[2:]))[keep]
     o_tm1, o_t = trajectory.observations[:-1], trajectory.observations[1:]
+    if final_observations is not None:
+      last = (trajectory.step_types == 2).reshape(trajectory.step_types.shape + (1,) * (o_t.dim() - 2))
+      o_t = self._torch.where(last, final_observations.to(o_t.dtype), o_t)
     self.add_batch([flat(o_tm1), flat(trajectory.actions), flat(trajectory.rewards), flat(trajectory.discounts), flat(o_t)])
     return int(keep.sum())
 

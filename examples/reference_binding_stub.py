@@ -33,7 +33,8 @@ class Config(ctypes.Structure):           # struct bsb_config, field for field (
 
 
 class Outputs(ctypes.Structure):          # struct bsb_outputs
-  _fields_ = [(name, ctypes.c_void_p) for name in ('observation', 'reward', 'reward_f64', 'discount', 'step_type')]
+  _fields_ = [(name, ctypes.c_void_p)
+              for name in ('observation', 'reward', 'reward_f64', 'discount', 'step_type', 'final_observation')]
 
 
 _lib = ctypes.CDLL(LIBRARY)

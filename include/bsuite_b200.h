@@ -23,7 +23,8 @@
  *   - the library owns only lane state, RNG counters and config tables.
  *   - calls on one handle are not thread-safe; distinct handles are independent.
  *   - a lane whose previous timestep was LAST ignores its action and emits
- *     FIRST (base.py:59-65).  FIRST lanes carry reward = 0, discount = 0; the
+ *     FIRST (base.py:59-65), unless the handle was created with
+ *     BSB_FLAG_SAME_STEP_RESET (see there).  FIRST lanes carry reward = 0, discount = 0; the
  *     reference's `None` is recovered from step_type == BSB_FIRST.
  */
 #ifndef BSUITE_B200_H_
@@ -35,7 +36,7 @@
 extern "C" {
 #endif
 
-#define BSB_ABI_VERSION 8
+#define BSB_ABI_VERSION 9
 #define BSB_DEVICE_HOST (-1)
 #define BSB_MAX_INFO 4
 
@@ -163,6 +164,25 @@ typedef struct bsb_config {
 /* bsb_config.flags */
 #define BSB_FLAG_TRACK_EPISODES 1u /* keep the Logging-wrapper accumulators
                                       (wrappers.py:85-110) per lane on device */
+/*
+ * Same-step auto-reset, fixed at bsb_create (needs BSB_RNG_PHILOX; MT19937
+ * returns BSB_UNSUPPORTED).  A lane whose step returns LAST runs reset() in
+ * the SAME call: that call returns LAST with the transition's reward and
+ * discount, but its observation is the next episode's FIRST observation, and
+ * the lane's next call is an ordinary step.  FIRST is then only returned by
+ * the first call of a fresh handle and by bsb_reset.  Per lane this is the
+ * reference's own call sequence with every LAST merged into the reset call
+ * that follows it: the random draws happen in the reference's order (the
+ * step's, the LAST observation's, the reset's, the FIRST observation's), so
+ * every value the reference produces appears exactly once.  The observation
+ * the reference returned with the LAST goes to bsb_outputs.final_observation
+ * when that is given.  Log rows, bsuite_info() and the Logging columns equal
+ * the reference's on that folded trace (episode_len / episode_return keep the
+ * finished episode's values until the lane steps again).  The snapshot of a
+ * same-step handle that tracks episodes holds one more float64 [B] block.
+ * Without the flag, behaviour is exactly the default next-step convention.
+ */
+#define BSB_FLAG_SAME_STEP_RESET 2u
 
 /*
  * Caller-allocated outputs of one lock-step transition.  For bsb_rollout each
@@ -178,6 +198,13 @@ typedef struct bsb_config {
  *   reward_f64  : float64 [B]   (the reference's double-precision reward)
  *   discount    : float32 [B]   1 (MID) / 0 (LAST) / 0 (FIRST = None)
  *   step_type   : int32   [B]   bsb_step_type
+ *   final_observation : [B, obs_numel] in the handle's obs_dtype, or NULL.
+ *                 Same-step handles only (BSB_FLAG_SAME_STEP_RESET; non-NULL
+ *                 on another handle returns BSB_INVALID_ARGUMENT): the row of
+ *                 each lane whose step_type is LAST receives the observation
+ *                 the reference returned with that LAST timestep; the rows of
+ *                 other lanes are left untouched.  Not through bsb_step_host
+ *                 (BSB_UNSUPPORTED).
  */
 typedef struct bsb_outputs {
   float* observation;
@@ -185,6 +212,7 @@ typedef struct bsb_outputs {
   double* reward_f64;
   float* discount;
   int32_t* step_type;
+  float* final_observation;
 } bsb_outputs;
 
 typedef struct bsb_env bsb_env; /* opaque handle */
@@ -341,6 +369,8 @@ int32_t bsb_set_state(bsb_env* env, const void* src_host, int64_t nbytes,
  *       afterwards sees complete observations; without it, order a consumer by
  *       the next call on this handle (every entry point waits for the step) or
  *       set BSB_HOST_EARLY=0 to make the call wait for the whole kernel.
+ *       Same-step handles (BSB_FLAG_SAME_STEP_RESET) always run host steps in
+ *       one phase.
  *   BSB_HOST_PRELAUNCH  (pinned buffers only) after ringing this step, the NEXT
  *       step's kernel is enqueued at once; it becomes resident as this one drains
  *       and polls the mailbox doorbell, so the next call costs neither a launch
