@@ -5,6 +5,7 @@ Public surface (mirrors `bsuite/__init__.py:18-24` and `bsuite/bsuite.py`):
   load_from_id(bsuite_id)                      -> B = 1 dm_env.Environment (drop-in)
   load_from_id(bsuite_id, batch=B, device=...) -> BatchedEnvironment (torch tensors)
   load(experiment_name, kwargs, ...)           -> same, from explicit kwargs
+  load_experiment(experiment_name, L, ...)     -> every setting of an experiment in one BatchedEnvironment
   make(environment_class, batch=..., **kwargs) -> construct a raw environment class
   sweep                                        -> SETTINGS / SWEEP / TAGS / TESTING / EPISODES
   EXPERIMENT_NAME_TO_ENVIRONMENT               -> experiment name -> loader
@@ -29,6 +30,7 @@ from bsuite_b200.registry import (  # noqa: E402,F401
     load_and_record,
     load_and_record_to_csv,
     load_and_record_to_terminal,
+    load_experiment,
     load_from_id,
     make,
     unpack_bsuite_id,

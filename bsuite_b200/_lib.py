@@ -13,9 +13,10 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BSB_LIBRARY points the binding at another build of the SAME library (tools/host_sanitize.sh: ASan/UBSan build)
 LIB_PATH = os.environ.get('BSB_LIBRARY') or os.path.join(_HERE, 'libbsuite_b200.so')
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 DEVICE_HOST = -1
 MAX_INFO = 4
+MAX_PACKED_SETTINGS = 64      # bsb_create_packed: settings per handle
 COMM_ID_BYTES = 128
 
 # enum bsb_family
@@ -84,6 +85,10 @@ EXPORTS = {
     'bsb_last_error': (ctypes.c_char_p, []),
     'bsb_create': (ctypes.c_int32, [ctypes.POINTER(Config), ctypes.c_int64, ctypes.c_int32, ctypes.c_uint64,
                                     ctypes.c_uint64, ctypes.POINTER(ctypes.c_void_p)]),
+    'bsb_create_packed': (ctypes.c_int32, [ctypes.POINTER(Config), ctypes.c_int32, ctypes.c_int64, ctypes.c_int32,
+                                           ctypes.POINTER(ctypes.c_uint64), ctypes.c_uint64,
+                                           ctypes.POINTER(ctypes.c_void_p)]),
+    'bsb_packed_layout': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int64)]),
     'bsb_destroy': (ctypes.c_int32, [ctypes.c_void_p]),
     'bsb_obs_numel': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64)]),
     'bsb_obs_shape': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32)]),

@@ -36,8 +36,9 @@ template <> struct HostEmit<Mnist> {
 
 // Observations of type O other than float32: each lane's float32 observation is rendered into `f32` and converted
 // element by element with obs_cast, the function the kernels use.  kSameStep: a lane whose step returned LAST is reset
-// in the same call, and its final observation goes to a.final_obs when that is given.
-template <class F, int RK, class O, bool kSameStep = false>
+// in the same call, and its final observation goes to a.final_obs when that is given.  kPacked: every lane runs with
+// its setting's parameters (pack_lane_params), as the packed kernels do.
+template <class F, int RK, class O, bool kSameStep = false, bool kPacked = false>
 void host_run(const EnvParams& p, const LaunchArgs& a) {
   typedef typename RngOf<RK>::type R;
   const int64_t B = p.batch;
@@ -48,22 +49,25 @@ void host_run(const EnvParams& p, const LaunchArgs& a) {
   const bool noise = p.wrapper == BSB_WRAP_REWARD_NOISE && a.mode != MODE_INIT;
   const bool track = p.ep != nullptr && a.mode != MODE_INIT;
   const MailFields out = {a.actions, a.obs, a.reward, a.reward_f64, a.discount, a.step_type, 0, 0};
-  auto render = [&](const typename F::Lane& L, R& rng, O* dst) {
+  EnvParams setting_p;                    // packed handles: p with the current lane's setting
+  auto render = [&](const EnvParams& lp, const typename F::Lane& L, R& rng, O* dst) {
     if constexpr (std::is_same<O, float>::value) {
-      HostEmit<F>::run(p, L, rng, dst);
+      HostEmit<F>::run(lp, L, rng, dst);
     } else {
-      HostEmit<F>::run(p, L, rng, f32.data());
+      HostEmit<F>::run(lp, L, rng, f32.data());
       for (int e = 0; e < K; ++e) dst[e] = obs_cast<O>(f32[(size_t)e]);
     }
   };
   for (int64_t lane = 0; lane < B; ++lane) {
+    if constexpr (kPacked) { setting_p = p; pack_lane_params(setting_p, lane); }
+    const EnvParams& lp = kPacked ? setting_p : p;
     typename F::Lane L;
     R rng, wrng;
     EpisodeStats ep;
     ActionStream action_stream;
     action_stream.open();
-    lane_open<F>(p, lane, L, rng, wrng, ep, a.mode, noise, track);
-    if (a.mode == MODE_INIT) F::ctor_draws(p, L, rng);
+    lane_open<F>(lp, lane, L, rng, wrng, ep, a.mode, noise, track);
+    if (a.mode == MODE_INIT) F::ctor_draws(lp, L, rng);
     MergedReset<F, R> merged;
     F::init(p, merged.last);
     merged.done = false;
@@ -72,14 +76,14 @@ void host_run(const EnvParams& p, const LaunchArgs& a) {
       int32_t action = 0;
       if (a.mode == MODE_STEP) {
         action = a.actions ? a.actions[off]
-                           : action_stream.sample(a.action_seed, p.lane_offset + (uint64_t)lane, (uint64_t)(a.step0 + t), p.num_actions);
+                           : action_stream.sample(a.action_seed, lp.lane_offset + (uint64_t)lane, (uint64_t)(a.step0 + t), p.num_actions);
         if (a.actions_out) a.actions_out[off] = action;
       }
-      lane_step<F, R, kSameStep>(p, lane, L, rng, wrng, ep, action, a.mode, noise, track, a.step0 + t, out, off, &merged);
-      if constexpr (kSameStep) { if (merged.done && fin) render(merged.last, merged.rng, fin + off * (int64_t)K); }
-      render(L, rng, obs + off * (int64_t)K);
+      lane_step<F, R, kSameStep>(lp, lane, L, rng, wrng, ep, action, a.mode, noise, track, a.step0 + t, out, off, &merged);
+      if constexpr (kSameStep) { if (merged.done && fin) render(lp, merged.last, merged.rng, fin + off * (int64_t)K); }
+      render(lp, L, rng, obs + off * (int64_t)K);
     }
-    lane_close<F>(p, lane, L, rng, wrng, ep, noise, track);
+    lane_close<F>(lp, lane, L, rng, wrng, ep, noise, track);
   }
 }
 
@@ -321,9 +325,29 @@ BSB_SAME_STEP(DeepSea) BSB_SAME_STEP(Catch) BSB_SAME_STEP(Cartpole) BSB_SAME_STE
 BSB_SAME_STEP(MemoryChain) BSB_SAME_STEP(Bandit) BSB_SAME_STEP(UmbrellaChain) BSB_SAME_STEP(DiscountingChain) BSB_SAME_STEP(Mnist)
 #undef BSB_SAME_STEP
 
+// Packed handles (bsb_create_packed): float32, next-step auto-reset, Philox, every family but deep_sea (whose
+// settings differ in observation shape).  Instantiated in translation units of their own (pk_<family>.cu): an
+// ordinary handle never loads their modules.  Host steps take the single-phase kernel.
+template <class F> struct Packable { static const bool value = !std::is_same<F, DeepSea>::value; };
+template <class F>
+int run_packed(bsb_env* e, const LaunchArgs& a, cudaStream_t stream) {
+  if (e->device < 0) { host_run<F, 0, float, false, true>(e->p, a); return BSB_OK; }
+  return with_flags(e, a, [&](auto noise, auto track) {
+    LaunchArgs la = a;
+    Geometry g;
+    const int rc = plan_launch<F, float>(e, la, g);
+    return rc != BSB_OK ? rc : launch(e, la, g, stream, transition_kernel<Packed<F>, 0, decltype(noise)::value, decltype(track)::value>, e->p, la);
+  });
+}
+#define BSB_PACKED(F) extern template int run_packed<F>(bsb_env*, const LaunchArgs&, cudaStream_t);
+BSB_PACKED(Catch) BSB_PACKED(Cartpole) BSB_PACKED(CartpoleSwingup) BSB_PACKED(MountainCar) BSB_PACKED(MemoryChain)
+BSB_PACKED(Bandit) BSB_PACKED(UmbrellaChain) BSB_PACKED(DiscountingChain) BSB_PACKED(Mnist)
+#undef BSB_PACKED
+
 // Kernels and host path of the handle's auto-reset mode and observation dtype.
 template <class F>
 int run_family(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr) {
+  if constexpr (Packable<F>::value) { if (e->packed) return run_packed<F>(e, a, stream); }
   if (e->same_step) return run_same_step<F>(e, a, stream);
   if (e->obs_dtype != BSB_OBS_FLOAT32) return run_reduced<F>(e, a, stream, two_phase);
   return run_family_as<F, float>(e, a, stream, two_phase);

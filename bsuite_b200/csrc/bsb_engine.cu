@@ -234,9 +234,9 @@ int mailbox_open(bsb_env* e) {
 // lane out, 4 B in): deep_sea from N = 16 up (>= 1 KB of observation per lane).  catch (200 B per lane) is bound
 // by the 2 MB of scalars per step either way and keeps the single-phase kernel.  The rule counts float32 bytes
 // whatever the handle's obs_dtype, so a reduced-dtype handle takes the same path as its float32 twin.
-// Same-step handles always take the single-phase kernel.
+// Same-step and packed handles always take the single-phase kernel.
 bool family_obs_from_state(const bsb_env* e) {
-  return !e->same_step && (e->p.family == BSB_DEEP_SEA || e->p.family == BSB_CATCH) && (size_t)e->p.obs_numel * sizeof(float) >= 1024;
+  return !e->same_step && !e->packed && (e->p.family == BSB_DEEP_SEA || e->p.family == BSB_CATCH) && (size_t)e->p.obs_numel * sizeof(float) >= 1024;
 }
 
 int mailbox_launch(bsb_env* e, unsigned long long ticket, int64_t step0, const MailFields* fields, bool wait_doorbell, bool split = false) {
@@ -418,7 +418,11 @@ int32_t bsb_abi_version(void) { return BSB_ABI_VERSION; }
 const char* bsb_last_error(void) { return bsb::last_error_cstr(); }
 int64_t bsb_launch_count(void) { return g_launches.load(); }
 
-int32_t bsb_create(const bsb_config* config, int64_t batch, int32_t device, uint64_t seed, uint64_t lane_offset, bsb_env** out) {
+// bsb_create, and bsb_create_packed with `n_settings` > 0 (`config` is then configs[0], the validated settings are
+// `configs` with their `seeds`; `batch` = n_settings * lanes_per_setting).
+static int32_t create_env(const bsb_config* config, int64_t batch, int32_t device, uint64_t seed, uint64_t lane_offset,
+                          bsb_env** out, const bsb_config* configs = nullptr, const uint64_t* seeds = nullptr,
+                          int32_t n_settings = 0) {
   if (!config || !out) return fail(BSB_INVALID_ARGUMENT, "null argument");
   *out = nullptr;
   const bsb_config& c = *config;
@@ -440,7 +444,10 @@ int32_t bsb_create(const bsb_config* config, int64_t batch, int32_t device, uint
   memset(&e->p, 0, sizeof(e->p));
   e->device = device; e->steps_done = 0;
   e->obs_dtype = c.obs_dtype; e->obs_elem_bytes = c.obs_dtype == BSB_OBS_BFLOAT16 ? 2 : c.obs_dtype == BSB_OBS_UINT8 ? 1 : 4;
-  e->same_step = (c.flags & BSB_FLAG_SAME_STEP_RESET) != 0; e->graph_safe = false; e->clock = nullptr; e->sum_scratch = nullptr; e->names = info_names(c.family);
+  e->same_step = (c.flags & BSB_FLAG_SAME_STEP_RESET) != 0;
+  e->packed = n_settings > 0; e->n_settings = n_settings > 0 ? n_settings : 1;
+  e->lanes_per_setting = n_settings > 0 ? batch / n_settings : batch;
+  e->graph_safe = false; e->clock = nullptr; e->sum_scratch = nullptr; e->names = info_names(c.family);
   {  // tuning knobs (environment variables, read once per handle)
     auto flag = [](const char* name, int dflt) { const char* v = getenv(name); return v ? (atoi(v) != 0 ? 1 : 0) : dflt; };
     const char* bt = getenv("BSB_BLOCK_THREADS");
@@ -512,9 +519,12 @@ int32_t bsb_create(const bsb_config* config, int64_t batch, int32_t device, uint
     BSB_TRY(env_upload(e, d, bits.data(), bits.size() * 4));
     p.mapping_bits = d;
   } else if (c.family == BSB_BANDIT || c.family == BSB_DISCOUNTING_CHAIN) {
+    // a packed handle stacks its settings' tables (all of one size), setting k at k * table_bytes / 8
+    const size_t tables = e->packed ? (size_t)n_settings : 1;
     double* d = nullptr;
-    BSB_TRY(env_alloc_t(e, &d, (size_t)c.table_bytes / 8, false));
-    BSB_TRY(env_upload(e, d, c.table, (size_t)c.table_bytes));
+    BSB_TRY(env_alloc_t(e, &d, tables * (size_t)c.table_bytes / 8, false));
+    for (size_t k = 0; k < tables; ++k)
+      BSB_TRY(env_upload(e, d + k * (size_t)c.table_bytes / 8, e->packed ? configs[k].table : c.table, (size_t)c.table_bytes));
     p.reward_table = d;
   } else if (c.family == BSB_MNIST) {
     int8_t* d = nullptr; uint8_t* l = nullptr;
@@ -578,6 +588,24 @@ int32_t bsb_create(const bsb_config* config, int64_t batch, int32_t device, uint
       BSB_TRY(env_alloc_t(e, &p.wmt_idx, B, true)); BSB_TRY(env_upload(e, p.wmt_idx, idx.data(), B * 4));
     }
   }
+  if (e->packed) {      // the per-setting values every lane of a packed handle picks up (pack_lane_params)
+    std::vector<char> blob(sizeof(PackTable) + (size_t)n_settings * sizeof(PackSetting));
+    PackTable* t = reinterpret_cast<PackTable*>(blob.data());
+    t->lanes_per_setting = e->lanes_per_setting; t->n_settings = n_settings;
+    PackSetting* s = reinterpret_cast<PackSetting*>(t + 1);
+    for (int32_t k = 0; k < n_settings; ++k) {
+      const bsb_config& ck = configs[k];
+      s[k].seed = seeds[k];
+      s[k].table_offset = p.reward_table ? (int64_t)k * (c.table_bytes / 8) : 0;
+      s[k].height_threshold = ck.height_threshold; s[k].x_reward_threshold = ck.x_reward_threshold;
+      s[k].noise_scale = ck.noise_scale; s[k].reward_scale = ck.reward_scale;
+      s[k].memory_length = ck.memory_length; s[k].chain_length = ck.chain_length;
+    }
+    void* d = nullptr;
+    BSB_TRY(env_alloc(e, &d, blob.size(), false));
+    BSB_TRY(env_upload(e, d, blob.data(), blob.size()));
+    p.pack = static_cast<const PackTable*>(d);
+  }
   // constructor: _reset_next_step = True and the constructor's RNG draws
   LaunchArgs a = make_args(e, nullptr, nullptr, 0, MODE_INIT);
   BSB_TRY(run(e, a, nullptr));
@@ -587,6 +615,63 @@ int32_t bsb_create(const bsb_config* config, int64_t batch, int32_t device, uint
   }
 #undef BSB_TRY
   *out = e;
+  return BSB_OK;
+}
+
+int32_t bsb_create(const bsb_config* config, int64_t batch, int32_t device, uint64_t seed, uint64_t lane_offset, bsb_env** out) {
+  return create_env(config, batch, device, seed, lane_offset, out);
+}
+
+// The first field in which two settings of a packed handle differ although they may not (nullptr: none).  Allowed
+// to differ: the seed (seeds[]), the contents of `table` (bandit / discounting_chain reward tables), memory_length,
+// chain_length, height_threshold, x_reward_threshold, noise_scale, reward_scale.
+static const char* packed_mismatch(const bsb_config& a, const bsb_config& b) {
+#define BSB_SAME(field) if (memcmp(&a.field, &b.field, sizeof(a.field)) != 0) return #field;
+  BSB_SAME(family) BSB_SAME(wrapper) BSB_SAME(rng_kind) BSB_SAME(flags) BSB_SAME(size) BSB_SAME(deterministic)
+  BSB_SAME(rows) BSB_SAME(columns) BSB_SAME(num_bits) BSB_SAME(n_distractor) BSB_SAME(num_actions) BSB_SAME(max_steps)
+  BSB_SAME(num_data) BSB_SAME(image_rows) BSB_SAME(image_cols) BSB_SAME(obs_dtype) BSB_SAME(unscaled_move_cost)
+  BSB_SAME(x_threshold) BSB_SAME(timescale) BSB_SAME(max_time) BSB_SAME(init_range) BSB_SAME(theta_dot_threshold)
+  BSB_SAME(move_cost) BSB_SAME(table_bytes) BSB_SAME(table2_bytes) BSB_SAME(log_schedule_len)
+#undef BSB_SAME
+  if (a.family == BSB_MNIST && a.table_bytes == b.table_bytes && a.table != b.table &&
+      (!a.table || !b.table || memcmp(a.table, b.table, (size_t)a.table_bytes) != 0)) return "table";
+  if (a.table2_bytes == b.table2_bytes && a.table2 != b.table2 &&
+      (!a.table2 || !b.table2 || memcmp(a.table2, b.table2, (size_t)a.table2_bytes) != 0)) return "table2";
+  if (a.log_schedule_len == b.log_schedule_len && a.log_schedule != b.log_schedule && a.log_schedule_len > 0 &&
+      (!a.log_schedule || !b.log_schedule ||
+       memcmp(a.log_schedule, b.log_schedule, (size_t)a.log_schedule_len * sizeof(int64_t)) != 0)) return "log_schedule";
+  return nullptr;
+}
+
+int32_t bsb_create_packed(const bsb_config* configs, int32_t n_settings, int64_t lanes_per_setting, int32_t device,
+                          const uint64_t* seeds, uint64_t lane_offset, bsb_env** out) {
+  if (!configs || !seeds || !out) return fail(BSB_INVALID_ARGUMENT, "null argument");
+  *out = nullptr;
+  if (n_settings < 1 || n_settings > BSB_MAX_PACKED_SETTINGS)
+    return fail(BSB_INVALID_ARGUMENT, "n_settings must be in [1, " + std::to_string(BSB_MAX_PACKED_SETTINGS) + "]");
+  if (lanes_per_setting < 1 || lanes_per_setting > INT64_MAX / n_settings)
+    return fail(BSB_INVALID_ARGUMENT, "lanes_per_setting must be positive (and n_settings * lanes_per_setting an int64)");
+  for (int32_t k = 0; k < n_settings; ++k) {
+    int rows = 0, cols = 0, n_actions = 0;
+    const int rc = validate(configs[k], lanes_per_setting, &rows, &cols, &n_actions);
+    if (rc != BSB_OK) return fail(rc, "setting " + std::to_string(k) + ": " + last_error_cstr());
+  }
+  const bsb_config& c = configs[0];
+  if (c.family == BSB_DEEP_SEA) return fail(BSB_UNSUPPORTED, "deep_sea has no packed kernel (its settings differ in size)");
+  if (c.rng_kind == BSB_RNG_MT19937) return fail(BSB_UNSUPPORTED, "packed handles need rng_kind BSB_RNG_PHILOX");
+  if (c.obs_dtype != BSB_OBS_FLOAT32) return fail(BSB_UNSUPPORTED, "packed handles write float32 observations only");
+  if (c.flags & BSB_FLAG_SAME_STEP_RESET) return fail(BSB_UNSUPPORTED, "packed handles do not take BSB_FLAG_SAME_STEP_RESET");
+  for (int32_t k = 1; k < n_settings; ++k)
+    if (const char* field = packed_mismatch(c, configs[k]))
+      return fail(BSB_UNSUPPORTED, std::string("settings 0 and ") + std::to_string(k) + " differ in `" + field +
+                                       "`, which the settings of a packed handle must share");
+  return create_env(&c, (int64_t)n_settings * lanes_per_setting, device, seeds[0], lane_offset, out, configs, seeds,
+                    n_settings);
+}
+
+int32_t bsb_packed_layout(const bsb_env* env, int32_t* n_settings, int64_t* lanes_per_setting) {
+  if (!env || !n_settings || !lanes_per_setting) return fail(BSB_INVALID_ARGUMENT, "null argument");
+  *n_settings = env->n_settings; *lanes_per_setting = env->lanes_per_setting;
   return BSB_OK;
 }
 

@@ -34,6 +34,11 @@ struct bsb_env {
   int obs_dtype;          // bsb_obs_dtype of the observations this handle writes
   int obs_elem_bytes;     // ... and their size: 4, 2 or 1
   bool same_step;         // BSB_FLAG_SAME_STEP_RESET: a LAST lane is reset in the same call
+  // bsb_create_packed: n_settings settings of lanes_per_setting lanes each (p.pack holds their values); an ordinary
+  // handle has packed = false, n_settings = 1, lanes_per_setting = batch
+  bool packed;
+  int32_t n_settings;
+  int64_t lanes_per_setting;
   int64_t steps_done;     // step() calls so far (host counter; frozen at the switch to graph-safe mode)
   // Graph-safe mode: entered for good when a launch of this handle is first captured into a CUDA graph.  From
   // then on the device clock counts the steps (kernel comment in bsb_kernels.cuh) and steps = steps_done + clock[0].
@@ -90,7 +95,7 @@ struct bsb_env {
 namespace bsb {
 // One entry per family, each defined in its own translation unit (fam_<name>.cu).
 // deep_sea and catch also run the two-phase host step (`two_phase`: its arguments).  Each also reaches its same-step
-// (ss_<name>.cu) and reduced-dtype (obs_<name>.cu) instantiations.
+// (ss_<name>.cu), reduced-dtype (obs_<name>.cu) and, but deep_sea, packed (pk_<name>.cu) instantiations.
 int run_deep_sea(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs* two_phase = nullptr);
 int run_catch(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs* two_phase = nullptr);
 int run_cartpole(bsb_env*, const LaunchArgs&, cudaStream_t);

@@ -23,6 +23,8 @@ BSB_HD StepOut make_first() { StepOut o; o.reward = 0.0; o.discount = 0.0f; o.st
 BSB_HD StepOut make_mid(double r) { StepOut o; o.reward = r; o.discount = 1.0f; o.step_type = MID; return o; }
 BSB_HD StepOut make_last(double r) { StepOut o; o.reward = r; o.discount = 0.0f; o.step_type = LAST; return o; }
 
+struct PackTable;
+
 // Device-resident (or host-resident) description of one environment batch.
 // Passed BY VALUE to kernels.
 struct EnvParams {
@@ -42,8 +44,11 @@ struct EnvParams {
   double cp_force_mag, cp_pl, cp_length, cp_mass_pole, cp_mass_total, cp_gravity, cp_four_thirds, cp_two_pi;
 
   // tables
-  const uint32_t* mapping_bits;  // deep_sea: bit (row*N+col) of the action mapping
-  const double* reward_table;    // bandit / discounting_chain
+  union {
+    const uint32_t* mapping_bits;  // deep_sea: bit (row*N+col) of the action mapping
+    const PackTable* pack;         // packed handles (bsb_create_packed; never deep_sea): the per-setting values
+  };
+  const double* reward_table;    // bandit / discounting_chain (packed handles: the settings' tables, stacked)
   const int8_t* images;          // mnist
   const uint8_t* labels;         // mnist
 
@@ -65,6 +70,32 @@ struct EnvParams {
   uint32_t* mt_key;  int32_t* mt_idx;   // [624][B], [B]  (rng_kind == MT19937)
   uint32_t* wmt_key; int32_t* wmt_idx;
 };
+
+// Packed handles (bsb_create_packed): the settings of one experiment side by side, `lanes_per_setting` lanes each,
+// so lane i belongs to setting i / lanes_per_setting.  A PackTable is followed in memory by one PackSetting per
+// setting: the EnvParams fields that may differ between the settings of an experiment.
+struct PackSetting {
+  uint64_t seed;
+  int64_t table_offset;          // bandit / discounting_chain: first double of this setting's reward table
+  double height_threshold, x_reward_threshold, noise_scale, reward_scale;
+  int32_t memory_length, chain_length;
+};
+struct PackTable { int64_t lanes_per_setting, n_settings; };
+
+// Turns `q` (a copy of a packed handle's parameters) into the parameters lane i sees: those of its setting k's own
+// handle, in which it is lane j = i - k * lanes_per_setting.  The RNG streams and the action stream are keyed by
+// lane_offset + lane index, so lowering lane_offset by k * lanes_per_setting keys them by the setting's lane j.
+BSB_HD void pack_lane_params(EnvParams& q, int64_t i) {
+  const PackTable* t = q.pack;
+  const int64_t k = i / t->lanes_per_setting;
+  const PackSetting& s = reinterpret_cast<const PackSetting*>(t + 1)[k];
+  q.seed = s.seed;
+  q.lane_offset -= (uint64_t)(k * t->lanes_per_setting);
+  if (q.reward_table) q.reward_table += s.table_offset;
+  q.height_threshold = s.height_threshold; q.x_reward_threshold = s.x_reward_threshold;
+  q.noise_scale = s.noise_scale; q.reward_scale = s.reward_scale;
+  q.memory_length = s.memory_length; q.chain_length = s.chain_length;
+}
 
 static const uint32_t NEEDS_RESET = 0x80000000u;
 

@@ -156,6 +156,12 @@ template <class Family, class O> struct IsSameStep<SameStep<Family, O> > { stati
 // Kernel argument F for observations of type O in either auto-reset mode.
 template <class Family, class O, bool kSameStep> struct KernelTag { typedef typename KernelFamily<Family, O>::type type; };
 template <class Family, class O> struct KernelTag<Family, O, true> { typedef SameStep<Family, O> type; };
+// Packed handles (bsb_create_packed; float32, next-step): the first template argument of transition_kernel is
+// Packed<family>.  Every lane runs with its setting's parameters (pack_lane_params), found once per launch.
+template <class Family> struct Packed {};
+template <class Family> struct FamilyOf<Packed<Family> > { typedef Family type; };
+template <class F> struct IsPacked { static const bool value = false; };
+template <class Family> struct IsPacked<Packed<Family> > { static const bool value = true; };
 
 // ----- RNG plumbing ---------------------------------------------------------
 template <int RK> struct RngOf;
@@ -991,10 +997,11 @@ __device__ __forceinline__ void signal_done(const LaunchArgs& a, unsigned long l
 // single-phase host step.
 template <class F, int RK, bool kNoise, bool kTrack>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kernel(const EnvParams p, const LaunchArgs a) {
-  typedef typename FamilyOf<F>::type Fam;          // F is the family, ObsAs<family, O> (observations of type O) or
-  typedef typename ObsElemOf<F>::type O;           // SameStep<family, O> (same-step auto-reset)
+  typedef typename FamilyOf<F>::type Fam;          // F is the family, ObsAs<family, O> (observations of type O),
+  typedef typename ObsElemOf<F>::type O;           // SameStep<family, O> (same-step auto-reset) or Packed<family>
   typedef typename RngOf<RK>::type R;
   constexpr bool kSameStep = IsSameStep<F>::value;
+  constexpr bool kPacked = IsPacked<F>::value;
   const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
   const int64_t B = p.batch;
   const int K = p.obs_numel;
@@ -1032,15 +1039,20 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
     const bool active = tid < n_lanes;
     const bool bulk = chunk_is_bulk<Fam, O>(p, a, vec, n_lanes);
     ws.any_bulk = ws.any_bulk || bulk;
+    // The parameters this lane runs with: p itself, or (packed kernels) a copy with its setting's values, which it
+    // keeps for all T steps of the launch.
+    EnvParams setting_p;
+    if constexpr (kPacked) { setting_p = p; if (active) pack_lane_params(setting_p, lane); }
+    const EnvParams& lp = kPacked ? setting_p : p;
 
     typename Fam::Lane L;
     R rng, wrng;
     EpisodeStats ep;
     ActionStream action_stream;
     action_stream.open();
-    if (active) lane_open<Fam>(p, lane, L, rng, wrng, ep, a.mode, kNoise, kTrack);
+    if (active) lane_open<Fam>(lp, lane, L, rng, wrng, ep, a.mode, kNoise, kTrack);
     else Fam::init(p, L);
-    if (a.mode == MODE_INIT && active) Fam::ctor_draws(p, L, rng);      // the constructor runs no step (T = 0)
+    if (a.mode == MODE_INIT && active) Fam::ctor_draws(lp, L, rng);      // the constructor runs no step (T = 0)
     MergedReset<Fam, R> merged;            // same-step kernels only
     if constexpr (kSameStep) { Fam::init(p, merged.last); merged.done = false; }
 
@@ -1057,22 +1069,22 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
               action = action < 0 ? 0 : p.num_actions - 1;
             }
           } else {
-            action = action_stream.sample(a.action_seed, p.lane_offset + (uint64_t)lane, (uint64_t)(step0 + t), p.num_actions);
+            action = action_stream.sample(a.action_seed, lp.lane_offset + (uint64_t)lane, (uint64_t)(step0 + t), p.num_actions);
           }
           if (a.actions_out) a.actions_out[off] = action;
         }
         if constexpr (kSameStep) lane_step<Fam, R, true>(p, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, io, off, &merged);
-        else lane_step<Fam>(p, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, io, off);
+        else lane_step<Fam>(lp, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, io, off);
       }
       if constexpr (kSameStep) {
         if (!a.mailbox && a.final_obs)
           emit_final<Fam>(p, a, ws, merged, reinterpret_cast<O*>(a.final_obs) + t * B * (int64_t)K, warp_base, n_lanes,
                           lane, active, a.final_vec_ok != 0, bulk);
       }
-      emit_obs<Fam>(p, a, ws, L, rng, obs + t * B * (int64_t)K, warp_base, n_lanes, lane, active, bulk, vec);
+      emit_obs<Fam>(lp, a, ws, L, rng, obs + t * B * (int64_t)K, warp_base, n_lanes, lane, active, bulk, vec);
     }
 
-    if (active) lane_close<Fam>(p, lane, L, rng, wrng, ep, kNoise, kTrack);
+    if (active) lane_close<Fam>(lp, lane, L, rng, wrng, ep, kNoise, kTrack);
     if (dynamic && lazy) cur_chunk = fetch_chunk(a, total_warps);        // lazy: nothing was reserved while working
   }
   retire_warp(a, ws, a.mailbox != nullptr);

@@ -104,6 +104,23 @@ class _Handle:
     del keep
     self.ptr = ptr
 
+  @classmethod
+  def packed(cls, specs, lanes_per_setting: int, device_ordinal: int, seeds, lane_offset: int, flags: int,
+             log_schedule=None):
+    """One handle for the settings `specs` (Philox, float32): bsb_create_packed."""
+    self = cls.__new__(cls)
+    self.ptr = None
+    self.lib = _lib.load()
+    built = [_make_config(spec, _lib.RNG_PHILOX, flags, log_schedule) for spec in specs]
+    configs = (_lib.Config * len(built))(*[cfg for cfg, _ in built])
+    seed_array = (ctypes.c_uint64 * len(seeds))(*[int(s) & _MASK64 for s in seeds])
+    ptr = ctypes.c_void_p()
+    _lib.check(self.lib.bsb_create_packed(configs, len(built), int(lanes_per_setting), device_ordinal, seed_array,
+                                          lane_offset & _MASK64, ctypes.byref(ptr)))
+    del built
+    self.ptr = ptr
+    return self
+
   def close(self):
     if self.ptr is not None and self.ptr.value:
       self.lib.bsb_destroy(self.ptr)
@@ -209,11 +226,17 @@ class BatchedEnvironment:
   call is a transition.  The observation that came with the LAST goes to `final_observation` of buffers made with
   `make_buffers(..., final_observation=True)`.  Per lane, the outputs are the reference's own trace with each LAST
   merged into the reset that follows it (same random draws, same order), and info, episode statistics and log rows
-  are the reference's on that trace."""
+  are the reference's on that trace.
+
+  A packed environment (`bsuite_b200.load_experiment`) holds several settings of one experiment side by side:
+  `bsuite_ids[k]` owns the lanes `lanes_of(bsuite_ids[k])`, and lane j of that slice is lane j of
+  `load_from_id(bsuite_ids[k], batch=lanes_per_setting, seed=setting_seeds[k], lane_offset=lane_offset)`, bit for
+  bit.  An ordinary environment has `bsuite_ids` None."""
 
   def __init__(self, spec: EnvSpec, batch: int, device='cuda', seed: Optional[int] = None,
                rng: str = 'philox', lane_offset: int = 0, track_episodes: bool = False,
-               reward_dtype='float32', record_rows: bool = False, obs_dtype='float32', autoreset: str = 'next_step'):
+               reward_dtype='float32', record_rows: bool = False, obs_dtype='float32', autoreset: str = 'next_step',
+               _pack=None):
     import torch
     self._torch = torch
     self._spec = spec
@@ -247,8 +270,15 @@ class BatchedEnvironment:
       self._log_schedule = recording.log_schedule(spec.bsuite_num_episodes)
     self._reward_dtype = torch.float64 if str(reward_dtype).endswith('64') else torch.float32
     self._obs_dtype, obs_code = _obs_dtype(obs_dtype)
-    self._handle = _Handle(spec, self._batch, self._ordinal, self._seed, self._lane_offset, self._rng_kind, flags,
-                           self._log_schedule, obs_code)
+    # _pack: (bsuite_ids, specs, seeds, lanes_per_setting) of a packed environment (load_experiment)
+    self._pack = _pack
+    if _pack is not None:
+      ids, pack_specs, seeds, lanes = _pack
+      self._handle = _Handle.packed(pack_specs, lanes, self._ordinal, seeds, self._lane_offset, flags,
+                                    self._log_schedule)
+    else:
+      self._handle = _Handle(spec, self._batch, self._ordinal, self._seed, self._lane_offset, self._rng_kind, flags,
+                             self._log_schedule, obs_code)
     self._lib = self._handle.lib
     n = ctypes.c_int32()
     _lib.check(self._lib.bsb_info_count(self._handle.ptr, ctypes.byref(n)))
@@ -266,6 +296,19 @@ class BatchedEnvironment:
   info_names = property(lambda self: self._info_names)
   obs_dtype = property(lambda self: self._obs_dtype)      # torch dtype of the observation tensors
   autoreset = property(lambda self: self._autoreset)      # 'next_step' or 'same_step'
+  # packed environments: one bsuite_id and one seed per setting, lanes_per_setting lanes each (ordinary: None, batch)
+  bsuite_ids = property(lambda self: None if self._pack is None else self._pack[0])
+  setting_seeds = property(lambda self: None if self._pack is None else self._pack[2])
+  lanes_per_setting = property(lambda self: self._batch if self._pack is None else self._pack[3])
+
+  def lanes_of(self, bsuite_id: str) -> slice:
+    """The slice of the lane axis that holds setting `bsuite_id` of a packed environment."""
+    if self._pack is None:
+      raise ValueError('lanes_of needs a packed environment (load_experiment)')
+    if bsuite_id not in self._pack[0]:
+      raise KeyError(f'{bsuite_id!r} is not packed in this environment ({", ".join(self._pack[0])})')
+    k, lanes = self._pack[0].index(bsuite_id), self._pack[3]
+    return slice(k * lanes, (k + 1) * lanes)
 
   def observation_spec(self):
     """Per-lane spec, identical to the reference environment's (float32 values).  The observation tensors this
@@ -512,11 +555,12 @@ class BatchedEnvironment:
     """Host mirror of the on-device action sampler for this environment's lanes."""
     if first_step is None:
       first_step = self.steps_done
-    out = np.empty((int(num_steps), self._batch), dtype=np.int32)
-    _lib.check(self._lib.bsb_random_actions(int(action_seed) & _MASK64, self._lane_offset, self._batch,
+    lanes = self.lanes_per_setting      # a packed environment keys every setting's lanes by the lane within it
+    out = np.empty((int(num_steps), lanes), dtype=np.int32)
+    _lib.check(self._lib.bsb_random_actions(int(action_seed) & _MASK64, self._lane_offset, lanes,
                                             int(first_step), int(num_steps), self._spec.num_actions,
                                             ctypes.c_void_p(out.ctypes.data)))
-    return out
+    return out if lanes == self._batch else np.tile(out, (1, self._batch // lanes))
 
   @property
   def steps_done(self) -> int:
@@ -607,6 +651,13 @@ class BatchedEnvironment:
     for table in (self._spec.table, self._spec.table2):
       if table is not None:
         h.update(np.ascontiguousarray(table).tobytes())
+    if self._pack is not None:             # every setting's fields, tables and seed, and the packing
+      ids, pack_specs, seeds, lanes = self._pack
+      h.update(repr(('packed', tuple(ids), tuple(int(s) for s in seeds), int(lanes),
+                     tuple(tuple(sorted(s.fields.items())) for s in pack_specs))).encode())
+      for spec in pack_specs:
+        if spec.table is not None:
+          h.update(np.ascontiguousarray(spec.table).tobytes())
     return h.hexdigest()[:16]
 
   def close(self):

@@ -39,8 +39,8 @@ def log_schedule(num_episodes: int) -> 'list[int]':
 _INT_COLUMNS = frozenset(['steps', 'episode', 'episode_len', 'total_bad_episodes', 'total_perfect'])
 
 
-def write_lane_csvs(env, bsuite_id: str, results_root: str, lanes: Optional[Sequence[int]] = None,
-                    overwrite: bool = False) -> 'list[str]':
+def write_lane_csvs(env, bsuite_id: Optional[str] = None, results_root: Optional[str] = None,
+                    lanes: Optional[Sequence[int]] = None, overwrite: bool = False) -> 'list[str]':
   """Writes the rows a `record_rows=True` batched environment has recorded, one results directory per lane.
 
   Every lane is an independent run of `bsuite_id` (its own seed), so each gets what the reference's
@@ -48,7 +48,18 @@ def write_lane_csvs(env, bsuite_id: str, results_root: str, lanes: Optional[Sequ
   (logging/csv_logging.py:29-31, 73-89), one row per log point with the columns `steps, episode, total_return,
   episode_len, episode_return` + the `bsuite_info()` keys.  Each directory loads with the reference's
   `csv_load.load_one_result_set` / `load_bsuite` (csv_load.py:29-57).  Returns the directories written.
+
+  A packed environment (`load_experiment`) writes every setting it holds (or only `bsuite_id`): lane j of every
+  setting goes to `lane_<lane_offset + j>/`, so each such directory holds one complete run of the experiment, and
+  each file is byte for byte the one `write_lane_csvs` writes for that setting's own environment.  `lanes` then
+  counts within a setting.
   """
+  if results_root is None:
+    raise TypeError('write_lane_csvs needs results_root')
+  if getattr(env, 'bsuite_ids', None) is not None:
+    return _write_packed_csvs(env, bsuite_id, results_root, lanes, overwrite)
+  if bsuite_id is None:
+    raise TypeError('write_lane_csvs needs the bsuite_id of an environment that is not packed')
   logged = env.logged_rows()
   columns = list(logged['columns'])
   rows = logged['rows'].cpu().numpy()              # [n_points, n_columns, B]
@@ -69,6 +80,34 @@ def write_lane_csvs(env, bsuite_id: str, results_root: str, lanes: Optional[Sequ
       for k in range(int(counts[lane])):
         writer.writerow([int(v) if c in _INT_COLUMNS else float(v) for c, v in zip(columns, rows[k, :, lane])])
     written.append(directory)
+  return written
+
+
+def _write_packed_csvs(env, bsuite_id, results_root, lanes, overwrite):
+  logged = env.logged_rows()
+  columns = list(logged['columns'])
+  rows = logged['rows'].cpu().numpy()              # [n_points, n_columns, B]
+  counts = logged['counts'].cpu().numpy()
+  ids = env.bsuite_ids if bsuite_id is None else (bsuite_id,)
+  lanes = range(env.lanes_per_setting) if lanes is None else lanes
+  written = []
+  for setting_id in ids:
+    first = env.lanes_of(setting_id).start
+    filename = f"{BSUITE_PREFIX}{setting_id.replace('/', SAFE_SEPARATOR)}.csv"
+    for lane in lanes:
+      directory = os.path.join(results_root, f'lane_{env.lane_offset + lane:07d}')
+      os.makedirs(directory, exist_ok=True)
+      path = os.path.join(directory, filename)
+      if os.path.exists(path) and not overwrite:
+        raise ValueError(f'File {path} already exists. Specify a different directory, or set overwrite=True '
+                         'to overwrite existing data.')
+      with open(path, 'w', newline='') as fh:
+        writer = csv.writer(fh)
+        writer.writerow(columns)
+        for k in range(int(counts[first + lane])):
+          writer.writerow([int(v) if c in _INT_COLUMNS else float(v) for c, v in zip(columns, rows[k, :, first + lane])])
+      if directory not in written:
+        written.append(directory)
   return written
 
 

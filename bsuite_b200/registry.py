@@ -6,11 +6,11 @@ contract); with `batch=B` it is a `BatchedEnvironment` of B lanes.
 """
 
 import functools
-from typing import Any, Mapping, Optional, Tuple
+from typing import Any, Mapping, Optional, Sequence, Tuple
 
 from bsuite_b200 import experiments
 from bsuite_b200 import sweep
-from bsuite_b200.environment import BatchedEnvironment, DmEnvAdapter
+from bsuite_b200.environment import BatchedEnvironment, DmEnvAdapter, _fresh_seed
 
 
 def unpack_bsuite_id(bsuite_id: str) -> Tuple[str, int]:
@@ -48,6 +48,48 @@ def load_from_id(bsuite_id: str, batch: Optional[int] = None, device='cuda', see
   kwargs = sweep.SETTINGS[bsuite_id]
   experiment_name, _ = unpack_bsuite_id(bsuite_id)
   return load(experiment_name, kwargs, batch=batch, device=device, seed=seed, rng=rng, **engine_kwargs)
+
+
+# Fields whose value may differ between the settings of a packed environment (bsb_create_packed); a field outside
+# this set that changes the observation shape keeps an experiment out of load_experiment.
+_PER_SETTING_FIELDS = frozenset(['memory_length', 'chain_length', 'height_threshold', 'x_reward_threshold',
+                                 'noise_scale', 'reward_scale'])
+
+
+def load_experiment(experiment_name: str, lanes_per_setting: int, settings: Optional[Sequence[int]] = None,
+                    device='cuda', seed: Optional[int] = None, lane_offset: int = 0, track_episodes: bool = False,
+                    record_rows: bool = False, reward_dtype='float32') -> BatchedEnvironment:
+  """Every setting of one experiment (or the `settings` indices into `sweep.BY_EXPERIMENT[experiment_name]`) in ONE
+  batched environment of `len(settings) * lanes_per_setting` lanes: a step of the experiment is one kernel launch and
+  one observation tensor.  Lane j of `env.lanes_of(bsuite_id)` is lane j of
+  `load_from_id(bsuite_id, batch=lanes_per_setting, seed=env.setting_seeds[k], lane_offset=lane_offset)`, bit for
+  bit, so sharding works as it does for single ids.
+
+  An explicit `seed` is used by every setting, as `load_from_id(bsuite_id, seed=seed)` would use it; otherwise each
+  setting takes its experiment's own seed (memory_len fixes 0) or fresh OS entropy.  Experiments whose settings
+  differ in observation shape (deep_sea, deep_sea_stochastic: `size`; memory_size: `num_bits`; umbrella_distract:
+  `n_distractor`) raise ValueError.  Packed environments use the Philox bit source, float32 observations and the
+  next-step auto-reset convention."""
+  if experiment_name not in sweep.BY_EXPERIMENT:
+    raise ValueError(f'unknown experiment {experiment_name!r}')
+  all_ids = sweep.BY_EXPERIMENT[experiment_name]
+  indices = list(range(len(all_ids))) if settings is None else [int(k) for k in settings]
+  if not indices:
+    raise ValueError('settings must name at least one setting')
+  ids = tuple(all_ids[k] for k in indices)
+  if len(set(ids)) != len(ids):
+    raise ValueError('settings must not repeat a setting')
+  specs = [experiments.EXPERIMENT_NAME_TO_SPEC[experiment_name](**sweep.SETTINGS[i]) for i in ids]
+  for spec in specs[1:]:
+    if spec.obs_shape != specs[0].obs_shape:
+      changed = [k for k in specs[0].fields if specs[0].fields[k] != spec.fields.get(k) and k not in _PER_SETTING_FIELDS]
+      raise ValueError(f'the settings of {experiment_name} differ in `{changed[0] if changed else "obs_shape"}`, which '
+                       'changes the observation shape: load them with load_from_id one by one')
+  seeds = tuple(int(seed) if seed is not None else (s.seed if s.seed is not None else _fresh_seed()) for s in specs)
+  lanes = int(lanes_per_setting)
+  return BatchedEnvironment(specs[0], batch=len(specs) * lanes, device=device, seed=seeds[0], lane_offset=lane_offset,
+                            track_episodes=track_episodes, record_rows=record_rows, reward_dtype=reward_dtype,
+                            _pack=(ids, tuple(specs), seeds, lanes))
 
 
 def make(environment_class: str, batch: Optional[int] = None, device='cuda', seed: Optional[int] = None,

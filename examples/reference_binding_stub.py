@@ -40,6 +40,10 @@ class Outputs(ctypes.Structure):          # struct bsb_outputs
 _lib = ctypes.CDLL(LIBRARY)
 _lib.bsb_create.argtypes = [ctypes.POINTER(Config), ctypes.c_int64, ctypes.c_int32, ctypes.c_uint64, ctypes.c_uint64,
                             ctypes.POINTER(ctypes.c_void_p)]
+# ABI 10: every setting of one experiment in one handle (lane k * lanes_per_setting + j = lane j of setting k)
+_lib.bsb_create_packed.argtypes = [ctypes.POINTER(Config), ctypes.c_int32, ctypes.c_int64, ctypes.c_int32,
+                                   ctypes.POINTER(ctypes.c_uint64), ctypes.c_uint64, ctypes.POINTER(ctypes.c_void_p)]
+_lib.bsb_packed_layout.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int64)]
 _lib.bsb_reset.argtypes = [ctypes.c_void_p, ctypes.POINTER(Outputs), ctypes.c_void_p]
 _lib.bsb_step.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Outputs), ctypes.c_void_p]
 _lib.bsb_read_info.argtypes = [ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]

@@ -36,9 +36,10 @@
 extern "C" {
 #endif
 
-#define BSB_ABI_VERSION 9
+#define BSB_ABI_VERSION 10
 #define BSB_DEVICE_HOST (-1)
 #define BSB_MAX_INFO 4
+#define BSB_MAX_PACKED_SETTINGS 64 /* bsb_create_packed: settings per handle */
 
 typedef enum bsb_status {
   BSB_OK = 0,
@@ -233,6 +234,39 @@ const char* bsb_last_error(void);
  */
 int32_t bsb_create(const bsb_config* config, int64_t batch, int32_t device,
                    uint64_t seed, uint64_t lane_offset, bsb_env** out);
+
+/*
+ * Packed handle: the settings of one experiment (bsuite_ids that share
+ * everything that shapes the kernel and the observation) in ONE handle, so a
+ * step of the whole experiment is one launch and one output tensor.  The
+ * handle has batch B = n_settings * lanes_per_setting, and lane
+ * k * lanes_per_setting + j of it is, bit for bit, lane j of
+ *   bsb_create(&configs[k], lanes_per_setting, device, seeds[k], lane_offset)
+ * -- its outputs, info, Logging columns, log rows, clamping of device actions,
+ * and the actions bsb_rollout samples for it (keyed by lane_offset + j, the
+ * lane within its setting).  Random streams therefore do not depend on the
+ * packing, and a rank that owns lanes [a, b) of every setting creates its
+ * pack with lanes_per_setting = b - a and lane_offset = a.
+ * Settings may differ in their seed (seeds[k]; configs[k].seed is not a
+ * field), the contents of `table` (bandit / discounting_chain rewards),
+ * memory_length, chain_length, height_threshold, x_reward_threshold,
+ * noise_scale and reward_scale; every other field must be equal, including
+ * table sizes, mnist's images and labels and the log schedule
+ * (BSB_UNSUPPORTED, naming the first field that differs).  n_settings in
+ * [1, BSB_MAX_PACKED_SETTINGS] and lanes_per_setting >= 1, else
+ * BSB_INVALID_ARGUMENT.  Not available (BSB_UNSUPPORTED): deep_sea (its
+ * settings differ in size), BSB_RNG_MT19937, obs_dtype other than float32,
+ * BSB_FLAG_SAME_STEP_RESET.  Every other entry point takes a packed handle as
+ * a batch of B lanes; bsb_step_host runs it in one phase.
+ */
+int32_t bsb_create_packed(const bsb_config* configs, int32_t n_settings,
+                          int64_t lanes_per_setting, int32_t device,
+                          const uint64_t* seeds, uint64_t lane_offset,
+                          bsb_env** out);
+
+/* Settings and lanes per setting of a handle (1 and B for bsb_create's). */
+int32_t bsb_packed_layout(const bsb_env* env, int32_t* n_settings,
+                          int64_t* lanes_per_setting);
 
 int32_t bsb_destroy(bsb_env* env);
 
