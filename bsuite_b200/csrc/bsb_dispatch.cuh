@@ -92,13 +92,12 @@ void host_run(const EnvParams& p, const LaunchArgs& a) {
 struct Geometry { int threads = 0; size_t smem = 0; int64_t n_chunks = 0, grid = 0; int extra_blocks = 0; };
 
 // Chunk lanes, emitter plan (group lanes, stage rows), CTA size, shared memory and grid of a launch; fills a's
-// emitter fields and, for a persistent grid, its chunk counter.  The rest is for two-phase host steps: `group` > 0
-// sets the lanes per deep_sea bulk store; `no_obs`: no observation (no shared memory: co-resident with another
-// handle's observation stream), one chunk per warp; `extra_threads` > 0 puts g.extra_blocks blocks of that many
-// threads in all (at least one) in front of the chunk owners; `ctas_per_sm` > 0 caps a persistent grid per SM.
+// emitter fields and, for a persistent grid (the deep_sea and mnist bulk paths, once the grid exceeds what is
+// resident), its chunk counter.  The rest is for two-phase host steps: `no_obs`: no observation (no shared memory:
+// co-resident with another handle's observation stream), one chunk per warp; `extra_threads` > 0 puts
+// g.extra_blocks blocks of that many threads in all (at least one) in front of the chunk owners.
 template <class F, class O>
-int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int group = 0, bool no_obs = false, int extra_threads = 0,
-                int ctas_per_sm = 0) {
+int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, bool no_obs = false, int extra_threads = 0) {
   const int K = e->p.obs_numel;
   const bool is_onehot = EmitKind<F>::value == EMIT_ONEHOT;
   const bool is_image = EmitKind<F>::value == EMIT_IMAGE;
@@ -107,8 +106,6 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int group = 0, bool no_o
   a.group_lanes = 1;
   a.work_counter = nullptr;
   a.work_base = 0;
-  a.lazy_fetch = e->lazy_fetch;
-  a.l2_hint = e->l2_hint;
   // Row / board stages per warp: two (the next row block is rendered while the TMA unit still reads the previous
   // one) unless that costs resident warps -- 16 warps per SM fit the register budget, so a warp can afford
   // ~14 KB of shared memory.  umbrella_distract (103-float rows, 13 KB per stage) would hold 8 warps per SM
@@ -139,12 +136,11 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int group = 0, bool no_o
     int m = 1;
     while (m < 16 && (size_t)(2 * m) * tile <= 40 * 1024) m <<= 1;
     if (e->deep_sea_group > 0) m = e->deep_sea_group;
-    if (group > 0) m = group;
     if (m > chunk) m = chunk;               // a group never spans chunks
     if (((size_t)m * tile) % 16 != 0 || (size_t)TILE_STAGES * m * tile > 100 * 1024) {
       a.emit_bulk = 0;                      // tiles too large (or misaligned) for the staged path: vector stores
     } else {
-      a.group_lanes = m; threads = 32; persistent = e->deep_sea_persistent != 0;
+      a.group_lanes = m; threads = 32; persistent = true;
     }
   }
   if (is_image && a.emit_bulk) {
@@ -164,7 +160,7 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int group = 0, bool no_o
     if ((K & 15) != 0 || (size_t)stages * m * tile > 64 * 1024) {
       a.emit_bulk = 0;
     } else {
-      a.group_lanes = m; a.stage_rows = stages; threads = 128; a.cta_extra_elems = mz * K; persistent = e->deep_sea_persistent != 0;
+      a.group_lanes = m; a.stage_rows = stages; threads = 128; a.cta_extra_elems = mz * K; persistent = true;
       if (g.n_chunks < 2 * (int64_t)e->num_sms) threads = 64;      // small batches: more, smaller CTAs
     }
   }
@@ -191,7 +187,6 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int group = 0, bool no_o
     // draw chunks from the environment's global counter.
     int64_t per_sm = (int64_t)((227 * 1024) / (smem + 1024));
     per_sm = per_sm < 1 ? 1 : (per_sm > 16 ? 16 : per_sm);
-    if (ctas_per_sm > 0 && per_sm > ctas_per_sm) per_sm = ctas_per_sm;
     const int64_t resident = (int64_t)e->num_sms * per_sm;
     if (g.grid > resident) {      // else everything is resident anyway: one chunk per warp
       g.grid = resident;
@@ -238,12 +233,10 @@ template <class F, int RK, bool kNoise, bool kTrack, class O>
 int two_phase_launch(bsb_env* e, LaunchArgs a, TwoPhaseArgs h, cudaStream_t stream) {
   if (a.clock) return fail(BSB_INTERNAL, "a host step reached graph-safe mode, which turns the mailbox path off");
   // Copiers: enough of them for ~512 threads, i.e. ~64 KB of 16-byte loads in flight.  The observation-only launch
-  // of a split step has none and may take its own group size (BSB_SPLIT_GROUP) and leave room for ANOTHER handle's
-  // observation stream on every SM (BSB_SPLIT_CTAS_PER_SM).
+  // of a split step has none.
   Geometry g;
   const bool obs_only = h.phase == 2;
-  const int rc = plan_launch<F, O>(e, a, g, obs_only ? e->split_group : 0, h.phase == 1, obs_only ? 0 : 512,
-                                obs_only ? e->split_ctas_per_sm : 0);
+  const int rc = plan_launch<F, O>(e, a, g, h.phase == 1, obs_only ? 0 : 512);
   if (rc != BSB_OK) return rc;
   h.copiers = g.extra_blocks;
   return launch(e, a, g, stream, two_phase_host_kernel<typename KernelFamily<F, O>::type, RK, kNoise, kTrack>, e->p, a, h);

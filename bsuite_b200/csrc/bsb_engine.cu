@@ -459,10 +459,7 @@ static int32_t create_env(const bsb_config* config, int64_t batch, int32_t devic
       if (e->deep_sea_group < 0 || e->deep_sea_group > 32 || (e->deep_sea_group & (e->deep_sea_group - 1))) e->deep_sea_group = 0; }
     e->use_pdl = flag("BSB_PDL", 1);
     e->graph_pdl = flag("BSB_GRAPH_PDL", 1);
-    e->deep_sea_persistent = flag("BSB_DEEP_SEA_PERSISTENT", 1);
     e->zero_copy = flag("BSB_ZERO_COPY", 1);
-    e->lazy_fetch = flag("BSB_LAZY_FETCH", 1);
-    { const char* v = getenv("BSB_L2_HINT"); e->l2_hint = v ? atoi(v) : 1; if (e->l2_hint < 0 || e->l2_hint > 2) e->l2_hint = 1; }
     { const char* v = getenv("BSB_IMAGE_STAGES"); e->image_stages = (v && atoi(v) == 2) ? 2 : 1; }
     { const char* v = getenv("BSB_IMAGE_GROUP"); const int g = v ? atoi(v) : 4; e->image_group = (g == 1 || g == 2) ? g : 4; }
     { const char* v = getenv("BSB_CHUNK_LANES"); e->chunk_lanes = v ? atoi(v) : 0;
@@ -477,10 +474,6 @@ static int32_t create_env(const bsb_config* config, int64_t batch, int32_t devic
   { const char* v = getenv("BSB_HOST_SPIN"); e->host_spin = v ? (atoi(v) != 0) : 1; }
   { const char* v = getenv("BSB_HOST_EARLY"); e->host_early = v ? (atoi(v) != 0) : 1; }
   { const char* v = getenv("BSB_HOST_SPLIT"); e->host_split = v ? (atoi(v) != 0) : 1; }
-  { const char* v = getenv("BSB_SPLIT_GROUP"); e->split_group = v ? atoi(v) : 0;
-    if (e->split_group < 0 || e->split_group > 32 || (e->split_group & (e->split_group - 1))) e->split_group = 0; }
-  { const char* v = getenv("BSB_SPLIT_CTAS_PER_SM"); e->split_ctas_per_sm = v ? atoi(v) : 0;
-    if (e->split_ctas_per_sm < 0 || e->split_ctas_per_sm > 16) e->split_ctas_per_sm = 0; }
   { const char* v = getenv("BSB_HOST_STAGE_ACTIONS"); e->host_stage_actions = v ? (atoi(v) != 0) : 1; }
   e->h2d_stream = nullptr; e->h2d_event = nullptr;
   e->early_inflight = false;

@@ -50,14 +50,11 @@ struct bsb_env {
   int emit_bulk;          // TMA bulk stores for the row / board emitters
   int deep_sea_bulk;      // TMA bulk stores for deep_sea tiles (else 16-byte streaming stores)
   int deep_sea_group;     // lanes per deep_sea bulk store (0 = automatic)
-  int deep_sea_persistent; // persistent grid + dynamic chunk dealing for the deep_sea bulk path
   unsigned long long* work_counter;  // device counter of the dynamic chunk scheduler
   unsigned long long work_base;      // its value when the next launch starts
   int use_pdl;            // programmatic dependent launch between consecutive steps
   int graph_pdl;          // ... also between launches captured into a CUDA graph (programmatic graph edges)
   int zero_copy;          // bsb_step_host: kernel reads/writes pinned host buffers directly
-  int lazy_fetch;         // persistent kernel: fetch the next chunk lazily (default) or one chunk ahead
-  int l2_hint;            // L2 eviction hint of the observation bulk stores (0 none, 1 evict_first, 2 evict_last)
   int image_stages;       // mnist TMA path: staging buffers per warp (1 or 2)
   int image_group;        // mnist TMA path: tiles per staged store (1, 2 or 4)
   int chunk_lanes;        // lanes per chunk: 0 = automatic (32; 16 / 8 for small mnist batches), BSB_CHUNK_LANES forces
@@ -83,9 +80,6 @@ struct bsb_env {
   unsigned long long doorbell_timeout_ns;
   int host_spin;                      // BSB_HOST_SPIN (default 1): completion through the mailbox instead of a synchronise
   int host_split;                     // BSB_HOST_SPLIT (default 1): BSB_HOST_NO_WAIT two-phase steps run as two launches (transitions, observations)
-  int split_group;                    // BSB_SPLIT_GROUP (default 0 = as ordinary steps): lanes per bulk store of the observation-only launch of a split step
-  int split_ctas_per_sm;              // BSB_SPLIT_CTAS_PER_SM (default 0 = no cap): persistent CTAs per SM of that launch, so that the
-                                      // observation streams of two handles can be co-resident (shared memory) instead of taking turns
   int host_early;                     // BSB_HOST_EARLY (default 1): two-phase host steps (scalars first) where the family allows
   bool early_inflight;                // a two-phase host step may still be streaming observations on copy_stream
   int host_stage_actions;             // BSB_HOST_STAGE_ACTIONS (default 1): two-phase steps get their actions by DMA on a side stream instead of reading them in place

@@ -181,7 +181,7 @@ __global__ void __launch_bounds__(IMG_THREADS) to_image_kernel(const ImageParams
       const unsigned mis = (unsigned)(reinterpret_cast<uintptr_t>(g) & 15u);
       if (mis == 0) {
         const int body = len & ~3;
-        if (tid == 0 && body > 0) bulk_store_obs(g, buf, (uint32_t)body * 4u, 1);
+        if (tid == 0 && body > 0) bulk_store_obs(g, buf, (uint32_t)body * 4u);
         if (tid < len - body) st_stream(g + body + tid, buf[body + tid]);
       } else {                                          // 16-byte streaming stores between a scalar head and tail
         const int head = min(len, (int)((16u - mis) >> 2));

@@ -64,8 +64,6 @@ struct LaunchArgs {
   int32_t emit_bulk;        // use TMA bulk stores where the emitter supports them
   int32_t use_pdl;          // launched with programmatic stream serialization
   int32_t group_lanes;      // deep_sea bulk path: lanes per bulk store (power of two, 1..32)
-  int32_t lazy_fetch;       // persistent launches: 1 = fetch the next chunk only when the current one is issued
-  int32_t l2_hint;          // L2 policy of the observation bulk stores: 0 none, 1 evict_first (default), 2 evict_last
   int32_t final_vec_ok;     // same-step handles: final_obs base and per-step stride are 16-byte aligned
   unsigned long long* work_counter;  // persistent launches: monotonically increasing chunk counter (device)
   unsigned long long work_base;      // value of *work_counter at which this launch's chunk 0 starts
@@ -360,27 +358,19 @@ __device__ __forceinline__ void st_stream(uint2* dst, uint2 v) { __stcs(dst, v);
 __device__ __forceinline__ void st_stream(unsigned int* dst, unsigned int v) { __stcs(dst, v); }
 
 // ----- TMA bulk store (shared::cta -> global) and PDL primitives --------------
-__device__ __forceinline__ void bulk_store_s2g(void* gdst, const void* ssrc, uint32_t bytes) {
-  const uint32_t s = (uint32_t)__cvta_generic_to_shared(ssrc);
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(s), "r"(bytes) : "memory");
-}
-// Same store with an L2 eviction-priority hint (policy from createpolicy.fractional.L2::evict_first / evict_last).
+// Bulk store with an L2 eviction-priority hint (policy from createpolicy.fractional.L2::evict_first).
 __device__ __forceinline__ void bulk_store_s2g_hint(void* gdst, const void* ssrc, uint32_t bytes, uint64_t policy) {
   const uint32_t s = (uint32_t)__cvta_generic_to_shared(ssrc);
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;" ::"l"(gdst), "r"(s), "r"(bytes), "l"(policy) : "memory");
 }
+// Not volatile: the policy is a pure value, so the compiler may create it once and reuse it across stores.
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {
-  uint64_t p; asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p)); return p;
+  uint64_t p; asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p)); return p;
 }
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-  uint64_t p; asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p)); return p;
-}
-// Bulk store with the launch's L2 policy: observations are written once and never re-read by this kernel, so they
-// are marked evict_first (default; BSB_L2_HINT selects none / evict_last for A/B runs).
-__device__ __forceinline__ void bulk_store_obs(void* gdst, const void* ssrc, uint32_t bytes, int l2_hint) {
-  if (l2_hint == 1) bulk_store_s2g_hint(gdst, ssrc, bytes, l2_policy_evict_first());
-  else if (l2_hint == 2) bulk_store_s2g_hint(gdst, ssrc, bytes, l2_policy_evict_last());
-  else bulk_store_s2g(gdst, ssrc, bytes);
+// Observation bulk store: observations are written once and never re-read by this kernel, so they are marked
+// evict_first (DESIGN.md §3 records the H100 A/B against the other policies).
+__device__ __forceinline__ void bulk_store_obs(void* gdst, const void* ssrc, uint32_t bytes) {
+  bulk_store_s2g_hint(gdst, ssrc, bytes, l2_policy_evict_first());
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
@@ -565,7 +555,7 @@ __device__ __forceinline__ float4 pixels4(uint32_t w) {
 template <class O>
 __device__ __forceinline__ void emit_image_bulk(const EnvParams& p, O* stage, const O* cta_zero, O* obs_t,
                                                 int64_t warp_base, int n_lanes, int K, int image, int m, int mz,
-                                                int l2_hint, int stages, unsigned& emitted) {
+                                                int stages, unsigned& emitted) {
   constexpr int MAXM = 4;
   const int tid = threadIdx.x & 31;
   O* tiles = reinterpret_cast<O*>(reinterpret_cast<float*>(stage) + 256);
@@ -576,7 +566,7 @@ __device__ __forceinline__ void emit_image_bulk(const EnvParams& p, O* stage, co
     const unsigned block_mask = (in_block >= 32 ? 0xffffffffu : ((1u << in_block) - 1u));
     if (((showing >> z0) & block_mask) == 0u) {
       if (tid == 0) {
-        bulk_store_obs(obs_t + (warp_base + z0) * (int64_t)K, cta_zero, (uint32_t)in_block * (uint32_t)K * (uint32_t)sizeof(O), l2_hint);
+        bulk_store_obs(obs_t + (warp_base + z0) * (int64_t)K, cta_zero, (uint32_t)in_block * (uint32_t)K * (uint32_t)sizeof(O));
         bulk_commit();
       }
       continue;
@@ -617,7 +607,7 @@ __device__ __forceinline__ void emit_image_bulk(const EnvParams& p, O* stage, co
       }
       fence_proxy_async_smem();
       __syncwarp();
-      if (tid == 0) { bulk_store_obs(dst, buf, bytes, l2_hint); bulk_commit(); }
+      if (tid == 0) { bulk_store_obs(dst, buf, bytes); bulk_commit(); }
       ++emitted;
     }
   }
@@ -874,7 +864,7 @@ __device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a
         if (tid == 0) {
           O* tile_dst = obs_t + (warp_base + g0) * (int64_t)K;
           const uint32_t tile_bytes = (uint32_t)in_group * (uint32_t)K * (uint32_t)sizeof(O);
-          bulk_store_obs(tile_dst, group, tile_bytes, a.l2_hint);
+          bulk_store_obs(tile_dst, group, tile_bytes);
           bulk_commit();
         }
         ++ws.emitted;
@@ -898,7 +888,7 @@ __device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a
       if (buf) { ws.poked_a1 = new_a; ws.poked_b1 = new_b; } else { ws.poked_a0 = new_a; ws.poked_b0 = new_b; }
       fence_proxy_async_smem();
       __syncwarp();
-      if (tid == 0) { bulk_store_obs(obs_t + warp_base * (int64_t)K, boards, (uint32_t)n_lanes * (uint32_t)K * (uint32_t)sizeof(O), a.l2_hint); bulk_commit(); }
+      if (tid == 0) { bulk_store_obs(obs_t + warp_base * (int64_t)K, boards, (uint32_t)n_lanes * (uint32_t)K * (uint32_t)sizeof(O)); bulk_commit(); }
       ++ws.emitted;
     } else {
       emit_twohot_vec(obs_t, warp_base, n_lanes, K, hot_a, hot_b, vec);
@@ -906,7 +896,7 @@ __device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a
   } else if (kEmit == EMIT_IMAGE) {
     const int image = Descriptor<F>::a(L);
     if (bulk) emit_image_bulk(p, ws.stage, ws.cta_zero, obs_t, warp_base, n_lanes, K, active ? image : -1, a.group_lanes,
-                              a.cta_extra_elems / K, a.l2_hint, a.stage_rows, ws.emitted);
+                              a.cta_extra_elems / K, a.stage_rows, ws.emitted);
     else emit_image(p, reinterpret_cast<const float*>(ws.stage), obs_t, warp_base, n_lanes, K, image, vec && (K & 3) == 0);
   } else if (!a.stage_rows) {
     // observation rows too long for a shared-memory stage: every thread renders its row in place.  Never taken by
@@ -920,7 +910,7 @@ __device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a
     if (bulk) {
       fence_proxy_async_smem();
       __syncwarp();
-      if (tid == 0) { bulk_store_obs(obs_t + warp_base * (int64_t)K, rows, (uint32_t)n_lanes * (uint32_t)K * (uint32_t)sizeof(O), a.l2_hint); bulk_commit(); }
+      if (tid == 0) { bulk_store_obs(obs_t + warp_base * (int64_t)K, rows, (uint32_t)n_lanes * (uint32_t)K * (uint32_t)sizeof(O)); bulk_commit(); }
     } else {
       __syncwarp();
       flush_rows_vec(rows, obs_t, warp_base, n_lanes, K, vec);
@@ -1019,7 +1009,6 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
   const int cl = a.chunk_lanes;
   const int64_t n_chunks = (B + cl - 1) / cl;
   const bool dynamic = a.work_counter != nullptr;
-  const bool lazy = a.lazy_fetch != 0;
   const int64_t total_warps = (int64_t)gridDim.x * warps_per_cta;
   if (cancelled) {
     // A stood-down launch still owes the chunk counter its share: a launch over C chunks advances it by exactly C.
@@ -1032,8 +1021,6 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
 
   while (cur_chunk < n_chunks) {
     const int64_t warp_base = cur_chunk * cl;
-    // eager policy: reserve the next chunk now; lazy (default): only after this chunk's stores are issued
-    cur_chunk = (dynamic && !lazy) ? fetch_chunk(a, total_warps) : n_chunks;
     const int n_lanes = (B - warp_base) < cl ? (int)(B - warp_base) : cl;
     const int64_t lane = warp_base + tid;
     const bool active = tid < n_lanes;
@@ -1085,7 +1072,8 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
     }
 
     if (active) lane_close<Fam>(lp, lane, L, rng, wrng, ep, kNoise, kTrack);
-    if (dynamic && lazy) cur_chunk = fetch_chunk(a, total_warps);        // lazy: nothing was reserved while working
+    // a persistent warp reserves its next chunk only once this one's stores are issued
+    cur_chunk = dynamic ? fetch_chunk(a, total_warps) : n_chunks;
   }
   retire_warp(a, ws, a.mailbox != nullptr);
   if (a.mailbox) signal_done(a, a.ticket);

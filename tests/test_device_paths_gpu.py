@@ -18,7 +18,8 @@ also go through oracle.run_lanes, which anchors the comparison outside the engin
   group A  every instantiation transition_kernel<family, Philox | MT19937, noise, track> once (80 kernels);
   group B  the paths the default dispatch selects, at batch sizes derived from its rules (margins quoted for the
            132 SMs of an H100 SXM);
-  group C  every non-default value of the A/B tuning knobs, read from the environment when a handle is created;
+  group C  every non-default value of the tuning knobs still open to A/B runs, read from the environment when a
+           handle is created;
   group H  every instantiation two_phase_host_kernel<deep_sea | catch, Philox | MT19937, noise, track> (16 kernels),
            driven by host steps (bsb_step_host on pinned buffers): waited for, pre-launched, and BSB_HOST_NO_WAIT
            (which splits the step over two launches).
@@ -193,16 +194,11 @@ GROUP_C = (
     # lanes per deep_sea bulk store; N = 32 (default 8; 16 = 128 KB of stages: vector stores), N = 33 (K odd)
     + [_knob('deep_sea', b, dict(DS, size=n), BSB_DEEP_SEA_GROUP=g) for n, b in ((32, 3001), (33, 3004))
        for g in (1, 2, 4, 16)]
-    # chunk dealing of the persistent grids
-    + [_knob(*c, **kv) for c in (('deep_sea', 140003, dict(DS, size=10)), ('mnist', 40001, dict(images=28)))
-       for kv in (dict(BSB_LAZY_FETCH=0), dict(BSB_DEEP_SEA_PERSISTENT=0))]
     # vector stores instead of TMA bulk stores
     + [_knob(*c, BSB_EMIT_BULK=0) for c in (ROWS, ('mountain_car', 1000, {}), CATCH, MNIST)]
     # mnist staging
     + [_knob(*MNIST, BSB_IMAGE_STAGES=2), _knob('mnist', 40001, dict(images=28), BSB_IMAGE_STAGES=2),
        _knob(*MNIST, BSB_IMAGE_GROUP=1), _knob(*MNIST, BSB_IMAGE_GROUP=2)]
-    # L2 policy of the bulk stores
-    + [_knob(*c, BSB_L2_HINT=h) for c in (ROWS, CATCH, ('deep_sea', 3001, dict(DS, size=32)), MNIST) for h in (0, 2)]
     # single steps without programmatic dependent launch
     + [_knob(*c, BSB_PDL=0) for c in (ROWS, CATCH, ('deep_sea', 5000, dict(DS, size=10)), ('mnist', 1001, dict(images=28)))]
 )

@@ -8,7 +8,8 @@ ulp).
 
   group A  transition_kernel<ObsAs<family, Bf16 | uint8_t>, Philox, noise, track> (48 kernels) at B = 97;
   group B  dispatch paths whose rules count bytes: group sizes, tails, stages, alignment;
-  group C  every non-default BSB_* knob for uint8 deep_sea and bfloat16 catch;
+  group C  the non-default values of the launch-geometry and store knobs still open to A/B runs, for uint8 deep_sea
+           and bfloat16 catch;
   group H  two_phase_host_kernel<ObsAs<deep_sea | catch, Bf16 | uint8_t>, Philox, noise, track> (16 kernels).
 """
 
@@ -93,7 +94,6 @@ def _knob(family, batch, kwargs, obs_dtype, **knobs):
 
 
 DS_U8 = ('deep_sea', 3001, dict(DS, size=32), 'uint8')
-DS_U8_BIG = ('deep_sea', 140003, dict(DS, size=10), 'uint8')
 CATCH_BF16 = ('catch', 1000, {}, 'bfloat16')
 GROUP_C = (
     [_knob(*c, BSB_CHUNK_LANES=n) for c in (DS_U8, CATCH_BF16, ('deep_sea', 20004, dict(DS, size=15), 'uint8'))
@@ -101,9 +101,7 @@ GROUP_C = (
     + [_knob(*c, BSB_BLOCK_THREADS=n) for c in (DS_U8, CATCH_BF16) for n in (32, 128)]
     + [_knob(*DS_U8, BSB_DEEP_SEA_GROUP=g) for g in (1, 2, 4, 8, 32)]
     + [_knob('deep_sea', 3004, dict(DS, size=33), 'uint8', BSB_DEEP_SEA_GROUP=g) for g in (4, 16)]
-    + [_knob(*DS_U8_BIG, **kv) for kv in (dict(BSB_LAZY_FETCH=0), dict(BSB_DEEP_SEA_PERSISTENT=0))]
     + [_knob(*DS_U8, BSB_DEEP_SEA_BULK=0), _knob(*CATCH_BF16, BSB_EMIT_BULK=0)]
-    + [_knob(*c, BSB_L2_HINT=h) for c in (DS_U8, CATCH_BF16) for h in (0, 2)]
     + [_knob(*c, BSB_PDL=0) for c in (DS_U8, CATCH_BF16)]
 )
 
@@ -117,13 +115,11 @@ GROUP_H += [(case('deep_sea', 30001, H_KWARGS['deep_sea'], obs_dtype='uint8', tr
 
 # host-step knobs (read when a handle is created) for uint8 deep_sea and bfloat16 catch: (knobs, mode, observation
 # copied to the host as well).  BSB_ZERO_COPY=0 takes the staged path (device scratch sized in bytes, staged copies);
-# a host observation turns the zero-copy path's mailbox off (bsb_step + a copy); the split knobs set the group and
-# the CTAs of the observation-only launch of a BSB_HOST_NO_WAIT step.
+# a host observation turns the zero-copy path's mailbox off (bsb_step + a copy); BSB_HOST_SPLIT=0 runs a
+# BSB_HOST_NO_WAIT step as one launch instead of two.
 HOST_KNOBS = [({}, 'wait', True), (dict(BSB_ZERO_COPY=0), 'wait', True), (dict(BSB_ZERO_COPY=0), 'wait', False),
               (dict(BSB_HOST_SPIN=0), 'wait', False), (dict(BSB_HOST_EARLY=0), 'wait', False),
-              (dict(BSB_HOST_STAGE_ACTIONS=0), 'wait', False), (dict(BSB_HOST_SPLIT=0), 'no_wait', False),
-              (dict(BSB_SPLIT_GROUP=4), 'no_wait', False), (dict(BSB_SPLIT_GROUP=32), 'no_wait', False),
-              (dict(BSB_SPLIT_CTAS_PER_SM=2), 'no_wait', False)]
+              (dict(BSB_HOST_STAGE_ACTIONS=0), 'wait', False), (dict(BSB_HOST_SPLIT=0), 'no_wait', False)]
 GROUP_HK = [(case(f, 1001, H_KWARGS[f], obs_dtype=d, track=True, knobs={k: str(v) for k, v in knobs.items()}), mode,
              with_obs)
             for f, d in (('deep_sea', 'uint8'), ('catch', 'bfloat16')) for knobs, mode, with_obs in HOST_KNOBS]

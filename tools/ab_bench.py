@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """A/B of engine knobs on ONE box: alternates the variants several times (fresh handle each) and prints medians.
 
-    python tools/ab_bench.py BSB_LAZY_FETCH=0 BSB_LAZY_FETCH=1 [--track] [--host]
+    python tools/ab_bench.py BSB_BLOCK_THREADS=64 BSB_BLOCK_THREADS=128 [--track] [--host]
 """
 import os
 import statistics

@@ -55,9 +55,9 @@ def main():
   args = ap.parse_args()
   rows = []
   calibrate_writes(rows)
-  variants = [dict(threads=64, bulk=0, pdl=1, group=0, persistent=0), dict(threads=64, bulk=1, pdl=1, group=0, persistent=0),
-              dict(threads=64, bulk=1, pdl=1, group=0, persistent=1), dict(threads=64, bulk=1, pdl=0, group=0, persistent=1),
-              dict(threads=64, bulk=1, pdl=1, group=4, persistent=1), dict(threads=64, bulk=1, pdl=1, group=16, persistent=1)]
+  variants = [dict(threads=64, bulk=0, pdl=1, group=0), dict(threads=64, bulk=1, pdl=1, group=0),
+              dict(threads=64, bulk=1, pdl=0, group=0), dict(threads=64, bulk=1, pdl=1, group=4),
+              dict(threads=64, bulk=1, pdl=1, group=16)]
   for bsuite_id, batch in (('deep_sea/11', 65536), ('deep_sea/20', 32768), ('deep_sea/3', 262144), ('deep_sea/0', 262144)):
     size = bsuite_b200.sweep.SETTINGS[bsuite_id]['size']
     bytes_per = 4 * size * size + 24
@@ -70,7 +70,6 @@ def main():
       os.environ['BSB_DEEP_SEA_BULK'] = str(v['bulk'])
       os.environ['BSB_PDL'] = str(v['pdl'])
       os.environ['BSB_DEEP_SEA_GROUP'] = str(v['group'])
-      os.environ['BSB_DEEP_SEA_PERSISTENT'] = str(v['persistent'])
       env = bsuite_b200.load_from_id(bsuite_id, batch=batch, device='cuda', seed=0)
       ring_n = max(2, int(400e6 // (batch * size * size * 4)) + 1)
       ring = [env.make_buffers() for _ in range(ring_n)]
@@ -93,7 +92,7 @@ def main():
                  step_us=step_s * 1e6, step_gbs=batch * bytes_per / step_s / 1e9,
                  rollout_us=roll_s * 1e6, rollout_gbs=batch * bytes_per / roll_s / 1e9)
       rows.append(row)
-      print(f"{bsuite_id:14s} threads={v['threads']:<4d} bulk={v['bulk']} group={v['group']:<2d} pers={v['persistent']} pdl={v['pdl']}  step {row['step_us']:7.1f} us "
+      print(f"{bsuite_id:14s} threads={v['threads']:<4d} bulk={v['bulk']} group={v['group']:<2d} pdl={v['pdl']}  step {row['step_us']:7.1f} us "
             f"{row['step_gbs']:6.0f} GB/s | rollout {row['rollout_us']:7.1f} us/step {row['rollout_gbs']:6.0f} GB/s", flush=True)
       env.close()
       del ring, rbuf
