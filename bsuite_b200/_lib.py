@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BSB_LIBRARY points the binding at another build of the SAME library (tools/host_sanitize.sh: ASan/UBSan build)
 LIB_PATH = os.environ.get('BSB_LIBRARY') or os.path.join(_HERE, 'libbsuite_b200.so')
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 DEVICE_HOST = -1
 MAX_INFO = 4
 MAX_PACKED_SETTINGS = 64      # bsb_create_packed: settings per handle
@@ -131,6 +131,10 @@ EXPORTS = {
     'bsb_image_plan_create': (ctypes.c_int32, [ctypes.POINTER(ImageDesc), ctypes.c_int32, ctypes.POINTER(ctypes.c_void_p)]),
     'bsb_image_plan_destroy': (ctypes.c_int32, [ctypes.c_void_p]),
     'bsb_to_image': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
+    'bsb_obs_malloc': (ctypes.c_void_p, [ctypes.c_ssize_t, ctypes.c_int, ctypes.c_void_p]),
+    'bsb_obs_free': (None, [ctypes.c_void_p, ctypes.c_ssize_t, ctypes.c_int, ctypes.c_void_p]),
+    'bsb_obs_memory_info': (ctypes.c_int32, [ctypes.c_int, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_uint64),
+                                             ctypes.POINTER(ctypes.c_uint64)]),
 }
 
 _lib = None

@@ -129,6 +129,11 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, bool no_obs = false, int
   int threads = e->block_threads;
   bool persistent = false;
   const size_t tile = (size_t)K * elem;
+  // deep_sea tiles written to compressible memory (bsb_obs_malloc) leave as 16-byte streaming stores once the batch
+  // fills the GPU (>= 4 chunks per SM): there the bulk path gains nothing from compression, and the streaming stores
+  // run up to 1.22x faster than the bulk path on plain memory.  Smaller batches keep the bulk path, which overlaps
+  // a warp's stores with its next steps (DESIGN.md §7, "Compressible observation memory").
+  if (is_onehot && a.emit_bulk && g.n_chunks >= 4 * (int64_t)e->num_sms && in_compressed_block(a.obs)) a.emit_bulk = 0;
   if (is_onehot && a.emit_bulk) {
     // Lanes per bulk store: the largest power of two <= 16 with one store <= 40 KB (BSB_DEEP_SEA_GROUP overrides).
     // N = 32 -> 8 lanes (32 KB stores), N = 50 -> 4 lanes (40 KB); tools/bench_variants.py compares group sizes.

@@ -17,6 +17,7 @@ struct InfoNames { int n; const char* names[BSB_MAX_INFO]; };
 int fail(int code, const std::string& msg);           // records the thread-local error string
 const char* last_error_cstr();
 extern std::atomic<int64_t> g_launches;                // kernels launched by this library
+bool in_compressed_block(const void* p);               // p lies in a compressed bsb_obs_malloc block (bsb_memory.cu)
 
 #define BSB_CUDA(expr)                                                                   \
   do {                                                                                   \

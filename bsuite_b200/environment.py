@@ -20,6 +20,7 @@ import numpy as np
 
 from bsuite_b200 import _lib
 from bsuite_b200 import dm_env
+from bsuite_b200 import obs_memory
 from bsuite_b200.experiments import EnvSpec
 
 specs = dm_env.specs
@@ -334,13 +335,14 @@ class BatchedEnvironment:
     lead = (self._batch,) if num_steps is None else (int(num_steps), self._batch)
     kw = dict(device=self._device)
     obs_shape = lead + tuple(self._spec.obs_shape)
+    obs_args = (obs_shape, self._obs_dtype, self._device, self._spec.family)
     return StepBuffers(
-        observation=torch.empty(obs_shape, dtype=self._obs_dtype, **kw),
+        observation=obs_memory.empty(*obs_args),
         reward=torch.empty(lead, dtype=self._reward_dtype, **kw),
         discount=torch.empty(lead, dtype=torch.float32, **kw),
         step_type=torch.empty(lead, dtype=torch.int32, **kw),
         actions=torch.empty(lead, dtype=torch.int32, **kw) if with_actions else None,
-        final_observation=torch.zeros(obs_shape, dtype=self._obs_dtype, **kw) if final_observation else None)
+        final_observation=obs_memory.empty(*obs_args, zero=True) if final_observation else None)
 
   def _stream(self):
     if self._ordinal < 0:
@@ -397,8 +399,8 @@ class BatchedEnvironment:
     if self._ordinal < 0:
       return self.make_buffers()
     host = self.make_host_buffers()
-    return StepBuffers(observation=torch.empty((self._batch,) + tuple(self._spec.obs_shape), dtype=self._obs_dtype,
-                                               device=self._device),
+    return StepBuffers(observation=obs_memory.empty((self._batch,) + tuple(self._spec.obs_shape), self._obs_dtype,
+                                                    self._device, self._spec.family),
                        reward=host.reward, discount=host.discount, step_type=host.step_type)
 
   def make_host_buffers(self, with_observation: bool = False) -> StepBuffers:

@@ -30,13 +30,14 @@
 #ifndef BSUITE_B200_H_
 #define BSUITE_B200_H_
 
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
 extern "C" {
 #endif
 
-#define BSB_ABI_VERSION 10
+#define BSB_ABI_VERSION 11
 #define BSB_DEVICE_HOST (-1)
 #define BSB_MAX_INFO 4
 #define BSB_MAX_PACKED_SETTINGS 64 /* bsb_create_packed: settings per handle */
@@ -553,6 +554,32 @@ int32_t bsb_image_plan_destroy(bsb_image_plan* plan);
  */
 int32_t bsb_to_image(bsb_image_plan* plan, const float* in, int64_t batch,
                      float* out, void* stream);
+
+/*
+ * Device memory for observation buffers.  Observations are mostly zero (a
+ * deep_sea tile holds at most one 1.0 in 1 024 floats), and memory created
+ * with generic compression is compressed by the L2 on its way to DRAM, so
+ * kernels that write such tiles move fewer DRAM bytes.  Kernels, copies and
+ * the host see ordinary memory holding the values written.
+ *
+ * bsb_obs_malloc returns `size` bytes on CUDA device `device` (rounded up to
+ * the compressible granularity), or NULL with bsb_last_error() set when the
+ * device does not exist or memory is exhausted.  It falls back to plain
+ * cudaMalloc memory when the device cannot compress, the compressible backing
+ * store is used up, or the driver does not grant compression; it never fails
+ * where cudaMalloc would succeed.  bsb_obs_free waits for the device, then
+ * releases a pointer bsb_obs_malloc returned.  `stream` is unused by both.
+ * The signatures are those of torch.cuda.memory.CUDAPluggableAllocator.
+ * Host environments (BSB_DEVICE_HOST) use plain host memory.
+ *
+ * bsb_obs_memory_info: *supported = the device's generic-compression
+ * attribute; *compressed_bytes / *plain_bytes = bytes of live bsb_obs_malloc
+ * blocks on `device` that were / were not granted compression.
+ */
+void* bsb_obs_malloc(ptrdiff_t size, int device, void* stream);
+void bsb_obs_free(void* ptr, ptrdiff_t size, int device, void* stream);
+int32_t bsb_obs_memory_info(int device, int32_t* supported,
+                            uint64_t* compressed_bytes, uint64_t* plain_bytes);
 
 #ifdef __cplusplus
 }

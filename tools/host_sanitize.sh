@@ -7,9 +7,11 @@
 set -e
 OUT=/tmp/bsb_asan
 LOG=${1:-/tmp/bsb_asan/run.log}
-mkdir -p $OUT
+mkdir -p $OUT && rm -f $OUT/*.o
 cd "$(dirname "$0")/../bsuite_b200/csrc"
-ls bsb_engine.cu bsb_comm.cu bsb_image.cu fam_*.cu obs_*.cu | xargs -P 16 -I{} sh -c "nvcc -gencode arch=compute_90a,code=sm_90a -O1 -std=c++17 --fmad=false \
+# the translation units of the library as bsuite_b200/build.py lists them
+python -c "import sys; sys.path.insert(0, '../..'); from bsuite_b200 import build; print('\n'.join(build.SOURCES))" \
+  | xargs -P 16 -I{} sh -c "nvcc -gencode arch=compute_90a,code=sm_90a -O1 -std=c++17 --fmad=false \
   -Xcompiler -fPIC,-ffp-contract=off,-O1,-g,-fsanitize=address,-fsanitize=undefined,-fno-omit-frame-pointer -c {} -o $OUT/\$(basename {} .cu).o"
 nvcc -shared -o $OUT/libbsuite_b200.so $OUT/*.o -cudart static -ldl -Xcompiler -fsanitize=address,-fsanitize=undefined 2>/dev/null
 cd ../..
