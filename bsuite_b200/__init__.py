@@ -8,6 +8,7 @@ Public surface (mirrors `bsuite/__init__.py:18-24` and `bsuite/bsuite.py`):
   load_experiment(experiment_name, L, ...)     -> every setting of an experiment in one BatchedEnvironment
   make(environment_class, batch=..., **kwargs) -> construct a raw environment class
   sweep                                        -> SETTINGS / SWEEP / TAGS / TESTING / EPISODES
+  analysis.bsuite_score(envs)                  -> bsuite scores of every lane from the recorded log rows
   EXPERIMENT_NAME_TO_ENVIRONMENT               -> experiment name -> loader
 
 The compute lives in `libbsuite_b200.so` (hand-written sm_90a CUDA behind the C
@@ -23,7 +24,7 @@ except ImportError:  # this image: use the bundled compatible module
   from bsuite_b200 import dm_env_compat as dm_env  # noqa: F401
 _sys.modules.setdefault('bsuite_b200.dm_env', dm_env)
 
-from bsuite_b200 import sweep  # noqa: E402,F401
+from bsuite_b200 import analysis, sweep  # noqa: E402,F401
 from bsuite_b200.registry import (  # noqa: E402,F401
     EXPERIMENT_NAME_TO_ENVIRONMENT,
     load,

@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BSB_LIBRARY points the binding at another build of the SAME library (tools/host_sanitize.sh: ASan/UBSan build)
 LIB_PATH = os.environ.get('BSB_LIBRARY') or os.path.join(_HERE, 'libbsuite_b200.so')
 
-ABI_VERSION = 11
+ABI_VERSION = 12
 DEVICE_HOST = -1
 MAX_INFO = 4
 MAX_PACKED_SETTINGS = 64      # bsb_create_packed: settings per handle
@@ -79,6 +79,24 @@ class Outputs(ctypes.Structure):
               ('discount', ctypes.c_void_p), ('step_type', ctypes.c_void_p), ('final_observation', ctypes.c_void_p)]
 
 
+SCORE_MAX_SOURCES = 512      # bsb_score: sources per call
+# enum bsb_score_quantity: the row columns a score reads
+SCORE_QUANTITIES = ('episode', 'total_return', 'total_regret', 'raw_return', 'best_episode', 'total_perfect',
+                    'total_bad_episodes')
+
+
+class ScoreSource(ctypes.Structure):
+  """struct bsb_score_source."""
+  _fields_ = [
+      ('env', ctypes.c_void_p), ('rows', ctypes.c_void_p), ('counts', ctypes.c_void_p),
+      ('n_points', ctypes.c_int32), ('n_columns', ctypes.c_int32), ('lane_stride', ctypes.c_int64),
+      ('device', ctypes.c_int32), ('experiment', ctypes.c_int32), ('setting', ctypes.c_int32),
+      ('reserved0', ctypes.c_int32), ('first_lane', ctypes.c_int64), ('lanes', ctypes.c_int64),
+      ('group_key', ctypes.c_double), ('columns', ctypes.c_int32 * len(SCORE_QUANTITIES)),
+      ('reserved1', ctypes.c_int32),
+  ]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     'bsb_abi_version': (ctypes.c_int32, []),
@@ -133,6 +151,8 @@ EXPORTS = {
     'bsb_to_image': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_void_p]),
     'bsb_obs_malloc': (ctypes.c_void_p, [ctypes.c_ssize_t, ctypes.c_int, ctypes.c_void_p]),
     'bsb_obs_free': (None, [ctypes.c_void_p, ctypes.c_ssize_t, ctypes.c_int, ctypes.c_void_p]),
+    'bsb_score': (ctypes.c_int32, [ctypes.POINTER(ScoreSource), ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p,
+                                   ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     'bsb_obs_memory_info': (ctypes.c_int32, [ctypes.c_int, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_uint64),
                                              ctypes.POINTER(ctypes.c_uint64)]),
 }

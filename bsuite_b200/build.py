@@ -18,11 +18,11 @@ CSRC = os.path.join(HERE, 'csrc')
 FAMILIES = ('deep_sea', 'catch', 'cartpole', 'cartpole_swingup', 'mountain_car', 'memory_chain', 'bandit',
             'umbrella_chain', 'discounting_chain', 'mnist')
 SOURCES = [os.path.join(CSRC, 'bsb_engine.cu'), os.path.join(CSRC, 'bsb_comm.cu'), os.path.join(CSRC, 'bsb_image.cu'),
-           os.path.join(CSRC, 'bsb_memory.cu')] + [os.path.join(CSRC, f'fam_{name}.cu') for name in FAMILIES] + [
+           os.path.join(CSRC, 'bsb_memory.cu'), os.path.join(CSRC, 'bsb_score.cu')] + [os.path.join(CSRC, f'fam_{name}.cu') for name in FAMILIES] + [
     os.path.join(CSRC, f'obs_{name}.cu') for name in FAMILIES] + [os.path.join(CSRC, f'ss_{name}.cu') for name in FAMILIES] + [
     os.path.join(CSRC, f'pk_{name}.cu') for name in FAMILIES if name != 'deep_sea']
 HEADERS = [os.path.join(CSRC, f) for f in ('bsb_obs_dtype.h', 'bsb_rng.cuh', 'bsb_families.cuh', 'bsb_kernels.cuh', 'bsb_env.h',
-                                           'bsb_dispatch.cuh')] + [
+                                           'bsb_dispatch.cuh', 'bsb_score.cuh')] + [
     os.path.join(os.path.dirname(HERE), 'include', 'bsuite_b200.h')]
 OUTPUT = os.path.join(HERE, 'libbsuite_b200.so')
 OBJ_DIR = os.path.join(HERE, 'build')

@@ -357,6 +357,10 @@ void destroy_env(bsb_env* e) {
 
 }  // namespace
 
+namespace bsb {
+int drain_log_rows(bsb_env* e) { return drain_host_steps(e); }
+}  // namespace bsb
+
 __global__ void episode_stat_kernel(const EnvParams p, int field, int64_t calls, const unsigned long long* clock, double* dst) {
   if (clock) calls += (int64_t)*clock;      // graph-safe mode: steps since the switch are counted on the device
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;

@@ -18,6 +18,10 @@ int fail(int code, const std::string& msg);           // records the thread-loca
 const char* last_error_cstr();
 extern std::atomic<int64_t> g_launches;                // kernels launched by this library
 bool in_compressed_block(const void* p);               // p lies in a compressed bsb_obs_malloc block (bsb_memory.cu)
+}  // namespace bsb
+struct bsb_env;
+namespace bsb {
+int drain_log_rows(bsb_env* e);                         // waits out host steps in flight, as bsb_read_log_rows does
 
 #define BSB_CUDA(expr)                                                                   \
   do {                                                                                   \

@@ -273,6 +273,7 @@ class BatchedEnvironment:
     self._obs_dtype, obs_code = _obs_dtype(obs_dtype)
     # _pack: (bsuite_ids, specs, seeds, lanes_per_setting) of a packed environment (load_experiment)
     self._pack = _pack
+    self._bsuite_id = None          # set by load_from_id
     if _pack is not None:
       ids, pack_specs, seeds, lanes = _pack
       self._handle = _Handle.packed(pack_specs, lanes, self._ordinal, seeds, self._lane_offset, flags,
@@ -299,6 +300,8 @@ class BatchedEnvironment:
   autoreset = property(lambda self: self._autoreset)      # 'next_step' or 'same_step'
   # packed environments: one bsuite_id and one seed per setting, lanes_per_setting lanes each (ordinary: None, batch)
   bsuite_ids = property(lambda self: None if self._pack is None else self._pack[0])
+  # the bsuite_id an ordinary environment was loaded from (load_from_id), else None
+  bsuite_id = property(lambda self: self._bsuite_id)
   setting_seeds = property(lambda self: None if self._pack is None else self._pack[2])
   lanes_per_setting = property(lambda self: self._batch if self._pack is None else self._pack[3])
 

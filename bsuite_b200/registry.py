@@ -47,7 +47,10 @@ def load_from_id(bsuite_id: str, batch: Optional[int] = None, device='cuda', see
   """Returns a bsuite environment given a bsuite_id (bsuite.py:101-108)."""
   kwargs = sweep.SETTINGS[bsuite_id]
   experiment_name, _ = unpack_bsuite_id(bsuite_id)
-  return load(experiment_name, kwargs, batch=batch, device=device, seed=seed, rng=rng, **engine_kwargs)
+  env = load(experiment_name, kwargs, batch=batch, device=device, seed=seed, rng=rng, **engine_kwargs)
+  if isinstance(env, BatchedEnvironment):
+    env._bsuite_id = bsuite_id      # pylint: disable=protected-access
+  return env
 
 
 # Fields whose value may differ between the settings of a packed environment (bsb_create_packed); a field outside

@@ -49,7 +49,7 @@ class SweepBatch:
 
   def __init__(self, bsuite_ids: Optional[Sequence[str]] = None, lanes: int = 4096, device='cuda', seed: int = 0,
                rank: int = 0, world: int = 1, track_episodes: bool = True, ring: int = 1,
-               autoreset: str = 'next_step'):
+               autoreset: str = 'next_step', record_rows: bool = False):
     import torch
     self._torch = torch
     self.bsuite_ids = list(bsuite_ids) if bsuite_ids is not None else one_per_experiment()
@@ -57,7 +57,8 @@ class SweepBatch:
     self.lanes, self.local_lanes, self.lane_offset = lanes, count, first
     self.envs = {
         bsuite_id: registry.load_from_id(bsuite_id, batch=count, device=device, seed=seed, lane_offset=first,
-                                         track_episodes=track_episodes, autoreset=autoreset)
+                                         track_episodes=track_episodes, autoreset=autoreset,
+                                         record_rows=record_rows)
         for bsuite_id in self.bsuite_ids
     }
     self._device = next(iter(self.envs.values())).device

@@ -37,7 +37,7 @@
 extern "C" {
 #endif
 
-#define BSB_ABI_VERSION 11
+#define BSB_ABI_VERSION 12
 #define BSB_DEVICE_HOST (-1)
 #define BSB_MAX_INFO 4
 #define BSB_MAX_PACKED_SETTINGS 64 /* bsb_create_packed: settings per handle */
@@ -363,6 +363,93 @@ int32_t bsb_sum_episode_stats_many(bsb_env* const* envs, int32_t count,
  */
 int32_t bsb_log_layout(const bsb_env* env, int32_t* n_points, int32_t* n_columns);
 int32_t bsb_read_log_rows(bsb_env* env, double* rows, int32_t* counts, void* stream);
+
+/*
+ * bsuite scores from the log rows (experiments/summary_analysis.py:111-171,
+ * bsuite_score and ave_score_by_tag, on the results directory of each lane).
+ * Lane j of every source is one run of the sweep, as lane j's directory of
+ * CSV files (recording.write_lane_csvs) is for the reference: scores[e][j]
+ * is the score experiment e gets from those files, finished[e][j] whether
+ * each of its settings present reached NUM_EPISODES, and tag_scores[t][j]
+ * the mean over the experiments tagged t (NaN scores skipped).  An
+ * experiment with no row at lane j scores NaN and is not finished.
+ * Experiments are numbered in sorted name order and tags in sorted tag order.
+ */
+typedef enum bsb_experiment {
+  BSB_EXP_BANDIT = 0, BSB_EXP_BANDIT_NOISE, BSB_EXP_BANDIT_SCALE,
+  BSB_EXP_CARTPOLE, BSB_EXP_CARTPOLE_NOISE, BSB_EXP_CARTPOLE_SCALE,
+  BSB_EXP_CARTPOLE_SWINGUP, BSB_EXP_CATCH, BSB_EXP_CATCH_NOISE,
+  BSB_EXP_CATCH_SCALE, BSB_EXP_DEEP_SEA, BSB_EXP_DEEP_SEA_STOCHASTIC,
+  BSB_EXP_DISCOUNTING_CHAIN, BSB_EXP_MEMORY_LEN, BSB_EXP_MEMORY_SIZE,
+  BSB_EXP_MNIST, BSB_EXP_MNIST_NOISE, BSB_EXP_MNIST_SCALE,
+  BSB_EXP_MOUNTAIN_CAR, BSB_EXP_MOUNTAIN_CAR_NOISE,
+  BSB_EXP_MOUNTAIN_CAR_SCALE, BSB_EXP_UMBRELLA_DISTRACT,
+  BSB_EXP_UMBRELLA_LENGTH, BSB_NUM_EXPERIMENTS
+} bsb_experiment;
+
+typedef enum bsb_tag {
+  BSB_TAG_BASIC = 0, BSB_TAG_CREDIT_ASSIGNMENT, BSB_TAG_EXPLORATION,
+  BSB_TAG_GENERALIZATION, BSB_TAG_MEMORY, BSB_TAG_NOISE, BSB_TAG_SCALE,
+  BSB_NUM_TAGS
+} bsb_tag;
+
+/* The row columns a score reads: bsb_score_source.columns[quantity]. */
+typedef enum bsb_score_quantity {
+  BSB_Q_EPISODE = 0, BSB_Q_TOTAL_RETURN, BSB_Q_TOTAL_REGRET,
+  BSB_Q_RAW_RETURN, BSB_Q_BEST_EPISODE, BSB_Q_TOTAL_PERFECT,
+  BSB_Q_TOTAL_BAD_EPISODES, BSB_SCORE_NUM_QUANTITIES
+} bsb_score_quantity;
+
+#define BSB_SCORE_MAX_SOURCES 512
+
+/*
+ * One setting (bsuite_id) of one experiment: its rows, read in place.
+ *   env != NULL: the rows a handle created with a log schedule keeps
+ *       (bsb_read_log_rows' layout; any host step still in flight is
+ *       drained first).  rows, counts, n_points, n_columns, lane_stride and
+ *       device are then ignored.
+ *   env == NULL: caller-owned rows float64 [n_points][n_columns][lane_stride]
+ *       and counts int32 [lane_stride] in the memory space `device`.
+ * Lanes [first_lane, first_lane + lanes) of the store are lanes 0 .. lanes-1
+ * of the result (a packed handle's setting k starts at k * lanes_per_setting).
+ * `setting` is the index of the bsuite_id within its experiment, `group_key`
+ * the sweep value the experiment groups by (noise_scale, reward_scale, size,
+ * memory_length, num_bits, chain_length, n_distractor, height_threshold; 0
+ * when it groups by none), and columns[q] the column holding quantity q, or
+ * -1.  Rows must be recorded at strictly ascending episodes no larger than
+ * the experiment's NUM_EPISODES, as every handle's log schedule is.
+ */
+typedef struct bsb_score_source {
+  bsb_env* env;
+  const double* rows;
+  const int32_t* counts;
+  int32_t n_points, n_columns;
+  int64_t lane_stride;
+  int32_t device;
+  int32_t experiment;   /* bsb_experiment */
+  int32_t setting;
+  int32_t reserved0;
+  int64_t first_lane, lanes;
+  double group_key;
+  int32_t columns[BSB_SCORE_NUM_QUANTITIES];
+  int32_t reserved1;
+} bsb_score_source;
+
+/*
+ * Scores `count` sources (any order, at most BSB_SCORE_MAX_SOURCES, each
+ * setting once, all with `lanes` lanes and on one device) into scores
+ * float64 [BSB_NUM_EXPERIMENTS][lanes], finished uint8 [BSB_NUM_EXPERIMENTS]
+ * [lanes] (0 / 1) and tag_scores float64 [BSB_NUM_TAGS][lanes], all in the
+ * sources' memory space.  A device call enqueues two kernels on `stream`
+ * (one lane per thread and experiment, then the tag means) and neither
+ * allocates nor synchronises; a host call is synchronous.  The rows are only
+ * read.  BSB_INVALID_ARGUMENT: a handle without a log schedule, differing
+ * lane counts or devices, an unknown experiment, a column the experiment's
+ * score needs that is missing or out of range, a setting given twice.
+ */
+int32_t bsb_score(const bsb_score_source* sources, int32_t count, int64_t lanes,
+                  double* scores, uint8_t* finished, double* tag_scores,
+                  void* stream);
 
 /* Flat snapshot of all lane state (checkpoint/resume; absent in the reference). */
 int32_t bsb_state_bytes(const bsb_env* env, int64_t* nbytes);
