@@ -59,8 +59,6 @@ def is_stale() -> bool:
 
 def _compile(nvcc: str, source: str, verbose: bool):
   cmd = [nvcc] + NVCC_FLAGS + ['-c', source, '-o', _object_path(source)]
-  if os.environ.get('BSB_MIN_BLOCKS_PER_SM'):   # tuning experiment: cap registers via __launch_bounds__
-    cmd.append('-DBSB_MIN_BLOCKS_PER_SM=' + os.environ['BSB_MIN_BLOCKS_PER_SM'])
   if verbose:
     cmd += ['-Xptxas', '-v']
   proc = subprocess.run(cmd, capture_output=True, text=True)

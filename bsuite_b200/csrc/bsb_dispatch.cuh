@@ -102,7 +102,7 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, bool no_obs = false, int
   const bool is_onehot = EmitKind<F>::value == EMIT_ONEHOT;
   const bool is_image = EmitKind<F>::value == EMIT_IMAGE;
   const int64_t B = e->p.batch;
-  a.emit_bulk = is_onehot ? e->deep_sea_bulk : e->emit_bulk;
+  a.emit_bulk = 1;
   a.group_lanes = 1;
   a.work_counter = nullptr;
   a.work_base = 0;
@@ -123,10 +123,9 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, bool no_obs = false, int
   int chunk = 32;
   if (is_image)
     while (chunk > 8 && (B + chunk - 1) / chunk < 4 * (int64_t)e->num_sms) chunk >>= 1;
-  if (e->chunk_lanes > 0) chunk = e->chunk_lanes;
   a.chunk_lanes = chunk;
   g.n_chunks = (B + chunk - 1) / chunk;
-  int threads = e->block_threads;
+  int threads = 64;         // one chunk per warp: small CTAs spread evenly over the SMs (transition_kernel)
   bool persistent = false;
   const size_t tile = (size_t)K * elem;
   // deep_sea tiles written to compressible memory (bsb_obs_malloc) leave as 16-byte streaming stores once the batch
@@ -135,13 +134,12 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, bool no_obs = false, int
   // a warp's stores with its next steps (DESIGN.md §7, "Compressible observation memory").
   if (is_onehot && a.emit_bulk && g.n_chunks >= 4 * (int64_t)e->num_sms && in_compressed_block(a.obs)) a.emit_bulk = 0;
   if (is_onehot && a.emit_bulk) {
-    // Lanes per bulk store: the largest power of two <= 16 with one store <= 40 KB (BSB_DEEP_SEA_GROUP overrides).
-    // N = 32 -> 8 lanes (32 KB stores), N = 50 -> 4 lanes (40 KB); tools/bench_variants.py compares group sizes.
-    // Narrow tiles reach the 16-lane cap first: N = 32 in bfloat16 -> 16 lanes (32 KB), in uint8 -> 16 lanes (16 KB).
+    // Lanes per bulk store: the largest power of two <= 16 with one store <= 40 KB, so a group never spans a
+    // 32-lane chunk.  N = 32 -> 8 lanes (32 KB stores; 88.8 us per headline step against 91.9 with 4 lanes, DESIGN.md
+    // §3), N = 50 -> 4 lanes (40 KB).  Narrow tiles reach the 16-lane cap first: N = 32 in bfloat16 -> 16 lanes
+    // (32 KB), in uint8 -> 16 lanes (16 KB).
     int m = 1;
     while (m < 16 && (size_t)(2 * m) * tile <= 40 * 1024) m <<= 1;
-    if (e->deep_sea_group > 0) m = e->deep_sea_group;
-    if (m > chunk) m = chunk;               // a group never spans chunks
     if (((size_t)m * tile) % 16 != 0 || (size_t)TILE_STAGES * m * tile > 100 * 1024) {
       a.emit_bulk = 0;                      // tiles too large (or misaligned) for the staged path: vector stores
     } else {
@@ -150,26 +148,24 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, bool no_obs = false, int
   }
   if (is_image && a.emit_bulk) {
     // mnist through the TMA unit: groups of m tiles staged in shared memory + mz all-zero tiles per CTA for the LAST
-    // frames.  16-byte image loads need K % 16 == 0 (28 x 28 = 784 is).  Defaults (BSB_IMAGE_STAGES, BSB_IMAGE_GROUP):
-    // ONE staging buffer of m = 2 tiles per warp (6 KB) in 128-thread CTAs with mz = 8 zero tiles (25 KB, shared by
-    // the CTA's warps): 50 KB per CTA -> 4 CTAs = 16 warps per SM, the register limit.  The pixel conversion is
-    // issue-bound, so resident warps matter more than overlapping a warp's own fill with its own store (other
-    // warps fill that gap) or than the size of the staged stores; the zero frames still leave in 25 KB stores.
-    const int stages = e->image_stages;
-    int m = e->image_group;
-    while (m > 1 && (size_t)stages * m * tile > 28 * 1024) m >>= 1;
-    if (m > chunk) m = chunk;
+    // frames.  16-byte image loads need K % 16 == 0 (28 x 28 = 784 is).  ONE staging buffer of m <= 4 tiles per warp
+    // and mz <= 8 zero tiles per CTA, each halved until it fits 28 KB.  28 x 28 in float32: m = 4 (12.25 KB, plus
+    // the 1 KB pixel table: 13.25 KB per warp) and mz = 8 (24.5 KB, shared by the CTA's warps): 77.5 KB per
+    // 128-thread CTA -> 2 CTAs = 8 warps per SM (64-thread CTAs: 51 KB -> 4 CTAs, also 8 warps).  The pixel
+    // conversion is issue-bound, so resident warps matter more than overlapping a warp's own fill with its own store
+    // (other warps fill that gap); the zero frames, pure bandwidth, leave in 24.5 KB stores.
+    int m = 4;
+    while (m > 1 && (size_t)m * tile > 28 * 1024) m >>= 1;
     int mz = 8;
-    while (mz > 1 && ((size_t)mz * tile > 28 * 1024 || mz > chunk)) mz >>= 1;
-    if (mz < m) mz = m;
-    if ((K & 15) != 0 || (size_t)stages * m * tile > 64 * 1024) {
+    while (mz > 1 && (size_t)mz * tile > 28 * 1024) mz >>= 1;
+    if ((K & 15) != 0 || (size_t)m * tile > 64 * 1024) {
       a.emit_bulk = 0;
     } else {
-      a.group_lanes = m; a.stage_rows = stages; threads = 128; a.cta_extra_elems = mz * K; persistent = true;
+      a.group_lanes = m; a.stage_rows = 1; threads = 128; a.cta_extra_elems = mz * K; persistent = true;
       if (g.n_chunks < 2 * (int64_t)e->num_sms) threads = 64;      // small batches: more, smaller CTAs
     }
   }
-  a.use_pdl = (e->use_pdl && !a.no_pdl && a.mode == MODE_STEP && a.T == 1) ? 1 : 0;
+  a.use_pdl = (a.mode == MODE_STEP && a.T == 1) ? 1 : 0;
   if (no_obs) { a.emit_bulk = 0; a.stage_rows = 0; a.cta_extra_elems = 0; a.group_lanes = 1; threads = 128; persistent = false; }
   size_t per_warp = smem_elems_per_warp<F, O>(K, a.emit_bulk != 0, a.group_lanes, a.stage_rows) * elem;
   if ((EmitKind<F>::value == EMIT_ROWS || EmitKind<F>::value == EMIT_TWOHOT) && per_warp > 96 * 1024) {
@@ -264,8 +260,6 @@ int run_family_as(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const Tw
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
   if (!kF32 && mt) return fail(BSB_INTERNAL, "reduced obs_dtype or same-step auto-reset with MT19937");
   if (kSameStep && two_phase) return fail(BSB_INTERNAL, "a two-phase host step on a same-step handle");
-  // LaunchArgs::final_obs shares its word with doorbell_timeout_ns: a launch without a mailbox must carry a pointer
-  if (kSameStep && !a.mailbox && a.wait_doorbell) return fail(BSB_INTERNAL, "a doorbell launch without a mailbox");
   if (e->device < 0) {
     if constexpr (kF32) { if (mt) { host_run<F, 1, O>(e->p, a); return BSB_OK; } }
     host_run<F, 0, O, kSameStep>(e->p, a);

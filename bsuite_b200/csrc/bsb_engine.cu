@@ -89,7 +89,7 @@ int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseA
   if (e->device >= 0) {
     cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
     BSB_CUDA(cudaStreamIsCapturing(stream, &capture));
-    if (capture != cudaStreamCaptureStatusNone) { e->graph_safe = true; a.no_pdl = e->graph_pdl ? 0 : 1; }
+    if (capture != cudaStreamCaptureStatusNone) e->graph_safe = true;
     if (e->graph_safe) a.clock = e->clock;      // a.step0 == e->steps_done, which no longer moves
   }
   switch (e->p.family) {
@@ -245,9 +245,8 @@ int mailbox_launch(bsb_env* e, unsigned long long ticket, int64_t step0, const M
   LaunchArgs a = make_args(e, fields ? &out : nullptr, fields ? fields->actions : nullptr, 1, MODE_STEP);
   a.step0 = step0;
   a.mailbox = e->mailbox_dev; a.mail = e->mail; a.ticket = ticket; a.wait_doorbell = wait_doorbell ? 1 : 0;
-  a.doorbell_timeout_ns = e->doorbell_timeout_ns;
   { static const int timing = getenv("BSB_HOST_TIMING") ? atoi(getenv("BSB_HOST_TIMING")) : 0; a.timing = timing; }
-  if (!e->host_early || !family_obs_from_state(e)) return run(e, a, e->copy_stream);
+  if (!family_obs_from_state(e)) return run(e, a, e->copy_stream);
   // device staging of the scalars: reward | discount | step_type in one block (as the staged-copy path keeps them)
   const size_t B = (size_t)e->p.batch;
   if (!e->d_reward) {
@@ -260,7 +259,7 @@ int mailbox_launch(bsb_env* e, unsigned long long ticket, int64_t step0, const M
   memset(&h, 0, sizeof(h));
   h.stage.reward = e->d_reward; h.stage.reward_f64 = e->d_reward64; h.stage.discount = e->d_discount; h.stage.step_type = e->d_step_type;
   e->early_inflight = true;
-  if (split && e->host_split && !wait_doorbell) {
+  if (split && !wait_doorbell) {
     // BSB_HOST_NO_WAIT: the caller alternates between handles.  Two launches instead of one -- transitions + copiers
     // (no shared memory), then the observation stream -- so that THIS handle's transitions and PCIe traffic run
     // while the OTHER handle's observations have the SMs' shared memory and the HBM.
@@ -268,7 +267,6 @@ int mailbox_launch(bsb_env* e, unsigned long long ticket, int64_t step0, const M
     int rc = run(e, a, e->copy_stream, &h);
     if (rc != BSB_OK) return rc;
     a.mailbox = nullptr;
-    a.final_obs = nullptr;        // the word held the doorbell timeout: a launch without a mailbox reads it as final_obs
     h.phase = 2;
   }
   return run(e, a, e->copy_stream, &h);
@@ -452,33 +450,11 @@ static int32_t create_env(const bsb_config* config, int64_t batch, int32_t devic
   e->packed = n_settings > 0; e->n_settings = n_settings > 0 ? n_settings : 1;
   e->lanes_per_setting = n_settings > 0 ? batch / n_settings : batch;
   e->graph_safe = false; e->clock = nullptr; e->sum_scratch = nullptr; e->names = info_names(c.family);
-  {  // tuning knobs (environment variables, read once per handle)
-    auto flag = [](const char* name, int dflt) { const char* v = getenv(name); return v ? (atoi(v) != 0 ? 1 : 0) : dflt; };
-    const char* bt = getenv("BSB_BLOCK_THREADS");
-    e->block_threads = bt ? atoi(bt) : 64;
-    if (e->block_threads != 32 && e->block_threads != 64 && e->block_threads != 128) e->block_threads = 64;
-    e->emit_bulk = flag("BSB_EMIT_BULK", 1);
-    e->deep_sea_bulk = flag("BSB_DEEP_SEA_BULK", 1);
-    { const char* g = getenv("BSB_DEEP_SEA_GROUP"); e->deep_sea_group = g ? atoi(g) : 0;
-      if (e->deep_sea_group < 0 || e->deep_sea_group > 32 || (e->deep_sea_group & (e->deep_sea_group - 1))) e->deep_sea_group = 0; }
-    e->use_pdl = flag("BSB_PDL", 1);
-    e->graph_pdl = flag("BSB_GRAPH_PDL", 1);
-    e->zero_copy = flag("BSB_ZERO_COPY", 1);
-    { const char* v = getenv("BSB_IMAGE_STAGES"); e->image_stages = (v && atoi(v) == 2) ? 2 : 1; }
-    { const char* v = getenv("BSB_IMAGE_GROUP"); const int g = v ? atoi(v) : 4; e->image_group = (g == 1 || g == 2) ? g : 4; }
-    { const char* v = getenv("BSB_CHUNK_LANES"); e->chunk_lanes = v ? atoi(v) : 0;
-      if (e->chunk_lanes != 8 && e->chunk_lanes != 16 && e->chunk_lanes != 32) e->chunk_lanes = 0; }
-    e->work_counter = nullptr; e->work_base = 0;
-    e->num_sms = 132;
-    if (device >= 0) { int n = 0; if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) == cudaSuccess && n > 0) e->num_sms = n; }
-  }
+  e->work_counter = nullptr; e->work_base = 0;
+  e->num_sms = 132;
+  if (device >= 0) { int n = 0; if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) == cudaSuccess && n > 0) e->num_sms = n; }
   e->order_event = nullptr; e->fence_event = nullptr; e->bad_action_host = nullptr; e->bad_action_dev = nullptr;
   e->mailbox = nullptr; e->mailbox_dev = nullptr; e->mail = nullptr; e->next_ticket = 0; e->pending_ticket = 0; e->awaiting_ticket = 0;
-  { const char* v = getenv("BSB_DOORBELL_TIMEOUT_MS"); const long ms = v ? atol(v) : 200; e->doorbell_timeout_ns = (unsigned long long)(ms > 0 ? ms : 200) * 1000000ull; }
-  { const char* v = getenv("BSB_HOST_SPIN"); e->host_spin = v ? (atoi(v) != 0) : 1; }
-  { const char* v = getenv("BSB_HOST_EARLY"); e->host_early = v ? (atoi(v) != 0) : 1; }
-  { const char* v = getenv("BSB_HOST_SPLIT"); e->host_split = v ? (atoi(v) != 0) : 1; }
-  { const char* v = getenv("BSB_HOST_STAGE_ACTIONS"); e->host_stage_actions = v ? (atoi(v) != 0) : 1; }
   e->h2d_stream = nullptr; e->h2d_event = nullptr;
   e->early_inflight = false;
   e->h2d_actions = nullptr; e->d_reward = nullptr; e->d_reward64 = nullptr; e->d_discount = nullptr; e->d_step_type = nullptr; e->d_obs = nullptr;
@@ -996,115 +972,113 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
   // unified addressing), the transition kernel reads the actions from and writes reward / discount / step_type to
   // host memory directly over PCIe -- 1 MB per step, overlapped with the observation stream -- instead of three
   // separate copies with their launch and DMA latencies before and after the kernel.
-  if (env->zero_copy) {
-    void* d_actions = mapped_device_pointer(env, actions);
-    void* d_reward = host_out->reward ? mapped_device_pointer(env, host_out->reward) : nullptr;
-    void* d_reward64 = host_out->reward_f64 ? mapped_device_pointer(env, host_out->reward_f64) : nullptr;
-    void *d_discount = nullptr, *d_step_type = nullptr;
-    const bool packed_scalars = d_reward && host_out->discount == host_out->reward + B &&
-                                reinterpret_cast<char*>(host_out->step_type) == reinterpret_cast<char*>(host_out->reward + 2 * B);
-    if (packed_scalars) {       // reward | discount | step_type back to back in one pinned block: one query covers all
-      d_discount = static_cast<float*>(d_reward) + B;
-      d_step_type = static_cast<float*>(d_reward) + 2 * B;
-    } else {
-      d_discount = host_out->discount ? mapped_device_pointer(env, host_out->discount) : nullptr;
-      d_step_type = host_out->step_type ? mapped_device_pointer(env, host_out->step_type) : nullptr;
-    }
-    const bool all_mapped = d_actions && (!host_out->reward || d_reward) && (!host_out->reward_f64 || d_reward64) &&
-                            (!host_out->discount || d_discount) && (!host_out->step_type || d_step_type);
-    if (all_mapped) {
-      if (!device_obs && !env->d_obs) BSB_CUDA(cudaMalloc(&env->d_obs, obs_bytes));
-      MailFields f;
-      memset(&f, 0, sizeof(f));
-      f.actions = static_cast<const int32_t*>(d_actions);
-      f.obs = device_obs ? device_obs : env->d_obs;
-      f.reward = static_cast<float*>(d_reward);
-      f.reward_f64 = static_cast<double*>(d_reward64);
-      f.discount = static_cast<float*>(d_discount);
-      f.step_type = static_cast<int32_t*>(d_step_type);
-      f.obs_vec_ok = (reinterpret_cast<uintptr_t>(f.obs) % 16 == 0) ? 1 : 0;
-      cudaStream_t zs = env->copy_stream;
-      // Completion through the mailbox (BSB_HOST_SPIN=0 turns it off): the kernel's last CTA stores the ticket into
-      // pinned host memory after a system-scope fence and the host spins on that word -- a stream synchronise costs
-      // a wake-up per step.  Observations copied to the host, graph-safe handles and unaligned
-      // observation buffers keep the synchronise.
-      const bool spin = env->host_spin && !env->graph_safe && !host_out->observation && f.obs_vec_ok;
-      if (!spin) {
-        { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
-        bsb_outputs dev;
-        dev.final_observation = nullptr;
-        dev.observation = f.obs; dev.reward = f.reward; dev.reward_f64 = f.reward_f64; dev.discount = f.discount; dev.step_type = f.step_type;
-        int zrc = bsb_step(env, f.actions, &dev, zs);
-        if (zrc != BSB_OK) return zrc;
-        if (host_out->observation) BSB_CUDA(cudaMemcpyAsync(host_out->observation, dev.observation, obs_bytes, cudaMemcpyDeviceToHost, zs));
-        BSB_CUDA(cudaStreamSynchronize(zs));
-        return report_bad_actions(env);
-      }
-      { int mrc = mailbox_open(env); if (mrc != BSB_OK) return mrc; }
-      const bool prelaunch = (flags & BSB_HOST_PRELAUNCH) != 0;
-      for (int attempt = 0; attempt < 2; ++attempt) {
-        unsigned long long ticket;
-        if (env->pending_ticket) {
-          // The kernel of this step is already resident and polling: hand it the buffers and ring.
-          ticket = env->pending_ticket;
-          env->pending_ticket = 0;
-          env->mailbox->in = f;
-          std::atomic_thread_fence(std::memory_order_release);
-          env->mailbox->doorbell = ticket;
-        } else {
-          ticket = ++env->next_ticket;
-          if (env->host_stage_actions && env->host_early && family_obs_from_state(env)) {
-            // Two-phase step: phase 1 (the transitions of every lane) is all that stands between this launch and the
-            // observation stream, and reading 4 B per lane over PCIe from inside the kernel is most of it.  The DMA
-            // engine brings the actions over NOW, on a side stream, while the previous step's kernel is still
-            // streaming observations; the launch waits for that copy on the device.  (The previous kernel read its
-            // actions in phase 1, which ended before its completion word was seen: the buffer is free.)
-            if (!env->h2d_actions) BSB_CUDA(cudaMalloc(&env->h2d_actions, B * 4));
-            if (!env->h2d_stream) {
-              BSB_CUDA(cudaStreamCreateWithFlags(&env->h2d_stream, cudaStreamNonBlocking));
-              BSB_CUDA(cudaEventCreateWithFlags(&env->h2d_event, cudaEventDisableTiming));
-            }
-            BSB_CUDA(cudaMemcpyAsync(env->h2d_actions, actions, B * 4, cudaMemcpyHostToDevice, env->h2d_stream));
-            BSB_CUDA(cudaEventRecord(env->h2d_event, env->h2d_stream));
-            BSB_CUDA(cudaStreamWaitEvent(zs, env->h2d_event, 0));
-            f.actions = env->h2d_actions;
-          }
-          int lrc = mailbox_launch(env, ticket, env->steps_done, &f, false, (flags & BSB_HOST_NO_WAIT) != 0);
-          if (lrc != BSB_OK) return lrc;
-        }
-        if ((flags & BSB_HOST_FENCE_CALLER) && env->early_inflight) {
-          // Two-phase step: the observation stores outlive this call.  Fence the caller's stream behind the kernel
-          // (the event is recorded BEFORE the next step's kernel is queued, so it stands for this step only):
-          // whatever the caller enqueues there afterwards sees complete observations.
-          if (!env->fence_event) BSB_CUDA(cudaEventCreateWithFlags(&env->fence_event, cudaEventDisableTiming));
-          BSB_CUDA(cudaEventRecord(env->fence_event, zs));
-          BSB_CUDA(cudaStreamWaitEvent(static_cast<cudaStream_t>(caller_stream), env->fence_event, 0));
-        }
-        if (flags & BSB_HOST_NO_WAIT) {
-          // Split call: the completion word is collected by bsb_host_wait (or by whichever entry point of this handle
-          // runs next), so the caller can drive ANOTHER handle while this step's scalars cross PCIe.
-          env->awaiting_ticket = ticket;
-          return BSB_OK;
-        }
-        if (prelaunch) {
-          // Queue the NEXT step's kernel now: it becomes resident as this one drains and waits for its doorbell,
-          // so the next call pays neither a launch nor a wake-up.  It stands down by itself after
-          // BSB_DOORBELL_TIMEOUT_MS without a ring.
-          const unsigned long long next = ++env->next_ticket;
-          int lrc = mailbox_launch(env, next, env->steps_done + 1, nullptr, true);
-          if (lrc != BSB_OK) return lrc;
-          env->pending_ticket = next;
-        }
-        bool cancelled = false;
-        { int wrc = mailbox_wait(env, ticket, &cancelled); if (wrc != BSB_OK) return wrc; }
-        if (!cancelled) { env->steps_done += 1; return report_bad_actions(env); }
-        // The pre-launched kernel had given up waiting before the ring arrived: nothing was stepped.  The launch
-        // queued behind it carries the wrong step index now; stand it down and take the step again, launched now.
-        { int frc = flush_pending(env); if (frc != BSB_OK) return frc; }
-      }
-      return fail(BSB_INTERNAL, "host step: a freshly launched kernel reported a cancelled doorbell");
-    }
+  void* d_actions = mapped_device_pointer(env, actions);
+  void* d_reward = host_out->reward ? mapped_device_pointer(env, host_out->reward) : nullptr;
+  void* d_reward64 = host_out->reward_f64 ? mapped_device_pointer(env, host_out->reward_f64) : nullptr;
+  void *d_discount = nullptr, *d_step_type = nullptr;
+  const bool packed_scalars = d_reward && host_out->discount == host_out->reward + B &&
+                              reinterpret_cast<char*>(host_out->step_type) == reinterpret_cast<char*>(host_out->reward + 2 * B);
+  if (packed_scalars) {       // reward | discount | step_type back to back in one pinned block: one query covers all
+    d_discount = static_cast<float*>(d_reward) + B;
+    d_step_type = static_cast<float*>(d_reward) + 2 * B;
+  } else {
+    d_discount = host_out->discount ? mapped_device_pointer(env, host_out->discount) : nullptr;
+    d_step_type = host_out->step_type ? mapped_device_pointer(env, host_out->step_type) : nullptr;
   }
+  const bool all_mapped = d_actions && (!host_out->reward || d_reward) && (!host_out->reward_f64 || d_reward64) &&
+                          (!host_out->discount || d_discount) && (!host_out->step_type || d_step_type);
+  if (all_mapped) {
+    if (!device_obs && !env->d_obs) BSB_CUDA(cudaMalloc(&env->d_obs, obs_bytes));
+    MailFields f;
+    memset(&f, 0, sizeof(f));
+    f.actions = static_cast<const int32_t*>(d_actions);
+    f.obs = device_obs ? device_obs : env->d_obs;
+    f.reward = static_cast<float*>(d_reward);
+    f.reward_f64 = static_cast<double*>(d_reward64);
+    f.discount = static_cast<float*>(d_discount);
+    f.step_type = static_cast<int32_t*>(d_step_type);
+    f.obs_vec_ok = (reinterpret_cast<uintptr_t>(f.obs) % 16 == 0) ? 1 : 0;
+    cudaStream_t zs = env->copy_stream;
+    // Completion through the mailbox: the kernel's last CTA stores the ticket into pinned host memory after a
+    // system-scope fence and the host spins on that word -- a stream synchronise costs a wake-up per step.
+    // Observations copied to the host, graph-safe handles and unaligned observation buffers keep the synchronise.
+    const bool spin = !env->graph_safe && !host_out->observation && f.obs_vec_ok;
+    if (!spin) {
+      { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
+      bsb_outputs dev;
+      dev.final_observation = nullptr;
+      dev.observation = f.obs; dev.reward = f.reward; dev.reward_f64 = f.reward_f64; dev.discount = f.discount; dev.step_type = f.step_type;
+      int zrc = bsb_step(env, f.actions, &dev, zs);
+      if (zrc != BSB_OK) return zrc;
+      if (host_out->observation) BSB_CUDA(cudaMemcpyAsync(host_out->observation, dev.observation, obs_bytes, cudaMemcpyDeviceToHost, zs));
+      BSB_CUDA(cudaStreamSynchronize(zs));
+      return report_bad_actions(env);
+    }
+    { int mrc = mailbox_open(env); if (mrc != BSB_OK) return mrc; }
+    const bool prelaunch = (flags & BSB_HOST_PRELAUNCH) != 0;
+    for (int attempt = 0; attempt < 2; ++attempt) {
+      unsigned long long ticket;
+      if (env->pending_ticket) {
+        // The kernel of this step is already resident and polling: hand it the buffers and ring.
+        ticket = env->pending_ticket;
+        env->pending_ticket = 0;
+        env->mailbox->in = f;
+        std::atomic_thread_fence(std::memory_order_release);
+        env->mailbox->doorbell = ticket;
+      } else {
+        ticket = ++env->next_ticket;
+        if (family_obs_from_state(env)) {
+          // Two-phase step: phase 1 (the transitions of every lane) is all that stands between this launch and the
+          // observation stream, and reading 4 B per lane over PCIe from inside the kernel is most of it.  The DMA
+          // engine brings the actions over NOW, on a side stream, while the previous step's kernel is still
+          // streaming observations; the launch waits for that copy on the device.  (The previous kernel read its
+          // actions in phase 1, which ended before its completion word was seen: the buffer is free.)
+          if (!env->h2d_actions) BSB_CUDA(cudaMalloc(&env->h2d_actions, B * 4));
+          if (!env->h2d_stream) {
+            BSB_CUDA(cudaStreamCreateWithFlags(&env->h2d_stream, cudaStreamNonBlocking));
+            BSB_CUDA(cudaEventCreateWithFlags(&env->h2d_event, cudaEventDisableTiming));
+          }
+          BSB_CUDA(cudaMemcpyAsync(env->h2d_actions, actions, B * 4, cudaMemcpyHostToDevice, env->h2d_stream));
+          BSB_CUDA(cudaEventRecord(env->h2d_event, env->h2d_stream));
+          BSB_CUDA(cudaStreamWaitEvent(zs, env->h2d_event, 0));
+          f.actions = env->h2d_actions;
+        }
+        int lrc = mailbox_launch(env, ticket, env->steps_done, &f, false, (flags & BSB_HOST_NO_WAIT) != 0);
+        if (lrc != BSB_OK) return lrc;
+      }
+      if ((flags & BSB_HOST_FENCE_CALLER) && env->early_inflight) {
+        // Two-phase step: the observation stores outlive this call.  Fence the caller's stream behind the kernel
+        // (the event is recorded BEFORE the next step's kernel is queued, so it stands for this step only):
+        // whatever the caller enqueues there afterwards sees complete observations.
+        if (!env->fence_event) BSB_CUDA(cudaEventCreateWithFlags(&env->fence_event, cudaEventDisableTiming));
+        BSB_CUDA(cudaEventRecord(env->fence_event, zs));
+        BSB_CUDA(cudaStreamWaitEvent(static_cast<cudaStream_t>(caller_stream), env->fence_event, 0));
+      }
+      if (flags & BSB_HOST_NO_WAIT) {
+        // Split call: the completion word is collected by bsb_host_wait (or by whichever entry point of this handle
+        // runs next), so the caller can drive ANOTHER handle while this step's scalars cross PCIe.
+        env->awaiting_ticket = ticket;
+        return BSB_OK;
+      }
+      if (prelaunch) {
+        // Queue the NEXT step's kernel now: it becomes resident as this one drains and waits for its doorbell,
+        // so the next call pays neither a launch nor a wake-up.  It stands down by itself after
+        // DOORBELL_TIMEOUT_NS (200 ms) without a ring.
+        const unsigned long long next = ++env->next_ticket;
+        int lrc = mailbox_launch(env, next, env->steps_done + 1, nullptr, true);
+        if (lrc != BSB_OK) return lrc;
+        env->pending_ticket = next;
+      }
+      bool cancelled = false;
+      { int wrc = mailbox_wait(env, ticket, &cancelled); if (wrc != BSB_OK) return wrc; }
+      if (!cancelled) { env->steps_done += 1; return report_bad_actions(env); }
+      // The pre-launched kernel had given up waiting before the ring arrived: nothing was stepped.  The launch
+      // queued behind it carries the wrong step index now; stand it down and take the step again, launched now.
+      { int frc = flush_pending(env); if (frc != BSB_OK) return frc; }
+    }
+    return fail(BSB_INTERNAL, "host step: a freshly launched kernel reported a cancelled doorbell");
+  }
+  // Staged copies (a pageable buffer among them): actions in, bsb_step on device scratch, scalars out.
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
   if (!env->h2d_actions) BSB_CUDA(cudaMalloc(&env->h2d_actions, B * 4));
   // reward | discount | step_type live in ONE device block so that a caller who keeps its three host arrays

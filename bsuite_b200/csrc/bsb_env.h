@@ -50,19 +50,8 @@ struct bsb_env {
   bool graph_safe;
   unsigned long long* clock;         // device, CLOCK_WORDS words: step count (replicated), chunk counter, finished-CTA counters
   double* sum_scratch;               // device: bsb_sum_episode_stats partials [64][5] + the ticket
-  // tuning knobs (environment variables, read once per handle)
-  int block_threads;      // CTA size of the transition kernel (32 / 64 / 128)
-  int emit_bulk;          // TMA bulk stores for the row / board emitters
-  int deep_sea_bulk;      // TMA bulk stores for deep_sea tiles (else 16-byte streaming stores)
-  int deep_sea_group;     // lanes per deep_sea bulk store (0 = automatic)
   unsigned long long* work_counter;  // device counter of the dynamic chunk scheduler
   unsigned long long work_base;      // its value when the next launch starts
-  int use_pdl;            // programmatic dependent launch between consecutive steps
-  int graph_pdl;          // ... also between launches captured into a CUDA graph (programmatic graph edges)
-  int zero_copy;          // bsb_step_host: kernel reads/writes pinned host buffers directly
-  int image_stages;       // mnist TMA path: staging buffers per warp (1 or 2)
-  int image_group;        // mnist TMA path: tiles per staged store (1, 2 or 4)
-  int chunk_lanes;        // lanes per chunk: 0 = automatic (32; 16 / 8 for small mnist batches), BSB_CHUNK_LANES forces
   int num_sms;
   bsb::InfoNames names;
   std::vector<void*> allocs;
@@ -82,13 +71,8 @@ struct bsb_env {
   unsigned long long next_ticket;     // last ticket handed out
   unsigned long long awaiting_ticket; // a BSB_HOST_NO_WAIT step whose completion word has not been collected yet (0 = none)
   unsigned long long pending_ticket;  // pre-launched launch waiting for its doorbell (0 = none); it is for step steps_done
-  unsigned long long doorbell_timeout_ns;
-  int host_spin;                      // BSB_HOST_SPIN (default 1): completion through the mailbox instead of a synchronise
-  int host_split;                     // BSB_HOST_SPLIT (default 1): BSB_HOST_NO_WAIT two-phase steps run as two launches (transitions, observations)
-  int host_early;                     // BSB_HOST_EARLY (default 1): two-phase host steps (scalars first) where the family allows
   bool early_inflight;                // a two-phase host step may still be streaming observations on copy_stream
-  int host_stage_actions;             // BSB_HOST_STAGE_ACTIONS (default 1): two-phase steps get their actions by DMA on a side stream instead of reading them in place
-  cudaStream_t h2d_stream; cudaEvent_t h2d_event;
+  cudaStream_t h2d_stream; cudaEvent_t h2d_event;     // two-phase host steps: the actions' DMA on a side stream
 };
 
 namespace bsb {

@@ -70,7 +70,6 @@ struct LaunchArgs {
   // Device clock (graph-safe mode, see the kernel): {steps advanced in this mode, chunk counter, finished CTAs}.
   // Null in the default mode, where `step0` / `work_base` arrive as launch arguments from the host's counters.
   unsigned long long* clock;
-  int32_t no_pdl;           // set while the stream is being captured
   int32_t chunk_lanes;      // lanes per chunk (= per warp pass): 32, or 16 / 8 when the batch would under-fill the SMs
   int32_t stage_rows;       // row / board emitters: number of [32, K] shared-memory stages per warp (2: double buffered;
                             // 1: long rows, where a second stage would cost resident warps; 0: straight to global memory)
@@ -86,12 +85,8 @@ struct LaunchArgs {
   unsigned long long ticket;
   int32_t timing;                    // BSB_HOST_TIMING: leave %globaltimer stamps in the mailbox
   int32_t wait_doorbell;             // 1: pre-launched -- poll the doorbell for `ticket`, then take the buffers from the mailbox
-  // Host steps never deliver final observations, ordinary launches never wait for a doorbell: the two share a word,
-  // so that the kernels' argument layout is that of the next-step kernels.
-  union {
-    unsigned long long doorbell_timeout_ns;   // host steps (a.mailbox set)
-    float* final_obs;       // same-step handles, ordinary launches: [T,B,K] observations of the LAST timesteps
-  };                        // (bsb_outputs.final_observation), or null
+  float* final_obs;         // same-step handles: [T,B,K] observations of the LAST timesteps (bsb_outputs.final_observation),
+                            // or null (always null for host steps)
   int32_t* bad_action;      // pinned host flag (device alias): set to 1 when an action is outside [0, num_actions)
 };
 
@@ -322,8 +317,8 @@ __host__ __device__
 size_t smem_elems_per_warp(int K, bool emit_bulk, int group_lanes, int row_stages) {
   if (EmitKind<F>::value == EMIT_ROWS || EmitKind<F>::value == EMIT_TWOHOT) return (size_t)row_stages * 32 * (size_t)K;
   if (EmitKind<F>::value == EMIT_ONEHOT && emit_bulk) return (size_t)TILE_STAGES * (size_t)group_lanes * (size_t)K;
-  if (EmitKind<F>::value == EMIT_IMAGE)                    // int8 pixel -> float32 table (+ two staging buffers of m tiles)
-    return 256 * sizeof(float) / sizeof(O) + (emit_bulk ? (size_t)row_stages * (size_t)group_lanes * (size_t)K : 0);
+  if (EmitKind<F>::value == EMIT_IMAGE)                    // int8 pixel -> float32 table (+ one staging buffer of m tiles)
+    return 256 * sizeof(float) / sizeof(O) + (emit_bulk ? (size_t)group_lanes * (size_t)K : 0);
   return 0;
 }
 
@@ -547,18 +542,16 @@ __device__ __forceinline__ float4 pixels4(uint32_t w) {
 //   * otherwise the block goes in groups of `m` (<= 4) lanes: all 16-byte loads of the group's int8 images (49 per
 //     28 x 28 tile) are issued before the first conversion, the float32 tiles land in a staging buffer and leave
 //     as one bulk store of m * 4K bytes.
-// stage = [256 floats: table of the vector path][stages x m x K elements of O; a bfloat16 tile is converted after
-// pixel_div255]; `emitted` counts staged stores (buffer
-// parity).  Small staging buffers (m = 2, one stage: 6 KB per warp) keep 16 warps per SM resident -- the conversion
-// is issue-bound, so resident warps matter -- while the
-// zero frames, which are pure bandwidth, still leave in 25 KB stores.
+// stage = [256 floats: table of the vector path][m x K elements of O; a bfloat16 tile is converted after
+// pixel_div255].  One staging buffer per warp (13.25 KB at m = 4 in float32) keeps more warps resident than two --
+// the conversion is issue-bound, so resident warps matter -- while the zero frames, which are pure bandwidth, still
+// leave in 24.5 KB stores.
 template <class O>
 __device__ __forceinline__ void emit_image_bulk(const EnvParams& p, O* stage, const O* cta_zero, O* obs_t,
-                                                int64_t warp_base, int n_lanes, int K, int image, int m, int mz,
-                                                int stages, unsigned& emitted) {
+                                                int64_t warp_base, int n_lanes, int K, int image, int m, int mz) {
   constexpr int MAXM = 4;
   const int tid = threadIdx.x & 31;
-  O* tiles = reinterpret_cast<O*>(reinterpret_cast<float*>(stage) + 256);
+  O* const buf = reinterpret_cast<O*>(reinterpret_cast<float*>(stage) + 256);
   const int K16 = K >> 4;
   const unsigned showing = __ballot_sync(0xffffffffu, image >= 0);
   for (int z0 = 0; z0 < n_lanes; z0 += mz) {
@@ -575,9 +568,7 @@ __device__ __forceinline__ void emit_image_bulk(const EnvParams& p, O* stage, co
       const int in_group = (z0 + in_block - g0) < m ? (z0 + in_block - g0) : m;
       O* dst = obs_t + (warp_base + g0) * (int64_t)K;
       const uint32_t bytes = (uint32_t)in_group * (uint32_t)K * (uint32_t)sizeof(O);
-      O* buf = tiles + (size_t)(stages == 2 ? (emitted & 1u) : 0u) * m * K;
-      // two staging buffers: at most the newest store may still be reading, never this buffer; one: none may
-      if (tid == 0) { if (stages == 2) bulk_wait_read<1>(); else bulk_wait_read<0>(); }
+      if (tid == 0) bulk_wait_read<0>();      // the previous staged store has finished reading the buffer
       __syncwarp();
       int img[MAXM];
 #pragma unroll
@@ -608,7 +599,6 @@ __device__ __forceinline__ void emit_image_bulk(const EnvParams& p, O* stage, co
       fence_proxy_async_smem();
       __syncwarp();
       if (tid == 0) { bulk_store_obs(dst, buf, bytes); bulk_commit(); }
-      ++emitted;
     }
   }
 }
@@ -688,11 +678,7 @@ template <class F> struct MinBlocksPerSM { static const int value = 4; };       
 template <> struct MinBlocksPerSM<MemoryChain> { static const int value = 6; };   // <= 80
 template <> struct MinBlocksPerSM<Bandit> { static const int value = 8; };        // <= 64
 template <> struct MinBlocksPerSM<DiscountingChain> { static const int value = 8; };
-#ifdef BSB_MIN_BLOCKS_PER_SM   // build-time override for tuning experiments
-#define BSB_LAUNCH_MIN_BLOCKS(F) BSB_MIN_BLOCKS_PER_SM
-#else
 #define BSB_LAUNCH_MIN_BLOCKS(F) MinBlocksPerSM<typename FamilyOf<F>::type>::value
-#endif
 // System-scope accesses to the pinned mailbox (host memory over PCIe) and volatile accesses to its L2 relay.
 __device__ __forceinline__ unsigned long long ld_sys_u64(const volatile unsigned long long* ptr) {
   unsigned long long v; asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(ptr) : "memory"); return v;
@@ -762,7 +748,8 @@ __device__ __forceinline__ WarpStage<O> clear_stages(const EnvParams& p, const L
 
 // Caller-owned buffers of the launch: its arguments or -- pre-launched (doorbell) mode -- whatever the host wrote
 // into the mailbox before it rang this launch's ticket.  `cancelled`: the host stood the launch down, or nobody rang
-// before the timeout.  Every thread of the CTA calls it.
+// before DOORBELL_TIMEOUT_NS.  Every thread of the CTA calls it.
+static const unsigned long long DOORBELL_TIMEOUT_NS = 200000000ull;      // 200 ms
 __device__ __forceinline__ MailFields receive_doorbell(const LaunchArgs& a, bool& cancelled) {
   __shared__ MailFields mail_in;
   __shared__ int mail_cancel;
@@ -776,7 +763,7 @@ __device__ __forceinline__ MailFields receive_doorbell(const LaunchArgs& a, bool
     // before the doorbell, so this second read cannot be stale), parked in device memory, and the ticket is
     // relayed to the other blocks through L2.
     const volatile unsigned long long* line = &a.mailbox->doorbell;
-    const unsigned long long deadline = global_timer_ns() + a.doorbell_timeout_ns;
+    const unsigned long long deadline = global_timer_ns() + DOORBELL_TIMEOUT_NS;
     unsigned long long word = 0, seen;
     do {
       if (tid < 8) word = ld_sys_u64(line + tid);
@@ -896,7 +883,7 @@ __device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a
   } else if (kEmit == EMIT_IMAGE) {
     const int image = Descriptor<F>::a(L);
     if (bulk) emit_image_bulk(p, ws.stage, ws.cta_zero, obs_t, warp_base, n_lanes, K, active ? image : -1, a.group_lanes,
-                              a.cta_extra_elems / K, a.stage_rows, ws.emitted);
+                              a.cta_extra_elems / K);
     else emit_image(p, reinterpret_cast<const float*>(ws.stage), obs_t, warp_base, n_lanes, K, image, vec && (K & 3) == 0);
   } else if (!a.stage_rows) {
     // observation rows too long for a shared-memory stage: every thread renders its row in place.  Never taken by
@@ -1064,7 +1051,7 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
         else lane_step<Fam>(lp, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, io, off);
       }
       if constexpr (kSameStep) {
-        if (!a.mailbox && a.final_obs)
+        if (a.final_obs)
           emit_final<Fam>(p, a, ws, merged, reinterpret_cast<O*>(a.final_obs) + t * B * (int64_t)K, warp_base, n_lanes,
                           lane, active, a.final_vec_ok != 0, bulk);
       }

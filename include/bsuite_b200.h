@@ -333,7 +333,7 @@ int32_t bsb_read_episode_stats(bsb_env* env, int32_t field, double* dst,
  * counter (it indexes the on-device action stream and the Logging columns) and its chunk scheduler into device
  * memory, for good: replays and eager calls can then be mixed in any order, and bsb_steps_done / bsb_get_state
  * synchronise the device to read the counter back.  Consecutive captured steps keep their programmatic dependent
- * launch (it becomes a programmatic graph edge; BSB_GRAPH_PDL=0 turns that off).
+ * launch (it becomes a programmatic graph edge).
  * bsb_step_host (internal stream, host-side wait) cannot be captured.
  */
 
@@ -471,7 +471,7 @@ int32_t bsb_set_state(bsb_env* env, const void* src_host, int64_t nbytes,
  * When `actions` and the requested scalar outputs are PINNED host memory the
  * kernel accesses them in place over PCIe (zero-copy: no separate H2D / D2H
  * copies) and signals completion through a pinned mailbox word the host spins
- * on (no stream synchronise; BSB_HOST_SPIN=0 restores it); pageable buffers
+ * on (no stream synchronise); pageable buffers
  * take the staged-copy path.  Host actions are range-checked: an action outside
  * [0, num_actions) yields BSB_INVALID_ARGUMENT (the reference raises IndexError,
  * e.g. bandit.py:61).
@@ -489,8 +489,7 @@ int32_t bsb_set_state(bsb_env* env, const void* src_host, int64_t nbytes,
  *       decides its next action while the observations are still being written.  With this flag `caller_stream`
  *       is fenced (on the device) behind the step, so work enqueued there
  *       afterwards sees complete observations; without it, order a consumer by
- *       the next call on this handle (every entry point waits for the step) or
- *       set BSB_HOST_EARLY=0 to make the call wait for the whole kernel.
+ *       the next call on this handle (every entry point waits for the step).
  *       Same-step handles (BSB_FLAG_SAME_STEP_RESET) always run host steps in
  *       one phase.
  *   BSB_HOST_PRELAUNCH  (pinned buffers only) after ringing this step, the NEXT
@@ -498,8 +497,8 @@ int32_t bsb_set_state(bsb_env* env, const void* src_host, int64_t nbytes,
  *       and polls the mailbox doorbell, so the next call costs neither a launch
  *       nor a wake-up -- for agents whose policy runs on the HOST.  While it
  *       waits it occupies the SMs: other GPU work of the process queues behind it
- *       until the next call, bsb_host_flush, or BSB_DOORBELL_TIMEOUT_MS (default
- *       200) without a ring, after which it stands down by itself.  Every other
+ *       until the next call, bsb_host_flush, or 200 ms without a ring, after
+ *       which it stands down by itself.  Every other
  *       entry point of this handle stands it down first.
  *   BSB_HOST_NO_WAIT  (pinned buffers; otherwise the call is simply synchronous)
  *       the call returns once the step is enqueued; the host outputs are valid

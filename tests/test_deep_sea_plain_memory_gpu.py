@@ -14,7 +14,6 @@ import torch
 from bsuite_b200 import obs_memory
 from tests import test_cuda_graph_gpu as cg
 from tests import test_device_paths_gpu as dp
-from tests import test_full_size_gpu as fs
 from tests import test_obs_dtype_gpu as odg
 from tests import test_same_step_gpu as ss
 from tests.test_compressible_gpu import in_segments, pool_segments
@@ -87,8 +86,3 @@ def test_reduced_dtype_two_phase_host_steps_on_plain_memory(case_mode, image_dir
 def test_graph_replay_on_plain_memory(env_class, kwargs, batch, T, fused, mnist_dir, plain_observations):
   cg.test_replayed_graph_equals_eager_steps(env_class, kwargs, batch, T, fused, mnist_dir)
 
-
-@pytest.mark.parametrize('bsuite_id,batch', [('deep_sea/0', 100000), ('deep_sea/3', 70001), ('deep_sea/20', 20011),
-                                             ('deep_sea_stochastic/11', 40000)])
-def test_bulk_path_equals_vector_path_on_plain_memory(bsuite_id, batch, monkeypatch, plain_observations):
-  fs.test_deep_sea_bulk_path_equals_vector_path_at_scale(bsuite_id, batch, monkeypatch)

@@ -3,7 +3,8 @@
 The transition logic is one set of __host__ __device__ functions that the host path runs too.  What the CUDA side
 adds is how chunks of lanes are dealt to warps and how observations reach HBM: `device_launch` (bsb_dispatch.cuh)
 and `transition_kernel` (bsb_kernels.cuh) pick row stages, TMA bulk or vector stores, group sizes, CTA sizes and a
-persistent grid from the family, the batch, the observation size, T, the buffer alignment and the BSB_* knobs.
+persistent grid from the family, the batch, the observation size, T, the buffer alignment and the memory the
+buffer lies in.
 
 Every case creates the same environment twice, on the GPU and on the explicit host path (device='cpu': `host_run`,
 a plain per-lane loop that the golden and oracle tests pin to the reference), drives both through one script and
@@ -18,8 +19,8 @@ also go through oracle.run_lanes, which anchors the comparison outside the engin
   group A  every instantiation transition_kernel<family, Philox | MT19937, noise, track> once (80 kernels);
   group B  the paths the default dispatch selects, at batch sizes derived from its rules (margins quoted for the
            132 SMs of an H100 SXM);
-  group C  every non-default value of the tuning knobs still open to A/B runs, read from the environment when a
-           handle is created;
+  group C  the CTA sizes, deep_sea group sizes, vector fallbacks and mnist group sizes that only larger boards,
+           tiles and images reach;
   group H  every instantiation two_phase_host_kernel<deep_sea | catch, Philox | MT19937, noise, track> (16 kernels),
            driven by host steps (bsb_step_host on pinned buffers): waited for, pre-launched, and BSB_HOST_NO_WAIT
            (which splits the step over two launches).
@@ -55,7 +56,7 @@ STATE_RTOL = 1e-9
 # ------------------------------------------------------------------ cases
 def _case(family, batch, kwargs=None, **over):
   case = dict(family=family, kwargs=dict(kwargs or {}), batch=int(batch), rng='philox', noise=None, track=False,
-              seed=7, lane_offset=0, reward_dtype='float64', knobs={}, misalign=False,
+              seed=7, lane_offset=0, reward_dtype='float64', misalign=False,
               t_caller=3, t_sampled=3, n_steps=2, n_more=2)
   case.update(over)
   return case
@@ -74,7 +75,6 @@ def _case_id(case):
     parts.append(f"offset{case['lane_offset']}")
   if case['misalign']:
     parts.append('misaligned')
-  parts += [f'{k[4:]}={v}' for k, v in sorted(case['knobs'].items())]
   return '-'.join(parts)
 
 
@@ -178,30 +178,20 @@ GROUP_H = [(_case(f, 97, H_KWARGS[f], rng=r, noise=0.1 if n else None, track=t,
 GROUP_H += [(_case('deep_sea', 30001, H_KWARGS['deep_sea'], track=True), mode) for mode in HOST_MODES]
 
 
-def _knob(family, batch, kwargs=None, **knobs):
-  over = dict(t_caller=2, t_sampled=2) if batch > 50000 or family == 'mnist' and batch > 20000 else {}
-  return _case(family, batch, kwargs, knobs={k: str(v) for k, v in knobs.items()}, **over)
-
-
-ROWS = ('umbrella_chain', 1000, dict(UMB, n_distractor=100))
-CATCH = ('catch', 1000, {})
-MNIST = ('mnist', 5001, dict(images=28))
-GROUP_C = (
-    # lanes per chunk: rows, boards, and deep_sea (K = 225, B = 20 004: persistent at both sizes)
-    [_knob(*c, BSB_CHUNK_LANES=n) for c in (ROWS, CATCH, ('deep_sea', 20004, dict(DS, size=15))) for n in (8, 16)]
-    # CTA size (128: 52 KB of row stages, over the 48 KB default limit)
-    + [_knob(*c, BSB_BLOCK_THREADS=n) for c in (ROWS, CATCH, ('mnist', 3001, dict(images=26))) for n in (32, 128)]
-    # lanes per deep_sea bulk store; N = 32 (default 8; 16 = 128 KB of stages: vector stores), N = 33 (K odd)
-    + [_knob('deep_sea', b, dict(DS, size=n), BSB_DEEP_SEA_GROUP=g) for n, b in ((32, 3001), (33, 3004))
-       for g in (1, 2, 4, 16)]
-    # vector stores instead of TMA bulk stores
-    + [_knob(*c, BSB_EMIT_BULK=0) for c in (ROWS, ('mountain_car', 1000, {}), CATCH, MNIST)]
-    # mnist staging
-    + [_knob(*MNIST, BSB_IMAGE_STAGES=2), _knob('mnist', 40001, dict(images=28), BSB_IMAGE_STAGES=2),
-       _knob(*MNIST, BSB_IMAGE_GROUP=1), _knob(*MNIST, BSB_IMAGE_GROUP=2)]
-    # single steps without programmatic dependent launch
-    + [_knob(*c, BSB_PDL=0) for c in (ROWS, CATCH, ('deep_sea', 5000, dict(DS, size=10)), ('mnist', 1001, dict(images=28)))]
-)
+# group C: f32 deep_sea groups are the largest power of two <= 16 lanes with one store <= 40 KB (plan_launch); a group
+# whose store is not a multiple of 16 bytes (odd K needs m % 4 == 0), or whose two stages exceed 100 KB, takes the
+# vector path.  mnist groups of m <= 4 tiles and mz <= 8 zero tiles are halved until they fit 28 KB.
+GROUP_C = [
+    _case('catch', 1000, dict(rows=20, columns=20)),       # K = 400: 50 KB of boards per warp -> 32-thread CTAs
+    _case('deep_sea', 3001, dict(DS, size=80)),            # 25.6 KB tiles: m = 1
+    _case('deep_sea', 3001, dict(DS, size=64)),            # 16 KB tiles: m = 2
+    _case('deep_sea', 3001, dict(DS, size=50)),            # 10 KB tiles: m = 4 (40 KB stores)
+    _case('deep_sea', 3004, dict(DS, size=45)),            # K = 2 025 odd: m = 4 (32.4 KB stores); tail 28 % 4 == 0
+    _case('deep_sea', 3004, dict(DS, size=51)),            # K = 2 601 odd: m = 2, 20 808-byte stores: vector path
+    _case('deep_sea', 1000, dict(DS, size=120), t_caller=2, t_sampled=2),   # m = 1, 2 x 57.6 KB > 100 KB: vector path
+    _case('mnist', 5001, dict(images=48)),                 # 9 KB tiles: m = 2, mz = 2; 8-lane chunks, 128-thread CTAs
+    _case('mnist', 5001, dict(images=64)),                 # 16 KB tiles: m = 1, mz = 1
+]
 
 
 # ------------------------------------------------------------------ comparison
@@ -410,10 +400,7 @@ class Twins:
                 context=self.context)
 
 
-def drive(case, image_dirs, devices=('cuda', 'cpu'), monkeypatch=None):
-  if monkeypatch is not None:
-    for name, value in case['knobs'].items():
-      monkeypatch.setenv(name, value)
+def drive(case, image_dirs, devices=('cuda', 'cpu')):
   twins = Twins(case, devices, image_dirs)
   try:
     twins.run_script()
@@ -438,9 +425,10 @@ def _write_idx(directory, images):
 
 @pytest.fixture(scope='module')
 def image_dirs(tmp_path_factory):
-  """idx files of 28 x 28 (the table-free TMA path), 26 x 26 and 27 x 27 (the table path) images; every byte value."""
+  """idx files of 28 x 28, 48 x 48 and 64 x 64 (the table-free TMA path), 26 x 26 and 27 x 27 (the table path)
+  images; every byte value."""
   dirs = {}
-  for side in (28, 26, 27):
+  for side in (28, 26, 27, 48, 64):
     path = str(tmp_path_factory.mktemp(f'mnist_{side}'))
     images = np.random.RandomState(side).randint(0, 256, size=(64, side, side))
     images.reshape(64, -1)[:, :256] = np.arange(256)
@@ -531,8 +519,8 @@ def test_default_dispatch_paths_match_the_host_path(case, image_dirs):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('case', GROUP_C, ids=_case_id)
-def test_tuning_knobs_match_the_host_path(case, image_dirs, monkeypatch):
-  drive(case, image_dirs, monkeypatch=monkeypatch)
+def test_large_tile_and_board_paths_match_the_host_path(case, image_dirs):
+  drive(case, image_dirs)
 
 
 @pytest.mark.gpu

@@ -11,6 +11,7 @@ import pytest
 import torch
 
 import bsuite_b200
+from bsuite_b200 import obs_memory
 from oracle import bsuite_oracle as oracle
 
 pytestmark = pytest.mark.gpu
@@ -124,18 +125,27 @@ def test_float_dynamics_full_batch(bsuite_id, env_class, kwargs):
 
 @pytest.mark.parametrize('bsuite_id,batch', [('deep_sea/0', 100000), ('deep_sea/3', 70001), ('deep_sea/20', 20011),
                                              ('deep_sea_stochastic/11', 40000)])
-def test_deep_sea_bulk_path_equals_vector_path_at_scale(bsuite_id, batch, monkeypatch):
-  """Large (and ragged) batches take the persistent TMA bulk-store path; it must agree bit for bit with the plain
-  16-byte-store path on every lane, for fused rollouts and for single-step launches (PDL + chunk counter)."""
+def test_deep_sea_bulk_path_equals_vector_path_at_scale(bsuite_id, batch):
+  """Large (and ragged) batches written into plain `torch.empty` memory take the persistent TMA bulk-store path;
+  written into the compressible pool (`make_buffers`, >= 4 chunks per SM) they take 16-byte streaming stores.  The
+  two must agree bit for bit on every lane, for fused rollouts and for single-step launches (PDL + chunk counter)."""
+  if not (obs_memory.info(0)[0] and obs_memory.pool(0) is not None):
+    pytest.skip('this device grants no compressible memory: both legs would take the bulk path')
   results = []
-  for bulk in ('0', '1'):
-    monkeypatch.setenv('BSB_DEEP_SEA_BULK', bulk)
+  for plain in (True, False):
     env = bsuite_b200.load_from_id(bsuite_id, batch=batch, device='cuda', seed=11, reward_dtype='float64')
-    ts = env.rollout(12, action_seed=4)
+
+    def buffers(num_steps=None):
+      out = env.make_buffers(num_steps)
+      if plain:
+        out.observation = torch.empty(out.observation.shape, dtype=out.observation.dtype, device='cuda')
+      return out
+
+    ts = env.rollout(12, action_seed=4, out=buffers(12))
     got = [ts.step_type.clone(), ts.reward.clone(), ts.observation.clone()]
     more = torch.as_tensor(env.random_actions(5, action_seed=4))
     for k in range(5):
-      one = env.step(more[k])
+      one = env.step(more[k], out=buffers())
       got += [one.observation.clone(), one.reward.clone()]
     got += [v.clone() for v in env.bsuite_info().values()]
     results.append(got)

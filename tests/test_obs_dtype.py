@@ -174,15 +174,22 @@ class DtypeTwins:
       env.reset(out=out)
     self.check_call('reset()', outs, 0)
 
-  def step_host(self, mode, with_observation=False):
-    """One host step per twin; `with_observation`: the observation is copied to pinned host memory as well (the
-    staged copies of bsb_step_host), and that copy must equal the device observation."""
+  def step_host(self, mode, with_observation=False, pageable=False):
+    """One host step per twin; `with_observation`: the observation is copied to host memory as well, and that copy
+    must equal the device observation.  `pageable`: actions and host outputs in plain (not pinned) host memory, so
+    that bsb_step_host takes its staged copies.  The device observation is misaligned as the case says."""
     acts = self.rng.randint(self.envs[0].num_actions, size=self.case['batch']).astype(np.int32)
     outs = []
     for env in self.envs:
-      host, out = env.make_host_buffers(with_observation=with_observation), env.make_buffers()
+      host = env.make_host_buffers(with_observation=with_observation)
+      if pageable:
+        host = type(host)(**{f: None if getattr(host, f) is None else torch.empty(getattr(host, f).shape,
+                                                                                    dtype=getattr(host, f).dtype)
+                             for f in ('observation', 'reward', 'discount', 'step_type')})
+      out = buffers(env, None, False, self.case['misalign'])
       actions = torch.from_numpy(acts)
-      env.step_host(actions.pin_memory() if env.device.type == 'cuda' else actions, host, out=out,
+      pin = env.device.type == 'cuda' and not pageable
+      env.step_host(actions.pin_memory() if pin else actions, host, out=out,
                     prelaunch=mode == 'prelaunch', wait=mode != 'no_wait')
       if mode == 'no_wait':
         env.host_wait()
@@ -207,10 +214,7 @@ class DtypeTwins:
     self.check_state('end of script')
 
 
-def drive(c, image_dirs, device='cuda', monkeypatch=None):
-  if monkeypatch is not None:
-    for name, value in c['knobs'].items():
-      monkeypatch.setenv(name, value)
+def drive(c, image_dirs, device='cuda'):
   twins = DtypeTwins(c, device, image_dirs)
   try:
     twins.run_script()

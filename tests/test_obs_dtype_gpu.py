@@ -8,9 +8,9 @@ ulp).
 
   group A  transition_kernel<ObsAs<family, Bf16 | uint8_t>, Philox, noise, track> (48 kernels) at B = 97;
   group B  dispatch paths whose rules count bytes: group sizes, tails, stages, alignment;
-  group C  the non-default values of the launch-geometry and store knobs still open to A/B runs, for uint8 deep_sea
-           and bfloat16 catch;
-  group H  two_phase_host_kernel<ObsAs<deep_sea | catch, Bf16 | uint8_t>, Philox, noise, track> (16 kernels).
+  group C  uint8 deep_sea group sizes that only larger tiles reach;
+  group H  two_phase_host_kernel<ObsAs<deep_sea | catch, Bf16 | uint8_t>, Philox, noise, track> (16 kernels), and
+           the other host-step paths: staged copies, synchronised steps.
 """
 
 import itertools
@@ -88,22 +88,15 @@ GROUP_B = [
 ]
 
 
-def _knob(family, batch, kwargs, obs_dtype, **knobs):
-  over = dict(t_caller=2, t_sampled=2) if batch > 50000 else {}
-  return case(family, batch, kwargs, obs_dtype=obs_dtype, knobs={k: str(v) for k, v in knobs.items()}, **over)
-
-
-DS_U8 = ('deep_sea', 3001, dict(DS, size=32), 'uint8')
-CATCH_BF16 = ('catch', 1000, {}, 'bfloat16')
-GROUP_C = (
-    [_knob(*c, BSB_CHUNK_LANES=n) for c in (DS_U8, CATCH_BF16, ('deep_sea', 20004, dict(DS, size=15), 'uint8'))
-     for n in (8, 16)]
-    + [_knob(*c, BSB_BLOCK_THREADS=n) for c in (DS_U8, CATCH_BF16) for n in (32, 128)]
-    + [_knob(*DS_U8, BSB_DEEP_SEA_GROUP=g) for g in (1, 2, 4, 8, 32)]
-    + [_knob('deep_sea', 3004, dict(DS, size=33), 'uint8', BSB_DEEP_SEA_GROUP=g) for g in (4, 16)]
-    + [_knob(*DS_U8, BSB_DEEP_SEA_BULK=0), _knob(*CATCH_BF16, BSB_EMIT_BULK=0)]
-    + [_knob(*c, BSB_PDL=0) for c in (DS_U8, CATCH_BF16)]
-)
+# group C: uint8 deep_sea groups (1-byte cells: m lanes of N * N bytes, m <= 16, one store <= 40 KB); a group whose
+# store is not a multiple of 16 bytes takes the vector path (odd K: every m < 16)
+GROUP_C = [
+    case('deep_sea', 1000, dict(DS, size=144), obs_dtype='uint8'),      # 20.25 KB tiles: m = 1
+    case('deep_sea', 1000, dict(DS, size=104), obs_dtype='uint8'),      # 10.6 KB tiles: m = 2
+    case('deep_sea', 3001, dict(DS, size=80), obs_dtype='uint8'),       # 6.25 KB tiles: m = 4
+    case('deep_sea', 3001, dict(DS, size=64), obs_dtype='uint8'),       # 4 KB tiles: m = 8
+    case('deep_sea', 3004, dict(DS, size=51), obs_dtype='uint8'),       # K = 2 601 odd: m = 8, 20 808 bytes: vector path
+]
 
 H_KWARGS = dp.H_KWARGS
 GROUP_H = [(case(f, 97, H_KWARGS[f], obs_dtype=d, noise=0.1 if n else None, track=t,
@@ -113,21 +106,18 @@ GROUP_H = [(case(f, 97, H_KWARGS[f], obs_dtype=d, noise=0.1 if n else None, trac
 GROUP_H += [(case('deep_sea', 30001, H_KWARGS['deep_sea'], obs_dtype='uint8', track=True), mode) for mode in dp.HOST_MODES]
 
 
-# host-step knobs (read when a handle is created) for uint8 deep_sea and bfloat16 catch: (knobs, mode, observation
-# copied to the host as well).  BSB_ZERO_COPY=0 takes the staged path (device scratch sized in bytes, staged copies);
-# a host observation turns the zero-copy path's mailbox off (bsb_step + a copy); BSB_HOST_SPLIT=0 runs a
-# BSB_HOST_NO_WAIT step as one launch instead of two.
-HOST_KNOBS = [({}, 'wait', True), (dict(BSB_ZERO_COPY=0), 'wait', True), (dict(BSB_ZERO_COPY=0), 'wait', False),
-              (dict(BSB_HOST_SPIN=0), 'wait', False), (dict(BSB_HOST_EARLY=0), 'wait', False),
-              (dict(BSB_HOST_STAGE_ACTIONS=0), 'wait', False), (dict(BSB_HOST_SPLIT=0), 'no_wait', False)]
-GROUP_HK = [(case(f, 1001, H_KWARGS[f], obs_dtype=d, track=True, knobs={k: str(v) for k, v in knobs.items()}), mode,
-             with_obs)
-            for f, d in (('deep_sea', 'uint8'), ('catch', 'bfloat16')) for knobs, mode, with_obs in HOST_KNOBS]
+# other host-step paths of uint8 deep_sea and bfloat16 catch: (observation copied to the host as well, pageable host
+# memory, misaligned device observation).  A host observation turns the zero-copy path's mailbox off (bsb_step + a
+# copy and a stream synchronise), pageable buffers take the staged copies (device scratch sized in bytes), and a
+# misaligned device observation takes the synchronise as well.
+HOST_PATHS = [(True, False, False), (True, True, False), (False, True, False), (False, False, True)]
+GROUP_HK = [(case(f, 1001, H_KWARGS[f], obs_dtype=d, track=True, misalign=misalign), with_obs, pageable)
+            for f, d in (('deep_sea', 'uint8'), ('catch', 'bfloat16')) for with_obs, pageable, misalign in HOST_PATHS]
 
 
-def _hk_id(case_mode_obs):
-  c, mode, with_obs = case_mode_obs
-  return f'{case_id(c)}-{mode}' + ('-host_obs' if with_obs else '')
+def _hk_id(case_obs_pageable):
+  c, with_obs, pageable = case_obs_pageable
+  return case_id(c) + ('-host_obs' if with_obs else '') + ('-pageable' if pageable else '')
 
 
 def _h_id(case_mode):
@@ -148,8 +138,8 @@ def test_reduced_dtype_dispatch_paths(c, image_dirs):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('c', GROUP_C, ids=case_id)
-def test_reduced_dtype_tuning_knobs(c, image_dirs, monkeypatch):
-  od.drive(c, image_dirs, monkeypatch=monkeypatch)
+def test_reduced_dtype_large_tile_paths(c, image_dirs):
+  od.drive(c, image_dirs)
 
 
 @pytest.mark.gpu
@@ -170,33 +160,27 @@ def test_reduced_dtype_two_phase_host_kernel(case_mode, image_dirs):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('case_mode_obs', GROUP_HK, ids=_hk_id)
-def test_reduced_dtype_host_step_knobs(case_mode_obs, image_dirs, monkeypatch):
-  c, mode, with_obs = case_mode_obs
-  for name, value in c['knobs'].items():
-    monkeypatch.setenv(name, value)
+@pytest.mark.parametrize('case_obs_pageable', GROUP_HK, ids=_hk_id)
+def test_reduced_dtype_host_step_paths(case_obs_pageable, image_dirs):
+  c, with_obs, pageable = case_obs_pageable
   twins = od.DtypeTwins(c, 'cuda', image_dirs)
   try:
     for _ in range(3):
-      twins.step_host(mode, with_observation=with_obs)
+      twins.step_host('wait', with_observation=with_obs, pageable=pageable)
     twins.step()
     for _ in range(3):
-      twins.step_host(mode, with_observation=with_obs)
+      twins.step_host('wait', with_observation=with_obs, pageable=pageable)
     twins.check_state('end of script')
   finally:
     twins.close()
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('family,kwargs,dtype,knobs', [('deep_sea', dict(DS, size=32), 'uint8', {}),
-                                                       ('catch', {}, 'bfloat16', {}),
-                                                       ('mnist', dict(images=28), 'bfloat16', {}),
-                                                       ('deep_sea', dict(DS, size=32), 'uint8', dict(BSB_GRAPH_PDL='0')),
-                                                       ('catch', {}, 'bfloat16', dict(BSB_GRAPH_PDL='0'))])
+@pytest.mark.parametrize('family,kwargs,dtype', [('deep_sea', dict(DS, size=32), 'uint8'),
+                                                 ('catch', {}, 'bfloat16'),
+                                                 ('mnist', dict(images=28), 'bfloat16')])
 @pytest.mark.parametrize('fused', [False, True])
-def test_graph_replay_equals_an_uncaptured_twin(family, kwargs, dtype, knobs, fused, image_dirs, monkeypatch):
-  for name, value in knobs.items():
-    monkeypatch.setenv(name, value)
+def test_graph_replay_equals_an_uncaptured_twin(family, kwargs, dtype, fused, image_dirs):
   c = case(family, 4099, kwargs, obs_dtype=dtype)
   env, twin = (od.make(c, 'cuda', image_dirs, dtype) for _ in range(2))
   try:

@@ -146,7 +146,7 @@ def test_host_driven_steps_through_the_mailbox_equal_ordinary_steps(bsuite_id, p
       got_obs = got.observation
     else:
       if t == 20 and prelaunch:
-        time.sleep(0.35)                     # > BSB_DOORBELL_TIMEOUT_MS: the queued launch gives up, the step still happens
+        time.sleep(0.35)                     # > the 200 ms doorbell timeout: the queued launch gives up, the step still happens
       got, got_obs = b.step_host(actions[t], host, out=outs[t % 2], prelaunch=prelaunch)
     tol = cf.FLOAT_TOL if bsuite_id.startswith('cartpole') else 0
     for field in ('step_type', 'reward', 'discount'):

@@ -4,10 +4,9 @@
     python tools/e2e_breakdown.py [bsuite_id] [batch]
 
 Rows: the kernel rate (launches queued), a device-resident loop that synchronises after every step, then the
-host-buffer call `BatchedEnvironment.step_host` (pinned actions in, pinned scalars out) in its variants:
-stream synchronise (BSB_HOST_SPIN=0), mailbox completion, two-phase (scalars first), pre-launched doorbell
-kernels -- each through the Python face and through bare ctypes calls with prebuilt arguments (what a C caller
-of the ABI pays).
+host-buffer call `BatchedEnvironment.step_host` (pinned actions in, pinned scalars out) -- two-phase (scalars
+first), with and without pre-launched doorbell kernels, each through the Python face and through bare ctypes calls
+with prebuilt arguments (what a C caller of the ABI pays) -- and its staged copies from pageable buffers.
 """
 import ctypes
 import os
@@ -22,15 +21,6 @@ from bsuite_b200 import _lib
 
 BSUITE_ID = sys.argv[1] if len(sys.argv) > 1 else 'deep_sea/11'
 B = int(sys.argv[2]) if len(sys.argv) > 2 else 65536
-
-
-def make(**env_vars):
-  for k, v in env_vars.items():
-    os.environ[k] = v
-  env = bsuite_b200.load_from_id(BSUITE_ID, batch=B, device='cuda', seed=0, track_episodes=True)
-  for k in env_vars:
-    os.environ.pop(k)
-  return env
 
 
 def timed(fn, n=300, after=None):
@@ -48,7 +38,7 @@ def timed(fn, n=300, after=None):
   return (time.perf_counter() - t0) / n * 1e6
 
 
-env = make()
+env = bsuite_b200.load_from_id(BSUITE_ID, batch=B, device='cuda', seed=0, track_episodes=True)
 ring = [env.make_buffers() for _ in range(4)]
 n_act = env.num_actions
 dev_acts = torch.randint(0, n_act, (64, B), device='cuda', dtype=torch.int32)
@@ -82,9 +72,8 @@ def variants(e, label):
     print(f'step_host {label:34s} prelaunch={int(prelaunch)}  python {py:6.1f}  ctypes {raw:6.1f} us/step')
 
 
-variants(make(BSB_HOST_SPIN='0'), 'stream synchronise (round 1)')
-variants(make(BSB_HOST_EARLY='0'), 'mailbox completion')
-variants(make(), 'mailbox + two-phase (default)')
-os.environ['BSB_ZERO_COPY'] = '0'
-env2 = bsuite_b200.load_from_id(BSUITE_ID, batch=B, device='cuda', seed=0, track_episodes=True)
-print(f'step_host staged copies (BSB_ZERO_COPY=0)                {timed(lambda i: env2.step_host(prow[i % 64], host, out=ring[i % 4])):7.1f} us/step')
+variants(env, 'mailbox + two-phase')
+page = [torch.empty(B, dtype=torch.int32).copy_(row) for row in prow[:4]]      # pageable host memory
+page_host = type(host)(**{f: torch.empty(getattr(host, f).shape, dtype=getattr(host, f).dtype)
+                          for f in ('reward', 'discount', 'step_type')})
+print(f'step_host staged copies (pageable buffers)               {timed(lambda i: env.step_host(page[i % 4], page_host, out=ring[i % 4])):7.1f} us/step')

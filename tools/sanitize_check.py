@@ -52,19 +52,30 @@ if '--only-split' in sys.argv:
   print('sanitize workload (split steps) finished')
   sys.exit(0)
 
+def buffers(env, bsuite_id, plain, num_steps=None):
+  """Bulk stores land in `plain` torch.empty memory; the other leg writes where the store path changes: the
+  compressible pool (make_buffers) for deep_sea, whose large batches then take 16-byte streaming stores, and an
+  observation one float past a 16-byte boundary (vector / scalar stores) for every other family."""
+  out = env.make_buffers(num_steps)
+  n = out.observation.numel()
+  if plain:
+    out.observation = torch.empty(out.observation.shape, device='cuda')
+  elif not bsuite_id.startswith('deep_sea'):
+    out.observation = torch.empty(n + 4, device='cuda')[1:n + 1].view(out.observation.shape)
+  return out
+
+
 for bsuite_id, batch in (('deep_sea/11', 20000), ('deep_sea_stochastic/3', 40001), ('catch_noise/0', 5000), ('cartpole/0', 3000),
                          ('umbrella_length/3', 2000), ('umbrella_distract/22', 1500), ('mnist/0', 1500), ('mnist/0', 30000)):
   if bsuite_id.startswith('mnist'):
     from bsuite_b200 import datasets
     os.environ[datasets.ENV_VAR] = datasets.write_synthetic_mnist('/tmp/bsb_sanitize_mnist', 256, 16, 0)
   results = []
-  for bulk in ('1', '0'):
-    os.environ['BSB_DEEP_SEA_BULK'] = bulk
-    os.environ['BSB_EMIT_BULK'] = bulk
+  for plain in (True, False):
     env = bsuite_b200.load_from_id(bsuite_id, batch=batch, device='cuda', seed=3, track_episodes=True)
     acts = torch.as_tensor(env.random_actions(4, action_seed=1, first_step=0)).cuda()
-    outs = [env.step(acts[i]).observation.clone() for i in range(4)]
-    ts = env.rollout(3, action_seed=2)
+    outs = [env.step(acts[i], out=buffers(env, bsuite_id, plain)).observation.clone() for i in range(4)]
+    ts = env.rollout(3, action_seed=2, out=buffers(env, bsuite_id, plain, 3))
     results.append(outs + [ts.observation.clone(), ts.reward.clone(), ts.step_type.clone()])
     torch.cuda.synchronize()
     env.close()
