@@ -48,7 +48,7 @@ void host_run(const EnvParams& p, const LaunchArgs& a) {
   std::vector<float> f32(std::is_same<O, float>::value ? 0 : (size_t)K);
   const bool noise = p.wrapper == BSB_WRAP_REWARD_NOISE && a.mode != MODE_INIT;
   const bool track = p.ep != nullptr && a.mode != MODE_INIT;
-  const MailFields out = {a.actions, a.obs, a.reward, a.reward_f64, a.discount, a.step_type, 0, 0};
+  const MailFields out = {a.reward, a.reward_f64, a.discount, a.step_type};
   EnvParams setting_p;                    // packed handles: p with the current lane's setting
   auto render = [&](const EnvParams& lp, const typename F::Lane& L, R& rng, O* dst) {
     if constexpr (std::is_same<O, float>::value) {

@@ -214,7 +214,7 @@ inline void cpu_relax() {
 #endif
 }
 
-// ---- host-driven steps: mailbox completion and pre-launched doorbell kernels --------------------------------
+// ---- host-driven steps: completion through the mailbox ------------------------------------------------------
 int mailbox_open(bsb_env* e) {
   if (e->mailbox) return BSB_OK;
   void* host = nullptr; void* dev = nullptr;
@@ -228,8 +228,6 @@ int mailbox_open(bsb_env* e) {
   return BSB_OK;
 }
 
-// Enqueues one single-step launch that signals `ticket` through the mailbox.  wait_doorbell: the launch takes its
-// buffers from the mailbox once the host rings `ticket` (pre-launch); otherwise from `fields` right away.
 // Two-phase host steps pay off where the observation stream is long next to the scalar traffic over PCIe (12 B per
 // lane out, 4 B in): deep_sea from N = 16 up (>= 1 KB of observation per lane).  catch (200 B per lane) is bound
 // by the 2 MB of scalars per step either way and keeps the single-phase kernel.  The rule counts float32 bytes
@@ -239,12 +237,11 @@ bool family_obs_from_state(const bsb_env* e) {
   return !e->same_step && !e->packed && (e->p.family == BSB_DEEP_SEA || e->p.family == BSB_CATCH) && (size_t)e->p.obs_numel * sizeof(float) >= 1024;
 }
 
-int mailbox_launch(bsb_env* e, unsigned long long ticket, int64_t step0, const MailFields* fields, bool wait_doorbell, bool split = false) {
-  const bsb_outputs out = fields ? bsb_outputs{fields->obs, fields->reward, fields->reward_f64, fields->discount, fields->step_type, nullptr}
-                                : bsb_outputs{};
-  LaunchArgs a = make_args(e, fields ? &out : nullptr, fields ? fields->actions : nullptr, 1, MODE_STEP);
-  a.step0 = step0;
-  a.mailbox = e->mailbox_dev; a.mail = e->mail; a.ticket = ticket; a.wait_doorbell = wait_doorbell ? 1 : 0;
+// Enqueues the step of `actions` into the device-addressable buffers `out`, which signals `ticket` through the
+// mailbox.  `split`: BSB_HOST_NO_WAIT.
+int mailbox_launch(bsb_env* e, unsigned long long ticket, const int32_t* actions, const bsb_outputs& out, bool split) {
+  LaunchArgs a = make_args(e, &out, actions, 1, MODE_STEP);
+  a.mailbox = e->mailbox_dev; a.mail = e->mail; a.ticket = ticket;
   { static const int timing = getenv("BSB_HOST_TIMING") ? atoi(getenv("BSB_HOST_TIMING")) : 0; a.timing = timing; }
   if (!family_obs_from_state(e)) return run(e, a, e->copy_stream);
   // device staging of the scalars: reward | discount | step_type in one block (as the staged-copy path keeps them)
@@ -259,7 +256,7 @@ int mailbox_launch(bsb_env* e, unsigned long long ticket, int64_t step0, const M
   memset(&h, 0, sizeof(h));
   h.stage.reward = e->d_reward; h.stage.reward_f64 = e->d_reward64; h.stage.discount = e->d_discount; h.stage.step_type = e->d_step_type;
   e->early_inflight = true;
-  if (split && !wait_doorbell) {
+  if (split) {
     // BSB_HOST_NO_WAIT: the caller alternates between handles.  Two launches instead of one -- transitions + copiers
     // (no shared memory), then the observation stream -- so that THIS handle's transitions and PCIe traffic run
     // while the OTHER handle's observations have the SMs' shared memory and the HBM.
@@ -273,56 +270,39 @@ int mailbox_launch(bsb_env* e, unsigned long long ticket, int64_t step0, const M
 }
 
 // Spins on the mailbox until `ticket` is done (the kernel's last CTA stores it after a system-scope fence).
-int mailbox_wait(bsb_env* e, unsigned long long ticket, bool* cancelled) {
+int mailbox_wait(bsb_env* e, unsigned long long ticket) {
   const auto start = std::chrono::steady_clock::now();
-  unsigned long long seen;
   uint32_t spins = 0;
-  while (((seen = e->mailbox->done) & ~MAIL_CANCEL) < ticket) {
+  while (e->mailbox->done < ticket) {
     cpu_relax();
     if ((++spins & 0xfffffu) == 0 && std::chrono::steady_clock::now() - start > std::chrono::seconds(20)) {
       cudaError_t err = cudaStreamSynchronize(e->copy_stream);      // a faulted kernel never signals: surface its error
       if (err != cudaSuccess) return fail(BSB_CUDA_ERROR, std::string("host step: ") + cudaGetErrorString(err));
-      if ((e->mailbox->done & ~MAIL_CANCEL) >= ticket) { seen = e->mailbox->done; break; }
+      if (e->mailbox->done >= ticket) break;
       return fail(BSB_INTERNAL, "host step: the kernel finished without signalling the mailbox");
     }
   }
   std::atomic_thread_fence(std::memory_order_acquire);
-  *cancelled = (seen & MAIL_CANCEL) != 0;
   return BSB_OK;
 }
 
 // Collects a step issued with BSB_HOST_NO_WAIT: spins until its completion word is in and counts the step.
+// Every entry point that enqueues work for this handle or reads its state calls this first.
 int finish_awaited(bsb_env* e) {
   if (!e || e->device < 0 || !e->awaiting_ticket) return BSB_OK;
   const unsigned long long ticket = e->awaiting_ticket;
   e->awaiting_ticket = 0;
-  bool cancelled = false;
-  int rc = mailbox_wait(e, ticket, &cancelled);
+  int rc = mailbox_wait(e, ticket);
   if (rc != BSB_OK) return rc;
   e->steps_done += 1;
   return BSB_OK;
-}
-
-// Stands down the pre-launched launch, if any: rings its ticket with the cancel bit and waits for it to leave
-// (and collects a BSB_HOST_NO_WAIT step nobody waited for).
-// Every entry point that enqueues work for this handle or reads its state calls this first.
-int flush_pending(bsb_env* e) {
-  { int arc = finish_awaited(e); if (arc != BSB_OK) return arc; }
-  if (!e || e->device < 0 || !e->pending_ticket) return BSB_OK;
-  DeviceGuard guard(e->device);
-  const unsigned long long ticket = e->pending_ticket;
-  e->pending_ticket = 0;
-  std::atomic_thread_fence(std::memory_order_release);
-  e->mailbox->doorbell = ticket | MAIL_CANCEL;
-  bool cancelled = false;
-  return mailbox_wait(e, ticket, &cancelled);
 }
 
 // Two-phase host steps return when the scalars have landed; the observation stores of the latest one may still
 // be in flight on the handle's stream.  Anything that leaves that stream (work on a caller's stream, state reads,
 // destruction) waits for it here.
 int drain_host_steps(bsb_env* e) {
-  int rc = flush_pending(e);
+  int rc = finish_awaited(e);
   if (rc != BSB_OK) return rc;
   if (e && e->device >= 0 && e->early_inflight) {
     DeviceGuard guard(e->device);
@@ -454,7 +434,7 @@ static int32_t create_env(const bsb_config* config, int64_t batch, int32_t devic
   e->num_sms = 132;
   if (device >= 0) { int n = 0; if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) == cudaSuccess && n > 0) e->num_sms = n; }
   e->order_event = nullptr; e->fence_event = nullptr; e->bad_action_host = nullptr; e->bad_action_dev = nullptr;
-  e->mailbox = nullptr; e->mailbox_dev = nullptr; e->mail = nullptr; e->next_ticket = 0; e->pending_ticket = 0; e->awaiting_ticket = 0;
+  e->mailbox = nullptr; e->mailbox_dev = nullptr; e->mail = nullptr; e->next_ticket = 0; e->awaiting_ticket = 0;
   e->h2d_stream = nullptr; e->h2d_event = nullptr;
   e->early_inflight = false;
   e->h2d_actions = nullptr; e->d_reward = nullptr; e->d_reward64 = nullptr; e->d_discount = nullptr; e->d_step_type = nullptr; e->d_obs = nullptr;
@@ -683,7 +663,7 @@ static void advance_steps(bsb_env* env, int64_t n) { if (!env->graph_safe) env->
 
 int32_t bsb_steps_done(const bsb_env* env, int64_t* steps) {
   if (!env || !steps) return fail(BSB_INVALID_ARGUMENT, "null argument");
-  int rc = current_steps(env, steps);     // a pre-launched host step (if any) has not been counted: it is for step steps_done
+  int rc = current_steps(env, steps);
   if (rc == BSB_OK && env->awaiting_ticket) *steps += 1;      // a BSB_HOST_NO_WAIT step has been issued: it counts
   return rc;
 }
@@ -931,7 +911,7 @@ int32_t bsb_host_timing(bsb_env* env, uint64_t* stamps8) {
 
 int32_t bsb_host_flush(bsb_env* env) {
   if (!env) return fail(BSB_INVALID_ARGUMENT, "null argument");
-  return flush_pending(env);
+  return finish_awaited(env);
 }
 
 // Reports (and clears) an out-of-range action seen by the kernels of a synchronous host step.
@@ -989,94 +969,62 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
                           (!host_out->discount || d_discount) && (!host_out->step_type || d_step_type);
   if (all_mapped) {
     if (!device_obs && !env->d_obs) BSB_CUDA(cudaMalloc(&env->d_obs, obs_bytes));
-    MailFields f;
-    memset(&f, 0, sizeof(f));
-    f.actions = static_cast<const int32_t*>(d_actions);
-    f.obs = device_obs ? device_obs : env->d_obs;
-    f.reward = static_cast<float*>(d_reward);
-    f.reward_f64 = static_cast<double*>(d_reward64);
-    f.discount = static_cast<float*>(d_discount);
-    f.step_type = static_cast<int32_t*>(d_step_type);
-    f.obs_vec_ok = (reinterpret_cast<uintptr_t>(f.obs) % 16 == 0) ? 1 : 0;
+    bsb_outputs dev;
+    dev.observation = device_obs ? device_obs : env->d_obs;
+    dev.reward = static_cast<float*>(d_reward);
+    dev.reward_f64 = static_cast<double*>(d_reward64);
+    dev.discount = static_cast<float*>(d_discount);
+    dev.step_type = static_cast<int32_t*>(d_step_type);
+    dev.final_observation = nullptr;
+    const int32_t* dev_actions = static_cast<const int32_t*>(d_actions);
     cudaStream_t zs = env->copy_stream;
     // Completion through the mailbox: the kernel's last CTA stores the ticket into pinned host memory after a
     // system-scope fence and the host spins on that word -- a stream synchronise costs a wake-up per step.
     // Observations copied to the host, graph-safe handles and unaligned observation buffers keep the synchronise.
-    const bool spin = !env->graph_safe && !host_out->observation && f.obs_vec_ok;
+    const bool spin = !env->graph_safe && !host_out->observation && reinterpret_cast<uintptr_t>(dev.observation) % 16 == 0;
     if (!spin) {
       { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
-      bsb_outputs dev;
-      dev.final_observation = nullptr;
-      dev.observation = f.obs; dev.reward = f.reward; dev.reward_f64 = f.reward_f64; dev.discount = f.discount; dev.step_type = f.step_type;
-      int zrc = bsb_step(env, f.actions, &dev, zs);
+      int zrc = bsb_step(env, dev_actions, &dev, zs);
       if (zrc != BSB_OK) return zrc;
       if (host_out->observation) BSB_CUDA(cudaMemcpyAsync(host_out->observation, dev.observation, obs_bytes, cudaMemcpyDeviceToHost, zs));
       BSB_CUDA(cudaStreamSynchronize(zs));
       return report_bad_actions(env);
     }
     { int mrc = mailbox_open(env); if (mrc != BSB_OK) return mrc; }
-    const bool prelaunch = (flags & BSB_HOST_PRELAUNCH) != 0;
-    for (int attempt = 0; attempt < 2; ++attempt) {
-      unsigned long long ticket;
-      if (env->pending_ticket) {
-        // The kernel of this step is already resident and polling: hand it the buffers and ring.
-        ticket = env->pending_ticket;
-        env->pending_ticket = 0;
-        env->mailbox->in = f;
-        std::atomic_thread_fence(std::memory_order_release);
-        env->mailbox->doorbell = ticket;
-      } else {
-        ticket = ++env->next_ticket;
-        if (family_obs_from_state(env)) {
-          // Two-phase step: phase 1 (the transitions of every lane) is all that stands between this launch and the
-          // observation stream, and reading 4 B per lane over PCIe from inside the kernel is most of it.  The DMA
-          // engine brings the actions over NOW, on a side stream, while the previous step's kernel is still
-          // streaming observations; the launch waits for that copy on the device.  (The previous kernel read its
-          // actions in phase 1, which ended before its completion word was seen: the buffer is free.)
-          if (!env->h2d_actions) BSB_CUDA(cudaMalloc(&env->h2d_actions, B * 4));
-          if (!env->h2d_stream) {
-            BSB_CUDA(cudaStreamCreateWithFlags(&env->h2d_stream, cudaStreamNonBlocking));
-            BSB_CUDA(cudaEventCreateWithFlags(&env->h2d_event, cudaEventDisableTiming));
-          }
-          BSB_CUDA(cudaMemcpyAsync(env->h2d_actions, actions, B * 4, cudaMemcpyHostToDevice, env->h2d_stream));
-          BSB_CUDA(cudaEventRecord(env->h2d_event, env->h2d_stream));
-          BSB_CUDA(cudaStreamWaitEvent(zs, env->h2d_event, 0));
-          f.actions = env->h2d_actions;
-        }
-        int lrc = mailbox_launch(env, ticket, env->steps_done, &f, false, (flags & BSB_HOST_NO_WAIT) != 0);
-        if (lrc != BSB_OK) return lrc;
+    const unsigned long long ticket = ++env->next_ticket;
+    if (family_obs_from_state(env)) {
+      // Two-phase step: phase 1 (the transitions of every lane) is all that stands between this launch and the
+      // observation stream, and reading 4 B per lane over PCIe from inside the kernel is most of it.  The DMA
+      // engine brings the actions over NOW, on a side stream, while the previous step's kernel is still
+      // streaming observations; the launch waits for that copy on the device.  (The previous kernel read its
+      // actions in phase 1, which ended before its completion word was seen: the buffer is free.)
+      if (!env->h2d_actions) BSB_CUDA(cudaMalloc(&env->h2d_actions, B * 4));
+      if (!env->h2d_stream) {
+        BSB_CUDA(cudaStreamCreateWithFlags(&env->h2d_stream, cudaStreamNonBlocking));
+        BSB_CUDA(cudaEventCreateWithFlags(&env->h2d_event, cudaEventDisableTiming));
       }
-      if ((flags & BSB_HOST_FENCE_CALLER) && env->early_inflight) {
-        // Two-phase step: the observation stores outlive this call.  Fence the caller's stream behind the kernel
-        // (the event is recorded BEFORE the next step's kernel is queued, so it stands for this step only):
-        // whatever the caller enqueues there afterwards sees complete observations.
-        if (!env->fence_event) BSB_CUDA(cudaEventCreateWithFlags(&env->fence_event, cudaEventDisableTiming));
-        BSB_CUDA(cudaEventRecord(env->fence_event, zs));
-        BSB_CUDA(cudaStreamWaitEvent(static_cast<cudaStream_t>(caller_stream), env->fence_event, 0));
-      }
-      if (flags & BSB_HOST_NO_WAIT) {
-        // Split call: the completion word is collected by bsb_host_wait (or by whichever entry point of this handle
-        // runs next), so the caller can drive ANOTHER handle while this step's scalars cross PCIe.
-        env->awaiting_ticket = ticket;
-        return BSB_OK;
-      }
-      if (prelaunch) {
-        // Queue the NEXT step's kernel now: it becomes resident as this one drains and waits for its doorbell,
-        // so the next call pays neither a launch nor a wake-up.  It stands down by itself after
-        // DOORBELL_TIMEOUT_NS (200 ms) without a ring.
-        const unsigned long long next = ++env->next_ticket;
-        int lrc = mailbox_launch(env, next, env->steps_done + 1, nullptr, true);
-        if (lrc != BSB_OK) return lrc;
-        env->pending_ticket = next;
-      }
-      bool cancelled = false;
-      { int wrc = mailbox_wait(env, ticket, &cancelled); if (wrc != BSB_OK) return wrc; }
-      if (!cancelled) { env->steps_done += 1; return report_bad_actions(env); }
-      // The pre-launched kernel had given up waiting before the ring arrived: nothing was stepped.  The launch
-      // queued behind it carries the wrong step index now; stand it down and take the step again, launched now.
-      { int frc = flush_pending(env); if (frc != BSB_OK) return frc; }
+      BSB_CUDA(cudaMemcpyAsync(env->h2d_actions, actions, B * 4, cudaMemcpyHostToDevice, env->h2d_stream));
+      BSB_CUDA(cudaEventRecord(env->h2d_event, env->h2d_stream));
+      BSB_CUDA(cudaStreamWaitEvent(zs, env->h2d_event, 0));
+      dev_actions = env->h2d_actions;
     }
-    return fail(BSB_INTERNAL, "host step: a freshly launched kernel reported a cancelled doorbell");
+    { int lrc = mailbox_launch(env, ticket, dev_actions, dev, (flags & BSB_HOST_NO_WAIT) != 0); if (lrc != BSB_OK) return lrc; }
+    if ((flags & BSB_HOST_FENCE_CALLER) && env->early_inflight) {
+      // Two-phase step: the observation stores outlive this call.  Fence the caller's stream behind the kernel:
+      // whatever the caller enqueues there afterwards sees complete observations.
+      if (!env->fence_event) BSB_CUDA(cudaEventCreateWithFlags(&env->fence_event, cudaEventDisableTiming));
+      BSB_CUDA(cudaEventRecord(env->fence_event, zs));
+      BSB_CUDA(cudaStreamWaitEvent(static_cast<cudaStream_t>(caller_stream), env->fence_event, 0));
+    }
+    if (flags & BSB_HOST_NO_WAIT) {
+      // Split call: the completion word is collected by bsb_host_wait (or by whichever entry point of this handle
+      // runs next), so the caller can drive ANOTHER handle while this step's scalars cross PCIe.
+      env->awaiting_ticket = ticket;
+      return BSB_OK;
+    }
+    { int wrc = mailbox_wait(env, ticket); if (wrc != BSB_OK) return wrc; }
+    env->steps_done += 1;
+    return report_bad_actions(env);
   }
   // Staged copies (a pageable buffer among them): actions in, bsb_step on device scratch, scalars out.
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }

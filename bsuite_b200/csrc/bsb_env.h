@@ -65,12 +65,10 @@ struct bsb_env {
   // this pinned flag; bsb_step_host / bsb_invalid_actions report it.
   int32_t* bad_action_host; int32_t* bad_action_dev;
   // Host-driven steps without a stream synchronise (bsb_step_host on pinned buffers): the kernel signals completion
-  // through a pinned mailbox the host spins on; with BSB_HOST_PRELAUNCH the next step's kernel is already queued
-  // and waits for the mailbox doorbell (bsb_kernels.cuh, HostMailbox).
+  // through a pinned mailbox the host spins on (bsb_kernels.cuh, HostMailbox).
   bsb::HostMailbox* mailbox; bsb::HostMailbox* mailbox_dev; bsb::DeviceMail* mail;
   unsigned long long next_ticket;     // last ticket handed out
   unsigned long long awaiting_ticket; // a BSB_HOST_NO_WAIT step whose completion word has not been collected yet (0 = none)
-  unsigned long long pending_ticket;  // pre-launched launch waiting for its doorbell (0 = none); it is for step steps_done
   bool early_inflight;                // a two-phase host step may still be streaming observations on copy_stream
   cudaStream_t h2d_stream; cudaEvent_t h2d_event;     // two-phase host steps: the actions' DMA on a side stream
 };

@@ -30,7 +30,7 @@
 // completion through a pinned mailbox.  For deep_sea and catch with observations of 1 KB or more they run in two
 // phases in a kernel of their own, two_phase_host_kernel (all transitions first, the scalars shipped to the host by a
 // few copier blocks, then the observations).  Both kernels share the emitters, the lane open / step / close sequence
-// (which the host path runs too) and the mailbox protocol.  With use_pdl a kernel is launched with programmatic
+// (which the host path runs too) and the completion word.  With use_pdl a kernel is launched with programmatic
 // stream serialization: everything before griddepcontrol.wait (index math, zeroing the shared-memory stages)
 // overlaps the tail of the previous step's kernel.
 // Observations may be written as bfloat16 or uint8 instead (bsb_config.obs_dtype; ObsAs below): the emitters stage and
@@ -42,10 +42,10 @@
 
 namespace bsb {
 
-// Caller-owned buffers of one step (launch arguments, or the fields of the host mailbox below).
+// Scalar outputs of one step (null members are skipped): the caller's buffers, or the two-phase host step's device
+// staging of them.
 struct MailFields {
-  const int32_t* actions; float* obs; float* reward; double* reward_f64; float* discount; int32_t* step_type;
-  int32_t obs_vec_ok, pad;
+  float* reward; double* reward_f64; float* discount; int32_t* step_type;
 };
 
 struct LaunchArgs {
@@ -75,16 +75,13 @@ struct LaunchArgs {
                             // 1: long rows, where a second stage would cost resident warps; 0: straight to global memory)
   int32_t cta_extra_elems;  // observation elements of shared memory after the per-warp stages (mnist bulk path: the
                             // CTA's all-zero tiles)
-  // Host-driven steps (bsb_step_host, pinned buffers): completion is signalled through a pinned mailbox; with
-  // BSB_HOST_PRELAUNCH the launch is even enqueued BEFORE its inputs exist and waits for the host to ring
-  // `ticket`, taking pointers and actions from the mailbox.
+  // Host-driven steps (bsb_step_host, pinned buffers): completion is signalled through a pinned mailbox.
   struct HostMailbox* mailbox;       // pinned host memory, device alias (null: ordinary launch).  The last CTA to
                                      // finish stores `done = ticket` there: the host spins on it instead of
                                      // paying a stream synchronise.
-  struct DeviceMail* mail;           // device memory: doorbell relay + finished-CTA counter
+  struct DeviceMail* mail;           // device memory: finished-CTA counter and two-phase flags
   unsigned long long ticket;
   int32_t timing;                    // BSB_HOST_TIMING: leave %globaltimer stamps in the mailbox
-  int32_t wait_doorbell;             // 1: pre-launched -- poll the doorbell for `ticket`, then take the buffers from the mailbox
   float* final_obs;         // same-step handles: [T,B,K] observations of the LAST timesteps (bsb_outputs.final_observation),
                             // or null (always null for host steps)
   int32_t* bad_action;      // pinned host flag (device alias): set to 1 when an action is outside [0, num_actions)
@@ -99,29 +96,21 @@ struct TwoPhaseArgs {
   MailFields stage;         // device staging of reward / reward_f64 / discount / step_type
 };
 
-// Host <-> device mailbox of the doorbell mode.  The host fills `in` and then stores `doorbell = ticket` (release
-// order); block 0 of the waiting launch polls it over PCIe, copies `in` to device memory and relays the ticket to the
-// other blocks through L2.  The last block to finish stores `done = ticket` after a system-scope fence, so every
-// output written to host memory (reward / discount / step_type, zero-copy) is visible when the host sees it.
-static const unsigned long long MAIL_CANCEL = 1ull << 63;      // doorbell: skip the step; done: the step was skipped
+// Pinned host memory the host-step kernels signal through.  The last block to finish stores `done = ticket` after a
+// system-scope fence, so every output written to host memory (reward / discount / step_type, zero-copy) is visible
+// when the host sees it.
 struct HostMailbox {
-  volatile unsigned long long doorbell;   // host -> device, word 0 of the line the device polls
-  MailFields in;                          // words 1..7 of the same 64-byte line
-  unsigned long long pad0[8];
-  volatile unsigned long long done;     unsigned long long pad1[7];     // device -> host, a line of its own
+  volatile unsigned long long done;     unsigned long long pad[7];      // device -> host, a line of its own
   // BSB_HOST_TIMING=1 (tools/e2e_timeline.py): %globaltimer stamps of the latest two-phase launch, written by its
   // signaller before `done`: [0] block 0 past the dependency wait, [1] phase 1 complete on every block, [2] just
   // before `done`, [3] the latest exit of any block of the PREVIOUS launch
   volatile unsigned long long stamp[8];
 };
-static_assert(sizeof(MailFields) == 56, "doorbell + fields must fill exactly one 64-byte line");
 struct DeviceMail {
-  volatile unsigned long long relay;      // ticket (| MAIL_CANCEL) most recently taken from the host doorbell
   unsigned long long last_exit;           // BSB_HOST_TIMING: max %globaltimer at which a block of the latest launch left
   unsigned long long finished;            // blocks of the current launch that have finished (phase 1, if two-phase)
   volatile unsigned long long phase1;     // ticket of the latest two-phase launch whose phase 1 is complete
   unsigned long long copied;              // copier blocks of the current two-phase launch that have shipped their share
-  MailFields in;                          // the host's fields, copied once per launch by block 0
 };
 
 enum { MODE_STEP = 0, MODE_RESET = 1, MODE_INIT = 2 };
@@ -679,10 +668,7 @@ template <> struct MinBlocksPerSM<MemoryChain> { static const int value = 6; }; 
 template <> struct MinBlocksPerSM<Bandit> { static const int value = 8; };        // <= 64
 template <> struct MinBlocksPerSM<DiscountingChain> { static const int value = 8; };
 #define BSB_LAUNCH_MIN_BLOCKS(F) MinBlocksPerSM<typename FamilyOf<F>::type>::value
-// System-scope accesses to the pinned mailbox (host memory over PCIe) and volatile accesses to its L2 relay.
-__device__ __forceinline__ unsigned long long ld_sys_u64(const volatile unsigned long long* ptr) {
-  unsigned long long v; asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(ptr) : "memory"); return v;
-}
+// System-scope stores to the pinned mailbox (host memory over PCIe).
 __device__ __forceinline__ void st_sys_u64(volatile unsigned long long* ptr, unsigned long long v) {
   asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(ptr), "l"(v) : "memory");
 }
@@ -744,52 +730,6 @@ __device__ __forceinline__ WarpStage<O> clear_stages(const EnvParams& p, const L
     __syncthreads();
   }
   return ws;
-}
-
-// Caller-owned buffers of the launch: its arguments or -- pre-launched (doorbell) mode -- whatever the host wrote
-// into the mailbox before it rang this launch's ticket.  `cancelled`: the host stood the launch down, or nobody rang
-// before DOORBELL_TIMEOUT_NS.  Every thread of the CTA calls it.
-static const unsigned long long DOORBELL_TIMEOUT_NS = 200000000ull;      // 200 ms
-__device__ __forceinline__ MailFields receive_doorbell(const LaunchArgs& a, bool& cancelled) {
-  __shared__ MailFields mail_in;
-  __shared__ int mail_cancel;
-  MailFields io = {a.actions, a.obs, a.reward, a.reward_f64, a.discount, a.step_type, a.obs_vec_ok, 0};
-  cancelled = false;
-  if (!a.mailbox || !a.wait_doorbell) return io;
-  const int tid = threadIdx.x & 31;
-  if (blockIdx.x == 0 && (threadIdx.x >> 5) == 0) {
-    // The one poller of host memory: lanes 0..7 read the mailbox's first 64-byte line (doorbell + fields) with ONE
-    // coalesced request per poll; when the ring shows, the line is read once more (the host wrote the fields
-    // before the doorbell, so this second read cannot be stale), parked in device memory, and the ticket is
-    // relayed to the other blocks through L2.
-    const volatile unsigned long long* line = &a.mailbox->doorbell;
-    const unsigned long long deadline = global_timer_ns() + DOORBELL_TIMEOUT_NS;
-    unsigned long long word = 0, seen;
-    do {
-      if (tid < 8) word = ld_sys_u64(line + tid);
-      seen = __shfl_sync(0xffffffffu, word, 0);
-    } while ((seen & ~MAIL_CANCEL) < a.ticket && global_timer_ns() < deadline);
-    if ((seen & ~MAIL_CANCEL) < a.ticket) seen = a.ticket | MAIL_CANCEL;        // nobody rang: stand down
-    __threadfence_system();
-    if (tid < 8) word = ld_sys_u64(line + tid);
-    if (tid >= 1 && tid < 8) reinterpret_cast<unsigned long long*>(&a.mail->in)[tid - 1] = word;
-    __threadfence();
-    __syncwarp();
-    if (tid == 0) a.mail->relay = seen;
-  }
-  if (threadIdx.x == 0) {
-    unsigned long long seen;
-    do { seen = a.mail->relay; } while ((seen & ~MAIL_CANCEL) < a.ticket);
-    __threadfence();
-    mail_cancel = (seen & MAIL_CANCEL) ? 1 : 0;
-    const volatile unsigned long long* src = reinterpret_cast<const volatile unsigned long long*>(&a.mail->in);
-    unsigned long long* dst = reinterpret_cast<unsigned long long*>(&mail_in);
-    for (int k = 0; k < (int)(sizeof(MailFields) / 8); ++k) dst[k] = src[k];
-  }
-  __syncthreads();
-  io = mail_in;
-  cancelled = mail_cancel != 0;
-  return io;
 }
 
 // The elected lane draws chunk indices [total_warps, n_chunks) from the global counter and broadcasts them with a
@@ -959,14 +899,14 @@ __device__ __forceinline__ void retire_warp(const LaunchArgs& a, const WarpStage
 }
 
 // Completion of a host step: every CTA counts itself finished once its zero-copy outputs are visible to the host;
-// the last one stores `word` (the ticket, with MAIL_CANCEL if the launch stood down) into the mailbox.
-__device__ __forceinline__ void signal_done(const LaunchArgs& a, unsigned long long word) {
+// the last one stores the ticket into the mailbox.
+__device__ __forceinline__ void signal_done(const LaunchArgs& a) {
   __threadfence_system();                  // every thread: its zero-copy outputs are visible to the host ...
   __syncthreads();                         // ... before the CTA counts itself finished
   if (threadIdx.x == 0 && atomicAdd(&a.mail->finished, 1ull) == (unsigned long long)gridDim.x - 1ull) {
     a.mail->finished = 0ull;
     __threadfence_system();
-    st_sys_u64(&a.mailbox->done, word);
+    st_sys_u64(&a.mailbox->done, a.ticket);
   }
 }
 
@@ -988,22 +928,14 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
   if (a.use_pdl) { pdl_wait(); pdl_launch_dependents(); }
   int64_t step0 = a.step0;
   if (a.clock) step0 += (int64_t)*reinterpret_cast<volatile unsigned long long*>(a.clock + 16 * (blockIdx.x % CLOCK_GROUPS));
-  bool cancelled;
-  const MailFields io = receive_doorbell(a, cancelled);
-  const bool vec = io.obs_vec_ok != 0;
-  O* const obs = reinterpret_cast<O*>(io.obs);      // the ABI's float* addresses elements of type O
+  const MailFields out = {a.reward, a.reward_f64, a.discount, a.step_type};
+  const bool vec = a.obs_vec_ok != 0;
+  O* const obs = reinterpret_cast<O*>(a.obs);       // the ABI's float* addresses elements of type O
 
   const int cl = a.chunk_lanes;
   const int64_t n_chunks = (B + cl - 1) / cl;
   const bool dynamic = a.work_counter != nullptr;
   const int64_t total_warps = (int64_t)gridDim.x * warps_per_cta;
-  if (cancelled) {
-    // A stood-down launch still owes the chunk counter its share: a launch over C chunks advances it by exactly C.
-    if (dynamic && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(a.work_counter, (unsigned long long)n_chunks);
-    retire_warp(a, ws, false);
-    signal_done(a, a.ticket | MAIL_CANCEL);
-    return;                                  // host steps never carry the device clock
-  }
   int64_t cur_chunk = (int64_t)blockIdx.x * warps_per_cta + warp;
 
   while (cur_chunk < n_chunks) {
@@ -1035,9 +967,8 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
       if (active) {
         int32_t action = 0;
         if (a.mode == MODE_STEP) {
-          if (io.actions) {
-            // doorbell mode reads host memory the launch may have cached before the host wrote it: ld.cv
-            action = a.mailbox ? __ldcv(io.actions + off) : io.actions[off];
+          if (a.actions) {
+            action = a.actions[off];
             if ((uint32_t)action >= (uint32_t)p.num_actions) {      // never index a table or pack state with it
               if (a.bad_action) *a.bad_action = 1;
               action = action < 0 ? 0 : p.num_actions - 1;
@@ -1047,8 +978,8 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
           }
           if (a.actions_out) a.actions_out[off] = action;
         }
-        if constexpr (kSameStep) lane_step<Fam, R, true>(p, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, io, off, &merged);
-        else lane_step<Fam>(lp, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, io, off);
+        if constexpr (kSameStep) lane_step<Fam, R, true>(p, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, out, off, &merged);
+        else lane_step<Fam>(lp, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, out, off);
       }
       if constexpr (kSameStep) {
         if (a.final_obs)
@@ -1063,7 +994,7 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
     cur_chunk = dynamic ? fetch_chunk(a, total_warps) : n_chunks;
   }
   retire_warp(a, ws, a.mailbox != nullptr);
-  if (a.mailbox) signal_done(a, a.ticket);
+  if (a.mailbox) signal_done(a);
   if (a.clock) {
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -1120,22 +1051,12 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
   // The observation-only launch must not wait for its predecessor -- the transitions launch, whose copiers are
   // still shipping scalars over PCIe -- to END: it waits for that launch's phase-1 flag instead.
   if (a.use_pdl) { if (h.phase != 2) pdl_wait(); pdl_launch_dependents(); }
-  bool cancelled;
-  const MailFields io = receive_doorbell(a, cancelled);
-  const bool vec = io.obs_vec_ok != 0;
-  O* const obs = reinterpret_cast<O*>(io.obs);      // the ABI's float* addresses elements of type O
+  const bool vec = a.obs_vec_ok != 0;
+  O* const obs = reinterpret_cast<O*>(a.obs);       // the ABI's float* addresses elements of type O
 
   const int cl = a.chunk_lanes;
   const int64_t n_chunks = (B + cl - 1) / cl;
   const bool dynamic = a.work_counter != nullptr;
-  if (cancelled) {
-    // A stood-down launch still owes the chunk counter its share: C chunks plus one failing fetch per copier warp.
-    if (dynamic && blockIdx.x == 0 && threadIdx.x == 0)
-      atomicAdd(a.work_counter, (unsigned long long)n_chunks + (unsigned long long)h.copiers * warps_per_cta);
-    retire_warp(a, ws, false);
-    signal_done(a, a.ticket | MAIL_CANCEL);
-    return;
-  }
   const unsigned copier_blocks = (unsigned)h.copiers;
   const unsigned worker_blocks = gridDim.x - copier_blocks;
   const int64_t total_warps = (int64_t)worker_blocks * warps_per_cta;
@@ -1208,10 +1129,10 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
       char* tail_dst = reinterpret_cast<char*>(to) + (n16 << 4);
       for (int64_t i = me; i < (bytes & 15); i += n_thr) tail_dst[i] = tail_src[i];
     };
-    ship(h.stage.reward, io.reward, B * 4);
-    ship(h.stage.reward_f64, io.reward_f64, B * 8);
-    ship(h.stage.discount, io.discount, B * 4);
-    ship(h.stage.step_type, io.step_type, B * 4);
+    ship(h.stage.reward, a.reward, B * 4);
+    ship(h.stage.reward_f64, a.reward_f64, B * 8);
+    ship(h.stage.discount, a.discount, B * 4);
+    ship(h.stage.step_type, a.step_type, B * 4);
     __threadfence_system();
     __syncthreads();
     if (threadIdx.x == 0 && atomicAdd(&a.mail->copied, 1ull) == (unsigned long long)copier_blocks - 1ull) {
@@ -1229,8 +1150,8 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
   } else {
     constexpr int kAhead = 4;              // chunks whose loads (action, lane state, accumulators) are in flight together
     for (int64_t c0 = own; c0 < n_chunks; c0 += kAhead * total_warps) {
-      // every independent load of up to kAhead chunks first: one round trip to L2 (or over PCIe, when the actions
-      // were not staged on the device) instead of one per chunk -- a warp owns 4-5 chunks of a 65 536-lane batch
+      // every independent load of up to kAhead chunks first: one round trip to L2 instead of one per chunk -- a warp
+      // owns 4-5 chunks of a 65 536-lane batch
       int32_t fetched[kAhead];
       typename Fam::Lane lanes[kAhead];
       EpisodeStats eps[kAhead];
@@ -1242,7 +1163,7 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
         fetched[k] = 0;
         Fam::init(p, lanes[k]);
         if (live) {
-          fetched[k] = __ldcv(io.actions + lane);
+          fetched[k] = a.actions[lane];
           Fam::load(p, lane, lanes[k]);
           if (kTrack) eps[k].load(p, lane);
         }

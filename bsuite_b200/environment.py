@@ -439,10 +439,7 @@ class BatchedEnvironment:
     `reset()` / `step()` / `rollout()` on the current torch stream is waited for on the device (the handle's
     stream is fenced behind the current stream the first time a host-driven step follows such work).
 
-    `prelaunch=True` (pinned buffers, CUDA): the next step's kernel is queued immediately and waits for this
-    method's next call on a doorbell in pinned memory, so a call costs neither a kernel launch nor a stream
-    synchronise.  The waiting kernel occupies the GPU: use it for host-side policies in a tight loop; any other
-    method of this environment (or 200 ms without a call) stands it down.
+    `prelaunch` is accepted and has no effect (`BSB_HOST_PRELAUNCH`): the call runs the same waited step.
 
     `wait=False` (pinned buffers, CUDA): returns once the step is enqueued; `host` holds the results after
     `host_wait()`.  `rollouts.HostHalves` uses it to drive two half-batches alternately (`BSB_HOST_NO_WAIT`).
@@ -490,7 +487,8 @@ class BatchedEnvironment:
       _lib.check(status)
 
   def host_flush(self):
-    """Stands down a kernel queued by `step_host(..., prelaunch=True)` (every other method does so implicitly)."""
+    """Collects a `step_host(..., wait=False)` nobody waited for (no-op otherwise); unlike `host_wait()` it does not
+    report an out-of-range action of that step."""
     _lib.check(self._lib.bsb_host_flush(self._handle.ptr))
 
   def invalid_actions_seen(self) -> bool:

@@ -492,14 +492,10 @@ int32_t bsb_set_state(bsb_env* env, const void* src_host, int64_t nbytes,
  *       the next call on this handle (every entry point waits for the step).
  *       Same-step handles (BSB_FLAG_SAME_STEP_RESET) always run host steps in
  *       one phase.
- *   BSB_HOST_PRELAUNCH  (pinned buffers only) after ringing this step, the NEXT
- *       step's kernel is enqueued at once; it becomes resident as this one drains
- *       and polls the mailbox doorbell, so the next call costs neither a launch
- *       nor a wake-up -- for agents whose policy runs on the HOST.  While it
- *       waits it occupies the SMs: other GPU work of the process queues behind it
- *       until the next call, bsb_host_flush, or 200 ms without a ring, after
- *       which it stands down by itself.  Every other
- *       entry point of this handle stands it down first.
+ *   BSB_HOST_PRELAUNCH  accepted, no effect: the call runs the same waited step
+ *       as without it.  The mode it named (the next step's kernel queued ahead,
+ *       polling a doorbell in pinned memory) was retired because it lost to the
+ *       waited step on the H100.
  *   BSB_HOST_NO_WAIT  (pinned buffers; otherwise the call is simply synchronous)
  *       the call returns once the step is enqueued; the host outputs are valid
  *       after bsb_host_wait(env).  One step per handle may be outstanding (any
@@ -522,7 +518,8 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions,
                       const bsb_outputs* host_out, float* device_obs,
                       void* caller_stream, uint32_t flags);
 
-/* Stands down a launch queued by BSB_HOST_PRELAUNCH (no-op otherwise). */
+/* Collects a BSB_HOST_NO_WAIT step nobody waited for (no-op otherwise).  Unlike
+ * bsb_host_wait it does not report an out-of-range action of that step. */
 int32_t bsb_host_flush(bsb_env* env);
 
 /* Completes a step issued with BSB_HOST_NO_WAIT: returns when its host outputs

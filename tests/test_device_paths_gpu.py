@@ -22,8 +22,8 @@ also go through oracle.run_lanes, which anchors the comparison outside the engin
   group C  the CTA sizes, deep_sea group sizes, vector fallbacks and mnist group sizes that only larger boards,
            tiles and images reach;
   group H  every instantiation two_phase_host_kernel<deep_sea | catch, Philox | MT19937, noise, track> (16 kernels),
-           driven by host steps (bsb_step_host on pinned buffers): waited for, pre-launched, and BSB_HOST_NO_WAIT
-           (which splits the step over two launches).
+           driven by host steps (bsb_step_host on pinned buffers): waited for, and BSB_HOST_NO_WAIT (which splits
+           the step over two launches).
 
 Exactness follows tests/conftest.py: integer / grid families bit for bit (step_type, discount, reward, observation,
 bsuite_info, episode_stats, log rows, state blob); float dynamics, the reward-noise wrapper and stochastic deep_sea
@@ -169,7 +169,7 @@ GROUP_B = [
 
 # group H: observations of >= 1 KB take the two-phase host step (deep_sea N = 16, catch 16 x 16)
 H_KWARGS = dict(deep_sea=dict(DS, size=16), catch=dict(rows=16, columns=16))
-HOST_MODES = ('wait', 'prelaunch', 'no_wait')
+HOST_MODES = ('wait', 'no_wait')
 GROUP_H = [(_case(f, 97, H_KWARGS[f], rng=r, noise=0.1 if n else None, track=t,
                   reward_dtype='float64' if t else 'float32'), mode)
            for f, r, n, t in itertools.product(('deep_sea', 'catch'), RNGS, (False, True), (False, True))
@@ -358,7 +358,7 @@ class Twins:
       host, out = env.make_host_buffers(), env.make_buffers()
       actions = torch.from_numpy(acts)
       env.step_host(actions.pin_memory() if env.device.type == 'cuda' else actions, host, out=out,
-                    prelaunch=mode == 'prelaunch', wait=mode != 'no_wait')
+                    wait=mode != 'no_wait')
       if mode == 'no_wait':
         env.host_wait()
       outs.append(type(out)(observation=out.observation, reward=host.reward, discount=host.discount,
@@ -526,8 +526,7 @@ def test_large_tile_and_board_paths_match_the_host_path(case, image_dirs):
 @pytest.mark.gpu
 @pytest.mark.parametrize('case_mode', GROUP_H, ids=_h_id)
 def test_two_phase_host_kernel_matches_the_host_path(case_mode, image_dirs):
-  """Host steps around an ordinary step: every call compared with the host twin, then the state (which stands a
-  pre-launched kernel down: the cancelled case)."""
+  """Host steps around an ordinary step: every call compared with the host twin, then the state."""
   case, mode = case_mode
   twins = Twins(case, ('cuda', 'cpu'), image_dirs)
   try:

@@ -189,8 +189,7 @@ class DtypeTwins:
       out = buffers(env, None, False, self.case['misalign'])
       actions = torch.from_numpy(acts)
       pin = env.device.type == 'cuda' and not pageable
-      env.step_host(actions.pin_memory() if pin else actions, host, out=out,
-                    prelaunch=mode == 'prelaunch', wait=mode != 'no_wait')
+      env.step_host(actions.pin_memory() if pin else actions, host, out=out, wait=mode != 'no_wait')
       if mode == 'no_wait':
         env.host_wait()
       if with_observation:

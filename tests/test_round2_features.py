@@ -1,7 +1,5 @@
 """Round-2 additions: action validation, Logging bookkeeping across mid-episode resets, snapshot fingerprints,
-seed precedence, host-driven steps through the mailbox (spin / pre-launch), staged-emitter fallbacks."""
-
-import time
+seed precedence, host-driven steps through the mailbox, staged-emitter fallbacks."""
 
 import numpy as np
 import pytest
@@ -129,9 +127,8 @@ def test_an_explicit_engine_seed_overrides_the_experiment_default():
 @pytest.mark.parametrize('bsuite_id', ['deep_sea/11', 'catch_noise/2', 'cartpole/0', 'mnist/0', 'umbrella_length/10'])
 @pytest.mark.parametrize('prelaunch', [False, True])
 def test_host_driven_steps_through_the_mailbox_equal_ordinary_steps(bsuite_id, prelaunch, mnist_dir):
-  """bsb_step_host on pinned buffers: completion through the pinned mailbox (no stream synchronise) and, with
-  prelaunch, kernels queued ahead that wait for the doorbell.  Interleaved with ordinary calls (which stand a
-  queued launch down) and with a pause longer than the doorbell timeout (the queued launch stands down by itself)."""
+  """bsb_step_host on pinned buffers: completion through the pinned mailbox (no stream synchronise), interleaved
+  with an ordinary call.  `prelaunch` (BSB_HOST_PRELAUNCH, accepted with no effect) runs the same waited step."""
   B, T = 4096, 36
   a = bsuite_b200.load_from_id(bsuite_id, batch=B, device='cuda', seed=3, track_episodes=True)
   b = bsuite_b200.load_from_id(bsuite_id, batch=B, device='cuda', seed=3, track_episodes=True)
@@ -141,34 +138,20 @@ def test_host_driven_steps_through_the_mailbox_equal_ordinary_steps(bsuite_id, p
   a.reset(); b.reset()                       # b: no synchronise -- step_host must order itself behind this
   for t in range(T):
     want = a.step(actions[t].cuda())
-    if t == 12:                              # an ordinary call in the middle: the queued launch must stand down
+    if t == 12:                              # an ordinary call in the middle
       got = b.step(actions[t].cuda())
       got_obs = got.observation
     else:
-      if t == 20 and prelaunch:
-        time.sleep(0.35)                     # > the 200 ms doorbell timeout: the queued launch gives up, the step still happens
       got, got_obs = b.step_host(actions[t], host, out=outs[t % 2], prelaunch=prelaunch)
     tol = cf.FLOAT_TOL if bsuite_id.startswith('cartpole') else 0
     for field in ('step_type', 'reward', 'discount'):
       np.testing.assert_allclose(_np(getattr(got, field)), _np(getattr(want, field)), rtol=0, atol=tol, err_msg=f'{field} t={t}')
     assert torch.equal(got_obs, want.observation), t
+  b.host_flush()
   assert a.steps_done == b.steps_done == T + 1
   assert torch.equal(a.episode_stat_sums(), b.episode_stat_sums())
   np.testing.assert_array_equal(a.state_dict()['blob'], b.state_dict()['blob'])
   b.close(); a.close()
-
-
-@pytest.mark.gpu
-def test_closing_an_environment_with_a_queued_launch_does_not_hang():
-  env = bsuite_b200.load_from_id('catch/0', batch=1024, device='cuda', seed=0)
-  host = env.make_host_buffers()
-  actions = torch.zeros(1024, dtype=torch.int32).pin_memory()
-  for _ in range(3):
-    env.step_host(actions, host, prelaunch=True)
-  env.host_flush()
-  env.step_host(actions, host, prelaunch=True)
-  env.close()
-  torch.cuda.synchronize()
 
 
 # ---------------------------------------------------------------------------- emitters

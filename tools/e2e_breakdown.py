@@ -4,9 +4,9 @@
     python tools/e2e_breakdown.py [bsuite_id] [batch]
 
 Rows: the kernel rate (launches queued), a device-resident loop that synchronises after every step, then the
-host-buffer call `BatchedEnvironment.step_host` (pinned actions in, pinned scalars out) -- two-phase (scalars
-first), with and without pre-launched doorbell kernels, each through the Python face and through bare ctypes calls
-with prebuilt arguments (what a C caller of the ABI pays) -- and its staged copies from pageable buffers.
+host-buffer call `BatchedEnvironment.step_host` (pinned actions in, pinned scalars out; two-phase, scalars first,
+for deep_sea) through the Python face and through bare ctypes calls with prebuilt arguments (what a C caller of the
+ABI pays), and its staged copies from pageable buffers.
 """
 import ctypes
 import os
@@ -23,17 +23,13 @@ BSUITE_ID = sys.argv[1] if len(sys.argv) > 1 else 'deep_sea/11'
 B = int(sys.argv[2]) if len(sys.argv) > 2 else 65536
 
 
-def timed(fn, n=300, after=None):
+def timed(fn, n=300):
   for i in range(20):
     fn(i)
-  if after:
-    after()
   torch.cuda.synchronize()
   t0 = time.perf_counter()
   for i in range(n):
     fn(i)
-  if after:
-    after()
   torch.cuda.synchronize()
   return (time.perf_counter() - t0) / n * 1e6
 
@@ -65,15 +61,13 @@ def variants(e, label):
   acts = [ctypes.c_void_p(p.data_ptr()) for p in prow]
   obs = [ctypes.c_void_p(r.observation.data_ptr()) for r in ring]
   ref = ctypes.byref(houts)
-  for prelaunch in (False, True):
-    flags = _lib.HOST_PRELAUNCH if prelaunch else 0
-    py = timed(lambda i: e.step_host(prow[i % 64], host, out=ring[i % 4], prelaunch=prelaunch), after=e.host_flush)
-    raw = timed(lambda i: lib.bsb_step_host(handle, acts[i % 64], ref, obs[i % 4], None, flags), after=e.host_flush)
-    print(f'step_host {label:34s} prelaunch={int(prelaunch)}  python {py:6.1f}  ctypes {raw:6.1f} us/step')
+  py = timed(lambda i: e.step_host(prow[i % 64], host, out=ring[i % 4]))
+  raw = timed(lambda i: lib.bsb_step_host(handle, acts[i % 64], ref, obs[i % 4], None, 0))
+  print(f'step_host {label:34s}  python {py:6.1f}  ctypes {raw:6.1f} us/step')
 
 
 variants(env, 'mailbox + two-phase')
 page = [torch.empty(B, dtype=torch.int32).copy_(row) for row in prow[:4]]      # pageable host memory
-page_host = type(host)(**{f: torch.empty(getattr(host, f).shape, dtype=getattr(host, f).dtype)
-                          for f in ('reward', 'discount', 'step_type')})
+page_host = type(host)(observation=None, **{f: torch.empty(getattr(host, f).shape, dtype=getattr(host, f).dtype)
+                                              for f in ('reward', 'discount', 'step_type')})
 print(f'step_host staged copies (pageable buffers)               {timed(lambda i: env.step_host(page[i % 4], page_host, out=ring[i % 4])):7.1f} us/step')

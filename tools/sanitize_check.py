@@ -106,8 +106,7 @@ for bsuite_id, batch in (('deep_sea/11', 20000), ('catch/0', 5000)):
   assert torch.equal(env.episode_stat_sums(), twin.episode_stat_sums()) and env.steps_done == twin.steps_done == 7
   print(bsuite_id, batch, 'graph replay == eager: True', flush=True)
   env.close(); twin.close()
-# Host-driven steps: completion through the pinned mailbox, pre-launched doorbell kernels (under the sanitizer launches
-# are serialised, so a pre-launched kernel times out and stands down: the cancel path), out-of-range actions.
+# Host-driven steps: completion through the pinned mailbox, out-of-range actions.
 for bsuite_id, batch in (('deep_sea/11', 20000), ('catch/0', 3000), ('mnist/0', 1500)):
   env = bsuite_b200.load_from_id(bsuite_id, batch=batch, device='cuda', seed=3, track_episodes=True)
   twin = bsuite_b200.load_from_id(bsuite_id, batch=batch, device='cuda', seed=3, track_episodes=True)
@@ -115,7 +114,7 @@ for bsuite_id, batch in (('deep_sea/11', 20000), ('catch/0', 3000), ('mnist/0', 
   acts = torch.as_tensor(env.random_actions(6, action_seed=1, first_step=0)).pin_memory()
   env.reset(); twin.reset()
   for t in range(6):
-    got, obs = env.step_host(acts[t], host, prelaunch=(t >= 3))
+    got, obs = env.step_host(acts[t], host)
     want = twin.step(acts[t].cuda())
     torch.cuda.synchronize()
     assert torch.equal(obs, want.observation) and torch.equal(got.reward, want.reward.cpu()) and torch.equal(got.step_type, want.step_type.cpu())
