@@ -128,11 +128,17 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, bool no_obs = false, int
   int threads = 64;         // one chunk per warp: small CTAs spread evenly over the SMs (transition_kernel)
   bool persistent = false;
   const size_t tile = (size_t)K * elem;
-  // deep_sea tiles written to compressible memory (bsb_obs_malloc) leave as 16-byte streaming stores once the batch
-  // fills the GPU (>= 4 chunks per SM): there the bulk path gains nothing from compression, and the streaming stores
-  // run up to 1.22x faster than the bulk path on plain memory.  Smaller batches keep the bulk path, which overlaps
-  // a warp's stores with its next steps (DESIGN.md §7, "Compressible observation memory").
-  if (is_onehot && a.emit_bulk && g.n_chunks >= 4 * (int64_t)e->num_sms && in_compressed_block(a.obs)) a.emit_bulk = 0;
+  // deep_sea tiles written to compressible memory (bsb_obs_malloc) once the batch fills the GPU (>= 4 chunks per SM)
+  // skip the bulk path, which gains nothing from compression there.  A launch of one step compares every tile with
+  // what the destination holds and stores only the lines that differ (emit_onehot_reuse): compressed one-hot tiles
+  // read back faster than any emitter can write them.  Fused rollouts (T > 1) ran slower that way and keep the 16-byte
+  // streaming stores.  Smaller batches keep the bulk path, which overlaps a warp's stores with its next steps
+  // (DESIGN.md §7, "Compressible observation memory").
+  a.emit_reuse = 0;
+  if (is_onehot && a.emit_bulk && g.n_chunks >= 4 * (int64_t)e->num_sms && in_compressed_block(a.obs)) {
+    a.emit_bulk = 0;
+    a.emit_reuse = a.T == 1 ? 1 : 0;
+  }
   if (is_onehot && a.emit_bulk) {
     // Lanes per bulk store: the largest power of two <= 16 with one store <= 40 KB, so a group never spans a
     // 32-lane chunk.  N = 32 -> 8 lanes (32 KB stores; 88.8 us per headline step against 91.9 with 4 lanes, DESIGN.md
@@ -166,8 +172,8 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, bool no_obs = false, int
     }
   }
   a.use_pdl = (a.mode == MODE_STEP && a.T == 1) ? 1 : 0;
-  if (no_obs) { a.emit_bulk = 0; a.stage_rows = 0; a.cta_extra_elems = 0; a.group_lanes = 1; threads = 128; persistent = false; }
-  size_t per_warp = smem_elems_per_warp<F, O>(K, a.emit_bulk != 0, a.group_lanes, a.stage_rows) * elem;
+  if (no_obs) { a.emit_bulk = 0; a.emit_reuse = 0; a.stage_rows = 0; a.cta_extra_elems = 0; a.group_lanes = 1; threads = 128; persistent = false; }
+  size_t per_warp = smem_elems_per_warp<F, O>(K, a.emit_bulk != 0, a.emit_reuse != 0, a.group_lanes, a.stage_rows) * elem;
   if ((EmitKind<F>::value == EMIT_ROWS || EmitKind<F>::value == EMIT_TWOHOT) && per_warp > 96 * 1024) {
     // rows / boards too long for a per-warp stage: long rows always get ONE stage (above), so the limit is
     // 32 * K * 4 bytes > 96 KB, i.e. K > 768 in float32 (catch boards of more than 768 cells such as 28 x 28,

@@ -21,7 +21,11 @@
 //     Large stores matter: the TMA unit pays a fixed cost per operation, which 4 KB stores cannot amortise
 //     and 32 KB stores can.  Unaligned tiles (odd N) use 16-byte streaming
 //     stores instead: the warp walks its lanes, every thread writes part of each lane's tile, the hot cell
-//     chosen per float4 from a descriptor broadcast by __shfl_sync.
+//     chosen per float4 from a descriptor broadcast by __shfl_sync.  Tiles in compressible memory (bsb_obs_malloc)
+//     of a single-step launch that fills the GPU are compared, not written: the warp reads each tile (cp.async into a
+//     small ring in shared memory) and stores only the 128-byte lines that differ from the new observation -- two
+//     per tile when the destination holds an earlier observation, as a reused output buffer does.  A destination
+//     holding anything else falls back to the streaming stores after a 512-byte probe of the chunk's first tile.
 //   * mnist: groups of 4 gathered int8 images -> float32 tiles in shared memory -> one bulk store; the all-zero
 //     LAST frames of a group leave as one bulk store from zero tiles the CTA's warps share.
 //
@@ -62,6 +66,7 @@ struct LaunchArgs {
   int32_t mode;             // 0 = step, 1 = reset every lane, 2 = constructor init
   int32_t obs_vec_ok;       // obs base and per-step stride are 16-byte aligned
   int32_t emit_bulk;        // use TMA bulk stores where the emitter supports them
+  int32_t emit_reuse;       // one-hot tiles without bulk stores: store only the words that differ (emit_onehot_reuse)
   int32_t use_pdl;          // launched with programmatic stream serialization
   int32_t group_lanes;      // deep_sea bulk path: lanes per bulk store (power of two, 1..32)
   int32_t final_vec_ok;     // same-step handles: final_obs base and per-step stride are 16-byte aligned
@@ -292,6 +297,9 @@ template <> struct EmitKind<Catch> { static const int value = EMIT_TWOHOT; };
 template <> struct EmitKind<Mnist> { static const int value = EMIT_IMAGE; };
 static const int ROW_STAGES = 2;      // at most: double-buffered [32, K] stage per warp (LaunchArgs::stage_rows)
 static const int TILE_STAGES = 2;     // deep_sea bulk path: double-buffered groups of `group_lanes` tiles per warp
+static const int REUSE_WORDS = 256;   // compare-then-store tiles: 16-byte words per pass (8 per thread) ...
+static const int REUSE_STAGES = 2;    // ... and passes in flight per warp (emit_onehot_reuse)
+static const int REUSE_STORE_WORDS = 8;   // ... and a differing word is stored with its whole 128-byte line
 
 // Families whose observations hold only 0 and 1, so that uint8 represents them exactly (obs_dtype uint8).
 template <class F> struct BinaryObs {
@@ -303,9 +311,10 @@ template <class F, class O> inline
 #if defined(__CUDACC__)
 __host__ __device__
 #endif
-size_t smem_elems_per_warp(int K, bool emit_bulk, int group_lanes, int row_stages) {
+size_t smem_elems_per_warp(int K, bool emit_bulk, bool emit_reuse, int group_lanes, int row_stages) {
   if (EmitKind<F>::value == EMIT_ROWS || EmitKind<F>::value == EMIT_TWOHOT) return (size_t)row_stages * 32 * (size_t)K;
   if (EmitKind<F>::value == EMIT_ONEHOT && emit_bulk) return (size_t)TILE_STAGES * (size_t)group_lanes * (size_t)K;
+  if (EmitKind<F>::value == EMIT_ONEHOT && emit_reuse) return (size_t)REUSE_STAGES * REUSE_WORDS * 16 / sizeof(O);
   if (EmitKind<F>::value == EMIT_IMAGE)                    // int8 pixel -> float32 table (+ one staging buffer of m tiles)
     return 256 * sizeof(float) / sizeof(O) + (emit_bulk ? (size_t)group_lanes * (size_t)K : 0);
   return 0;
@@ -405,6 +414,94 @@ __device__ __forceinline__ void emit_onehot_vec(O* obs_t, int64_t warp_base, int
       for (int e = tid; e < K; e += 32) st_stream(dst + e, obs_cast<O>(e == h ? 1.f : 0.f));
     }
   }
+}
+
+// Compare-then-store one-hot tiles (LaunchArgs::emit_reuse; every tile a whole number of 16-byte words): the warp
+// reads each tile and stores only the 128-byte lines that hold a word whose bits differ from the word this step
+// produces, so a destination that already holds an earlier one-hot observation costs a read of the tile and at most
+// two line stores (the old hot cell's and the new one's).  Bits are compared, not values, so -0.0 and NaN payloads
+// are rewritten: the result is bit-identical to a full write whatever the destination held.  Whole lines, not single
+// 16-byte words: a partial store into a line of compressible memory made single steps 1.5x slower than full writes
+// (DESIGN.md §7, "Compressible observation memory").
+// The tiles are read in PASSES of REUSE_WORDS words (8 per thread; one pass per 4 KB tile) through a ring of
+// REUSE_STAGES passes in the warp's shared memory, with cp.async (the loads in flight hold no registers): the next
+// pass is always in flight while the current one is compared.  Every thread compares exactly the words it loaded, so
+// no warp barrier is needed between the two.
+// A destination that does not hold an observation must not pay a read on top of every write.  A PROBE of the first
+// 512 bytes of the chunk's first tile decides whether the chunk is read at all; after it, any pass that holds more
+// than two differing words turns the rest of the chunk blind: streaming stores of every word, as emit_onehot_vec.
+__device__ __forceinline__ void cp_async16(void* sdst, const void* gsrc) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(sdst)), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+// Issues pass s of the chunk's tiles into ring slot s % REUSE_STAGES as one commit group (empty past the last pass).
+template <class O>
+__device__ __forceinline__ void reuse_load(uint4* ring, const O* obs_t, int64_t warp_base, int n_lanes, int K, int s) {
+  const int KV = K >> Vec16<O>::shift;                      // 16-byte words per tile
+  const int passes = (KV + REUSE_WORDS - 1) / REUSE_WORDS;
+  if (s < n_lanes * passes) {
+    const int j = s / passes, q0 = (s - j * passes) * REUSE_WORDS;
+    const uint4* src = reinterpret_cast<const uint4*>(obs_t + (warp_base + j) * (int64_t)K) + q0;
+    uint4* slot = ring + (s % REUSE_STAGES) * REUSE_WORDS;
+    for (int q = threadIdx.x & 31; q < REUSE_WORDS && q0 + q < KV; q += 32) cp_async16(slot + q, src + q);
+  }
+  cp_async_commit();
+}
+// What word `q` of a one-hot tile whose hot element is `h` (-1: none) holds: zero, or the hot word.
+template <class O>
+__device__ __forceinline__ uint4 onehot_word(int h, int q) {
+  constexpr int S = Vec16<O>::shift;
+  uint4 v = make_uint4(0u, 0u, 0u, 0u);
+  if (h >= 0 && q == (h >> S)) {
+    const int hb = (h & ((1 << S) - 1)) * (int)sizeof(O), part = hb >> 2;
+    const uint32_t bits = (sizeof(O) == 4 ? 0x3f800000u : one_bits<O>()) << ((hb & 3) * 8);
+    if (part == 0) v.x = bits; else if (part == 1) v.y = bits; else if (part == 2) v.z = bits; else v.w = bits;
+  }
+  return v;
+}
+__device__ __forceinline__ bool bits_differ(uint4 a, uint4 b) { return ((a.x ^ b.x) | (a.y ^ b.y) | (a.z ^ b.z) | (a.w ^ b.w)) != 0u; }
+template <class O>
+__device__ __forceinline__ void emit_onehot_reuse(uint4* ring, O* obs_t, int64_t warp_base, int n_lanes, int K, int hot) {
+  constexpr int S = Vec16<O>::shift;
+  const int tid = threadIdx.x & 31;
+  const int KV = K >> S;
+  const int passes = (KV + REUSE_WORDS - 1) / REUSE_WORDS;
+  const int n = n_lanes * passes;
+  // The probe: the first 32 words (512 bytes) of the chunk's first tile decide whether the chunk is read at all.
+  const int h0 = __shfl_sync(0xffffffffu, hot, 0);
+  const uint4* tile0 = reinterpret_cast<const uint4*>(obs_t + warp_base * (int64_t)K);
+  if (tid < KV) cp_async16(ring + tid, tile0 + tid);
+  cp_async_commit();
+  cp_async_wait<0>();
+  bool blind = __popc(__ballot_sync(0xffffffffu, tid < KV && bits_differ(ring[tid], onehot_word<O>(h0, tid)))) > 2;
+  if (!blind) for (int k = 0; k < REUSE_STAGES; ++k) reuse_load(ring, obs_t, warp_base, n_lanes, K, k);
+  for (int s = 0; s < n; ++s) {
+    const int j = s / passes, q0 = (s - j * passes) * REUSE_WORDS;
+    const int h = __shfl_sync(0xffffffffu, hot, j);
+    uint4* dst = reinterpret_cast<uint4*>(obs_t + (warp_base + j) * (int64_t)K) + q0;
+    const uint4* slot = ring + (s % REUSE_STAGES) * REUSE_WORDS;
+    if (!blind) cp_async_wait<REUSE_STAGES - 1>();           // this thread's words of pass s have landed
+    unsigned differing = 0;
+#pragma unroll 2
+    for (int u = 0; u < REUSE_WORDS / 32 && u * 32 < KV - q0; ++u) {
+      const int q = u * 32 + tid;
+      const bool in = q0 + q < KV;
+      const uint4 v = onehot_word<O>(h, q0 + q);
+      const bool differs = in && (blind || bits_differ(slot[q], v));
+      const unsigned mask = __ballot_sync(0xffffffffu, differs);
+      differing += __popc(mask);
+      // a differing word is stored with the rest of its REUSE_STORE_WORDS-word block
+      const unsigned block = (unsigned)((1ull << REUSE_STORE_WORDS) - 1ull) << (tid & ~(REUSE_STORE_WORDS - 1));
+      if (in && (mask & block) != 0u) __stcs(dst + q, v);
+    }
+    if (!blind) {
+      blind = differing > 2u;
+      if (!blind) reuse_load(ring, obs_t, warp_base, n_lanes, K, s + REUSE_STAGES);     // into the slot just compared
+    }
+  }
+  cp_async_wait<0>();                                       // nothing lands in the ring after the emitter returns
 }
 
 // Boards with up to two hot cells; the warp's boards form one contiguous span.  Its start is 16-byte aligned
@@ -711,7 +808,7 @@ __device__ __forceinline__ WarpStage<O> clear_stages(const EnvParams& p, const L
   constexpr int kEmit = EmitKind<F>::value;
   const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
   constexpr int S = Vec16<O>::shift;
-  const size_t stage_elems = smem_elems_per_warp<F, O>(p.obs_numel, a.emit_bulk != 0, a.group_lanes, a.stage_rows);
+  const size_t stage_elems = smem_elems_per_warp<F, O>(p.obs_numel, a.emit_bulk != 0, a.emit_reuse != 0, a.group_lanes, a.stage_rows);
   WarpStage<O> ws;
   ws.stage = reinterpret_cast<O*>(smem_raw) + (size_t)warp * stage_elems;
   ws.cta_zero = reinterpret_cast<O*>(smem_raw) + (size_t)warps_per_cta * stage_elems;
@@ -754,13 +851,20 @@ __device__ __forceinline__ bool chunk_is_bulk(const EnvParams& p, const LaunchAr
   if (kEmit == EMIT_IMAGE) bulk = bulk && (K & 3) == 0;
   return bulk;
 }
+// Whether a one-hot chunk that does not go through the TMA unit goes through emit_onehot_reuse: the launch asks for
+// it and the tiles are whole 16-byte words.
+template <class O>
+__device__ __forceinline__ bool reuse_chunk(const LaunchArgs& a, bool vec, int K) {
+  return a.emit_reuse && vec && (K & ((1 << Vec16<O>::shift) - 1)) == 0;
+}
 
 // Observation emitter of the warp for one chunk and step.  Every element is converted where it is written to the
-// stage or to global memory (obs_cast).
+// stage or to global memory (obs_cast).  `reuse`: one-hot tiles may go through emit_onehot_reuse (the launch's
+// observations; final observations of same-step handles, whose buffer the launch plan did not look at, never do).
 template <class F, class O, class R>
 __device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a, WarpStage<O>& ws, const typename F::Lane& L,
                                          R& rng, O* obs_t, int64_t warp_base, int n_lanes, int64_t lane, bool active,
-                                         bool bulk, bool vec) {
+                                         bool bulk, bool vec, bool reuse = true) {
   constexpr int kEmit = EmitKind<F>::value;
   constexpr int V1 = (1 << Vec16<O>::shift) - 1;
   const int tid = threadIdx.x & 31;
@@ -796,6 +900,8 @@ __device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a
         }
         ++ws.emitted;
       }
+    } else if (reuse && reuse_chunk<O>(a, vec, K)) {
+      emit_onehot_reuse(reinterpret_cast<uint4*>(ws.stage), obs_t, warp_base, n_lanes, K, hot);
     } else {
       emit_onehot_vec(obs_t, warp_base, n_lanes, K, hot, vec && (K & V1) == 0);
     }
@@ -849,7 +955,7 @@ __device__ __forceinline__ void emit_obs(const EnvParams& p, const LaunchArgs& a
 // Same-step handles: the final observation of every lane whose step returned LAST, rendered from the lane as it was
 // before the merged reset; the rows of other lanes are left untouched.  Lanes step in lock-step and most episodes
 // have a fixed length, so usually the whole chunk finishes together: then its rows leave through the observation's
-// own emitter (bulk, vector or scalar stores, by the same rules).  Otherwise only the finished lanes' rows are
+// own emitter (bulk, vector or scalar stores, by the same rules; never compare-then-store).  Otherwise only the finished lanes' rows are
 // written, each by the whole warp with streaming stores (rows: by the lane's own thread).
 // Rows are the exception to "the same rules": their stages serve bulk and non-bulk emits alike, and a non-bulk emit
 // neither waits for the TMA unit's reads of a stage nor keeps the stage parity in step with the committed groups.
@@ -868,7 +974,7 @@ __device__ __forceinline__ void emit_final(const EnvParams& p, const LaunchArgs&
   const bool bulk = chunk_is_bulk<F, O>(p, a, vec, n_lanes);
   if (done == (n_lanes >= 32 ? 0xffffffffu : ((1u << n_lanes) - 1u)) && (kEmit != EMIT_ROWS || bulk == obs_bulk)) {
     ws.any_bulk = ws.any_bulk || bulk;
-    emit_obs<F>(p, a, ws, m.last, m.rng, fin_t, warp_base, n_lanes, lane, active, bulk, vec);
+    emit_obs<F>(p, a, ws, m.last, m.rng, fin_t, warp_base, n_lanes, lane, active, bulk, vec, /*reuse=*/false);
     return;
   }
   if (kEmit == EMIT_ROWS) {

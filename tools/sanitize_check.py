@@ -54,7 +54,8 @@ if '--only-split' in sys.argv:
 
 def buffers(env, bsuite_id, plain, num_steps=None):
   """Bulk stores land in `plain` torch.empty memory; the other leg writes where the store path changes: the
-  compressible pool (make_buffers) for deep_sea, whose large batches then take 16-byte streaming stores, and an
+  compressible pool (make_buffers) for deep_sea, whose large batches then compare each tile with the destination
+  (single steps) or take 16-byte streaming stores (rollouts), and an
   observation one float past a 16-byte boundary (vector / scalar stores) for every other family."""
   out = env.make_buffers(num_steps)
   n = out.observation.numel()
