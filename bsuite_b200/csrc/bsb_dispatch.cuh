@@ -93,11 +93,10 @@ struct Geometry { int threads = 0; size_t smem = 0; int64_t n_chunks = 0, grid =
 
 // Chunk lanes, emitter plan (group lanes, stage rows), CTA size, shared memory and grid of a launch; fills a's
 // emitter fields and, for a persistent grid (the deep_sea and mnist bulk paths, once the grid exceeds what is
-// resident), its chunk counter.  The rest is for two-phase host steps: `no_obs`: no observation (no shared memory:
-// co-resident with another handle's observation stream), one chunk per warp; `extra_threads` > 0 puts
-// g.extra_blocks blocks of that many threads in all (at least one) in front of the chunk owners.
+// resident), its chunk counter.  `extra_threads` > 0 (the copiers of two-phase host steps) puts g.extra_blocks
+// blocks of that many threads in all (at least one) in front of the chunk owners.
 template <class F, class O>
-int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, bool no_obs = false, int extra_threads = 0) {
+int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int extra_threads = 0) {
   const int K = e->p.obs_numel;
   const bool is_onehot = EmitKind<F>::value == EMIT_ONEHOT;
   const bool is_image = EmitKind<F>::value == EMIT_IMAGE;
@@ -172,7 +171,6 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, bool no_obs = false, int
     }
   }
   a.use_pdl = (a.mode == MODE_STEP && a.T == 1) ? 1 : 0;
-  if (no_obs) { a.emit_bulk = 0; a.emit_reuse = 0; a.stage_rows = 0; a.cta_extra_elems = 0; a.group_lanes = 1; threads = 128; persistent = false; }
   size_t per_warp = smem_elems_per_warp<F, O>(K, a.emit_bulk != 0, a.emit_reuse != 0, a.group_lanes, a.stage_rows) * elem;
   if ((EmitKind<F>::value == EMIT_ROWS || EmitKind<F>::value == EMIT_TWOHOT) && per_warp > 96 * 1024) {
     // rows / boards too long for a per-warp stage: long rows always get ONE stage (above), so the limit is
@@ -235,15 +233,13 @@ int device_launch(bsb_env* e, LaunchArgs a, cudaStream_t stream) {
   return rc != BSB_OK ? rc : launch(e, a, g, stream, transition_kernel<typename KernelTag<F, O, kSameStep>::type, RK, kNoise, kTrack>, e->p, a);
 }
 
-// Two-phase host step (DeepSea, Catch): one launch (h.phase 0) or one of the two launches of a split step.
+// Two-phase host step (DeepSea, Catch): one launch per step.
 template <class F, int RK, bool kNoise, bool kTrack, class O>
 int two_phase_launch(bsb_env* e, LaunchArgs a, TwoPhaseArgs h, cudaStream_t stream) {
   if (a.clock) return fail(BSB_INTERNAL, "a host step reached graph-safe mode, which turns the mailbox path off");
-  // Copiers: enough of them for ~512 threads, i.e. ~64 KB of 16-byte loads in flight.  The observation-only launch
-  // of a split step has none.
+  // Copiers: enough of them for ~512 threads, i.e. ~64 KB of 16-byte loads in flight.
   Geometry g;
-  const bool obs_only = h.phase == 2;
-  const int rc = plan_launch<F, O>(e, a, g, h.phase == 1, obs_only ? 0 : 512);
+  const int rc = plan_launch<F, O>(e, a, g, 512);
   if (rc != BSB_OK) return rc;
   h.copiers = g.extra_blocks;
   return launch(e, a, g, stream, two_phase_host_kernel<typename KernelFamily<F, O>::type, RK, kNoise, kTrack>, e->p, a, h);

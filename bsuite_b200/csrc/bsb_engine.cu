@@ -237,35 +237,38 @@ bool family_obs_from_state(const bsb_env* e) {
   return !e->same_step && !e->packed && (e->p.family == BSB_DEEP_SEA || e->p.family == BSB_CATCH) && (size_t)e->p.obs_numel * sizeof(float) >= 1024;
 }
 
-// Enqueues the step of `actions` into the device-addressable buffers `out`, which signals `ticket` through the
-// mailbox.  `split`: BSB_HOST_NO_WAIT.
-int mailbox_launch(bsb_env* e, unsigned long long ticket, const int32_t* actions, const bsb_outputs& out, bool split) {
-  LaunchArgs a = make_args(e, &out, actions, 1, MODE_STEP);
-  a.mailbox = e->mailbox_dev; a.mail = e->mail; a.ticket = ticket;
-  { static const int timing = getenv("BSB_HOST_TIMING") ? atoi(getenv("BSB_HOST_TIMING")) : 0; a.timing = timing; }
-  if (!family_obs_from_state(e)) return run(e, a, e->copy_stream);
-  // device staging of the scalars: reward | discount | step_type in one block (as the staged-copy path keeps them)
+// Device staging of the scalars of host steps: reward | discount | step_type in ONE block, so that a caller who
+// keeps its three host arrays back to back (BatchedEnvironment.make_host_buffers does) gets them with a single D2H
+// copy; float64 rewards in a block of their own when `f64`.
+int alloc_scalar_staging(bsb_env* e, bool f64) {
   const size_t B = (size_t)e->p.batch;
   if (!e->d_reward) {
     BSB_CUDA(cudaMalloc(&e->d_reward, 3 * B * 4));
     e->d_discount = e->d_reward + B;
     e->d_step_type = reinterpret_cast<int32_t*>(e->d_reward + 2 * B);
   }
-  if (!e->d_reward64) BSB_CUDA(cudaMalloc(&e->d_reward64, B * 8));
+  if (f64 && !e->d_reward64) BSB_CUDA(cudaMalloc(&e->d_reward64, B * 8));
+  return BSB_OK;
+}
+
+// True when the caller's reward, discount and step_type arrays lie back to back in one block of 3 * B words.
+bool scalars_back_to_back(const bsb_outputs& out, size_t B) {
+  return out.reward && out.discount == out.reward + B &&
+         reinterpret_cast<char*>(out.step_type) == reinterpret_cast<char*>(out.reward + 2 * B);
+}
+
+// Enqueues the step of `actions` into the device-addressable buffers `out`, which signals `ticket` through the
+// mailbox.
+int mailbox_launch(bsb_env* e, unsigned long long ticket, const int32_t* actions, const bsb_outputs& out) {
+  LaunchArgs a = make_args(e, &out, actions, 1, MODE_STEP);
+  a.mailbox = e->mailbox_dev; a.mail = e->mail; a.ticket = ticket;
+  { static const int timing = getenv("BSB_HOST_TIMING") ? atoi(getenv("BSB_HOST_TIMING")) : 0; a.timing = timing; }
+  if (!family_obs_from_state(e)) return run(e, a, e->copy_stream);
+  { int src = alloc_scalar_staging(e, true); if (src != BSB_OK) return src; }
   TwoPhaseArgs h;
   memset(&h, 0, sizeof(h));
   h.stage.reward = e->d_reward; h.stage.reward_f64 = e->d_reward64; h.stage.discount = e->d_discount; h.stage.step_type = e->d_step_type;
   e->early_inflight = true;
-  if (split) {
-    // BSB_HOST_NO_WAIT: the caller alternates between handles.  Two launches instead of one -- transitions + copiers
-    // (no shared memory), then the observation stream -- so that THIS handle's transitions and PCIe traffic run
-    // while the OTHER handle's observations have the SMs' shared memory and the HBM.
-    h.phase = 1;
-    int rc = run(e, a, e->copy_stream, &h);
-    if (rc != BSB_OK) return rc;
-    a.mailbox = nullptr;
-    h.phase = 2;
-  }
   return run(e, a, e->copy_stream, &h);
 }
 
@@ -956,9 +959,7 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
   void* d_reward = host_out->reward ? mapped_device_pointer(env, host_out->reward) : nullptr;
   void* d_reward64 = host_out->reward_f64 ? mapped_device_pointer(env, host_out->reward_f64) : nullptr;
   void *d_discount = nullptr, *d_step_type = nullptr;
-  const bool packed_scalars = d_reward && host_out->discount == host_out->reward + B &&
-                              reinterpret_cast<char*>(host_out->step_type) == reinterpret_cast<char*>(host_out->reward + 2 * B);
-  if (packed_scalars) {       // reward | discount | step_type back to back in one pinned block: one query covers all
+  if (d_reward && scalars_back_to_back(*host_out, B)) {      // one pinned block: one query covers all three
     d_discount = static_cast<float*>(d_reward) + B;
     d_step_type = static_cast<float*>(d_reward) + 2 * B;
   } else {
@@ -1008,7 +1009,7 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
       BSB_CUDA(cudaStreamWaitEvent(zs, env->h2d_event, 0));
       dev_actions = env->h2d_actions;
     }
-    { int lrc = mailbox_launch(env, ticket, dev_actions, dev, (flags & BSB_HOST_NO_WAIT) != 0); if (lrc != BSB_OK) return lrc; }
+    { int lrc = mailbox_launch(env, ticket, dev_actions, dev); if (lrc != BSB_OK) return lrc; }
     if ((flags & BSB_HOST_FENCE_CALLER) && env->early_inflight) {
       // Two-phase step: the observation stores outlive this call.  Fence the caller's stream behind the kernel:
       // whatever the caller enqueues there afterwards sees complete observations.
@@ -1017,8 +1018,8 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
       BSB_CUDA(cudaStreamWaitEvent(static_cast<cudaStream_t>(caller_stream), env->fence_event, 0));
     }
     if (flags & BSB_HOST_NO_WAIT) {
-      // Split call: the completion word is collected by bsb_host_wait (or by whichever entry point of this handle
-      // runs next), so the caller can drive ANOTHER handle while this step's scalars cross PCIe.
+      // The completion word is collected by bsb_host_wait (or by whichever entry point of this handle runs next),
+      // so the caller can drive ANOTHER handle while this step's scalars cross PCIe.
       env->awaiting_ticket = ticket;
       return BSB_OK;
     }
@@ -1029,14 +1030,7 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
   // Staged copies (a pageable buffer among them): actions in, bsb_step on device scratch, scalars out.
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
   if (!env->h2d_actions) BSB_CUDA(cudaMalloc(&env->h2d_actions, B * 4));
-  // reward | discount | step_type live in ONE device block so that a caller who keeps its three host arrays
-  // back to back (BatchedEnvironment.make_host_buffers does) gets them with a single D2H copy.
-  if (!env->d_reward) {
-    BSB_CUDA(cudaMalloc(&env->d_reward, 3 * B * 4));
-    env->d_discount = env->d_reward + B;
-    env->d_step_type = reinterpret_cast<int32_t*>(env->d_reward + 2 * B);
-  }
-  if (host_out->reward_f64 && !env->d_reward64) BSB_CUDA(cudaMalloc(&env->d_reward64, B * 8));
+  { int src = alloc_scalar_staging(env, host_out->reward_f64 != nullptr); if (src != BSB_OK) return src; }
   if (!device_obs && !env->d_obs) BSB_CUDA(cudaMalloc(&env->d_obs, obs_bytes));
   { int vrc = check_host_actions(env, actions, (int64_t)B); if (vrc != BSB_OK) return vrc; }
   cudaStream_t s = env->copy_stream;
@@ -1050,10 +1044,7 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
   dev.step_type = host_out->step_type ? env->d_step_type : nullptr;
   int rc = bsb_step(env, env->h2d_actions, &dev, s);
   if (rc != BSB_OK) return rc;
-  const bool packed = host_out->reward && host_out->discount && host_out->step_type &&
-                      host_out->discount == host_out->reward + B &&
-                      reinterpret_cast<char*>(host_out->step_type) == reinterpret_cast<char*>(host_out->reward + 2 * B);
-  if (packed) {
+  if (scalars_back_to_back(*host_out, B)) {
     BSB_CUDA(cudaMemcpyAsync(host_out->reward, env->d_reward, 3 * B * 4, cudaMemcpyDeviceToHost, s));
   } else {
     if (host_out->reward) BSB_CUDA(cudaMemcpyAsync(host_out->reward, dev.reward, B * 4, cudaMemcpyDeviceToHost, s));

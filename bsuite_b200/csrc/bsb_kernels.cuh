@@ -95,9 +95,6 @@ struct LaunchArgs {
 // The arguments only two_phase_host_kernel takes.
 struct TwoPhaseArgs {
   int32_t copiers;          // blocks [0, copiers) own no chunks at first: they ship the scalars to the host (see the kernel)
-  int32_t phase;            // step split over TWO launches (BSB_HOST_NO_WAIT): 1 = transitions + copiers only (no shared
-                            // memory: co-resident with another handle's observation stream), 2 = observations only
-                            // (waits for mail->phase1 == ticket, not for launch 1 to END); 0 = one launch
   MailFields stage;         // device staging of reward / reward_f64 / discount / step_type
 };
 
@@ -1141,9 +1138,8 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
 // the last one stores the completion word; then they join phase 2 through the chunk counter like everybody else.
 // (PTX memory model: workers release / copiers acquire at gpu scope; the copiers' own stores, fence.sc.sys and the
 // completion word are program-ordered; the host's acquire load of the word therefore sees every scalar.)
-// A step split over two launches (h.phase 1 / 2, BSB_HOST_NO_WAIT) runs phase 1 with the copiers in the first and
-// phase 2 in the second, which waits for mail->phase1 instead of for the first launch to end.  Host steps never
-// run in graph-safe mode (the launcher checks): there is no device clock here.
+// Every host step, BSB_HOST_NO_WAIT included, is one launch of this kernel.  Host steps never run in graph-safe
+// mode (the launcher checks): there is no device clock here.
 template <class F, int RK, bool kNoise, bool kTrack>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F))
 two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs h) {
@@ -1154,9 +1150,7 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
   const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
   const int64_t B = p.batch;
   WarpStage<O> ws = clear_stages<Fam, O>(p, a);
-  // The observation-only launch must not wait for its predecessor -- the transitions launch, whose copiers are
-  // still shipping scalars over PCIe -- to END: it waits for that launch's phase-1 flag instead.
-  if (a.use_pdl) { if (h.phase != 2) pdl_wait(); pdl_launch_dependents(); }
+  if (a.use_pdl) { pdl_wait(); pdl_launch_dependents(); }
   const bool vec = a.obs_vec_ok != 0;
   O* const obs = reinterpret_cast<O*>(a.obs);       // the ABI's float* addresses elements of type O
 
@@ -1250,9 +1244,6 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
     }
     // join phase 2: the copiers own no chunk of their own, the counter deals them the rest
     render_stored(dynamic ? fetch_chunk(a, total_warps) : n_chunks, false, keep);
-  } else if (h.phase == 2) {
-    // observation-only launch: the transitions launch ahead of it in the stream stored every lane's state
-    render_stored(own, false, keep);
   } else {
     constexpr int kAhead = 4;              // chunks whose loads (action, lane state, accumulators) are in flight together
     for (int64_t c0 = own; c0 < n_chunks; c0 += kAhead * total_warps) {
@@ -1297,7 +1288,7 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
     __threadfence();                       // gpu scope (device memory only): the copiers do the system-scope one
     __syncthreads();
     if (threadIdx.x == 0) atomicAdd(&a.mail->finished, 1ull);
-    render_stored(h.phase == 1 ? n_chunks : own, true, keep);      // split step: the observations are the next launch's
+    render_stored(own, true, keep);
   }
   retire_warp(a, ws, false);
 }

@@ -506,9 +506,9 @@ int32_t bsb_set_state(bsb_env* env, const void* src_host, int64_t nbytes,
  *       half remains the reference's strict loop (act on what the previous step
  *       returned) and the GPU is not left idle in between (two to four handles).
  *       Pass BSB_HOST_FENCE_CALLER with it: without the fence's event record between
- *       a handle's observation launch and its next launch, the next launch parks
- *       its CTAs behind the other handles' work and the loop slows down.  Not with
- *       BSB_HOST_PRELAUNCH.
+ *       a handle's consecutive launches, the next launch becomes a programmatic
+ *       dependent of the previous one, parks its CTAs behind the other handles'
+ *       work and the loop slows down.  Not with BSB_HOST_PRELAUNCH.
  */
 #define BSB_HOST_ORDER_AFTER_STREAM 1u
 #define BSB_HOST_PRELAUNCH 2u

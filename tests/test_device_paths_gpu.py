@@ -22,8 +22,8 @@ also go through oracle.run_lanes, which anchors the comparison outside the engin
   group C  the CTA sizes, deep_sea group sizes, vector fallbacks and mnist group sizes that only larger boards,
            tiles and images reach;
   group H  every instantiation two_phase_host_kernel<deep_sea | catch, Philox | MT19937, noise, track> (16 kernels),
-           driven by host steps (bsb_step_host on pinned buffers): waited for, and BSB_HOST_NO_WAIT (which splits
-           the step over two launches).
+           driven by host steps (bsb_step_host on pinned buffers): waited for, and BSB_HOST_NO_WAIT (the same
+           launch, collected by host_wait()).
 
 Exactness follows tests/conftest.py: integer / grid families bit for bit (step_type, discount, reward, observation,
 bsuite_info, episode_stats, log rows, state blob); float dynamics, the reward-noise wrapper and stochastic deep_sea

@@ -224,7 +224,7 @@ def test_two_phase_host_steps_with_ragged_batches_and_float64_rewards(bsuite_id,
   np.testing.assert_array_equal(a.state_dict()['blob'], b.state_dict()['blob'])
 
 
-# ---------------------------------------------------------------------------- split host steps (BSB_HOST_NO_WAIT)
+# ---------------------------------------------------------------------------- host steps in flight (BSB_HOST_NO_WAIT)
 @pytest.mark.gpu
 @pytest.mark.parametrize('bsuite_id,batch', [('deep_sea/11', 8192 + 37), ('deep_sea_stochastic/3', 300), ('catch/0', 1000),
                                              ('cartpole/0', 777), ('bandit_noise/0', 2)])
@@ -293,6 +293,44 @@ def test_a_step_in_flight_is_collected_by_whatever_runs_next_and_reports_bad_act
   status = env._lib.bsb_step_host(env._handle.ptr, actions[0].data_ptr(), host.as_outputs(), env.make_buffers().observation.data_ptr(),
                                   None, _lib.HOST_NO_WAIT | _lib.HOST_PRELAUNCH)
   assert status != 0
+  env.close(); twin.close()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('name', ['deep_sea/11', 'catch_16x16'])
+def test_a_no_wait_two_phase_host_step_is_the_launch_of_a_waited_step(name):
+  """A BSB_HOST_NO_WAIT step of a two-phase handle (deep_sea N = 32; a catch board of 256 cells, the smallest that
+  takes the two-phase step) is one launch, like a waited step, and after host_wait() it has the waited step's outputs."""
+  from bsuite_b200 import experiments
+  B, T = 4096, 12
+
+  def make():
+    if name == 'catch_16x16':
+      return bsuite_b200.BatchedEnvironment(experiments.catch(rows=16, columns=16), batch=B, device='cuda', seed=4,
+                                            track_episodes=True)
+    return bsuite_b200.load_from_id(name, batch=B, device='cuda', seed=4, track_episodes=True)
+
+  lib = _lib.load()
+  env, twin = make(), make()
+  host, twin_host = env.make_host_buffers(), twin.make_host_buffers()
+  out, twin_out = env.make_buffers(), twin.make_buffers()
+  actions = torch.as_tensor(np.random.RandomState(5).randint(env.num_actions, size=(T, B)).astype(np.int32)).pin_memory()
+  env.reset(); twin.reset()
+  torch.cuda.synchronize()
+  for t in range(T):
+    before = lib.bsb_launch_count()
+    twin.step_host(actions[t], twin_host, out=twin_out)
+    waited = lib.bsb_launch_count() - before
+    before = lib.bsb_launch_count()
+    env.step_host(actions[t], host, out=out, wait=False)
+    assert lib.bsb_launch_count() - before == waited == 1, t
+    env.host_wait()
+    assert lib.bsb_launch_count() - before == 1, t
+    for field in ('step_type', 'reward', 'discount'):
+      np.testing.assert_array_equal(_np(getattr(host, field)), _np(getattr(twin_host, field)), err_msg=f'{field} t={t}')
+    torch.cuda.synchronize()
+    assert torch.equal(out.observation, twin_out.observation), t
+  np.testing.assert_array_equal(env.state_dict()['blob'], twin.state_dict()['blob'])
   env.close(); twin.close()
 
 

@@ -14,8 +14,8 @@ import bsuite_b200
 
 
 def split_steps():
-  """Split host steps (BSB_HOST_NO_WAIT: transitions + copiers, then the observation-only launch that waits for the
-  phase-1 flag) on 2 / 3 handles driven round-robin, against one ordinary environment."""
+  """Host steps left in flight (BSB_HOST_NO_WAIT) on 2 / 3 handles driven round-robin, against one ordinary
+  environment."""
   from bsuite_b200 import rollouts
   for bsuite_id, batch, parts in (('deep_sea/11', 12000 + 5, 3), ('deep_sea_stochastic/3', 9000, 2)):
     group = rollouts.HostParts(bsuite_id, batch, device='cuda', seed=3, track_episodes=True, parts=parts)
@@ -43,7 +43,7 @@ def split_steps():
         check(p, t - 1, *group.collect(p)); group.submit(p, rows[p][t])
     for p in range(parts):
       check(p, T - 1, *group.collect(p))
-    print(bsuite_id, batch, f'{parts} parts, split host steps == ordinary steps: True', flush=True)
+    print(bsuite_id, batch, f'{parts} parts, round-robin host steps == ordinary steps: True', flush=True)
     group.close(); twin.close()
 
 
