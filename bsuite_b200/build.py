@@ -8,6 +8,7 @@ and depends on nothing from torch.
 """
 
 import os
+import re
 import shutil
 import subprocess
 import sys
@@ -17,10 +18,25 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 FAMILIES = ('deep_sea', 'catch', 'cartpole', 'cartpole_swingup', 'mountain_car', 'memory_chain', 'bandit',
             'umbrella_chain', 'discounting_chain', 'mnist')
-SOURCES = [os.path.join(CSRC, 'bsb_engine.cu'), os.path.join(CSRC, 'bsb_comm.cu'), os.path.join(CSRC, 'bsb_image.cu'),
-           os.path.join(CSRC, 'bsb_memory.cu'), os.path.join(CSRC, 'bsb_score.cu')] + [os.path.join(CSRC, f'fam_{name}.cu') for name in FAMILIES] + [
-    os.path.join(CSRC, f'obs_{name}.cu') for name in FAMILIES] + [os.path.join(CSRC, f'ss_{name}.cu') for name in FAMILIES] + [
-    os.path.join(CSRC, f'pk_{name}.cu') for name in FAMILIES if name != 'deep_sea']
+VARIANTS = os.path.join(CSRC, 'bsb_variants.cu')
+SOURCES = [os.path.join(CSRC, f) for f in ('bsb_engine.cu', 'bsb_comm.cu', 'bsb_image.cu', 'bsb_memory.cu', 'bsb_score.cu')] + [
+    VARIANTS]
+
+
+def variant_list():
+  """The kernel-variant list of bsb_kernels.cuh, {unit: [(family, O, mode, mt, two_phase), ...]}: one
+  `#define BSB_UNIT_<unit>(X)` per translation unit of bsb_variants.cu, one X(...) per variant it compiles."""
+  with open(os.path.join(CSRC, 'bsb_kernels.cuh')) as fh:
+    units = re.findall(r'^#define BSB_UNIT_(\w+)\(X\) (.*)$', fh.read(), re.M)
+  return {unit: [(family, obs, mode, mt == '1', two_phase == '1')
+                 for family, obs, mode, mt, two_phase in re.findall(r'X\((\w+), (\w+), (\w+), ([01]), ([01])\)', row)]
+          for unit, row in units}
+
+
+# Translation units as (object name, source, extra nvcc defines): each source but bsb_variants.cu once, and
+# bsb_variants.cu once per unit of the variant list, with its slice of the list.
+UNITS = [(os.path.basename(src)[:-3], src, []) for src in SOURCES if src != VARIANTS] + [
+    (unit, VARIANTS, [f'-DBSB_UNIT=BSB_UNIT_{unit}']) for unit in variant_list()]
 HEADERS = [os.path.join(CSRC, f) for f in ('bsb_obs_dtype.h', 'bsb_rng.cuh', 'bsb_families.cuh', 'bsb_kernels.cuh', 'bsb_env.h',
                                            'bsb_dispatch.cuh', 'bsb_score.cuh')] + [
     os.path.join(os.path.dirname(HERE), 'include', 'bsuite_b200.h')]
@@ -42,8 +58,8 @@ def find_nvcc() -> str:
   raise RuntimeError('nvcc not found: bsuite_b200 needs the CUDA toolkit to build (no CPU-only build exists)')
 
 
-def _object_path(source: str) -> str:
-  return os.path.join(OBJ_DIR, os.path.basename(source)[:-3] + '.o')
+def _object_path(name: str) -> str:
+  return os.path.join(OBJ_DIR, name + '.o')
 
 
 def _stale(target: str, deps) -> bool:
@@ -57,8 +73,9 @@ def is_stale() -> bool:
   return _stale(OUTPUT, SOURCES + HEADERS)
 
 
-def _compile(nvcc: str, source: str, verbose: bool):
-  cmd = [nvcc] + NVCC_FLAGS + ['-c', source, '-o', _object_path(source)]
+def _compile(nvcc: str, unit, verbose: bool):
+  name, source, defines = unit
+  cmd = [nvcc] + NVCC_FLAGS + defines + ['-c', source, '-o', _object_path(name)]
   if verbose:
     cmd += ['-Xptxas', '-v']
   proc = subprocess.run(cmd, capture_output=True, text=True)
@@ -75,12 +92,12 @@ def build_library(force: bool = False, verbose: bool = False) -> str:
   nvcc = find_nvcc()
   os.makedirs(OBJ_DIR, exist_ok=True)
   start = time.time()
-  todo = [src for src in SOURCES if force or _stale(_object_path(src), [src] + HEADERS)]
+  todo = [unit for unit in UNITS if force or _stale(_object_path(unit[0]), [unit[1]] + HEADERS)]
   with concurrent.futures.ThreadPoolExecutor(max_workers=min(len(todo) or 1, os.cpu_count() or 1)) as pool:
-    for log in pool.map(lambda src: _compile(nvcc, src, verbose), todo):
+    for log in pool.map(lambda unit: _compile(nvcc, unit, verbose), todo):
       if verbose:
         sys.stderr.write(log)
-  cmd = [nvcc, '-shared'] + ARCH + ['-o', OUTPUT] + [_object_path(s) for s in SOURCES] + ['-ldl']
+  cmd = [nvcc, '-shared'] + ARCH + ['-o', OUTPUT] + [_object_path(unit[0]) for unit in UNITS] + ['-ldl']
   proc = subprocess.run(cmd, capture_output=True, text=True)
   if proc.returncode != 0:
     raise RuntimeError('link failed:\n' + ' '.join(cmd) + '\n' + proc.stdout + proc.stderr)

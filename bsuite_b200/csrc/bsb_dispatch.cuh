@@ -1,4 +1,5 @@
-// Host path and kernel launch, instantiated once per family (fam_<name>.cu).
+// Host path and kernel launch, instantiated once per kernel variant in the translation unit the variant list gives it
+// (bsb_variants.cu).
 #pragma once
 #include <type_traits>
 #include <vector>
@@ -38,8 +39,11 @@ template <> struct HostEmit<Mnist> {
 // element by element with obs_cast, the function the kernels use.  kSameStep: a lane whose step returned LAST is reset
 // in the same call, and its final observation goes to a.final_obs when that is given.  kPacked: every lane runs with
 // its setting's parameters (pack_lane_params), as the packed kernels do.
-template <class F, int RK, class O, bool kSameStep = false, bool kPacked = false>
+template <class V, int RK>
 void host_run(const EnvParams& p, const LaunchArgs& a) {
+  typedef typename V::Fam F;
+  typedef typename V::Obs O;
+  constexpr bool kSameStep = V::kSameStep, kPacked = V::kPacked;
   typedef typename RngOf<RK>::type R;
   const int64_t B = p.batch;
   const int K = p.obs_numel;
@@ -226,23 +230,16 @@ int launch(bsb_env* e, const LaunchArgs& a, const Geometry& g, cudaStream_t stre
   return BSB_OK;
 }
 
-template <class F, int RK, bool kNoise, bool kTrack, class O, bool kSameStep = false>
-int device_launch(bsb_env* e, LaunchArgs a, cudaStream_t stream) {
-  Geometry g;
-  const int rc = plan_launch<F, O>(e, a, g);
-  return rc != BSB_OK ? rc : launch(e, a, g, stream, transition_kernel<typename KernelTag<F, O, kSameStep>::type, RK, kNoise, kTrack>, e->p, a);
-}
-
 // Two-phase host step (DeepSea, Catch): one launch per step.
-template <class F, int RK, bool kNoise, bool kTrack, class O>
+template <class V, int RK, bool kNoise, bool kTrack>
 int two_phase_launch(bsb_env* e, LaunchArgs a, TwoPhaseArgs h, cudaStream_t stream) {
   if (a.clock) return fail(BSB_INTERNAL, "a host step reached graph-safe mode, which turns the mailbox path off");
   // Copiers: enough of them for ~512 threads, i.e. ~64 KB of 16-byte loads in flight.
   Geometry g;
-  const int rc = plan_launch<F, O>(e, a, g, 512);
+  const int rc = plan_launch<typename V::Fam, typename V::Obs>(e, a, g, 512);
   if (rc != BSB_OK) return rc;
   h.copiers = g.extra_blocks;
-  return launch(e, a, g, stream, two_phase_host_kernel<typename KernelFamily<F, O>::type, RK, kNoise, kTrack>, e->p, a, h);
+  return launch(e, a, g, stream, two_phase_host_kernel<V, RK, kNoise, kTrack>, e->p, a, h);
 }
 
 // Runs `launch(noise, track)` with the template flags of the launch's wrappers (none for the constructor).
@@ -254,97 +251,33 @@ int with_flags(const bsb_env* e, const LaunchArgs& a, Launch launch) {
   return track ? launch(std::false_type(), std::true_type()) : launch(std::false_type(), std::false_type());
 }
 
-// Float32 observations: both bit sources.  Reduced dtypes and same-step handles: Philox only (bsb_create refuses
-// MT19937 with them).  Same-step handles never take the two-phase host step.
-template <class F, class O, bool kSameStep = false>
-int run_family_as(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoPhaseArgs* two_phase) {
-  constexpr bool kF32 = std::is_same<O, float>::value && !kSameStep;
+// Kernels and host path of variant V, the runner bsb_create stores in the handle.  The bit sources and kernels are
+// those the variant list (BSB_VARIANTS) compiles for V: bsb_create picks no runner for an MT19937 handle whose variant
+// lacks MT19937, and only a variant with two_phase_host_kernel is given `two_phase` (a two-phase host step).
+template <class V>
+int run_variant(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoPhaseArgs* two_phase) {
+  constexpr bool kMt = Compiled<V>::kMt;
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
-  if (!kF32 && mt) return fail(BSB_INTERNAL, "reduced obs_dtype or same-step auto-reset with MT19937");
-  if (kSameStep && two_phase) return fail(BSB_INTERNAL, "a two-phase host step on a same-step handle");
   if (e->device < 0) {
-    if constexpr (kF32) { if (mt) { host_run<F, 1, O>(e->p, a); return BSB_OK; } }
-    host_run<F, 0, O, kSameStep>(e->p, a);
+    if constexpr (kMt) { if (mt) { host_run<V, 1>(e->p, a); return BSB_OK; } }
+    host_run<V, 0>(e->p, a);
     return BSB_OK;
   }
   return with_flags(e, a, [&](auto noise, auto track) {
     constexpr bool kNoise = decltype(noise)::value, kTrack = decltype(track)::value;
-    if constexpr (ObsFromState<F>::value && !kSameStep) {
-      if constexpr (kF32) {
-        if (two_phase) return mt ? two_phase_launch<F, 1, kNoise, kTrack, O>(e, a, *two_phase, stream)
-                                 : two_phase_launch<F, 0, kNoise, kTrack, O>(e, a, *two_phase, stream);
-      } else {
-        if (two_phase) return two_phase_launch<F, 0, kNoise, kTrack, O>(e, a, *two_phase, stream);
+    if constexpr (Compiled<V>::kTwoPhase) {
+      if (two_phase) {
+        if constexpr (kMt) { if (mt) return two_phase_launch<V, 1, kNoise, kTrack>(e, a, *two_phase, stream); }
+        return two_phase_launch<V, 0, kNoise, kTrack>(e, a, *two_phase, stream);
       }
     }
-    if constexpr (kF32) {
-      if (mt) return device_launch<F, 1, kNoise, kTrack, O>(e, a, stream);
-    }
-    return device_launch<F, 0, kNoise, kTrack, O, kSameStep>(e, a, stream);
-  });
-}
-
-// bfloat16 for every family, uint8 for the 0 / 1 observations of deep_sea and catch (BinaryObs).  Instantiated in
-// translation units of their own (obs_<family>.cu): a float32 handle never loads their modules.
-template <class F>
-int run_reduced(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoPhaseArgs* two_phase) {
-  switch (e->obs_dtype) {
-    case BSB_OBS_BFLOAT16: return run_family_as<F, Bf16>(e, a, stream, two_phase);
-    case BSB_OBS_UINT8:
-      if constexpr (BinaryObs<F>::value) return run_family_as<F, uint8_t>(e, a, stream, two_phase);
-      break;
-  }
-  return fail(BSB_INTERNAL, "obs_dtype not compiled for this family");
-}
-#define BSB_REDUCED(F) extern template int run_reduced<F>(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs*);
-BSB_REDUCED(DeepSea) BSB_REDUCED(Catch) BSB_REDUCED(Cartpole) BSB_REDUCED(CartpoleSwingup) BSB_REDUCED(MountainCar)
-BSB_REDUCED(MemoryChain) BSB_REDUCED(Bandit) BSB_REDUCED(UmbrellaChain) BSB_REDUCED(DiscountingChain) BSB_REDUCED(Mnist)
-#undef BSB_REDUCED
-
-// Same-step auto-reset (BSB_FLAG_SAME_STEP_RESET), every obs_dtype, Philox.  Instantiated in translation units of
-// their own (ss_<family>.cu): a next-step handle never loads their modules.
-template <class F>
-int run_same_step(bsb_env* e, const LaunchArgs& a, cudaStream_t stream) {
-  switch (e->obs_dtype) {
-    case BSB_OBS_FLOAT32: return run_family_as<F, float, true>(e, a, stream, nullptr);
-    case BSB_OBS_BFLOAT16: return run_family_as<F, Bf16, true>(e, a, stream, nullptr);
-    case BSB_OBS_UINT8:
-      if constexpr (BinaryObs<F>::value) return run_family_as<F, uint8_t, true>(e, a, stream, nullptr);
-      break;
-  }
-  return fail(BSB_INTERNAL, "obs_dtype not compiled for this family");
-}
-#define BSB_SAME_STEP(F) extern template int run_same_step<F>(bsb_env*, const LaunchArgs&, cudaStream_t);
-BSB_SAME_STEP(DeepSea) BSB_SAME_STEP(Catch) BSB_SAME_STEP(Cartpole) BSB_SAME_STEP(CartpoleSwingup) BSB_SAME_STEP(MountainCar)
-BSB_SAME_STEP(MemoryChain) BSB_SAME_STEP(Bandit) BSB_SAME_STEP(UmbrellaChain) BSB_SAME_STEP(DiscountingChain) BSB_SAME_STEP(Mnist)
-#undef BSB_SAME_STEP
-
-// Packed handles (bsb_create_packed): float32, next-step auto-reset, Philox, every family but deep_sea (whose
-// settings differ in observation shape).  Instantiated in translation units of their own (pk_<family>.cu): an
-// ordinary handle never loads their modules.  Host steps take the single-phase kernel.
-template <class F> struct Packable { static const bool value = !std::is_same<F, DeepSea>::value; };
-template <class F>
-int run_packed(bsb_env* e, const LaunchArgs& a, cudaStream_t stream) {
-  if (e->device < 0) { host_run<F, 0, float, false, true>(e->p, a); return BSB_OK; }
-  return with_flags(e, a, [&](auto noise, auto track) {
     LaunchArgs la = a;
     Geometry g;
-    const int rc = plan_launch<F, float>(e, la, g);
-    return rc != BSB_OK ? rc : launch(e, la, g, stream, transition_kernel<Packed<F>, 0, decltype(noise)::value, decltype(track)::value>, e->p, la);
+    const int rc = plan_launch<typename V::Fam, typename V::Obs>(e, la, g);
+    if (rc != BSB_OK) return rc;
+    if constexpr (kMt) { if (mt) return launch(e, la, g, stream, transition_kernel<V, 1, kNoise, kTrack>, e->p, la); }
+    return launch(e, la, g, stream, transition_kernel<V, 0, kNoise, kTrack>, e->p, la);
   });
-}
-#define BSB_PACKED(F) extern template int run_packed<F>(bsb_env*, const LaunchArgs&, cudaStream_t);
-BSB_PACKED(Catch) BSB_PACKED(Cartpole) BSB_PACKED(CartpoleSwingup) BSB_PACKED(MountainCar) BSB_PACKED(MemoryChain)
-BSB_PACKED(Bandit) BSB_PACKED(UmbrellaChain) BSB_PACKED(DiscountingChain) BSB_PACKED(Mnist)
-#undef BSB_PACKED
-
-// Kernels and host path of the handle's auto-reset mode and observation dtype.
-template <class F>
-int run_family(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr) {
-  if constexpr (Packable<F>::value) { if (e->packed) return run_packed<F>(e, a, stream); }
-  if (e->same_step) return run_same_step<F>(e, a, stream);
-  if (e->obs_dtype != BSB_OBS_FLOAT32) return run_reduced<F>(e, a, stream, two_phase);
-  return run_family_as<F, float>(e, a, stream, two_phase);
 }
 
 }  // namespace bsb

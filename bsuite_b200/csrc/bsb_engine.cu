@@ -92,19 +92,7 @@ int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseA
     if (capture != cudaStreamCaptureStatusNone) e->graph_safe = true;
     if (e->graph_safe) a.clock = e->clock;      // a.step0 == e->steps_done, which no longer moves
   }
-  switch (e->p.family) {
-    case BSB_DEEP_SEA: return run_deep_sea(e, a, stream, two_phase);
-    case BSB_CATCH: return run_catch(e, a, stream, two_phase);
-    case BSB_CARTPOLE: return run_cartpole(e, a, stream);
-    case BSB_CARTPOLE_SWINGUP: return run_cartpole_swingup(e, a, stream);
-    case BSB_MOUNTAIN_CAR: return run_mountain_car(e, a, stream);
-    case BSB_MEMORY_CHAIN: return run_memory_chain(e, a, stream);
-    case BSB_BANDIT: return run_bandit(e, a, stream);
-    case BSB_UMBRELLA_CHAIN: return run_umbrella_chain(e, a, stream);
-    case BSB_DISCOUNTING_CHAIN: return run_discounting_chain(e, a, stream);
-    case BSB_MNIST: return run_mnist(e, a, stream);
-  }
-  return fail(BSB_INVALID_ARGUMENT, "unknown family");
+  return e->variant->run(e, a, stream, two_phase);
 }
 
 LaunchArgs make_args(const bsb_env* e, const bsb_outputs* out, const int32_t* actions, int64_t T, int mode) {
@@ -117,6 +105,29 @@ LaunchArgs make_args(const bsb_env* e, const bsb_outputs* out, const int32_t* ac
   a.obs_vec_ok = (out && (reinterpret_cast<uintptr_t>(out->observation) % 16 == 0) && (T == 1 || step_bytes % 16 == 0)) ? 1 : 0;
   a.final_vec_ok = (a.final_obs && (reinterpret_cast<uintptr_t>(a.final_obs) % 16 == 0) && (T == 1 || step_bytes % 16 == 0)) ? 1 : 0;
   return a;
+}
+
+// The bsb_family of each family and the bsb_obs_dtype of each observation element type.
+template <class F> struct FamilyId;
+#define BSB_FAMILY_ID(F, id) template <> struct FamilyId<F> { static const int value = id; };
+BSB_FAMILY_ID(DeepSea, BSB_DEEP_SEA) BSB_FAMILY_ID(Catch, BSB_CATCH) BSB_FAMILY_ID(Cartpole, BSB_CARTPOLE)
+BSB_FAMILY_ID(CartpoleSwingup, BSB_CARTPOLE_SWINGUP) BSB_FAMILY_ID(MountainCar, BSB_MOUNTAIN_CAR)
+BSB_FAMILY_ID(MemoryChain, BSB_MEMORY_CHAIN) BSB_FAMILY_ID(Bandit, BSB_BANDIT) BSB_FAMILY_ID(UmbrellaChain, BSB_UMBRELLA_CHAIN)
+BSB_FAMILY_ID(DiscountingChain, BSB_DISCOUNTING_CHAIN) BSB_FAMILY_ID(Mnist, BSB_MNIST)
+#undef BSB_FAMILY_ID
+template <class O> constexpr int obs_dtype_id() {
+  return std::is_same<O, float>::value ? BSB_OBS_FLOAT32 : std::is_same<O, Bf16>::value ? BSB_OBS_BFLOAT16 : BSB_OBS_UINT8;
+}
+
+#define BSB_ENTRY(F, O, mode, mt, two_phase) {FamilyId<F>::value, obs_dtype_id<O>(), mode, mt, two_phase, &run_variant<Variant<F, O, mode> >},
+const VariantEntry kVariants[] = {BSB_VARIANTS(BSB_ENTRY)};
+#undef BSB_ENTRY
+
+// The compiled variant of a family, obs_dtype and mode that runs bit source `rng_kind`, or nullptr.
+const VariantEntry* find_variant(int family, int obs_dtype, int mode, int rng_kind) {
+  for (const VariantEntry& v : kVariants)
+    if (v.family == family && v.obs_dtype == obs_dtype && v.mode == mode && (rng_kind != BSB_RNG_MT19937 || v.mt)) return &v;
+  return nullptr;
 }
 
 int validate(const bsb_config& c, int64_t batch, int* obs_rows, int* obs_cols, int* n_actions) {
@@ -160,11 +171,11 @@ int validate(const bsb_config& c, int64_t batch, int* obs_rows, int* obs_cols, i
     default: return fail(BSB_INVALID_ARGUMENT, "unknown family");
   }
   if (c.obs_dtype < BSB_OBS_FLOAT32 || c.obs_dtype > BSB_OBS_UINT8) return fail(BSB_INVALID_ARGUMENT, "unknown obs_dtype");
-  if (c.obs_dtype == BSB_OBS_UINT8 && c.family != BSB_DEEP_SEA && c.family != BSB_CATCH)
+  if (!find_variant(c.family, c.obs_dtype, NEXT_STEP, BSB_RNG_PHILOX))
     return fail(BSB_UNSUPPORTED, "obs_dtype uint8 is only available for deep_sea and catch, whose observations are 0 / 1");
-  if (c.obs_dtype != BSB_OBS_FLOAT32 && c.rng_kind == BSB_RNG_MT19937)
+  if (!find_variant(c.family, c.obs_dtype, NEXT_STEP, c.rng_kind))
     return fail(BSB_UNSUPPORTED, "a bfloat16 or uint8 obs_dtype needs rng_kind BSB_RNG_PHILOX");
-  if ((c.flags & BSB_FLAG_SAME_STEP_RESET) && c.rng_kind == BSB_RNG_MT19937)
+  if ((c.flags & BSB_FLAG_SAME_STEP_RESET) && !find_variant(c.family, c.obs_dtype, SAME_STEP, c.rng_kind))
     return fail(BSB_UNSUPPORTED, "BSB_FLAG_SAME_STEP_RESET needs rng_kind BSB_RNG_PHILOX");
   if (c.log_schedule_len < 0 || c.log_schedule_len > 4096) return fail(BSB_INVALID_ARGUMENT, "log_schedule_len must be in [0, 4096]");
   if (c.log_schedule_len > 0) {
@@ -232,9 +243,9 @@ int mailbox_open(bsb_env* e) {
 // lane out, 4 B in): deep_sea from N = 16 up (>= 1 KB of observation per lane).  catch (200 B per lane) is bound
 // by the 2 MB of scalars per step either way and keeps the single-phase kernel.  The rule counts float32 bytes
 // whatever the handle's obs_dtype, so a reduced-dtype handle takes the same path as its float32 twin.
-// Same-step and packed handles always take the single-phase kernel.
+// Only the variants the list compiles two_phase_host_kernel for (deep_sea and catch, next-step) take it.
 bool family_obs_from_state(const bsb_env* e) {
-  return !e->same_step && !e->packed && (e->p.family == BSB_DEEP_SEA || e->p.family == BSB_CATCH) && (size_t)e->p.obs_numel * sizeof(float) >= 1024;
+  return e->variant->two_phase && (size_t)e->p.obs_numel * sizeof(float) >= 1024;
 }
 
 // Device staging of the scalars of host steps: reward | discount | step_type in ONE block, so that a caller who
@@ -414,6 +425,9 @@ static int32_t create_env(const bsb_config* config, int64_t batch, int32_t devic
   int obs_rows = 0, obs_cols = 0, n_actions = 0;
   int rc = validate(c, batch, &obs_rows, &obs_cols, &n_actions);
   if (rc != BSB_OK) return rc;
+  const int mode = n_settings > 0 ? PACKED : (c.flags & BSB_FLAG_SAME_STEP_RESET) ? SAME_STEP : NEXT_STEP;
+  const VariantEntry* variant = find_variant(c.family, c.obs_dtype, mode, c.rng_kind);
+  if (!variant) return fail(BSB_INTERNAL, "no compiled kernel variant for this family, obs_dtype, mode and rng_kind");
   if (device >= 0) {
     int count = 0;
     cudaError_t err = cudaGetDeviceCount(&count);
@@ -430,6 +444,7 @@ static int32_t create_env(const bsb_config* config, int64_t batch, int32_t devic
   e->device = device; e->steps_done = 0;
   e->obs_dtype = c.obs_dtype; e->obs_elem_bytes = c.obs_dtype == BSB_OBS_BFLOAT16 ? 2 : c.obs_dtype == BSB_OBS_UINT8 ? 1 : 4;
   e->same_step = (c.flags & BSB_FLAG_SAME_STEP_RESET) != 0;
+  e->variant = variant;
   e->packed = n_settings > 0; e->n_settings = n_settings > 0 ? n_settings : 1;
   e->lanes_per_setting = n_settings > 0 ? batch / n_settings : batch;
   e->graph_safe = false; e->clock = nullptr; e->sum_scratch = nullptr; e->names = info_names(c.family);
@@ -613,9 +628,10 @@ int32_t bsb_create_packed(const bsb_config* configs, int32_t n_settings, int64_t
     if (rc != BSB_OK) return fail(rc, "setting " + std::to_string(k) + ": " + last_error_cstr());
   }
   const bsb_config& c = configs[0];
-  if (c.family == BSB_DEEP_SEA) return fail(BSB_UNSUPPORTED, "deep_sea has no packed kernel (its settings differ in size)");
-  if (c.rng_kind == BSB_RNG_MT19937) return fail(BSB_UNSUPPORTED, "packed handles need rng_kind BSB_RNG_PHILOX");
-  if (c.obs_dtype != BSB_OBS_FLOAT32) return fail(BSB_UNSUPPORTED, "packed handles write float32 observations only");
+  if (!find_variant(c.family, BSB_OBS_FLOAT32, PACKED, BSB_RNG_PHILOX))
+    return fail(BSB_UNSUPPORTED, "deep_sea has no packed kernel (its settings differ in size)");
+  if (!find_variant(c.family, BSB_OBS_FLOAT32, PACKED, c.rng_kind)) return fail(BSB_UNSUPPORTED, "packed handles need rng_kind BSB_RNG_PHILOX");
+  if (!find_variant(c.family, c.obs_dtype, PACKED, c.rng_kind)) return fail(BSB_UNSUPPORTED, "packed handles write float32 observations only");
   if (c.flags & BSB_FLAG_SAME_STEP_RESET) return fail(BSB_UNSUPPORTED, "packed handles do not take BSB_FLAG_SAME_STEP_RESET");
   for (int32_t k = 1; k < n_settings; ++k)
     if (const char* field = packed_mismatch(c, configs[k]))

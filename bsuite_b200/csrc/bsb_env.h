@@ -1,4 +1,4 @@
-// Internal declarations shared by the engine and the per-family translation units.
+// Internal declarations shared by the engine and the kernel-variant translation units.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -23,6 +23,16 @@ struct bsb_env;
 namespace bsb {
 int drain_log_rows(bsb_env* e);                         // waits out host steps in flight, as bsb_read_log_rows does
 
+// Kernels and host path of kernel variant V (bsb_dispatch.cuh), explicitly instantiated for each entry of the variant
+// list (BSB_VARIANTS) in the translation unit the list gives it (bsb_variants.cu).  `two_phase`: a two-phase host step.
+template <class V> int run_variant(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs* two_phase);
+// An entry of the variant list, as bsb_create looks it up (bsb_engine.cu).
+struct VariantEntry {
+  int family, obs_dtype, mode;
+  bool mt, two_phase;
+  int (*run)(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs*);
+};
+
 #define BSB_CUDA(expr)                                                                   \
   do {                                                                                   \
     cudaError_t e__ = (expr);                                                            \
@@ -39,6 +49,7 @@ struct bsb_env {
   int obs_dtype;          // bsb_obs_dtype of the observations this handle writes
   int obs_elem_bytes;     // ... and their size: 4, 2 or 1
   bool same_step;         // BSB_FLAG_SAME_STEP_RESET: a LAST lane is reset in the same call
+  const bsb::VariantEntry* variant;   // the compiled variant of the handle's family, obs_dtype and mode: its runner
   // bsb_create_packed: n_settings settings of lanes_per_setting lanes each (p.pack holds their values); an ordinary
   // handle has packed = false, n_settings = 1, lanes_per_setting = batch
   bool packed;
@@ -73,18 +84,3 @@ struct bsb_env {
   cudaStream_t h2d_stream; cudaEvent_t h2d_event;     // two-phase host steps: the actions' DMA on a side stream
 };
 
-namespace bsb {
-// One entry per family, each defined in its own translation unit (fam_<name>.cu).
-// deep_sea and catch also run the two-phase host step (`two_phase`: its arguments).  Each also reaches its same-step
-// (ss_<name>.cu), reduced-dtype (obs_<name>.cu) and, but deep_sea, packed (pk_<name>.cu) instantiations.
-int run_deep_sea(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs* two_phase = nullptr);
-int run_catch(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs* two_phase = nullptr);
-int run_cartpole(bsb_env*, const LaunchArgs&, cudaStream_t);
-int run_cartpole_swingup(bsb_env*, const LaunchArgs&, cudaStream_t);
-int run_mountain_car(bsb_env*, const LaunchArgs&, cudaStream_t);
-int run_memory_chain(bsb_env*, const LaunchArgs&, cudaStream_t);
-int run_bandit(bsb_env*, const LaunchArgs&, cudaStream_t);
-int run_umbrella_chain(bsb_env*, const LaunchArgs&, cudaStream_t);
-int run_discounting_chain(bsb_env*, const LaunchArgs&, cudaStream_t);
-int run_mnist(bsb_env*, const LaunchArgs&, cudaStream_t);
-}  // namespace bsb

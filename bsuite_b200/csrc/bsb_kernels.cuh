@@ -1,4 +1,4 @@
-// Fused transition kernels: one per environment family (template F), specialised
+// Fused transition kernels: one per kernel variant (template V: family, observation type, auto-reset mode), specialised
 // on the bit source (Philox / MT19937), on whether the RewardNoise wrapper stream
 // is live, and on whether the Logging accumulators are tracked.
 //
@@ -37,10 +37,12 @@
 // (which the host path runs too) and the completion word.  With use_pdl a kernel is launched with programmatic
 // stream serialization: everything before griddepcontrol.wait (index math, zeroing the shared-memory stages)
 // overlaps the tail of the previous step's kernel.
-// Observations may be written as bfloat16 or uint8 instead (bsb_config.obs_dtype; ObsAs below): the emitters stage and
-// store elements of that type, each the float32 value converted by obs_cast (bsb_obs_dtype.h).
-// Same-step handles (BSB_FLAG_SAME_STEP_RESET; SameStep below) reset a lane in the call whose step returned LAST
-// (lane_step) and can emit that LAST's observation as well (emit_final).
+// Both kernels take a Variant (below) as their first template argument, e.g. transition_kernel<Variant<DeepSea, float,
+// NEXT_STEP>, 0, false, true>: the family, the observation element type and the auto-reset mode.  Observations may be
+// written as bfloat16 or uint8 instead of float32 (bsb_config.obs_dtype): the emitters stage and store elements of
+// that type, each the float32 value converted by obs_cast (bsb_obs_dtype.h).  Same-step handles
+// (BSB_FLAG_SAME_STEP_RESET) reset a lane in the call whose step returned LAST (lane_step) and can emit that LAST's
+// observation as well (emit_final).
 #pragma once
 #include "bsb_families.cuh"
 
@@ -117,35 +119,88 @@ struct DeviceMail {
 
 enum { MODE_STEP = 0, MODE_RESET = 1, MODE_INIT = 2 };
 
-// Observation element type of a kernel (bsb_config.obs_dtype).  The first template argument of both kernels is the
-// family F itself for float32 observations, or ObsAs<F, O> for observations written as O (Bf16, uint8_t): the
-// float32 kernels keep their template arguments, their names and their code.
-template <class Family, class O> struct ObsAs {};
-template <class F> struct FamilyOf { typedef F type; };
-template <class Family, class O> struct FamilyOf<ObsAs<Family, O> > { typedef Family type; };
-template <class F> struct ObsElemOf { typedef float type; };
-template <class Family, class O> struct ObsElemOf<ObsAs<Family, O> > { typedef O type; };
-// Kernel argument F for observations of type O.
-template <class Family, class O> struct KernelFamily { typedef ObsAs<Family, O> type; };
-template <class Family> struct KernelFamily<Family, float> { typedef Family type; };
+// ----- kernel variants --------------------------------------------------------------------------------------------
+// The first template argument of both kernels and of the host path: the family, the observation element type O
+// (bsb_config.obs_dtype: float, Bf16 or uint8_t; the emitters stage and store elements of that type) and the
+// auto-reset mode.  NEXT_STEP: bsb_create.  SAME_STEP (BSB_FLAG_SAME_STEP_RESET): a lane whose step returned LAST is
+// reset in the same call (lane_step), and that LAST's observation can be emitted as well (emit_final).  PACKED
+// (bsb_create_packed): every lane runs with its setting's parameters (pack_lane_params), found once per launch.
+enum { NEXT_STEP = 0, SAME_STEP = 1, PACKED = 2 };
+template <class Family, class O, int kMode> struct Variant {
+  typedef Family Fam;
+  typedef O Obs;
+  static const bool kSameStep = kMode == SAME_STEP;
+  static const bool kPacked = kMode == PACKED;
+};
+
+// Every compiled variant, X(family, O, mode, mt, two_phase), by the translation unit that holds its kernels and host
+// path: build.py compiles bsb_variants.cu once per BSB_UNIT_<unit> below.  `mt`: MT19937 is compiled beside Philox
+// (float32 next-step only).  `two_phase`: two_phase_host_kernel is compiled beside transition_kernel (deep_sea and
+// catch, whose observations are rendered from the stored lane state, next-step).  Units: fam_ float32 next-step,
+// obs_ reduced dtypes (uint8 only for the 0 / 1 observations of deep_sea and catch), ss_ same-step, pk_ packed (all
+// but deep_sea, whose settings differ in observation shape); a handle loads only the modules of its own unit.
+#define BSB_UNIT_fam_deep_sea(X) X(DeepSea, float, NEXT_STEP, 1, 1)
+#define BSB_UNIT_fam_catch(X) X(Catch, float, NEXT_STEP, 1, 1)
+#define BSB_UNIT_fam_cartpole(X) X(Cartpole, float, NEXT_STEP, 1, 0)
+#define BSB_UNIT_fam_cartpole_swingup(X) X(CartpoleSwingup, float, NEXT_STEP, 1, 0)
+#define BSB_UNIT_fam_mountain_car(X) X(MountainCar, float, NEXT_STEP, 1, 0)
+#define BSB_UNIT_fam_memory_chain(X) X(MemoryChain, float, NEXT_STEP, 1, 0)
+#define BSB_UNIT_fam_bandit(X) X(Bandit, float, NEXT_STEP, 1, 0)
+#define BSB_UNIT_fam_umbrella_chain(X) X(UmbrellaChain, float, NEXT_STEP, 1, 0)
+#define BSB_UNIT_fam_discounting_chain(X) X(DiscountingChain, float, NEXT_STEP, 1, 0)
+#define BSB_UNIT_fam_mnist(X) X(Mnist, float, NEXT_STEP, 1, 0)
+#define BSB_UNIT_obs_deep_sea(X) X(DeepSea, Bf16, NEXT_STEP, 0, 1) X(DeepSea, uint8_t, NEXT_STEP, 0, 1)
+#define BSB_UNIT_obs_catch(X) X(Catch, Bf16, NEXT_STEP, 0, 1) X(Catch, uint8_t, NEXT_STEP, 0, 1)
+#define BSB_UNIT_obs_cartpole(X) X(Cartpole, Bf16, NEXT_STEP, 0, 0)
+#define BSB_UNIT_obs_cartpole_swingup(X) X(CartpoleSwingup, Bf16, NEXT_STEP, 0, 0)
+#define BSB_UNIT_obs_mountain_car(X) X(MountainCar, Bf16, NEXT_STEP, 0, 0)
+#define BSB_UNIT_obs_memory_chain(X) X(MemoryChain, Bf16, NEXT_STEP, 0, 0)
+#define BSB_UNIT_obs_bandit(X) X(Bandit, Bf16, NEXT_STEP, 0, 0)
+#define BSB_UNIT_obs_umbrella_chain(X) X(UmbrellaChain, Bf16, NEXT_STEP, 0, 0)
+#define BSB_UNIT_obs_discounting_chain(X) X(DiscountingChain, Bf16, NEXT_STEP, 0, 0)
+#define BSB_UNIT_obs_mnist(X) X(Mnist, Bf16, NEXT_STEP, 0, 0)
+#define BSB_UNIT_ss_deep_sea(X) X(DeepSea, float, SAME_STEP, 0, 0) X(DeepSea, Bf16, SAME_STEP, 0, 0) X(DeepSea, uint8_t, SAME_STEP, 0, 0)
+#define BSB_UNIT_ss_catch(X) X(Catch, float, SAME_STEP, 0, 0) X(Catch, Bf16, SAME_STEP, 0, 0) X(Catch, uint8_t, SAME_STEP, 0, 0)
+#define BSB_UNIT_ss_cartpole(X) X(Cartpole, float, SAME_STEP, 0, 0) X(Cartpole, Bf16, SAME_STEP, 0, 0)
+#define BSB_UNIT_ss_cartpole_swingup(X) X(CartpoleSwingup, float, SAME_STEP, 0, 0) X(CartpoleSwingup, Bf16, SAME_STEP, 0, 0)
+#define BSB_UNIT_ss_mountain_car(X) X(MountainCar, float, SAME_STEP, 0, 0) X(MountainCar, Bf16, SAME_STEP, 0, 0)
+#define BSB_UNIT_ss_memory_chain(X) X(MemoryChain, float, SAME_STEP, 0, 0) X(MemoryChain, Bf16, SAME_STEP, 0, 0)
+#define BSB_UNIT_ss_bandit(X) X(Bandit, float, SAME_STEP, 0, 0) X(Bandit, Bf16, SAME_STEP, 0, 0)
+#define BSB_UNIT_ss_umbrella_chain(X) X(UmbrellaChain, float, SAME_STEP, 0, 0) X(UmbrellaChain, Bf16, SAME_STEP, 0, 0)
+#define BSB_UNIT_ss_discounting_chain(X) X(DiscountingChain, float, SAME_STEP, 0, 0) X(DiscountingChain, Bf16, SAME_STEP, 0, 0)
+#define BSB_UNIT_ss_mnist(X) X(Mnist, float, SAME_STEP, 0, 0) X(Mnist, Bf16, SAME_STEP, 0, 0)
+#define BSB_UNIT_pk_catch(X) X(Catch, float, PACKED, 0, 0)
+#define BSB_UNIT_pk_cartpole(X) X(Cartpole, float, PACKED, 0, 0)
+#define BSB_UNIT_pk_cartpole_swingup(X) X(CartpoleSwingup, float, PACKED, 0, 0)
+#define BSB_UNIT_pk_mountain_car(X) X(MountainCar, float, PACKED, 0, 0)
+#define BSB_UNIT_pk_memory_chain(X) X(MemoryChain, float, PACKED, 0, 0)
+#define BSB_UNIT_pk_bandit(X) X(Bandit, float, PACKED, 0, 0)
+#define BSB_UNIT_pk_umbrella_chain(X) X(UmbrellaChain, float, PACKED, 0, 0)
+#define BSB_UNIT_pk_discounting_chain(X) X(DiscountingChain, float, PACKED, 0, 0)
+#define BSB_UNIT_pk_mnist(X) X(Mnist, float, PACKED, 0, 0)
+#define BSB_VARIANTS(X)                                                                                                \
+  BSB_UNIT_fam_deep_sea(X) BSB_UNIT_fam_catch(X) BSB_UNIT_fam_cartpole(X) BSB_UNIT_fam_cartpole_swingup(X)             \
+  BSB_UNIT_fam_mountain_car(X) BSB_UNIT_fam_memory_chain(X) BSB_UNIT_fam_bandit(X) BSB_UNIT_fam_umbrella_chain(X)      \
+  BSB_UNIT_fam_discounting_chain(X) BSB_UNIT_fam_mnist(X)                                                              \
+  BSB_UNIT_obs_deep_sea(X) BSB_UNIT_obs_catch(X) BSB_UNIT_obs_cartpole(X) BSB_UNIT_obs_cartpole_swingup(X)             \
+  BSB_UNIT_obs_mountain_car(X) BSB_UNIT_obs_memory_chain(X) BSB_UNIT_obs_bandit(X) BSB_UNIT_obs_umbrella_chain(X)      \
+  BSB_UNIT_obs_discounting_chain(X) BSB_UNIT_obs_mnist(X)                                                              \
+  BSB_UNIT_ss_deep_sea(X) BSB_UNIT_ss_catch(X) BSB_UNIT_ss_cartpole(X) BSB_UNIT_ss_cartpole_swingup(X)                 \
+  BSB_UNIT_ss_mountain_car(X) BSB_UNIT_ss_memory_chain(X) BSB_UNIT_ss_bandit(X) BSB_UNIT_ss_umbrella_chain(X)          \
+  BSB_UNIT_ss_discounting_chain(X) BSB_UNIT_ss_mnist(X)                                                                \
+  BSB_UNIT_pk_catch(X) BSB_UNIT_pk_cartpole(X) BSB_UNIT_pk_cartpole_swingup(X) BSB_UNIT_pk_mountain_car(X)             \
+  BSB_UNIT_pk_memory_chain(X) BSB_UNIT_pk_bandit(X) BSB_UNIT_pk_umbrella_chain(X) BSB_UNIT_pk_discounting_chain(X)     \
+  BSB_UNIT_pk_mnist(X)
+
+// The list's flags of variant V (undefined for a variant the list does not compile).
+template <class V> struct Compiled;
+#define BSB_COMPILED(F, O, mode, mt, two_phase) \
+  template <> struct Compiled<Variant<F, O, mode> > { static const bool kMt = mt, kTwoPhase = two_phase; };
+BSB_VARIANTS(BSB_COMPILED)
+#undef BSB_COMPILED
+
 // log2 of the observation elements per 16-byte vector store.
 template <class O> struct Vec16 { static const int shift = sizeof(O) == 4 ? 2 : sizeof(O) == 2 ? 3 : 4; };
-// Same-step auto-reset (BSB_FLAG_SAME_STEP_RESET): the first template argument of transition_kernel is
-// SameStep<family, O> for every observation type, float32 included, so the next-step kernels above keep theirs.
-template <class Family, class O> struct SameStep {};
-template <class Family, class O> struct FamilyOf<SameStep<Family, O> > { typedef Family type; };
-template <class Family, class O> struct ObsElemOf<SameStep<Family, O> > { typedef O type; };
-template <class F> struct IsSameStep { static const bool value = false; };
-template <class Family, class O> struct IsSameStep<SameStep<Family, O> > { static const bool value = true; };
-// Kernel argument F for observations of type O in either auto-reset mode.
-template <class Family, class O, bool kSameStep> struct KernelTag { typedef typename KernelFamily<Family, O>::type type; };
-template <class Family, class O> struct KernelTag<Family, O, true> { typedef SameStep<Family, O> type; };
-// Packed handles (bsb_create_packed; float32, next-step): the first template argument of transition_kernel is
-// Packed<family>.  Every lane runs with its setting's parameters (pack_lane_params), found once per launch.
-template <class Family> struct Packed {};
-template <class Family> struct FamilyOf<Packed<Family> > { typedef Family type; };
-template <class F> struct IsPacked { static const bool value = false; };
-template <class Family> struct IsPacked<Packed<Family> > { static const bool value = true; };
 
 // ----- RNG plumbing ---------------------------------------------------------
 template <int RK> struct RngOf;
@@ -297,11 +352,6 @@ static const int TILE_STAGES = 2;     // deep_sea bulk path: double-buffered gro
 static const int REUSE_WORDS = 256;   // compare-then-store tiles: 16-byte words per pass (8 per thread) ...
 static const int REUSE_STAGES = 2;    // ... and passes in flight per warp (emit_onehot_reuse)
 static const int REUSE_STORE_WORDS = 8;   // ... and a differing word is stored with its whole 128-byte line
-
-// Families whose observations hold only 0 and 1, so that uint8 represents them exactly (obs_dtype uint8).
-template <class F> struct BinaryObs {
-  static const bool value = EmitKind<F>::value == EMIT_ONEHOT || EmitKind<F>::value == EMIT_TWOHOT;
-};
 
 // Dynamic shared memory per warp, in observation elements of type O (times sizeof(O): bytes).
 template <class F, class O> inline
@@ -761,7 +811,7 @@ template <class F> struct MinBlocksPerSM { static const int value = 4; };       
 template <> struct MinBlocksPerSM<MemoryChain> { static const int value = 6; };   // <= 80
 template <> struct MinBlocksPerSM<Bandit> { static const int value = 8; };        // <= 64
 template <> struct MinBlocksPerSM<DiscountingChain> { static const int value = 8; };
-#define BSB_LAUNCH_MIN_BLOCKS(F) MinBlocksPerSM<typename FamilyOf<F>::type>::value
+#define BSB_LAUNCH_MIN_BLOCKS(V) MinBlocksPerSM<typename V::Fam>::value
 // System-scope stores to the pinned mailbox (host memory over PCIe).
 __device__ __forceinline__ void st_sys_u64(volatile unsigned long long* ptr, unsigned long long v) {
   asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(ptr), "l"(v) : "memory");
@@ -1015,13 +1065,13 @@ __device__ __forceinline__ void signal_done(const LaunchArgs& a) {
 
 // The fused transition kernel: ordinary launches (constructor, reset, step, rollout), graph-safe mode and the
 // single-phase host step.
-template <class F, int RK, bool kNoise, bool kTrack>
-__global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kernel(const EnvParams p, const LaunchArgs a) {
-  typedef typename FamilyOf<F>::type Fam;          // F is the family, ObsAs<family, O> (observations of type O),
-  typedef typename ObsElemOf<F>::type O;           // SameStep<family, O> (same-step auto-reset) or Packed<family>
+template <class V, int RK, bool kNoise, bool kTrack>
+__global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) transition_kernel(const EnvParams p, const LaunchArgs a) {
+  typedef typename V::Fam Fam;
+  typedef typename V::Obs O;
   typedef typename RngOf<RK>::type R;
-  constexpr bool kSameStep = IsSameStep<F>::value;
-  constexpr bool kPacked = IsPacked<F>::value;
+  constexpr bool kSameStep = V::kSameStep;
+  constexpr bool kPacked = V::kPacked;
   const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
   const int64_t B = p.batch;
   const int K = p.obs_numel;
@@ -1140,11 +1190,12 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F)) transition_kern
 // completion word are program-ordered; the host's acquire load of the word therefore sees every scalar.)
 // Every host step, BSB_HOST_NO_WAIT included, is one launch of this kernel.  Host steps never run in graph-safe
 // mode (the launcher checks): there is no device clock here.
-template <class F, int RK, bool kNoise, bool kTrack>
-__global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(F))
+template <class V, int RK, bool kNoise, bool kTrack>
+__global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V))
 two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs h) {
-  typedef typename FamilyOf<F>::type Fam;          // F is the family, or ObsAs<family, O> (observations of type O)
-  typedef typename ObsElemOf<F>::type O;
+  typedef typename V::Fam Fam;
+  typedef typename V::Obs O;
+  static_assert(!V::kSameStep && !V::kPacked, "the two-phase host step runs next-step handles");
   static_assert(ObsFromState<Fam>::value, "the two-phase host step renders observations from the stored lane state");
   typedef typename RngOf<RK>::type R;
   const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;

@@ -1,7 +1,7 @@
 """Every compiled kernel and every launch path of the device engine, lane for lane against the host path.
 
 The transition logic is one set of __host__ __device__ functions that the host path runs too.  What the CUDA side
-adds is how chunks of lanes are dealt to warps and how observations reach HBM: `device_launch` (bsb_dispatch.cuh)
+adds is how chunks of lanes are dealt to warps and how observations reach HBM: `run_variant` (bsb_dispatch.cuh)
 and `transition_kernel` (bsb_kernels.cuh) pick row stages, TMA bulk or vector stores, group sizes, CTA sizes and a
 persistent grid from the family, the batch, the observation size, T, the buffer alignment and the memory the
 buffer lies in.
@@ -16,12 +16,14 @@ compares every output of every lane after every call:
 then bsuite_info(), episode_stats(), the recorded log rows and the state_dict() blob.  A few lanes of the host twin
 also go through oracle.run_lanes, which anchors the comparison outside the engine.
 
-  group A  every instantiation transition_kernel<family, Philox | MT19937, noise, track> once (80 kernels);
+  group A  every instantiation transition_kernel<Variant<family, float, NEXT_STEP>, Philox | MT19937, noise, track>
+           once (80 kernels);
   group B  the paths the default dispatch selects, at batch sizes derived from its rules (margins quoted for the
            132 SMs of an H100 SXM);
   group C  the CTA sizes, deep_sea group sizes, vector fallbacks and mnist group sizes that only larger boards,
            tiles and images reach;
-  group H  every instantiation two_phase_host_kernel<deep_sea | catch, Philox | MT19937, noise, track> (16 kernels),
+  group H  every instantiation two_phase_host_kernel<Variant<deep_sea | catch, float, NEXT_STEP>, Philox | MT19937,
+           noise, track> (16 kernels),
            driven by host steps (bsb_step_host on pinned buffers): waited for, and BSB_HOST_NO_WAIT (the same
            launch, collected by host_wait()).
 
@@ -96,7 +98,7 @@ GROUP_A = [_case(f, 97, A_KWARGS[f], rng=r, noise=0.1 if n else None, track=t, r
 
 UMB = dict(chain_length=6)
 DS = dict(mapping_seed=4)
-# Rules (device_launch / chunk_is_bulk): rows and boards take stage_rows = 2 when T > 1 and 2 * 32 * K * 4 <= 14 KB
+# Rules (plan_launch / chunk_is_bulk): rows and boards take stage_rows = 2 when T > 1 and 2 * 32 * K * 4 <= 14 KB
 # (K <= 56), 1 when T = 1 or the rows are longer, 0 (render in place, no bulk store) when one 32-row stage exceeds
 # 96 KB (K > 768).  A chunk leaves through the TMA unit only if the launch's buffer is 16-byte aligned with a
 # per-step stride that is a multiple of 16 bytes (obs_vec_ok; always true for T = 1 on an aligned buffer) and
@@ -438,23 +440,24 @@ def image_dirs(tmp_path_factory):
 
 
 # ------------------------------------------------------------------ CPU: the driver and the case lists
-def test_group_a_covers_every_kernel_instantiation():
+def test_groups_a_and_h_cover_every_float32_variant_of_the_list():
   """A new family, bit source or template flag of transition_kernel or two_phase_host_kernel cannot appear without a
   group A or group H case."""
-  csrc = bsb_build.CSRC
-  with open(os.path.join(csrc, 'bsb_kernels.cuh')) as fh:
+  with open(os.path.join(bsb_build.CSRC, 'bsb_kernels.cuh')) as fh:
     kernels = fh.read()
-  assert re.search(r'template <class F, int RK, bool kNoise, bool kTrack>\s*__global__ void[^\n]*\btransition_kernel\(', kernels)
-  assert re.search(r'template <class F, int RK, bool kNoise, bool kTrack>\s*__global__ void[^\n]*\n?'
+  assert re.search(r'template <class V, int RK, bool kNoise, bool kTrack>\s*__global__ void[^\n]*\btransition_kernel\(', kernels)
+  assert re.search(r'template <class V, int RK, bool kNoise, bool kTrack>\s*__global__ void[^\n]*\n?'
                    r'two_phase_host_kernel\(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs h\)', kernels)
-  # the two-phase kernel is instantiated for the families of ObsFromState, each in all four flag combinations
-  two_phase = sorted(re.findall(r'template <> struct ObsFromState<(\w+)> \{ static const bool value = true; \};', kernels))
-  assert two_phase == ['Catch', 'DeepSea']
+  # the float32 next-step units of the variant list: one variant per family, both bit sources, and the two-phase
+  # kernel for deep_sea and catch, each in all four flag combinations
+  units = {unit[4:]: rows for unit, rows in bsb_build.variant_list().items() if unit.startswith('fam_')}
+  assert sorted(FAMILIES) == sorted(units) == sorted(experiments.ENVIRONMENT_CLASSES)
+  assert all(len(rows) == 1 and rows[0][1:4] == ('float', 'NEXT_STEP', True) for rows in units.values())
+  two_phase = sorted(family for family, rows in units.items() if rows[0][4])
+  assert two_phase == ['catch', 'deep_sea']
   got = sorted((c['family'], c['rng'], c['noise'] is not None, c['track'], mode) for c, mode in GROUP_H if c['batch'] == 97)
-  assert got == sorted(itertools.product(('catch', 'deep_sea'), RNGS, (False, True), (False, True), HOST_MODES))
+  assert got == sorted(itertools.product(two_phase, RNGS, (False, True), (False, True), HOST_MODES))
   assert sorted(int(k) for k in re.findall(r'template <> struct RngOf<(\d+)>', kernels)) == list(range(len(RNGS)))
-  compiled = sorted(f[4:-3] for f in os.listdir(csrc) if f.startswith('fam_') and f.endswith('.cu'))
-  assert sorted(FAMILIES) == compiled == sorted(experiments.ENVIRONMENT_CLASSES)
   got = sorted((c['family'], c['rng'], c['noise'] is not None, c['track']) for c in GROUP_A)
   assert got == sorted(itertools.product(FAMILIES, RNGS, (False, True), (False, True)))
   ids = [_case_id(c) for c in GROUP_A + GROUP_B + GROUP_C] + [_h_id(h) for h in GROUP_H]

@@ -11,7 +11,6 @@ host twins; tests/test_obs_dtype_gpu.py runs the CUDA cases.
 import ctypes
 import itertools
 import os
-import re
 import shutil
 import subprocess
 
@@ -457,21 +456,20 @@ def test_state_dict_moves_between_float32_and_reduced_handles(family, kwargs, dt
 
 
 # ------------------------------------------------------------------ the GPU cases cover every new kernel
-def test_gpu_cases_cover_every_reduced_dtype_instantiation():
+def test_gpu_cases_cover_every_reduced_dtype_variant_of_the_list():
   """bf16 for every family and uint8 for the 0 / 1 families, Philox only, in both kernels: a new family, dtype or
   template flag cannot appear without a case in tests/test_obs_dtype_gpu.py."""
   from tests import test_obs_dtype_gpu as gpu
-  with open(os.path.join(bsb_build.CSRC, 'bsb_kernels.cuh')) as fh:
-    kernels = fh.read()
-  binary = sorted(re.findall(r'template <> struct EmitKind<(\w+)> \{ static const int value = EMIT_(?:ONEHOT|TWOHOT); \};',
-                             kernels))
-  assert binary == ['Catch', 'DeepSea']
-  with open(os.path.join(bsb_build.CSRC, 'bsb_dispatch.cuh')) as fh:
-    dispatch = fh.read()
-  assert 'case BSB_OBS_BFLOAT16: return run_family_as<F, Bf16>' in dispatch
-  compiled = sorted(f[4:-3] for f in os.listdir(bsb_build.CSRC) if f.startswith('obs_') and f.endswith('.cu'))
-  assert compiled == sorted(FAMILIES)
-  assert 'if constexpr (BinaryObs<F>::value) return run_family_as<F, uint8_t>' in dispatch
+  # the reduced-dtype units of the variant list: next-step, Philox only, bfloat16 for every family, uint8 and the
+  # two-phase kernel for deep_sea and catch
+  names = {'Bf16': 'bfloat16', 'uint8_t': 'uint8'}
+  units = {unit[4:]: rows for unit, rows in bsb_build.variant_list().items() if unit.startswith('obs_')}
+  assert sorted(units) == sorted(FAMILIES)
+  assert all(mode == 'NEXT_STEP' and not mt for rows in units.values() for _, _, mode, mt, _ in rows)
+  compiled = sorted((family, names[obs]) for family, rows in units.items() for _, obs, _, _, _ in rows)
+  assert compiled == sorted([(f, 'bfloat16') for f in FAMILIES] + [(f, 'uint8') for f in U8_FAMILIES])
+  two_phase = sorted((family, names[obs]) for family, rows in units.items() for _, obs, _, _, tp in rows if tp)
+  assert two_phase == sorted(itertools.product(U8_FAMILIES, ('bfloat16', 'uint8')))
   want = sorted(itertools.product(FAMILIES, ('bfloat16',), (False, True), (False, True))) + sorted(
       itertools.product(U8_FAMILIES, ('uint8',), (False, True), (False, True)))
   got = sorted((c['family'], c['obs_dtype'], c['noise'] is not None, c['track']) for c in gpu.GROUP_A)

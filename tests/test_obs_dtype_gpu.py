@@ -6,10 +6,12 @@ exactly), and the host path in the reduced dtype (bit for bit for integer and gr
 noise and stochastic deep_sea under the FLOAT_TOL policy of tests/test_device_paths_gpu.py widened by one bfloat16
 ulp).
 
-  group A  transition_kernel<ObsAs<family, Bf16 | uint8_t>, Philox, noise, track> (48 kernels) at B = 97;
+  group A  transition_kernel<Variant<family, Bf16 | uint8_t, NEXT_STEP>, Philox, noise, track> (48 kernels) at
+           B = 97;
   group B  dispatch paths whose rules count bytes: group sizes, tails, stages, alignment;
   group C  uint8 deep_sea group sizes that only larger tiles reach;
-  group H  two_phase_host_kernel<ObsAs<deep_sea | catch, Bf16 | uint8_t>, Philox, noise, track> (16 kernels), and
+  group H  two_phase_host_kernel<Variant<deep_sea | catch, Bf16 | uint8_t, NEXT_STEP>, Philox, noise, track>
+           (16 kernels), and
            the other host-step paths: staged copies, synchronised steps.
 """
 

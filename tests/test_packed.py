@@ -300,10 +300,12 @@ def test_step_host_on_a_packed_host_environment():
       assert torch.equal(obs[sl], pts.observation) and torch.equal(ts.reward[sl], pts.reward)
 
 
-def test_gpu_cases_cover_every_packed_instantiation(mnist_dir):
+def test_gpu_cases_cover_every_packed_variant_of_the_list(mnist_dir):
   """Every packed transition_kernel instantiation (nine families x noise x track) has a case in test_packed_gpu.py."""
   from tests import test_packed_gpu as g
-  compiled = sorted(f[3:-3] for f in os.listdir(bsb_build.CSRC) if f.startswith('pk_') and f.endswith('.cu'))
+  units = {unit[3:]: rows for unit, rows in bsb_build.variant_list().items() if unit.startswith('pk_')}
+  assert all(len(rows) == 1 and rows[0][1:] == ('float', 'PACKED', False, False) for rows in units.values())
+  compiled = sorted(units)
   assert compiled == sorted(f for f in bsb_build.FAMILIES if f != 'deep_sea')
   want = set(itertools.product(compiled, (False, True), (False, True)))
   assert len(want) == 36

@@ -378,6 +378,7 @@ def test_collect_and_replay_use_the_final_observation():
 
 # ------------------------------------------------------------------ coverage of the GPU file
 def test_gpu_cases_cover_every_same_step_instantiation():
+  from bsuite_b200 import build
   from tests import test_same_step_gpu as g
   want = set()
   for family in cf_families():
@@ -386,6 +387,10 @@ def test_gpu_cases_cover_every_same_step_instantiation():
       want.add((family, dtype, noise, track))
   got = {(c['family'], c['obs_dtype'], c['noise'] is not None, bool(c['track'])) for c in g.GROUP_S}
   assert len(want) == 88
+  names = {'float': 'float32', 'Bf16': 'bfloat16', 'uint8_t': 'uint8'}
+  units = {unit[3:]: rows for unit, rows in build.variant_list().items() if unit.startswith('ss_')}
+  assert all(mode == 'SAME_STEP' and not mt and not tp for rows in units.values() for _, _, mode, mt, tp in rows)
+  assert {(f, names[o]) for f, rows in units.items() for _, o, _, _, _ in rows} == {w[:2] for w in want}
   assert want <= got, sorted(want - got)
 
 

@@ -6,8 +6,8 @@ fused rollout with device-sampled actions, single steps (PDL), a mid-episode res
 handle, with `final_observation` on (compared too: rows of lanes that did not finish stay zero on both twins) or off,
 then compares info, episode statistics, log rows and the state blob, with the exactness policy of that file.
 
-  group S  every same-step instantiation transition_kernel<SameStep<family, float32 | bfloat16 | uint8>, Philox,
-           noise, track> (88 kernels) at B = 97;
+  group S  every same-step instantiation transition_kernel<Variant<family, float | Bf16 | uint8_t, SAME_STEP>,
+           Philox, noise, track> (88 kernels) at B = 97;
   group P  the dispatch paths the final observation's emitters take (bulk / vector / scalar, persistent grids, row
            stages, mnist chunks and the table path, unaligned buffers).
 """

@@ -9,10 +9,11 @@ OUT=/tmp/bsb_asan
 LOG=${1:-/tmp/bsb_asan/run.log}
 mkdir -p $OUT && rm -f $OUT/*.o
 cd "$(dirname "$0")/../bsuite_b200/csrc"
-# the translation units of the library as bsuite_b200/build.py lists them
-python -c "import sys; sys.path.insert(0, '../..'); from bsuite_b200 import build; print('\n'.join(build.SOURCES))" \
-  | xargs -P 16 -I{} sh -c "nvcc -gencode arch=compute_90a,code=sm_90a -O1 -std=c++17 --fmad=false \
-  -Xcompiler -fPIC,-ffp-contract=off,-O1,-g,-fsanitize=address,-fsanitize=undefined,-fno-omit-frame-pointer -c {} -o $OUT/\$(basename {} .cu).o"
+# the translation units of the library as bsuite_b200/build.py lists them: "name source [defines]" per line
+python -c "import sys; sys.path.insert(0, '../..'); from bsuite_b200 import build
+for name, source, defines in build.UNITS: print(name, source, *defines)" \
+  | xargs -P 16 -L 1 sh -c "nvcc -gencode arch=compute_90a,code=sm_90a -O1 -std=c++17 --fmad=false \
+  -Xcompiler -fPIC,-ffp-contract=off,-O1,-g,-fsanitize=address,-fsanitize=undefined,-fno-omit-frame-pointer \$2 -c \$1 -o $OUT/\$0.o"
 nvcc -shared -o $OUT/libbsuite_b200.so $OUT/*.o -cudart static -ldl -Xcompiler -fsanitize=address,-fsanitize=undefined 2>/dev/null
 cd ../..
 set +e
