@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BSB_LIBRARY points the binding at another build of the SAME library (tools/host_sanitize.sh: ASan/UBSan build)
 LIB_PATH = os.environ.get('BSB_LIBRARY') or os.path.join(_HERE, 'libbsuite_b200.so')
 
-ABI_VERSION = 12
+ABI_VERSION = 13
 DEVICE_HOST = -1
 MAX_INFO = 4
 MAX_PACKED_SETTINGS = 64      # bsb_create_packed: settings per handle
@@ -107,6 +107,11 @@ EXPORTS = {
                                            ctypes.POINTER(ctypes.c_uint64), ctypes.c_uint64,
                                            ctypes.POINTER(ctypes.c_void_p)]),
     'bsb_packed_layout': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int64)]),
+    'bsb_create_ragged': (ctypes.c_int32, [ctypes.POINTER(Config), ctypes.c_int32, ctypes.c_int64, ctypes.c_int32,
+                                           ctypes.POINTER(ctypes.c_uint64), ctypes.c_uint64,
+                                           ctypes.POINTER(ctypes.c_void_p)]),
+    'bsb_ragged_layout': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                           ctypes.POINTER(ctypes.c_int64)]),
     'bsb_destroy': (ctypes.c_int32, [ctypes.c_void_p]),
     'bsb_obs_numel': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64)]),
     'bsb_obs_shape': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32)]),

@@ -183,6 +183,8 @@ class ImageObservation(dm_env.Environment):
   engine on both faces (`bsuite_b200.imaging`; a B = 1 float32 observation takes the host path)."""
 
   def __init__(self, env, shape: Sequence[int]):
+    if getattr(env, 'ragged', False):
+      raise ValueError('ImageObservation needs one observation shape: a ragged pack has one per setting')
     self._env, self._shape = env, tuple(shape)
     self._batch_dims = 1 if hasattr(env, 'batch') else 0
 

@@ -38,16 +38,18 @@ template <> struct HostEmit<Mnist> {
 // Observations of type O other than float32: each lane's float32 observation is rendered into `f32` and converted
 // element by element with obs_cast, the function the kernels use.  kSameStep: a lane whose step returned LAST is reset
 // in the same call, and its final observation goes to a.final_obs when that is given.  kPacked: every lane runs with
-// its setting's parameters (pack_lane_params), as the packed kernels do.
+// its setting's parameters (pack_lane_params), as the packed kernels do.  kRagged: the same with ragged_setting_params,
+// and lane j of setting k writes row j of the setting's observation block.
 template <class V, int RK>
 void host_run(const EnvParams& p, const LaunchArgs& a) {
   typedef typename V::Fam F;
   typedef typename V::Obs O;
-  constexpr bool kSameStep = V::kSameStep, kPacked = V::kPacked;
+  constexpr bool kSameStep = V::kSameStep, kPacked = V::kPacked, kRagged = V::kRagged;
   typedef typename RngOf<RK>::type R;
   const int64_t B = p.batch;
   const int K = p.obs_numel;
   O* const obs = reinterpret_cast<O*>(a.obs);
+  const RaggedTable* ragged = kRagged ? reinterpret_cast<const RaggedTable*>(p.pack) : nullptr;
   O* const fin = reinterpret_cast<O*>(a.final_obs);
   std::vector<float> f32(std::is_same<O, float>::value ? 0 : (size_t)K);
   const bool noise = p.wrapper == BSB_WRAP_REWARD_NOISE && a.mode != MODE_INIT;
@@ -64,7 +66,17 @@ void host_run(const EnvParams& p, const LaunchArgs& a) {
   };
   for (int64_t lane = 0; lane < B; ++lane) {
     if constexpr (kPacked) { setting_p = p; pack_lane_params(setting_p, lane); }
-    const EnvParams& lp = kPacked ? setting_p : p;
+    O* lane_obs = obs + lane * (int64_t)K;      // step 0's observation row of this lane
+    int64_t step_elems = B * (int64_t)K;
+    if constexpr (kRagged) {
+      const int64_t k = lane / ragged->pack.lanes_per_setting;
+      const RaggedSetting& s = ragged_setting(ragged, k);
+      setting_p = p;
+      ragged_setting_params(setting_p, s, ragged->mapping_bits);
+      lane_obs = obs + s.obs_offset + (lane - s.lane_shift) * (int64_t)s.obs_numel;
+      step_elems = ragged->step_elems;
+    }
+    const EnvParams& lp = (kPacked || kRagged) ? setting_p : p;
     typename F::Lane L;
     R rng, wrng;
     EpisodeStats ep;
@@ -85,7 +97,7 @@ void host_run(const EnvParams& p, const LaunchArgs& a) {
       }
       lane_step<F, R, kSameStep>(lp, lane, L, rng, wrng, ep, action, a.mode, noise, track, a.step0 + t, out, off, &merged);
       if constexpr (kSameStep) { if (merged.done && fin) render(lp, merged.last, merged.rng, fin + off * (int64_t)K); }
-      render(lp, L, rng, obs + off * (int64_t)K);
+      render(lp, L, rng, lane_obs + t * step_elems);
     }
     lane_close<F>(lp, lane, L, rng, wrng, ep, noise, track);
   }
@@ -206,6 +218,65 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int extra_threads = 0) {
   return BSB_OK;
 }
 
+// The plan of a ragged pack's launch (float32 observations, the settings' shapes in e->obs_rows / obs_cols, their
+// deep_sea group sizes in e->group_lanes): plan_launch's rules with the chunk count of ragged_chunks.  Row stages are
+// sized for the largest K.  deep_sea tiles keep the grouped bulk store and its persistent grid, each setting with its
+// own group size; the stage holds two of the largest group (a.group_lanes * p.obs_numel elements each, p.obs_numel
+// being the largest K).  On compressible memory, where plan_launch would turn a batch of the same size to
+// compare-then-store or streaming stores, every chunk uses the streaming stores.
+template <class F>
+int plan_ragged_launch(bsb_env* e, LaunchArgs& a, Geometry& g) {
+  const int64_t K = e->p.obs_numel;
+  const bool is_onehot = EmitKind<F>::value == EMIT_ONEHOT;
+  a.emit_bulk = 1;
+  a.emit_reuse = 0;
+  a.group_lanes = 1;
+  a.work_counter = nullptr;
+  a.work_base = 0;
+  a.stage_rows = ((size_t)2 * 32 * (size_t)K * sizeof(float) <= 14 * 1024) ? 2 : 1;
+  if (a.T == 1 && EmitKind<F>::value == EMIT_ROWS) a.stage_rows = 1;
+  a.cta_extra_elems = 0;
+  a.bad_action = e->bad_action_dev;
+  a.chunk_lanes = 32;
+  g.n_chunks = (int64_t)e->n_settings * ((e->lanes_per_setting + 31) / 32);
+  int threads = 64;
+  bool persistent = false;
+  if (is_onehot && g.n_chunks >= 4 * (int64_t)e->num_sms && in_compressed_block(a.obs)) a.emit_bulk = 0;
+  if (is_onehot && a.emit_bulk) {
+    int64_t largest = 0;
+    for (int32_t k = 0; k < e->n_settings; ++k) {
+      const int64_t elems = (int64_t)e->group_lanes[k] * e->obs_rows[k] * e->obs_cols[k];
+      largest = elems > largest ? elems : largest;
+    }
+    if (largest == 0) {
+      a.emit_bulk = 0;
+    } else {
+      a.group_lanes = (int)((largest + K - 1) / K); threads = 32; persistent = true;
+    }
+  }
+  a.use_pdl = (a.mode == MODE_STEP && a.T == 1) ? 1 : 0;
+  size_t per_warp = smem_elems_per_warp<F, float>((int)K, a.emit_bulk != 0, false, a.group_lanes, a.stage_rows) * sizeof(float);
+  if (EmitKind<F>::value == EMIT_ROWS && per_warp > 96 * 1024) { a.emit_bulk = 0; a.stage_rows = 0; per_warp = 0; }
+  size_t smem = per_warp * (size_t)(threads / 32);
+  while (smem > 96 * 1024 && threads > 32) { threads >>= 1; smem = per_warp * (size_t)(threads / 32); }
+  if (smem > 200 * 1024) return fail(BSB_UNSUPPORTED, "observation too large for the staged emitter");
+  g.threads = threads;
+  g.smem = smem;
+  g.extra_blocks = 0;
+  g.grid = (g.n_chunks + threads / 32 - 1) / (threads / 32);
+  if (persistent) {
+    int64_t per_sm = (int64_t)((227 * 1024) / (smem + 1024));
+    per_sm = per_sm < 1 ? 1 : (per_sm > 16 ? 16 : per_sm);
+    const int64_t resident = (int64_t)e->num_sms * per_sm;
+    if (g.grid > resident) {
+      g.grid = resident;
+      a.work_counter = a.clock ? a.clock + CLOCK_CHUNK : e->work_counter;
+      a.work_base = a.clock ? 0ull : e->work_base;
+    }
+  }
+  return BSB_OK;
+}
+
 template <class Kernel, class... Args>
 int launch(bsb_env* e, const LaunchArgs& a, const Geometry& g, cudaStream_t stream, Kernel kernel, const Args&... args) {
   if (g.smem > 48 * 1024) BSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
@@ -273,10 +344,21 @@ int run_variant(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoP
     }
     LaunchArgs la = a;
     Geometry g;
-    const int rc = plan_launch<typename V::Fam, typename V::Obs>(e, la, g);
-    if (rc != BSB_OK) return rc;
-    if constexpr (kMt) { if (mt) return launch(e, la, g, stream, transition_kernel<V, 1, kNoise, kTrack>, e->p, la); }
-    return launch(e, la, g, stream, transition_kernel<V, 0, kNoise, kTrack>, e->p, la);
+    if constexpr (V::kRagged) {
+      // ragged packs take no reward wrapper (bsb_create_ragged): Logging off / on are their only kernels
+      if constexpr (kNoise) {
+        return fail(BSB_INTERNAL, "a ragged pack reached the RewardNoise kernel");
+      } else {
+        const int rc = plan_ragged_launch<typename V::Fam>(e, la, g);
+        if (rc != BSB_OK) return rc;
+        return launch(e, la, g, stream, transition_kernel<V, 0, false, kTrack>, e->p, la);
+      }
+    } else {
+      const int rc = plan_launch<typename V::Fam, typename V::Obs>(e, la, g);
+      if (rc != BSB_OK) return rc;
+      if constexpr (kMt) { if (mt) return launch(e, la, g, stream, transition_kernel<V, 1, kNoise, kTrack>, e->p, la); }
+      return launch(e, la, g, stream, transition_kernel<V, 0, kNoise, kTrack>, e->p, la);
+    }
   });
 }
 

@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #if defined(__x86_64__)
@@ -101,7 +102,7 @@ LaunchArgs make_args(const bsb_env* e, const bsb_outputs* out, const int32_t* ac
   a.actions = actions;
   if (out) { a.obs = out->observation; a.reward = out->reward; a.reward_f64 = out->reward_f64; a.discount = out->discount; a.step_type = out->step_type; a.final_obs = out->final_observation; }
   a.T = T; a.step0 = e->steps_done; a.mode = mode;
-  const size_t step_bytes = (size_t)e->p.batch * (size_t)e->p.obs_numel * (size_t)e->obs_elem_bytes;
+  const size_t step_bytes = (size_t)e->step_elems * (size_t)e->obs_elem_bytes;
   a.obs_vec_ok = (out && (reinterpret_cast<uintptr_t>(out->observation) % 16 == 0) && (T == 1 || step_bytes % 16 == 0)) ? 1 : 0;
   a.final_vec_ok = (a.final_obs && (reinterpret_cast<uintptr_t>(a.final_obs) % 16 == 0) && (T == 1 || step_bytes % 16 == 0)) ? 1 : 0;
   return a;
@@ -414,18 +415,21 @@ int32_t bsb_abi_version(void) { return BSB_ABI_VERSION; }
 const char* bsb_last_error(void) { return bsb::last_error_cstr(); }
 int64_t bsb_launch_count(void) { return g_launches.load(); }
 
-// bsb_create, and bsb_create_packed with `n_settings` > 0 (`config` is then configs[0], the validated settings are
-// `configs` with their `seeds`; `batch` = n_settings * lanes_per_setting).
+// Observation elements of a ragged pack's blocks are 128-byte aligned (32 float32 elements).
+static int64_t align_block(int64_t elems) { return (elems + 31) / 32 * 32; }
+
+// bsb_create, and bsb_create_packed / bsb_create_ragged with `n_settings` > 0 (`config` is then configs[0], the
+// validated settings are `configs` with their `seeds`; `batch` = n_settings * lanes_per_setting).
 static int32_t create_env(const bsb_config* config, int64_t batch, int32_t device, uint64_t seed, uint64_t lane_offset,
                           bsb_env** out, const bsb_config* configs = nullptr, const uint64_t* seeds = nullptr,
-                          int32_t n_settings = 0) {
+                          int32_t n_settings = 0, bool ragged = false) {
   if (!config || !out) return fail(BSB_INVALID_ARGUMENT, "null argument");
   *out = nullptr;
   const bsb_config& c = *config;
   int obs_rows = 0, obs_cols = 0, n_actions = 0;
   int rc = validate(c, batch, &obs_rows, &obs_cols, &n_actions);
   if (rc != BSB_OK) return rc;
-  const int mode = n_settings > 0 ? PACKED : (c.flags & BSB_FLAG_SAME_STEP_RESET) ? SAME_STEP : NEXT_STEP;
+  const int mode = ragged ? RAGGED : n_settings > 0 ? PACKED : (c.flags & BSB_FLAG_SAME_STEP_RESET) ? SAME_STEP : NEXT_STEP;
   const VariantEntry* variant = find_variant(c.family, c.obs_dtype, mode, c.rng_kind);
   if (!variant) return fail(BSB_INTERNAL, "no compiled kernel variant for this family, obs_dtype, mode and rng_kind");
   if (device >= 0) {
@@ -447,6 +451,20 @@ static int32_t create_env(const bsb_config* config, int64_t batch, int32_t devic
   e->variant = variant;
   e->packed = n_settings > 0; e->n_settings = n_settings > 0 ? n_settings : 1;
   e->lanes_per_setting = n_settings > 0 ? batch / n_settings : batch;
+  e->ragged = ragged;
+  {  // the observation blocks: one per setting, back to back (ragged packs: 128-byte aligned, each of its own shape)
+    const int32_t n = e->n_settings;
+    int64_t at = 0;
+    for (int32_t k = 0; k < n; ++k) {
+      int rows = obs_rows, cols = obs_cols, unused = 0;
+      if (ragged) validate(configs[k], batch, &rows, &cols, &unused);
+      e->obs_offset.push_back(at);
+      e->obs_rows.push_back(rows); e->obs_cols.push_back(cols);
+      at += e->lanes_per_setting * (int64_t)rows * cols;
+      if (ragged) at = align_block(at);
+    }
+    e->step_elems = at;
+  }
   e->graph_safe = false; e->clock = nullptr; e->sum_scratch = nullptr; e->names = info_names(c.family);
   e->work_counter = nullptr; e->work_base = 0;
   e->num_sms = 132;
@@ -465,6 +483,9 @@ static int32_t create_env(const bsb_config* config, int64_t batch, int32_t devic
   p.memory_length = c.memory_length; p.num_bits = c.num_bits; p.chain_length = c.chain_length; p.n_distractor = c.n_distractor;
   p.num_actions = n_actions; p.max_steps = c.max_steps; p.num_data = c.num_data; p.image_numel = c.family == BSB_MNIST ? c.image_rows * c.image_cols : 0;
   p.obs_rows = obs_rows; p.obs_cols = obs_cols; p.obs_numel = obs_rows * obs_cols; p.n_info = e->names.n;
+  if (ragged) {      // the launch plan sizes the stages for the largest observation; each chunk uses its setting's
+    for (int32_t k = 0; k < n_settings; ++k) p.obs_numel = std::max(p.obs_numel, e->obs_rows[k] * e->obs_cols[k]);
+  }
   p.batch = batch; p.seed = seed; p.lane_offset = lane_offset;
   if (c.family == BSB_DEEP_SEA) { p.move_cost_step = c.unscaled_move_cost / (double)c.size; p.inv_size = 1.0 / (double)c.size; }
   p.height_threshold = c.height_threshold; p.x_threshold = c.x_threshold; p.timescale = c.timescale; p.max_time = c.max_time;
@@ -480,11 +501,19 @@ static int32_t create_env(const bsb_config* config, int64_t batch, int32_t devic
 #define BSB_TRY(expr) do { rc = (expr); if (rc != BSB_OK) { destroy_env(e); return rc; } } while (0)
   const size_t B = (size_t)batch;
   // tables
+  std::vector<int64_t> mapping_offset(n_settings > 0 ? (size_t)n_settings : 1, 0);
   if (c.family == BSB_DEEP_SEA) {
-    const int cells = c.size * c.size;
-    std::vector<uint32_t> bits((size_t)(cells + 31) / 32, 0u);
-    const uint8_t* m = static_cast<const uint8_t*>(c.table);
-    for (int k = 0; k < cells; ++k) if (m[k]) bits[(size_t)k >> 5] |= 1u << (k & 31);
+    // a ragged pack stacks its settings' mapping bits, setting k from word mapping_offset[k]
+    std::vector<uint32_t> bits;
+    for (int32_t k = 0; k < (ragged ? n_settings : 1); ++k) {
+      const bsb_config& ck = ragged ? configs[k] : c;
+      const int cells = ck.size * ck.size;
+      mapping_offset[(size_t)k] = (int64_t)bits.size();
+      bits.resize(bits.size() + (size_t)(cells + 31) / 32, 0u);
+      uint32_t* word = bits.data() + mapping_offset[(size_t)k];
+      const uint8_t* m = static_cast<const uint8_t*>(ck.table);
+      for (int j = 0; j < cells; ++j) if (m[j]) word[(size_t)j >> 5] |= 1u << (j & 31);
+    }
     uint32_t* d = nullptr;
     BSB_TRY(env_alloc_t(e, &d, bits.size(), false));
     BSB_TRY(env_upload(e, d, bits.data(), bits.size() * 4));
@@ -559,7 +588,37 @@ static int32_t create_env(const bsb_config* config, int64_t batch, int32_t devic
       BSB_TRY(env_alloc_t(e, &p.wmt_idx, B, true)); BSB_TRY(env_upload(e, p.wmt_idx, idx.data(), B * 4));
     }
   }
-  if (e->packed) {      // the per-setting values every lane of a packed handle picks up (pack_lane_params)
+  if (ragged) {         // the per-setting values and observation blocks of a ragged pack (ragged_setting_params)
+    std::vector<char> blob(sizeof(RaggedTable) + (size_t)n_settings * sizeof(RaggedSetting), 0);
+    RaggedTable* t = reinterpret_cast<RaggedTable*>(blob.data());
+    t->pack.lanes_per_setting = e->lanes_per_setting; t->pack.n_settings = n_settings;
+    t->step_elems = e->step_elems;
+    t->mapping_bits = c.family == BSB_DEEP_SEA ? p.mapping_bits : nullptr;
+    RaggedSetting* s = reinterpret_cast<RaggedSetting*>(t + 1);
+    for (int32_t k = 0; k < n_settings; ++k) {
+      const bsb_config& ck = configs[k];
+      const int32_t K = e->obs_rows[(size_t)k] * e->obs_cols[(size_t)k];
+      s[k].seed = seeds[k];
+      s[k].lane_shift = (int64_t)k * e->lanes_per_setting;
+      s[k].obs_offset = e->obs_offset[(size_t)k];
+      s[k].mapping_offset = mapping_offset[(size_t)k];
+      s[k].size = ck.size;
+      if (c.family == BSB_DEEP_SEA) { s[k].inv_size = 1.0 / (double)ck.size; s[k].move_cost_step = ck.unscaled_move_cost / (double)ck.size; }
+      s[k].num_bits = ck.num_bits; s[k].n_distractor = ck.n_distractor; s[k].obs_numel = K;
+      s[k].memory_length = ck.memory_length; s[k].chain_length = ck.chain_length;
+      // deep_sea: lanes per bulk store by plan_launch's rule (the largest power of two <= 16 whose store is <= 40 KB),
+      // or 0 where that store is not a whole number of 16-byte words or two groups exceed 100 KB
+      int32_t m = 1;
+      const size_t tile = (size_t)K * sizeof(float);
+      while (m < 16 && (size_t)(2 * m) * tile <= 40 * 1024) m <<= 1;
+      s[k].group_lanes = (((size_t)m * tile) % 16 != 0 || (size_t)TILE_STAGES * m * tile > 100 * 1024) ? 0 : m;
+      e->group_lanes.push_back(c.family == BSB_DEEP_SEA ? s[k].group_lanes : 0);
+    }
+    void* d = nullptr;
+    BSB_TRY(env_alloc(e, &d, blob.size(), false));
+    BSB_TRY(env_upload(e, d, blob.data(), blob.size()));
+    p.pack = static_cast<const PackTable*>(d);
+  } else if (e->packed) {      // the per-setting values every lane of a packed handle picks up (pack_lane_params)
     std::vector<char> blob(sizeof(PackTable) + (size_t)n_settings * sizeof(PackSetting));
     PackTable* t = reinterpret_cast<PackTable*>(blob.data());
     t->lanes_per_setting = e->lanes_per_setting; t->n_settings = n_settings;
@@ -595,14 +654,20 @@ int32_t bsb_create(const bsb_config* config, int64_t batch, int32_t device, uint
 
 // The first field in which two settings of a packed handle differ although they may not (nullptr: none).  Allowed
 // to differ: the seed (seeds[]), the contents of `table` (bandit / discounting_chain reward tables), memory_length,
-// chain_length, height_threshold, x_reward_threshold, noise_scale, reward_scale.
-static const char* packed_mismatch(const bsb_config& a, const bsb_config& b) {
+// chain_length, height_threshold, x_reward_threshold, noise_scale, reward_scale.  The settings of a ragged pack
+// (`ragged`) may also differ in size with its deep_sea mapping table, num_bits and n_distractor.
+static const char* packed_mismatch(const bsb_config& a, const bsb_config& b, bool ragged = false) {
 #define BSB_SAME(field) if (memcmp(&a.field, &b.field, sizeof(a.field)) != 0) return #field;
-  BSB_SAME(family) BSB_SAME(wrapper) BSB_SAME(rng_kind) BSB_SAME(flags) BSB_SAME(size) BSB_SAME(deterministic)
-  BSB_SAME(rows) BSB_SAME(columns) BSB_SAME(num_bits) BSB_SAME(n_distractor) BSB_SAME(num_actions) BSB_SAME(max_steps)
+  BSB_SAME(family) BSB_SAME(wrapper) BSB_SAME(rng_kind) BSB_SAME(flags)
+  if (!ragged) { BSB_SAME(size) }
+  BSB_SAME(deterministic) BSB_SAME(rows) BSB_SAME(columns)
+  if (!ragged) { BSB_SAME(num_bits) BSB_SAME(n_distractor) }
+  BSB_SAME(num_actions) BSB_SAME(max_steps)
   BSB_SAME(num_data) BSB_SAME(image_rows) BSB_SAME(image_cols) BSB_SAME(obs_dtype) BSB_SAME(unscaled_move_cost)
   BSB_SAME(x_threshold) BSB_SAME(timescale) BSB_SAME(max_time) BSB_SAME(init_range) BSB_SAME(theta_dot_threshold)
-  BSB_SAME(move_cost) BSB_SAME(table_bytes) BSB_SAME(table2_bytes) BSB_SAME(log_schedule_len)
+  BSB_SAME(move_cost)
+  if (!ragged || a.family != BSB_DEEP_SEA) { BSB_SAME(table_bytes) }
+  BSB_SAME(table2_bytes) BSB_SAME(log_schedule_len)
 #undef BSB_SAME
   if (a.family == BSB_MNIST && a.table_bytes == b.table_bytes && a.table != b.table &&
       (!a.table || !b.table || memcmp(a.table, b.table, (size_t)a.table_bytes) != 0)) return "table";
@@ -647,14 +712,63 @@ int32_t bsb_packed_layout(const bsb_env* env, int32_t* n_settings, int64_t* lane
   return BSB_OK;
 }
 
+int32_t bsb_create_ragged(const bsb_config* configs, int32_t n_settings, int64_t lanes_per_setting, int32_t device,
+                          const uint64_t* seeds, uint64_t lane_offset, bsb_env** out) {
+  if (!configs || !seeds || !out) return fail(BSB_INVALID_ARGUMENT, "null argument");
+  *out = nullptr;
+  if (n_settings < 1 || n_settings > BSB_MAX_PACKED_SETTINGS)
+    return fail(BSB_INVALID_ARGUMENT, "n_settings must be in [1, " + std::to_string(BSB_MAX_PACKED_SETTINGS) + "]");
+  if (lanes_per_setting < 1 || lanes_per_setting > INT64_MAX / n_settings)
+    return fail(BSB_INVALID_ARGUMENT, "lanes_per_setting must be positive (and n_settings * lanes_per_setting an int64)");
+  for (int32_t k = 0; k < n_settings; ++k) {
+    int rows = 0, cols = 0, n_actions = 0;
+    const int rc = validate(configs[k], lanes_per_setting, &rows, &cols, &n_actions);
+    if (rc != BSB_OK) return fail(rc, "setting " + std::to_string(k) + ": " + last_error_cstr());
+  }
+  const bsb_config& c = configs[0];
+  if (!find_variant(c.family, BSB_OBS_FLOAT32, RAGGED, BSB_RNG_PHILOX))
+    return fail(BSB_UNSUPPORTED, "`family`: ragged packs hold deep_sea, memory_chain or umbrella_chain; the settings of "
+                                 "other families share one observation shape: use bsb_create_packed");
+  for (int32_t k = 0; k < n_settings; ++k) {
+    const bsb_config& ck = configs[k];
+    const char* field = ck.rng_kind != BSB_RNG_PHILOX ? "rng_kind` (ragged packs need BSB_RNG_PHILOX"
+                        : ck.obs_dtype != BSB_OBS_FLOAT32 ? "obs_dtype` (ragged packs write float32 observations"
+                        : (ck.flags & BSB_FLAG_SAME_STEP_RESET) ? "flags` (ragged packs do not take BSB_FLAG_SAME_STEP_RESET"
+                        : ck.wrapper != BSB_WRAP_NONE ? "wrapper` (ragged packs take no reward wrapper"
+                        : nullptr;
+    if (field) return fail(BSB_UNSUPPORTED, "setting " + std::to_string(k) + ": `" + field + ")");
+  }
+  for (int32_t k = 1; k < n_settings; ++k)
+    if (const char* field = packed_mismatch(c, configs[k], true))
+      return fail(BSB_UNSUPPORTED, std::string("settings 0 and ") + std::to_string(k) + " differ in `" + field +
+                                       "`, which the settings of a ragged pack must share");
+  return create_env(&c, (int64_t)n_settings * lanes_per_setting, device, seeds[0], lane_offset, out, configs, seeds,
+                    n_settings, true);
+}
+
+int32_t bsb_ragged_layout(const bsb_env* env, int64_t* offsets, int32_t* rows, int32_t* cols, int64_t* step_elems) {
+  if (!env || !offsets || !rows || !cols || !step_elems) return fail(BSB_INVALID_ARGUMENT, "null argument");
+  for (int32_t k = 0; k < env->n_settings; ++k) {
+    offsets[k] = env->obs_offset[(size_t)k]; rows[k] = env->obs_rows[(size_t)k]; cols[k] = env->obs_cols[(size_t)k];
+  }
+  *step_elems = env->step_elems;
+  return BSB_OK;
+}
+
 int32_t bsb_destroy(bsb_env* env) { if (env) destroy_env(env); return BSB_OK; }
 
+static int refuse_ragged(const bsb_env* env) {
+  if (env->ragged) return fail(BSB_UNSUPPORTED, "the settings of a ragged pack differ in observation shape: read them with bsb_ragged_layout");
+  return BSB_OK;
+}
 int32_t bsb_obs_numel(const bsb_env* env, int64_t* numel) {
   if (!env || !numel) return fail(BSB_INVALID_ARGUMENT, "null argument");
+  { int rc = refuse_ragged(env); if (rc != BSB_OK) return rc; }
   *numel = env->p.obs_numel; return BSB_OK;
 }
 int32_t bsb_obs_shape(const bsb_env* env, int32_t* rows, int32_t* cols) {
   if (!env || !rows || !cols) return fail(BSB_INVALID_ARGUMENT, "null argument");
+  { int rc = refuse_ragged(env); if (rc != BSB_OK) return rc; }
   *rows = env->p.obs_rows; *cols = env->p.obs_cols; return BSB_OK;
 }
 int32_t bsb_num_actions(const bsb_env* env, int32_t* n) {
@@ -955,8 +1069,8 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
   if ((flags & BSB_HOST_NO_WAIT) && (flags & BSB_HOST_PRELAUNCH)) return fail(BSB_INVALID_ARGUMENT, "BSB_HOST_NO_WAIT and BSB_HOST_PRELAUNCH exclude each other");
   DeviceGuard guard(env->device);
   { int arc = finish_awaited(env); if (arc != BSB_OK) return arc; }      // one step in flight per handle
-  const size_t B = (size_t)env->p.batch, K = (size_t)env->p.obs_numel;
-  const size_t obs_bytes = B * K * (size_t)env->obs_elem_bytes;
+  const size_t B = (size_t)env->p.batch;
+  const size_t obs_bytes = (size_t)env->step_elems * (size_t)env->obs_elem_bytes;
   if (!env->copy_stream) BSB_CUDA(cudaStreamCreateWithFlags(&env->copy_stream, cudaStreamNonBlocking));
   if (flags & BSB_HOST_ORDER_AFTER_STREAM) {
     // Work the caller enqueued earlier on ITS stream (bsb_reset / bsb_step / bsb_rollout of this handle) must have

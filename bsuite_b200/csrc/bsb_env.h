@@ -55,6 +55,13 @@ struct bsb_env {
   bool packed;
   int32_t n_settings;
   int64_t lanes_per_setting;
+  // bsb_create_ragged (packed is true as well): setting k's observations are a dense [lanes_per_setting, rows, cols]
+  // block at element obs_offset[k] of each step of step_elems elements; group_lanes[k] is the deep_sea bulk path's
+  // lanes per store (0: none).  Every other handle: one block per setting of lanes_per_setting * p.obs_numel elements.
+  bool ragged;
+  std::vector<int64_t> obs_offset;
+  std::vector<int32_t> obs_rows, obs_cols, group_lanes;
+  int64_t step_elems;
   int64_t steps_done;     // step() calls so far (host counter; frozen at the switch to graph-safe mode)
   // Graph-safe mode: entered for good when a launch of this handle is first captured into a CUDA graph.  From
   // then on the device clock counts the steps (kernel comment in bsb_kernels.cuh) and steps = steps_done + clock[0].

@@ -46,7 +46,8 @@ struct EnvParams {
   // tables
   union {
     const uint32_t* mapping_bits;  // deep_sea: bit (row*N+col) of the action mapping
-    const PackTable* pack;         // packed handles (bsb_create_packed; never deep_sea): the per-setting values
+    const PackTable* pack;         // packed handles (bsb_create_packed; never deep_sea): the per-setting values;
+                                   // ragged packs (bsb_create_ragged): their RaggedTable
   };
   const double* reward_table;    // bandit / discounting_chain (packed handles: the settings' tables, stacked)
   const int8_t* images;          // mnist
@@ -95,6 +96,40 @@ BSB_HD void pack_lane_params(EnvParams& q, int64_t i) {
   q.height_threshold = s.height_threshold; q.x_reward_threshold = s.x_reward_threshold;
   q.noise_scale = s.noise_scale; q.reward_scale = s.reward_scale;
   q.memory_length = s.memory_length; q.chain_length = s.chain_length;
+}
+
+// Ragged packs (bsb_create_ragged): the settings of one experiment whose observation shapes differ (deep_sea: size and
+// mapping, memory_chain: num_bits, umbrella_chain: n_distractor).  Lanes are laid out as in a pack; the observations of
+// setting k are a dense [lanes_per_setting, obs_numel] block at element `obs_offset` of every step of `step_elems`
+// elements.  The table begins with a PackTable, followed by the step size, the settings' stacked deep_sea mapping
+// bits, and one RaggedSetting per setting.
+struct RaggedSetting {
+  uint64_t seed;
+  int64_t lane_shift;            // k * lanes_per_setting: lane_offset is lowered by it, as pack_lane_params does
+  int64_t obs_offset;            // first element of this setting's observation block within a step
+  int64_t mapping_offset;        // deep_sea: first word of this setting's action mapping bits
+  double inv_size, move_cost_step;
+  int32_t size, num_bits, n_distractor, obs_numel, memory_length, chain_length;
+  int32_t group_lanes;           // deep_sea bulk path: lanes per bulk store (0: the tiles never go through the TMA unit)
+  int32_t pad;
+};
+struct RaggedTable {
+  PackTable pack;
+  int64_t step_elems;
+  const uint32_t* mapping_bits;  // deep_sea: every setting's mapping bits back to back (else null)
+};
+BSB_HD const RaggedSetting& ragged_setting(const RaggedTable* t, int64_t k) {
+  return reinterpret_cast<const RaggedSetting*>(t + 1)[k];
+}
+// Turns `q` (a copy of a ragged pack's parameters) into the parameters of setting s's own handle, as
+// pack_lane_params does for a pack.  The mapping pointer shares its word with `pack`, so it is set last.
+BSB_HD void ragged_setting_params(EnvParams& q, const RaggedSetting& s, const uint32_t* mapping_bits) {
+  q.seed = s.seed;
+  q.lane_offset -= (uint64_t)s.lane_shift;
+  q.size = s.size; q.inv_size = s.inv_size; q.move_cost_step = s.move_cost_step;
+  q.num_bits = s.num_bits; q.n_distractor = s.n_distractor; q.obs_numel = s.obs_numel;
+  q.memory_length = s.memory_length; q.chain_length = s.chain_length;
+  if (mapping_bits) q.mapping_bits = mapping_bits + s.mapping_offset;
 }
 
 static const uint32_t NEEDS_RESET = 0x80000000u;

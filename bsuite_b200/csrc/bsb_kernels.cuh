@@ -125,12 +125,15 @@ enum { MODE_STEP = 0, MODE_RESET = 1, MODE_INIT = 2 };
 // auto-reset mode.  NEXT_STEP: bsb_create.  SAME_STEP (BSB_FLAG_SAME_STEP_RESET): a lane whose step returned LAST is
 // reset in the same call (lane_step), and that LAST's observation can be emitted as well (emit_final).  PACKED
 // (bsb_create_packed): every lane runs with its setting's parameters (pack_lane_params), found once per launch.
-enum { NEXT_STEP = 0, SAME_STEP = 1, PACKED = 2 };
+// RAGGED (bsb_create_ragged): a pack whose settings differ in observation shape; chunks never straddle settings
+// (ragged_chunks).
+enum { NEXT_STEP = 0, SAME_STEP = 1, PACKED = 2, RAGGED = 3 };
 template <class Family, class O, int kMode> struct Variant {
   typedef Family Fam;
   typedef O Obs;
   static const bool kSameStep = kMode == SAME_STEP;
   static const bool kPacked = kMode == PACKED;
+  static const bool kRagged = kMode == RAGGED;
 };
 
 // Every compiled variant, X(family, O, mode, mt, two_phase), by the translation unit that holds its kernels and host
@@ -138,7 +141,8 @@ template <class Family, class O, int kMode> struct Variant {
 // (float32 next-step only).  `two_phase`: two_phase_host_kernel is compiled beside transition_kernel (deep_sea and
 // catch, whose observations are rendered from the stored lane state, next-step).  Units: fam_ float32 next-step,
 // obs_ reduced dtypes (uint8 only for the 0 / 1 observations of deep_sea and catch), ss_ same-step, pk_ packed (all
-// but deep_sea, whose settings differ in observation shape); a handle loads only the modules of its own unit.
+// but deep_sea, whose settings differ in observation shape), rg_ ragged packs (the three families whose settings
+// differ in observation shape); a handle loads only the modules of its own unit.
 #define BSB_UNIT_fam_deep_sea(X) X(DeepSea, float, NEXT_STEP, 1, 1)
 #define BSB_UNIT_fam_catch(X) X(Catch, float, NEXT_STEP, 1, 1)
 #define BSB_UNIT_fam_cartpole(X) X(Cartpole, float, NEXT_STEP, 1, 0)
@@ -178,6 +182,9 @@ template <class Family, class O, int kMode> struct Variant {
 #define BSB_UNIT_pk_umbrella_chain(X) X(UmbrellaChain, float, PACKED, 0, 0)
 #define BSB_UNIT_pk_discounting_chain(X) X(DiscountingChain, float, PACKED, 0, 0)
 #define BSB_UNIT_pk_mnist(X) X(Mnist, float, PACKED, 0, 0)
+#define BSB_UNIT_rg_deep_sea(X) X(DeepSea, float, RAGGED, 0, 0)
+#define BSB_UNIT_rg_memory_chain(X) X(MemoryChain, float, RAGGED, 0, 0)
+#define BSB_UNIT_rg_umbrella_chain(X) X(UmbrellaChain, float, RAGGED, 0, 0)
 #define BSB_VARIANTS(X)                                                                                                \
   BSB_UNIT_fam_deep_sea(X) BSB_UNIT_fam_catch(X) BSB_UNIT_fam_cartpole(X) BSB_UNIT_fam_cartpole_swingup(X)             \
   BSB_UNIT_fam_mountain_car(X) BSB_UNIT_fam_memory_chain(X) BSB_UNIT_fam_bandit(X) BSB_UNIT_fam_umbrella_chain(X)      \
@@ -190,7 +197,7 @@ template <class Family, class O, int kMode> struct Variant {
   BSB_UNIT_ss_discounting_chain(X) BSB_UNIT_ss_mnist(X)                                                                \
   BSB_UNIT_pk_catch(X) BSB_UNIT_pk_cartpole(X) BSB_UNIT_pk_cartpole_swingup(X) BSB_UNIT_pk_mountain_car(X)             \
   BSB_UNIT_pk_memory_chain(X) BSB_UNIT_pk_bandit(X) BSB_UNIT_pk_umbrella_chain(X) BSB_UNIT_pk_discounting_chain(X)     \
-  BSB_UNIT_pk_mnist(X)
+  BSB_UNIT_pk_mnist(X) BSB_UNIT_rg_deep_sea(X) BSB_UNIT_rg_memory_chain(X) BSB_UNIT_rg_umbrella_chain(X)
 
 // The list's flags of variant V (undefined for a variant the list does not compile).
 template <class V> struct Compiled;
@@ -1063,6 +1070,97 @@ __device__ __forceinline__ void signal_done(const LaunchArgs& a) {
   }
 }
 
+// The chunk loop of a ragged pack (Variant<F, float, RAGGED>).  Setting k owns ceil(L / chunk_lanes) chunks, the last
+// possibly partial, so a chunk never straddles two settings: the setting's parameters (K, N, mapping bits, group
+// size) are warp-uniform, looked up once per chunk and kept for all T steps.  Row j of setting k's observation block
+// receives lane j of the setting.  Tile groups and row stages sit at offsets that depend on the setting's K, so a
+// persistent warp (deep_sea bulk path) that moves on to another setting first waits until the TMA unit has read its
+// stages, then clears the cells it poked there with the old geometry: the stage is all zeros again before the new
+// setting's first poke.
+template <class Fam, class R, bool kNoise, bool kTrack>
+__device__ __forceinline__ void ragged_chunks(const EnvParams& p, const LaunchArgs& a, WarpStage<float>& ws, int64_t step0,
+                                              const MailFields& out, bool vec) {
+  constexpr int kEmit = EmitKind<Fam>::value;
+  const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
+  const RaggedTable* table = reinterpret_cast<const RaggedTable*>(p.pack);
+  const int64_t lanes = table->pack.lanes_per_setting, step_elems = table->step_elems;
+  const int cl = a.chunk_lanes;
+  const int64_t per_setting = (lanes + cl - 1) / cl;
+  const int64_t n_chunks = table->pack.n_settings * per_setting;
+  const bool dynamic = a.work_counter != nullptr;
+  const int64_t total_warps = (int64_t)gridDim.x * warps_per_cta;
+  int64_t cur_chunk = (int64_t)blockIdx.x * warps_per_cta + warp;
+  int64_t k_prev = -1;
+  EnvParams lp = p;              // setting k_prev's parameters
+  LaunchArgs la = a;             // ... its lanes per bulk store
+  float* obs_k = a.obs;          // ... and its observation block
+  bool tiles_bulk = false;       // ... whose tiles may go through the TMA unit
+  int group_stride = 0;          // elements from the stage's first tile group to its second
+
+  while (cur_chunk < n_chunks) {
+    const int64_t k = cur_chunk / per_setting;
+    const int64_t local_base = (cur_chunk - k * per_setting) * cl;      // first lane of the chunk within its setting
+    const int n_lanes = (lanes - local_base) < cl ? (int)(lanes - local_base) : cl;
+    const int64_t lane = k * lanes + local_base + tid;                 // the pack's lane: state, scalars, accumulators
+    const bool active = tid < n_lanes;
+    if (k != k_prev) {
+      if (k_prev >= 0 && ws.any_bulk) {
+        if (tid == 0) bulk_wait_read<0>();
+        __syncwarp();
+        if (kEmit == EMIT_ONEHOT) {
+          if (ws.tile_poked0 >= 0) ws.stage[ws.tile_poked0] = 0.f;
+          if (ws.tile_poked1 >= 0) ws.stage[group_stride + ws.tile_poked1] = 0.f;
+          ws.tile_poked0 = ws.tile_poked1 = -1;
+          __syncwarp();
+        }
+      }
+      const RaggedSetting& s = ragged_setting(table, k);
+      lp = p;
+      ragged_setting_params(lp, s, table->mapping_bits);
+      la.group_lanes = s.group_lanes > 0 ? s.group_lanes : 1;
+      tiles_bulk = s.group_lanes > 0;
+      group_stride = la.group_lanes * lp.obs_numel;
+      obs_k = a.obs + s.obs_offset;
+      k_prev = k;
+    }
+    const bool bulk = chunk_is_bulk<Fam, float>(lp, la, vec, n_lanes) && (kEmit != EMIT_ONEHOT || tiles_bulk);
+    ws.any_bulk = ws.any_bulk || bulk;
+
+    typename Fam::Lane L;
+    R rng, wrng;
+    EpisodeStats ep;
+    ActionStream action_stream;
+    action_stream.open();
+    if (active) lane_open<Fam>(lp, lane, L, rng, wrng, ep, a.mode, kNoise, kTrack);
+    else Fam::init(p, L);
+    if (a.mode == MODE_INIT && active) Fam::ctor_draws(lp, L, rng);      // the constructor runs no step (T = 0)
+
+    for (int64_t t = 0; t < a.T; ++t) {
+      const int64_t off = t * p.batch + lane;
+      if (active) {
+        int32_t action = 0;
+        if (a.mode == MODE_STEP) {
+          if (a.actions) {
+            action = a.actions[off];
+            if ((uint32_t)action >= (uint32_t)p.num_actions) {
+              if (a.bad_action) *a.bad_action = 1;
+              action = action < 0 ? 0 : p.num_actions - 1;
+            }
+          } else {
+            action = action_stream.sample(a.action_seed, lp.lane_offset + (uint64_t)lane, (uint64_t)(step0 + t), p.num_actions);
+          }
+          if (a.actions_out) a.actions_out[off] = action;
+        }
+        lane_step<Fam>(lp, lane, L, rng, wrng, ep, action, a.mode, kNoise, kTrack, step0 + t, out, off);
+      }
+      emit_obs<Fam>(lp, la, ws, L, rng, obs_k + t * step_elems, local_base, n_lanes, local_base + tid, active, bulk, vec);
+    }
+
+    if (active) lane_close<Fam>(lp, lane, L, rng, wrng, ep, kNoise, kTrack);
+    cur_chunk = dynamic ? fetch_chunk(a, total_warps) : n_chunks;
+  }
+}
+
 // The fused transition kernel: ordinary launches (constructor, reset, step, rollout), graph-safe mode and the
 // single-phase host step.
 template <class V, int RK, bool kNoise, bool kTrack>
@@ -1085,6 +1183,9 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) transition_kern
   const bool vec = a.obs_vec_ok != 0;
   O* const obs = reinterpret_cast<O*>(a.obs);       // the ABI's float* addresses elements of type O
 
+  if constexpr (V::kRagged) {
+    ragged_chunks<Fam, R, kNoise, kTrack>(p, a, ws, step0, out, vec);
+  } else {
   const int cl = a.chunk_lanes;
   const int64_t n_chunks = (B + cl - 1) / cl;
   const bool dynamic = a.work_counter != nullptr;
@@ -1146,6 +1247,7 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) transition_kern
     // a persistent warp reserves its next chunk only once this one's stores are issued
     cur_chunk = dynamic ? fetch_chunk(a, total_warps) : n_chunks;
   }
+  }  // !V::kRagged
   retire_warp(a, ws, a.mailbox != nullptr);
   if (a.mailbox) signal_done(a);
   if (a.clock) {

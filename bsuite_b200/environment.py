@@ -107,8 +107,8 @@ class _Handle:
 
   @classmethod
   def packed(cls, specs, lanes_per_setting: int, device_ordinal: int, seeds, lane_offset: int, flags: int,
-             log_schedule=None):
-    """One handle for the settings `specs` (Philox, float32): bsb_create_packed."""
+             log_schedule=None, ragged: bool = False):
+    """One handle for the settings `specs` (Philox, float32): bsb_create_packed, or bsb_create_ragged (`ragged`)."""
     self = cls.__new__(cls)
     self.ptr = None
     self.lib = _lib.load()
@@ -116,8 +116,9 @@ class _Handle:
     configs = (_lib.Config * len(built))(*[cfg for cfg, _ in built])
     seed_array = (ctypes.c_uint64 * len(seeds))(*[int(s) & _MASK64 for s in seeds])
     ptr = ctypes.c_void_p()
-    _lib.check(self.lib.bsb_create_packed(configs, len(built), int(lanes_per_setting), device_ordinal, seed_array,
-                                          lane_offset & _MASK64, ctypes.byref(ptr)))
+    create = self.lib.bsb_create_ragged if ragged else self.lib.bsb_create_packed
+    _lib.check(create(configs, len(built), int(lanes_per_setting), device_ordinal, seed_array,
+                      lane_offset & _MASK64, ctypes.byref(ptr)))
     del built
     self.ptr = ptr
     return self
@@ -212,6 +213,13 @@ class GraphedSteps:
     return self.timestep
 
 
+def _observation_spec(spec: EnvSpec):
+  if spec.obs_bounds is not None:
+    lo, hi = spec.obs_bounds
+    return specs.BoundedArray(shape=spec.obs_shape, dtype=np.float32, name=spec.obs_spec_name, minimum=lo, maximum=hi)
+  return specs.Array(shape=spec.obs_shape, dtype=np.float32, name=spec.obs_spec_name)
+
+
 class BatchedEnvironment:
   """`batch` independent lanes of one environment on one device.
 
@@ -232,12 +240,15 @@ class BatchedEnvironment:
   A packed environment (`bsuite_b200.load_experiment`) holds several settings of one experiment side by side:
   `bsuite_ids[k]` owns the lanes `lanes_of(bsuite_ids[k])`, and lane j of that slice is lane j of
   `load_from_id(bsuite_ids[k], batch=lanes_per_setting, seed=setting_seeds[k], lane_offset=lane_offset)`, bit for
-  bit.  An ordinary environment has `bsuite_ids` None."""
+  bit.  An ordinary environment has `bsuite_ids` None.  A ragged pack (`load_experiment(..., ragged=True)`) is a
+  packed environment whose settings differ in observation shape: its observation tensors are flat (`[step_elems]`
+  per step, `[T, step_elems]` per rollout), `obs_shape` is None, `obs_shapes` and `observation_spec()` give one
+  entry per setting, and `split_observation` returns each setting's `[L, *shape_k]` view."""
 
   def __init__(self, spec: EnvSpec, batch: int, device='cuda', seed: Optional[int] = None,
                rng: str = 'philox', lane_offset: int = 0, track_episodes: bool = False,
                reward_dtype='float32', record_rows: bool = False, obs_dtype='float32', autoreset: str = 'next_step',
-               _pack=None):
+               _pack=None, _ragged: bool = False):
     import torch
     self._torch = torch
     self._spec = spec
@@ -273,15 +284,32 @@ class BatchedEnvironment:
     self._obs_dtype, obs_code = _obs_dtype(obs_dtype)
     # _pack: (bsuite_ids, specs, seeds, lanes_per_setting) of a packed environment (load_experiment)
     self._pack = _pack
+    self._ragged = bool(_ragged)
     self._bsuite_id = None          # set by load_from_id
+    if self._ragged:
+      if autoreset != 'next_step':
+        raise ValueError("a ragged pack takes autoreset='next_step' only")
+      if self._obs_dtype is not torch.float32:
+        raise ValueError('a ragged pack writes float32 observations (obs_dtype)')
+      if self._rng_kind != _lib.RNG_PHILOX:
+        raise ValueError("a ragged pack needs rng='philox'")
     if _pack is not None:
       ids, pack_specs, seeds, lanes = _pack
       self._handle = _Handle.packed(pack_specs, lanes, self._ordinal, seeds, self._lane_offset, flags,
-                                    self._log_schedule)
+                                    self._log_schedule, ragged=self._ragged)
     else:
       self._handle = _Handle(spec, self._batch, self._ordinal, self._seed, self._lane_offset, self._rng_kind, flags,
                              self._log_schedule, obs_code)
     self._lib = self._handle.lib
+    # the observation buffer of one step: setting k's [lanes_per_setting, *shape_k] block at element offsets[k]
+    n = 1 if _pack is None else len(_pack[0])
+    offsets, rows, cols = (ctypes.c_int64 * n)(), (ctypes.c_int32 * n)(), (ctypes.c_int32 * n)()
+    step_elems = ctypes.c_int64()
+    _lib.check(self._lib.bsb_ragged_layout(self._handle.ptr, offsets, rows, cols, ctypes.byref(step_elems)))
+    self._offsets = tuple(offsets)
+    self._step_elems = step_elems.value
+    self._obs_shapes = (tuple(tuple(s.obs_shape) for s in _pack[1]) if _pack is not None
+                        else (tuple(spec.obs_shape),))
     n = ctypes.c_int32()
     _lib.check(self._lib.bsb_info_count(self._handle.ptr, ctypes.byref(n)))
     self._info_names = tuple(self._lib.bsb_info_name(self._handle.ptr, k).decode() for k in range(n.value))
@@ -292,7 +320,11 @@ class BatchedEnvironment:
   device = property(lambda self: self._device)
   seed = property(lambda self: self._seed)
   lane_offset = property(lambda self: self._lane_offset)
-  obs_shape = property(lambda self: self._spec.obs_shape)
+  # per-lane observation shape; None on a ragged pack, whose settings each have their own (obs_shapes)
+  obs_shape = property(lambda self: None if self._ragged else self._spec.obs_shape)
+  # one per setting, in bsuite_ids order (an ordinary environment: a 1-tuple)
+  obs_shapes = property(lambda self: self._obs_shapes)
+  ragged = property(lambda self: self._ragged)            # a ragged pack (load_experiment(..., ragged=True))
   family = property(lambda self: self._spec.family)
   num_actions = property(lambda self: self._spec.num_actions)
   info_names = property(lambda self: self._info_names)
@@ -316,12 +348,31 @@ class BatchedEnvironment:
 
   def observation_spec(self):
     """Per-lane spec, identical to the reference environment's (float32 values).  The observation tensors this
-    environment returns carry `obs_dtype`."""
-    if self._spec.obs_bounds is not None:
-      lo, hi = self._spec.obs_bounds
-      return specs.BoundedArray(shape=self._spec.obs_shape, dtype=np.float32, name=self._spec.obs_spec_name,
-                                minimum=lo, maximum=hi)
-    return specs.Array(shape=self._spec.obs_shape, dtype=np.float32, name=self._spec.obs_spec_name)
+    environment returns carry `obs_dtype`.  A ragged pack returns the tuple of its settings' specs, in `bsuite_ids`
+    order."""
+    if self._ragged:
+      return tuple(_observation_spec(s) for s in self._pack[1])
+    return _observation_spec(self._spec)
+
+  def split_observation(self, observation):
+    """The views (no copy) of `observation` ([B, ...] of a step, [T, B, ...] of a rollout, or the flat buffer of a
+    ragged pack) that hold each setting's observations, in `bsuite_ids` order: `[L, *shape_k]` or `[T, L, *shape_k]`.
+    An ordinary environment returns a 1-tuple.  The portable way to read observations of any environment."""
+    if self._ragged:
+      lead = tuple(observation.shape[:-1])
+      lanes = self._pack[3]
+      return tuple(observation[..., off:off + lanes * int(np.prod(shape))].view(lead + (lanes,) + shape)
+                   for off, shape in zip(self._offsets, self._obs_shapes))
+    if self._pack is None:
+      return (observation,)
+    axis = observation.dim() - len(self._spec.obs_shape) - 1
+    return tuple(observation.narrow(axis, self.lanes_of(i).start, self._pack[3]) for i in self._pack[0])
+
+  def _obs_shape_of(self, lead):
+    """Shape of an observation tensor with leading axes `lead` (the lane axis, or T and the lane axis)."""
+    if self._ragged:
+      return lead[:-1] + (self._step_elems,)
+    return lead + tuple(self._spec.obs_shape)
 
   def action_spec(self):
     return specs.DiscreteArray(self._spec.num_actions, dtype=self._spec.action_dtype, name='action')
@@ -337,8 +388,7 @@ class BatchedEnvironment:
       raise ValueError("final_observation needs autoreset='same_step'")
     lead = (self._batch,) if num_steps is None else (int(num_steps), self._batch)
     kw = dict(device=self._device)
-    obs_shape = lead + tuple(self._spec.obs_shape)
-    obs_args = (obs_shape, self._obs_dtype, self._device, self._spec.family)
+    obs_args = (self._obs_shape_of(lead), self._obs_dtype, self._device, self._spec.family)
     return StepBuffers(
         observation=obs_memory.empty(*obs_args),
         reward=torch.empty(lead, dtype=self._reward_dtype, **kw),
@@ -402,7 +452,7 @@ class BatchedEnvironment:
     if self._ordinal < 0:
       return self.make_buffers()
     host = self.make_host_buffers()
-    return StepBuffers(observation=obs_memory.empty((self._batch,) + tuple(self._spec.obs_shape), self._obs_dtype,
+    return StepBuffers(observation=obs_memory.empty(self._obs_shape_of((self._batch,)), self._obs_dtype,
                                                     self._device, self._spec.family),
                        reward=host.reward, discount=host.discount, step_type=host.step_type)
 
@@ -421,7 +471,7 @@ class BatchedEnvironment:
       reward = torch.empty(B, dtype=torch.float64, pin_memory=pin)
       discount = torch.empty(B, dtype=torch.float32, pin_memory=pin)
       step_type = torch.empty(B, dtype=torch.int32, pin_memory=pin)
-    observation = (torch.empty((B,) + tuple(self._spec.obs_shape), dtype=self._obs_dtype, pin_memory=pin)
+    observation = (torch.empty(self._obs_shape_of((B,)), dtype=self._obs_dtype, pin_memory=pin)
                    if with_observation else None)
     return StepBuffers(observation=observation, reward=reward, discount=discount, step_type=step_type)
 
@@ -661,6 +711,8 @@ class BatchedEnvironment:
       for spec in pack_specs:
         if spec.table is not None:
           h.update(np.ascontiguousarray(spec.table).tobytes())
+    if self._ragged:                       # ... and the observation layout
+      h.update(repr(('ragged', self._offsets, self._obs_shapes, self._step_elems)).encode())
     return h.hexdigest()[:16]
 
   def close(self):

@@ -8,6 +8,7 @@ contract); with `batch=B` it is a `BatchedEnvironment` of B lanes.
 import functools
 from typing import Any, Mapping, Optional, Sequence, Tuple
 
+from bsuite_b200 import _lib
 from bsuite_b200 import experiments
 from bsuite_b200 import sweep
 from bsuite_b200.environment import BatchedEnvironment, DmEnvAdapter, _fresh_seed
@@ -61,7 +62,7 @@ _PER_SETTING_FIELDS = frozenset(['memory_length', 'chain_length', 'height_thresh
 
 def load_experiment(experiment_name: str, lanes_per_setting: int, settings: Optional[Sequence[int]] = None,
                     device='cuda', seed: Optional[int] = None, lane_offset: int = 0, track_episodes: bool = False,
-                    record_rows: bool = False, reward_dtype='float32') -> BatchedEnvironment:
+                    record_rows: bool = False, reward_dtype='float32', ragged: bool = False) -> BatchedEnvironment:
   """Every setting of one experiment (or the `settings` indices into `sweep.BY_EXPERIMENT[experiment_name]`) in ONE
   batched environment of `len(settings) * lanes_per_setting` lanes: a step of the experiment is one kernel launch and
   one observation tensor.  Lane j of `env.lanes_of(bsuite_id)` is lane j of
@@ -71,8 +72,11 @@ def load_experiment(experiment_name: str, lanes_per_setting: int, settings: Opti
   An explicit `seed` is used by every setting, as `load_from_id(bsuite_id, seed=seed)` would use it; otherwise each
   setting takes its experiment's own seed (memory_len fixes 0) or fresh OS entropy.  Experiments whose settings
   differ in observation shape (deep_sea, deep_sea_stochastic: `size`; memory_size: `num_bits`; umbrella_distract:
-  `n_distractor`) raise ValueError.  Packed environments use the Philox bit source, float32 observations and the
-  next-step auto-reset convention."""
+  `n_distractor`) raise ValueError, unless `ragged=True`: then they load as a ragged pack, whose settings keep their
+  own observation shapes in one flat observation buffer (`env.split_observation` returns each setting's view).  With
+  `ragged=True` an experiment whose settings share a shape loads as an ordinary pack, so generic code may pass it for
+  every experiment.  Packed environments use the Philox bit source, float32 observations and the next-step
+  auto-reset convention."""
   if experiment_name not in sweep.BY_EXPERIMENT:
     raise ValueError(f'unknown experiment {experiment_name!r}')
   all_ids = sweep.BY_EXPERIMENT[experiment_name]
@@ -83,8 +87,10 @@ def load_experiment(experiment_name: str, lanes_per_setting: int, settings: Opti
   if len(set(ids)) != len(ids):
     raise ValueError('settings must not repeat a setting')
   specs = [experiments.EXPERIMENT_NAME_TO_SPEC[experiment_name](**sweep.SETTINGS[i]) for i in ids]
+  # a ragged pack where an ordinary one cannot hold the settings (deep_sea has no packed kernel at all)
+  shaped = ragged and (any(spec.obs_shape != specs[0].obs_shape for spec in specs) or specs[0].family == _lib.DEEP_SEA)
   for spec in specs[1:]:
-    if spec.obs_shape != specs[0].obs_shape:
+    if spec.obs_shape != specs[0].obs_shape and not ragged:
       changed = [k for k in specs[0].fields if specs[0].fields[k] != spec.fields.get(k) and k not in _PER_SETTING_FIELDS]
       raise ValueError(f'the settings of {experiment_name} differ in `{changed[0] if changed else "obs_shape"}`, which '
                        'changes the observation shape: load them with load_from_id one by one')
@@ -92,7 +98,7 @@ def load_experiment(experiment_name: str, lanes_per_setting: int, settings: Opti
   lanes = int(lanes_per_setting)
   return BatchedEnvironment(specs[0], batch=len(specs) * lanes, device=device, seed=seeds[0], lane_offset=lane_offset,
                             track_episodes=track_episodes, record_rows=record_rows, reward_dtype=reward_dtype,
-                            _pack=(ids, tuple(specs), seeds, lanes))
+                            _pack=(ids, tuple(specs), seeds, lanes), _ragged=shaped)
 
 
 def make(environment_class: str, batch: Optional[int] = None, device='cuda', seed: Optional[int] = None,

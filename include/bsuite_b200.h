@@ -37,7 +37,7 @@
 extern "C" {
 #endif
 
-#define BSB_ABI_VERSION 12
+#define BSB_ABI_VERSION 13
 #define BSB_DEVICE_HOST (-1)
 #define BSB_MAX_INFO 4
 #define BSB_MAX_PACKED_SETTINGS 64 /* bsb_create_packed: settings per handle */
@@ -268,6 +268,46 @@ int32_t bsb_create_packed(const bsb_config* configs, int32_t n_settings,
 /* Settings and lanes per setting of a handle (1 and B for bsb_create's). */
 int32_t bsb_packed_layout(const bsb_env* env, int32_t* n_settings,
                           int64_t* lanes_per_setting);
+
+/*
+ * Ragged pack: a packed handle whose settings differ in observation shape,
+ * with the same contract as bsb_create_packed -- lane k * lanes_per_setting
+ * + j is, bit for bit, lane j of
+ *   bsb_create(&configs[k], lanes_per_setting, device, seeds[k], lane_offset)
+ * (outputs, info, Logging columns, log rows, clamping of device actions and
+ * the actions bsb_rollout samples).  Beyond what packs allow, settings may
+ * differ in size together with the deep_sea mapping table, num_bits and
+ * n_distractor.  Families: deep_sea, memory_chain, umbrella_chain (any other
+ * returns BSB_UNSUPPORTED: use bsb_create_packed).  BSB_UNSUPPORTED, naming
+ * the field: BSB_RNG_MT19937, obs_dtype other than float32,
+ * BSB_FLAG_SAME_STEP_RESET, a reward wrapper, or a field the settings must
+ * share.  n_settings in [1, BSB_MAX_PACKED_SETTINGS] and
+ * lanes_per_setting >= 1, else BSB_INVALID_ARGUMENT.
+ *
+ * The observations of one step are ONE flat float32 buffer of step_elems
+ * elements (bsb_ragged_layout; a rollout's is [T][step_elems]): setting k's
+ * are a dense [lanes_per_setting, rows[k], cols[k]] block at element
+ * offsets[k].  Blocks follow setting order, each starts on a 128-byte
+ * boundary and step_elems is a multiple of 128 bytes; the gap elements
+ * between blocks are never written.  bsb_outputs.observation and
+ * bsb_step_host's device_obs / host_out->observation are that buffer;
+ * final_observation is refused.  bsb_obs_numel / bsb_obs_shape return
+ * BSB_UNSUPPORTED.  Every other entry point takes the handle as a batch of
+ * B = n_settings * lanes_per_setting lanes, as for a pack; bsb_step_host runs
+ * it in one phase.
+ */
+int32_t bsb_create_ragged(const bsb_config* configs, int32_t n_settings,
+                          int64_t lanes_per_setting, int32_t device,
+                          const uint64_t* seeds, uint64_t lane_offset,
+                          bsb_env** out);
+
+/* The observation buffer of a handle: offsets int64 [n_settings], rows and
+ * cols int32 [n_settings] (n_settings of bsb_packed_layout) and the elements
+ * of one step.  Every handle has one: an ordinary or uniformly packed handle
+ * reports offsets k * lanes_per_setting * obs_numel and step_elems
+ * B * obs_numel. */
+int32_t bsb_ragged_layout(const bsb_env* env, int64_t* offsets, int32_t* rows,
+                          int32_t* cols, int64_t* step_elems);
 
 int32_t bsb_destroy(bsb_env* env);
 
