@@ -39,9 +39,10 @@ template <> struct HostEmit<Mnist> {
 // element by element with obs_cast, the function the kernels use.  kSameStep: a lane whose step returned LAST is reset
 // in the same call, and its final observation goes to a.final_obs when that is given.  kPacked: every lane runs with
 // its setting's parameters (pack_lane_params), as the packed kernels do.  kRagged: the same with ragged_setting_params,
-// and lane j of setting k writes row j of the setting's observation block.
+// and lane j of setting k writes row j of the setting's observation block.  `mask` (masked calls, T = 1): lane i acts
+// only where mask[i] != 0; the others sit the call out (lane_sit_out) and their outputs are not written.
 template <class V, int RK>
-void host_run(const EnvParams& p, const LaunchArgs& a) {
+void host_run(const EnvParams& p, const LaunchArgs& a, const uint8_t* mask = nullptr) {
   typedef typename V::Fam F;
   typedef typename V::Obs O;
   constexpr bool kSameStep = V::kSameStep, kPacked = V::kPacked, kRagged = V::kRagged;
@@ -65,6 +66,10 @@ void host_run(const EnvParams& p, const LaunchArgs& a) {
     }
   };
   for (int64_t lane = 0; lane < B; ++lane) {
+    if (mask && !mask[lane]) {
+      if (track) lane_sit_out(p, lane);
+      continue;
+    }
     if constexpr (kPacked) { setting_p = p; pack_lane_params(setting_p, lane); }
     O* lane_obs = obs + lane * (int64_t)K;      // step 0's observation row of this lane
     int64_t step_elems = B * (int64_t)K;
@@ -360,6 +365,34 @@ int run_variant(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoP
       return launch(e, la, g, stream, transition_kernel<V, 0, kNoise, kTrack>, e->p, la);
     }
   });
+}
+
+// Masked calls of variant V (bsb_reset_masked / bsb_step_masked): the host path, or one launch of masked_kernel with
+// one chunk of 32 lanes per warp.
+template <class V>
+int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, cudaStream_t stream) {
+  constexpr bool kMt = Compiled<V>::kMt;
+  const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
+  if (e->device < 0) {
+    if constexpr (kMt) { if (mt) { host_run<V, 1>(e->p, a, mask); return BSB_OK; } }
+    host_run<V, 0>(e->p, a, mask);
+    return BSB_OK;
+  }
+  MaskArgs m;
+  m.mask = mask;
+  m.noise = e->p.wrapper == BSB_WRAP_REWARD_NOISE ? 1 : 0;
+  m.track = e->p.ep != nullptr ? 1 : 0;
+  LaunchArgs la = a;
+  la.bad_action = e->bad_action_dev;
+  la.use_pdl = 0;
+  la.work_counter = nullptr;
+  Geometry g;
+  g.threads = 64;
+  g.smem = 0;
+  g.n_chunks = V::kRagged ? (int64_t)e->n_settings * ((e->lanes_per_setting + 31) / 32) : (e->p.batch + 31) / 32;
+  g.grid = (g.n_chunks + g.threads / 32 - 1) / (g.threads / 32);
+  if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_kernel<V, 1>, e->p, la, m); }
+  return launch(e, la, g, stream, masked_kernel<V, 0>, e->p, la, m);
 }
 
 }  // namespace bsb

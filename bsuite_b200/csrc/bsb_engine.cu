@@ -83,8 +83,9 @@ template <class T> int env_alloc_t(bsb_env* e, T** out, size_t count, bool snaps
   return rc;
 }
 
-// `two_phase`: a two-phase host step (mailbox_launch; deep_sea and catch only).
-int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr) {
+// `two_phase`: a two-phase host step (mailbox_launch; deep_sea and catch only).  `mask`: a masked call.
+int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr,
+        const uint8_t* mask = nullptr) {
   DeviceGuard guard(e->device);
   LaunchArgs a = args;
   if (e->device >= 0) {
@@ -93,6 +94,7 @@ int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseA
     if (capture != cudaStreamCaptureStatusNone) e->graph_safe = true;
     if (e->graph_safe) a.clock = e->clock;      // a.step0 == e->steps_done, which no longer moves
   }
+  if (mask) return e->variant->run_masked(e, a, mask, stream);
   return e->variant->run(e, a, stream, two_phase);
 }
 
@@ -120,7 +122,8 @@ template <class O> constexpr int obs_dtype_id() {
   return std::is_same<O, float>::value ? BSB_OBS_FLOAT32 : std::is_same<O, Bf16>::value ? BSB_OBS_BFLOAT16 : BSB_OBS_UINT8;
 }
 
-#define BSB_ENTRY(F, O, mode, mt, two_phase) {FamilyId<F>::value, obs_dtype_id<O>(), mode, mt, two_phase, &run_variant<Variant<F, O, mode> >},
+#define BSB_ENTRY(F, O, mode, mt, two_phase) \
+  {FamilyId<F>::value, obs_dtype_id<O>(), mode, mt, two_phase, &run_variant<Variant<F, O, mode> >, &run_masked<Variant<F, O, mode> >},
 const VariantEntry kVariants[] = {BSB_VARIANTS(BSB_ENTRY)};
 #undef BSB_ENTRY
 
@@ -827,6 +830,37 @@ int32_t bsb_step(bsb_env* env, const int32_t* actions, const bsb_outputs* out, v
   int rc = run(env, a, static_cast<cudaStream_t>(stream));
   if (rc == BSB_OK) advance_steps(env, 1);
   return rc;
+}
+
+// bsb_reset_masked / bsb_step_masked: lane i makes the call only where mask[i] != 0 (run_masked).  Host handles
+// validate the actions of active lanes only: an inactive lane's action is never read.
+static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask, const bsb_outputs* out, void* stream,
+                       int mode) {
+  { int crc = check_final_observation(env, out); if (crc != BSB_OK) return crc; }
+  { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
+  if (env->device < 0 && mode == MODE_STEP) {
+    const uint32_t n = (uint32_t)env->p.num_actions;
+    for (int64_t k = 0; k < env->p.batch; ++k)
+      if (mask[k] && (uint32_t)actions[k] >= n)
+        return fail(BSB_INVALID_ARGUMENT, "action " + std::to_string(actions[k]) + " of active lane " + std::to_string(k) +
+                                              " is outside [0, " + std::to_string(n) + ")");
+  }
+  LaunchArgs a = make_args(env, out, mode == MODE_STEP ? actions : nullptr, 1, mode);
+  int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask);
+  if (rc == BSB_OK) advance_steps(env, 1);
+  return rc;
+}
+
+int32_t bsb_reset_masked(bsb_env* env, const uint8_t* mask, const bsb_outputs* out, void* stream) {
+  if (!env || !mask || !out || !out->observation)
+    return fail(BSB_INVALID_ARGUMENT, "bsb_reset_masked needs a mask and outputs with an observation buffer");
+  return masked_call(env, nullptr, mask, out, stream, MODE_RESET);
+}
+
+int32_t bsb_step_masked(bsb_env* env, const int32_t* actions, const uint8_t* mask, const bsb_outputs* out, void* stream) {
+  if (!env || !actions || !mask || !out || !out->observation)
+    return fail(BSB_INVALID_ARGUMENT, "bsb_step_masked needs actions, a mask and outputs with an observation buffer");
+  return masked_call(env, actions, mask, out, stream, MODE_STEP);
 }
 
 int32_t bsb_rollout(bsb_env* env, int64_t num_steps, const int32_t* actions, uint64_t action_seed,

@@ -343,6 +343,21 @@ BSB_HD void lane_step(const EnvParams& p, int64_t lane, typename F::Lane& L, R& 
   }
 }
 
+// A lane that sits out a masked call (bsb_step_masked / bsb_reset_masked) makes no call, but the handle's call count
+// still advances, and episode_stat / log_row_write read the lane's Logging columns from that global count.  So the
+// lane's own counters move instead: first_count and start_call each gain the skipped call, and steps = calls -
+// first_count and episode_len = calls - 1 - start_call keep the values of the lane's own call sequence.  Before the
+// lane's first call (first_count == 0 means "no episode yet" to episode_len) the first skip sets first_count to 1 and
+// leaves start_call at 0: after d skips first_count = d and start_call = d - 1, which read steps = episode_len = 0, and
+// the lane's first call overwrites start_call (it follows the constructor's _reset_next_step, as after a LAST).  The
+// same-step marker ep[5] waits for the lane's next call and is left alone.
+BSB_HD void lane_sit_out(const EnvParams& p, int64_t lane) {
+  double* first_count = p.ep + 3 * p.batch + lane;
+  double* start_call = p.ep + 4 * p.batch + lane;
+  if (*first_count != 0.0) *start_call += 1.0;
+  *first_count += 1.0;
+}
+
 // Observation emitter of each family.
 static const int EMIT_ROWS = 0, EMIT_ONEHOT = 1, EMIT_TWOHOT = 2, EMIT_IMAGE = 3;
 // Families whose observation is a pure function of the STORED lane state (F::describe after F::load): their
@@ -1444,6 +1459,147 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
     render_stored(own, true, keep);
   }
   retire_warp(a, ws, false);
+}
+
+// ----- masked calls -----------------------------------------------------------------------------------------------
+// bsb_step_masked / bsb_reset_masked: one call in which lane i acts only where mask[i] != 0.  An active lane makes the
+// call an unmasked reset / step would make; an inactive lane makes none (lane_sit_out) and none of its output entries
+// is written.  Noise and Logging are runtime flags here (lane_open / lane_step take them as arguments), so each
+// variant compiles one masked kernel per bit source.
+struct MaskArgs {
+  const uint8_t* mask;      // [B], device memory
+  int32_t noise, track;     // the RewardNoise stream is live / the Logging accumulators are tracked
+};
+
+// Writes lane j's observation `val(e)` (element e of K) with the whole warp: 16-byte streaming stores when `vec`
+// (the row starts 16-byte aligned and is a whole number of 16-byte words), else one element per store.
+template <class O, class Val>
+__device__ __forceinline__ void store_lane_obs(O* dst, int K, bool vec, const Val& val) {
+  constexpr int E = 16 / (int)sizeof(O);
+  const int tid = threadIdx.x & 31;
+  if (vec) {
+    for (int q = tid; q < K / E; q += 32) {
+      union { uint4 v; O o[E]; } w;
+#pragma unroll
+      for (int k = 0; k < E; ++k) w.o[k] = obs_cast<O>(val(q * E + k));
+      __stcs(reinterpret_cast<uint4*>(dst) + q, w.v);
+    }
+  } else {
+    for (int e = tid; e < K; e += 32) st_stream(dst + e, obs_cast<O>(val(e)));
+  }
+}
+
+// The observations of the warp's lanes for which `on` holds, into rows row0 + tid of `block` ([rows, K] elements of
+// O); the other rows are not touched.  Rows: each lane's thread renders its own row.  Tiles, boards and images: the
+// warp walks the lanes __ballot_sync selects and writes each one.  No TMA bulk store: a whole block would overwrite
+// the rows of inactive lanes.
+template <class F, class O, class R>
+__device__ __forceinline__ void emit_lane_subset(const EnvParams& lp, const typename F::Lane& L, R& rng, O* block, int K,
+                                                 int64_t row0, bool on, bool vec_base) {
+  constexpr int kEmit = EmitKind<F>::value;
+  const int tid = threadIdx.x & 31;
+  if (kEmit == EMIT_ROWS) {
+    if (on) RowRenderer<F, R>::run(lp, L, rng, block + (row0 + tid) * (int64_t)K);
+    return;
+  }
+  const bool vec = vec_base && ((int64_t)K * (int64_t)sizeof(O)) % 16 == 0;
+  const int da = Descriptor<F>::a(L), db = Descriptor<F>::b(L);
+  for (unsigned rest = __ballot_sync(0xffffffffu, on); rest != 0u; rest &= rest - 1u) {
+    const int j = __ffs(rest) - 1;
+    const int a0 = __shfl_sync(0xffffffffu, da, j), b0 = __shfl_sync(0xffffffffu, db, j);
+    O* dst = block + (row0 + j) * (int64_t)K;
+    if (kEmit == EMIT_IMAGE) {                 // a0 < 0: mnist's all-zero LAST frame (mnist.py:74)
+      const int8_t* src = lp.images + (int64_t)(a0 < 0 ? 0 : a0) * K;
+      store_lane_obs(dst, K, vec, [&](int e) { return a0 >= 0 ? Mnist::pixel(src[e]) : 0.f; });
+    } else {                                   // one-hot tiles (b0 = -1) and two-hot boards
+      store_lane_obs(dst, K, vec, [&](int e) { return (e == a0 || e == b0) ? 1.f : 0.f; });
+    }
+  }
+}
+
+// One masked call, T = 1.  One chunk of 32 lanes per warp; a ragged pack's chunks never straddle two settings (as in
+// ragged_chunks), and row j of setting k goes to the setting's block.  Graph-safe mode reads the call index from the
+// device clock and advances it by one, as transition_kernel does; the mask is read on every launch, so a graph
+// replays with whatever the mask buffer holds.
+template <class V, int RK>
+__global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(const EnvParams p, const LaunchArgs a, const MaskArgs m) {
+  typedef typename V::Fam Fam;
+  typedef typename V::Obs O;
+  typedef typename RngOf<RK>::type R;
+  const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
+  int64_t step0 = a.step0;
+  if (a.clock) step0 += (int64_t)*reinterpret_cast<volatile unsigned long long*>(a.clock + 16 * (blockIdx.x % CLOCK_GROUPS));
+  const MailFields out = {a.reward, a.reward_f64, a.discount, a.step_type};
+  const bool noise = m.noise != 0, track = m.track != 0;
+  const RaggedTable* table = V::kRagged ? reinterpret_cast<const RaggedTable*>(p.pack) : nullptr;
+  const int64_t lanes = V::kRagged ? table->pack.lanes_per_setting : p.batch;      // lanes per setting block
+  const int64_t per_setting = (lanes + 31) / 32;
+  const int64_t n_chunks = (V::kRagged ? table->pack.n_settings : 1) * per_setting;
+  const int64_t chunk = (int64_t)blockIdx.x * warps_per_cta + warp;
+
+  if (chunk < n_chunks) {
+    const int64_t k = chunk / per_setting;
+    const int64_t local_base = (chunk - k * per_setting) * 32;         // the chunk's first row within its block
+    const int64_t lane = k * lanes + local_base + tid;
+    const bool in = local_base + tid < lanes;
+    EnvParams lp = p;
+    O* block = reinterpret_cast<O*>(a.obs);
+    if constexpr (V::kRagged) {
+      const RaggedSetting& s = ragged_setting(table, k);
+      ragged_setting_params(lp, s, table->mapping_bits);
+      block += s.obs_offset;
+    } else if constexpr (V::kPacked) {
+      if (in) pack_lane_params(lp, lane);
+    }
+    const bool on = in && m.mask[lane] != 0;
+
+    typename Fam::Lane L;
+    R rng, wrng;
+    EpisodeStats ep;
+    Fam::init(p, L);
+    MergedReset<Fam, R> merged;            // same-step kernels only
+    if constexpr (V::kSameStep) { Fam::init(p, merged.last); merged.done = false; }
+    if (on) {
+      lane_open<Fam>(lp, lane, L, rng, wrng, ep, a.mode, noise, track);
+      int32_t action = 0;
+      if (a.mode == MODE_STEP) {
+        action = a.actions[lane];
+        if ((uint32_t)action >= (uint32_t)p.num_actions) {
+          if (a.bad_action) *a.bad_action = 1;
+          action = action < 0 ? 0 : p.num_actions - 1;
+        }
+      }
+      if constexpr (V::kSameStep) lane_step<Fam, R, true>(p, lane, L, rng, wrng, ep, action, a.mode, noise, track, step0, out, lane, &merged);
+      else lane_step<Fam>(lp, lane, L, rng, wrng, ep, action, a.mode, noise, track, step0, out, lane);
+    } else if (in && track) {
+      lane_sit_out(p, lane);
+    }
+    if constexpr (V::kSameStep) {
+      if (a.final_obs)
+        emit_lane_subset<Fam>(lp, merged.last, merged.rng, reinterpret_cast<O*>(a.final_obs), lp.obs_numel, local_base,
+                              on && merged.done, a.final_vec_ok != 0);
+    }
+    emit_lane_subset<Fam>(lp, L, rng, block, lp.obs_numel, local_base, on, a.obs_vec_ok != 0);
+    if (on) lane_close<Fam>(lp, lane, L, rng, wrng, ep, noise, track);
+  }
+
+  if (a.clock) {        // graph-safe mode: the last CTA advances the call count by one (transition_kernel's epilogue)
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      const unsigned groups = gridDim.x < (unsigned)CLOCK_GROUPS ? gridDim.x : (unsigned)CLOCK_GROUPS;
+      const unsigned g = blockIdx.x % groups;
+      const unsigned members = gridDim.x / groups + (g < gridDim.x % groups ? 1u : 0u);
+      unsigned long long* sub = a.clock + CLOCK_SUB0 + 16 * g;
+      if (atomicAdd(sub, 1ull) == (unsigned long long)members - 1ull) {
+        *sub = 0ull;
+        if (atomicAdd(a.clock + CLOCK_TOP, 1ull) == (unsigned long long)groups - 1ull) {
+          const unsigned long long steps = (unsigned long long)(step0 - a.step0) + 1ull;
+          for (int r = 0; r < CLOCK_GROUPS; ++r) a.clock[16 * r] = steps;
+          a.clock[CLOCK_TOP] = 0ull;
+        }
+      }
+    }
+  }
 }
 
 #endif  // __CUDACC__

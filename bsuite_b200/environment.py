@@ -416,17 +416,46 @@ class BatchedEnvironment:
     return actions
 
   # ---- dynamics ------------------------------------------------------------
-  def reset(self, out: Optional[StepBuffers] = None):
-    """base.Environment.reset for every lane (base.py:54-57)."""
+  def _mask(self, mask, out):
+    """The uint8 [B] tensor of a `mask` argument on the environment's device (a bool tensor is viewed, not copied)."""
+    torch = self._torch
+    if out is None:
+      raise ValueError('a masked call needs out=: the buffers that hold every lane\'s latest timestep (inactive '
+                       'lanes leave their entries as they are)')
+    if not isinstance(mask, torch.Tensor) or mask.dtype not in (torch.bool, torch.uint8):
+      raise ValueError(f'mask must be a bool or uint8 tensor, got {getattr(mask, "dtype", type(mask).__name__)}')
+    if tuple(mask.shape) != (self._batch,):
+      raise ValueError(f'mask must have shape ({self._batch},), got {tuple(mask.shape)}')
+    if mask.device != self._device:
+      raise ValueError(f'mask must live on {self._device}, got {mask.device}')
+    mask = mask.contiguous()
+    return mask.view(torch.uint8) if mask.dtype is torch.bool else mask
+
+  def reset(self, out: Optional[StepBuffers] = None, mask=None):
+    """base.Environment.reset for every lane (base.py:54-57).
+
+    `mask` (bool or uint8 tensor [B] on the environment's device; needs `out`): only the lanes where it is set
+    reset; the others make no call and their entries of `out` are left as they are (`bsb_reset_masked`)."""
+    if mask is not None:
+      mask = self._mask(mask, out)
     out = out or self.make_buffers()
     outputs = out.bind(self._obs_dtype)
     self._async_work = True
-    _lib.check(self._lib.bsb_reset(self._handle.ptr, ctypes.byref(outputs), self._stream()))
+    if mask is not None:
+      _lib.check(self._lib.bsb_reset_masked(self._handle.ptr, mask.data_ptr(), ctypes.byref(outputs), self._stream()))
+    else:
+      _lib.check(self._lib.bsb_reset(self._handle.ptr, ctypes.byref(outputs), self._stream()))
     return out.timestep()
 
-  def step(self, actions, out: Optional[StepBuffers] = None):
-    """base.Environment.step for every lane (base.py:59-65); actions int [B]."""
+  def step(self, actions, out: Optional[StepBuffers] = None, mask=None):
+    """base.Environment.step for every lane (base.py:59-65); actions int [B].
+
+    `mask` (bool or uint8 tensor [B] on the environment's device; needs `out`): only the lanes where it is set step;
+    the others make no call, their actions are ignored (never validated) and their entries of `out` are left as they
+    are (`bsb_step_masked`).  Every call, masked or not, counts once in `steps_done`."""
     torch = self._torch
+    if mask is not None:
+      return self._step_masked(actions, out, mask)
     if not (type(actions) is torch.Tensor and actions.dtype is torch.int32 and actions.dim() == 1
             and actions.shape[0] == self._batch and actions.is_contiguous()
             and (actions.device == self._device
@@ -442,6 +471,15 @@ class BatchedEnvironment:
     status = self._lib.bsb_step(self._handle.ptr, actions.data_ptr(), ctypes.byref(outputs), self._stream())
     if status:
       _lib.check(status)
+    return out.timestep()
+
+  def _step_masked(self, actions, out, mask):
+    mask = self._mask(mask, out)
+    actions = self._device_actions(actions, (self._batch,))
+    outputs = out.bind(self._obs_dtype)
+    self._async_work = True
+    _lib.check(self._lib.bsb_step_masked(self._handle.ptr, actions.data_ptr(), mask.data_ptr(), ctypes.byref(outputs),
+                                         self._stream()))
     return out.timestep()
 
   def make_mixed_buffers(self) -> StepBuffers:

@@ -77,6 +77,51 @@ def run(agent, environment, num_steps: int) -> None:
     timestep = new_timestep
 
 
+def run_episodes(agent, environment, num_episodes: Optional[int] = None, check_every: int = 16):
+  """`experiment.run` (baselines/experiment.py:24-57) for B lanes: every lane plays exactly its episode budget and
+  then stops, as the reference's loop stops after `num_episodes` episodes.
+
+  The budget is `num_episodes` for every lane, or by default each lane's `bsuite_num_episodes` (per setting on a
+  packed environment).  Lanes run in lock-step, so they reach their budgets at different calls; a lane that has
+  finished is masked out of the following calls (`step(..., mask=...)`), so its `bsuite_info()`, episode statistics
+  and log rows describe exactly the budget's episodes.  The agent sees the whole batch every call
+  (`select_action(timestep) -> int tensor [B]`, `update(timestep, actions, new_timestep)`); a finished lane's
+  entries of the timestep keep its final LAST.  The LAST counts stay on the device; the loop asks whether any lane
+  is still running once every `check_every` calls.  Returns the number of calls made after the first reset."""
+  torch = environment._torch
+  B, device = environment.batch, environment.device
+  if num_episodes is not None:
+    budget = torch.full((B,), int(num_episodes), dtype=torch.int64, device=device)
+  elif environment.bsuite_ids is not None:
+    lanes = environment.lanes_per_setting
+    per_setting = [spec.bsuite_num_episodes for spec in environment._pack[1]]
+    budget = torch.tensor(per_setting, dtype=torch.int64).repeat_interleave(lanes).to(device)
+  else:
+    budget = torch.full((B,), int(environment.bsuite_num_episodes), dtype=torch.int64, device=device)
+  finished = torch.zeros(B, dtype=torch.int64, device=device)
+  active = budget > 0
+  out = environment.make_buffers()
+  timestep = environment.reset(out=out, mask=active)
+  # the agent keeps the previous timestep while the same buffers receive the next one
+  spare = environment.make_buffers()
+  calls = 0
+  while True:
+    if calls % max(int(check_every), 1) == 0 and not bool(active.any()):
+      return calls
+    actions = agent.select_action(timestep)
+    spare.observation.copy_(out.observation)
+    spare.reward.copy_(out.reward)
+    spare.discount.copy_(out.discount)
+    spare.step_type.copy_(out.step_type)
+    previous = spare.timestep()
+    new_timestep = environment.step(actions, out=out, mask=active)
+    calls += 1
+    agent.update(previous, actions, new_timestep)
+    finished += ((new_timestep.step_type == 2) & active).to(torch.int64)
+    active = finished < budget
+    timestep = new_timestep
+
+
 class Replay:
   """Uniform replay of flat item tuples as device tensors (`bsuite/baselines/utils/replay.py:24-88`): a ring of
   `capacity` slots per item, `add(items)` writes one tuple, `sample(size)` returns a list of `[size, ...]` tensors

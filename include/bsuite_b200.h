@@ -37,7 +37,7 @@
 extern "C" {
 #endif
 
-#define BSB_ABI_VERSION 13
+#define BSB_ABI_VERSION 14
 #define BSB_DEVICE_HOST (-1)
 #define BSB_MAX_INFO 4
 #define BSB_MAX_PACKED_SETTINGS 64 /* bsb_create_packed: settings per handle */
@@ -324,6 +324,28 @@ int32_t bsb_reset(bsb_env* env, const bsb_outputs* out, void* stream);
 /* base.Environment.step (base.py:59-65) for all lanes; actions int32 [B]. */
 int32_t bsb_step(bsb_env* env, const int32_t* actions, const bsb_outputs* out,
                  void* stream);
+
+/*
+ * Masked calls: reset() / step() for the lanes i with mask[i] != 0 only.
+ * mask is uint8 [B] in the handle's memory space (device memory for a CUDA
+ * handle, host memory for BSB_DEVICE_HOST).  An active lane makes exactly the
+ * call bsb_reset / bsb_step would make for it (same transition, same random
+ * draws, same outputs).  An inactive lane makes no call: its state, RNG
+ * streams, info fields and Logging columns stay as they were, its action is
+ * never read (so it never raises the invalid-action flag), and none of its
+ * output entries -- observation row, reward, discount, step_type,
+ * final_observation -- is written.  Lane i of a handle driven by masked calls
+ * is, bit for bit, lane 0 of a one-lane handle with lane_offset + i driven by
+ * the calls in which mask[i] was set.  Every masked call advances the call
+ * count (bsb_steps_done) by one, even with an empty mask.  Works in
+ * graph-safe mode and may be captured; a replay reads the mask buffer as it
+ * is then.  Masked steps take explicit actions (int32 [B]) only.
+ */
+int32_t bsb_reset_masked(bsb_env* env, const uint8_t* mask,
+                         const bsb_outputs* out, void* stream);
+int32_t bsb_step_masked(bsb_env* env, const int32_t* actions,
+                        const uint8_t* mask, const bsb_outputs* out,
+                        void* stream);
 
 /*
  * T consecutive step() calls fused in one launch, lane state held in

@@ -125,6 +125,26 @@ for bsuite_id, batch in (('deep_sea/11', 20000), ('catch/0', 3000), ('mnist/0', 
   print(bsuite_id, batch, 'host-driven steps == ordinary steps: True', flush=True)
   env.close(); twin.close()
 split_steps()
+# Masked calls (masked_kernel): warp-written tiles / boards / rows of a lane subset, partial warps, same-step final
+# observations and a ragged pack, against the host path.
+for bsuite_id, batch, kw in (('deep_sea/11', 1001, {}), ('catch/0', 997, dict(autoreset='same_step')),
+                             ('umbrella_distract/3', 501, {}), ('mnist/0', 333, dict(obs_dtype='bfloat16'))):
+  plan = [(kind, torch.rand(batch, generator=torch.Generator().manual_seed(c)) < (0.5, 0.03, 1.0)[c % 3])
+          for c, kind in enumerate(('reset', 'step', 'step', 'step', 'reset', 'step'))]
+  got = []
+  for device in ('cuda', 'cpu'):
+    env = bsuite_b200.load_from_id(bsuite_id, batch=batch, device=device, seed=3, track_episodes=True, **kw)
+    out = env.make_buffers(final_observation='autoreset' in kw)
+    out.observation.fill_(5)
+    for kind, mask in plan:
+      if kind == 'reset':
+        env.reset(out=out, mask=mask.to(device))
+      else:
+        env.step(torch.ones(batch, dtype=torch.int32, device=device), out=out, mask=mask.to(device))
+    got.append([out.observation.cpu(), out.reward.cpu(), env.episode_stat_sums().cpu()])
+    env.close()
+  assert all(torch.equal(a, b) for a, b in zip(*got))
+  print(bsuite_id, batch, 'masked calls == host path: True', flush=True)
 # One-launch reduction over several environments and a whole lock-step in one graph.
 from bsuite_b200 import suite
 ids = ['catch/0', 'deep_sea/0', 'bandit_noise/0', 'cartpole/0', 'mnist/0', 'umbrella_length/0']
