@@ -148,11 +148,14 @@ BSB_HD double np_remainder(double a, double b) {
 // always equal to the correctly rounded x*x (about 1e-3 of inputs differ by one
 // ulp), so the host path calls pow to stay bit-identical with the reference
 // while the device uses the exact product (CUDA pow is looser than either).
+// The exponent is read through a volatile: with a constant 2.0, GCC folds the
+// call into x * x, which is exactly the product this function must not compute.
 BSB_HD double square_like_reference(double x) {
 #if defined(__CUDA_ARCH__)
   return x * x;
 #else
-  return pow(x, 2.0);
+  volatile double two = 2.0;
+  return pow(x, two);
 #endif
 }
 
