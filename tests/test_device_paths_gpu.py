@@ -30,7 +30,8 @@ also go through oracle.run_lanes, which anchors the comparison outside the engin
 Exactness follows tests/conftest.py: integer / grid families bit for bit (step_type, discount, reward, observation,
 bsuite_info, episode_stats, log rows, state blob); float dynamics, the reward-noise wrapper and stochastic deep_sea
 match step_type and discount exactly and the rest within FLOAT_TOL (CUDA sin / cos / log differ from glibc in the
-last ulp), without the blob (it holds float state and cached gaussians).
+last ulp), without the blob (it holds float state and cached gaussians).  The rewards of integer-dynamics families
+that draw a gaussian are held per element to the bound of one draw, `gauss_draw_reference.noise_reward_tolerance`.
 """
 
 import gzip
@@ -49,6 +50,7 @@ from bsuite_b200 import datasets
 from bsuite_b200 import experiments
 from oracle import bsuite_oracle as oracle
 from tests import conftest as cf
+from tests import gauss_draw_reference as gr
 
 FAMILIES = bsb_build.FAMILIES
 RNGS = ('philox', 'mt19937')
@@ -209,7 +211,7 @@ def compare(where, field, got, want, axes, step0=0, atol=0.0, rtol=0.0, context=
   """Raises TwinMismatch naming the first differing element; returns the largest |got - want| (0 if exact)."""
   if got.shape != want.shape or got.dtype != want.dtype:
     raise TwinMismatch(f'{where}: {field} has shape/dtype {got.shape}/{got.dtype}, want {want.shape}/{want.dtype} | {context}')
-  if atol == 0 and rtol == 0:
+  if not np.any(atol) and rtol == 0:
     bad, dev = got != want, 0.0
   else:
     diff = np.abs(got.astype(np.float64) - want.astype(np.float64))
@@ -222,7 +224,7 @@ def compare(where, field, got, want, axes, step0=0, atol=0.0, rtol=0.0, context=
       where_at['step'] += step0
     at = ', '.join(f'{k}={v}' for k, v in where_at.items())
     raise TwinMismatch(f'{where}: {field} differs first at {at}: got {got[first].item()!r}, want {want[first].item()!r} '
-                       f'({int(bad.sum())} of {bad.size} elements differ, atol={atol}, rtol={rtol}) | {context}')
+                       f'({int(bad.sum())} of {bad.size} elements differ, atol={np.max(atol)}, rtol={rtol}) | {context}')
   return dev
 
 
@@ -260,6 +262,11 @@ class Twins:
     self.tol = dict(step_type=0.0, discount=0.0, actions=0.0, reward=0.0 if self.exact else cf.FLOAT_TOL * scale,
                     observation=cf.FLOAT_TOL if case['family'] in cf.FLOAT_FAMILIES else 0.0)
     self.state_atol = 0.0 if self.exact else cf.FLOAT_TOL * scale
+    # integer dynamics whose reward draws a gaussian (RewardNoise, stochastic deep_sea's corner reward): the draws are
+    # the only inexact part of the reward, held per element to the bound of one draw (its scale: the sum of both)
+    stochastic_ds = case['family'] == 'deep_sea' and not case['kwargs'].get('deterministic', True)
+    self.draw_scale = (None if case['family'] in cf.FLOAT_FAMILIES or self.exact
+                       else abs(case['noise'] or 0.0) + (1.0 if stochastic_ds else 0.0))
     self.max_dev = {}
     self.envs = []
     try:
@@ -283,7 +290,7 @@ class Twins:
 
   def _cmp(self, where, field, got, want, axes, atol=0.0, rtol=0.0, step0=0):
     dev = compare(where, field, got, want, axes, step0, atol, rtol, self.context)
-    if atol or rtol:
+    if np.any(atol) or rtol:
       self.max_dev[field] = max(self.max_dev.get(field, 0.0), dev)
 
   def check_call(self, where, outs, num_steps, actions=None):
@@ -296,7 +303,10 @@ class Twins:
       if not num_steps:
         got, want = got[None], want[None]
       host[field] = want
-      self._cmp(where, field, got, want, axes, atol=self.tol[field], step0=self.t)
+      atol = self.tol[field]
+      if field == 'reward' and self.draw_scale is not None:
+        atol = gr.noise_reward_tolerance(self.draw_scale, want)
+      self._cmp(where, field, got, want, axes, atol=atol, step0=self.t)
     T = host['step_type'].shape[0]
     if actions is None:
       actions = host.get('actions', np.zeros((T, self.case['batch']), np.int32))

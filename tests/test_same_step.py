@@ -123,7 +123,8 @@ def run_folded_lane(meta, data, k, device='cpu', fused=False):
 
 
 def check_folded_lane(name, meta, data, k, calls, res, info, reward_tol=0.0, obs_tol=0.0):
-  """The folded outputs of lane k against the fixture: every reference value exactly once."""
+  """The folded outputs of lane k against the fixture: every reference value exactly once.  `reward_tol` is a number
+  or a function of the reward returned."""
   obs_shape = data['observation'].shape[2:]
   close = lambda got, want, where, tol: np.testing.assert_allclose(got, want, rtol=0, atol=tol, err_msg=where) if tol \
       else np.testing.assert_array_equal(got, want, err_msg=where)
@@ -136,7 +137,8 @@ def check_folded_lane(name, meta, data, k, calls, res, info, reward_tol=0.0, obs
     if st == 0:
       assert res['reward'][c].reshape(-1)[0] == 0.0 and res['discount'][c].reshape(-1)[0] == 0.0, where
     else:
-      close(res['reward'][c].reshape(-1)[0], data['reward'][t, k], where + ' reward', reward_tol)
+      got = res['reward'][c].reshape(-1)[0]
+      close(got, data['reward'][t, k], where + ' reward', reward_tol(got) if callable(reward_tol) else reward_tol)
       assert res['discount'][c].reshape(-1)[0] == data['discount'][t, k], where
     final = res['final_observation'][c].reshape(obs_shape)
     if st == 2:
