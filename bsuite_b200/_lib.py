@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BSB_LIBRARY points the binding at another build of the SAME library (tools/host_sanitize.sh: ASan/UBSan build)
 LIB_PATH = os.environ.get('BSB_LIBRARY') or os.path.join(_HERE, 'libbsuite_b200.so')
 
-ABI_VERSION = 14
+ABI_VERSION = 15
 DEVICE_HOST = -1
 MAX_INFO = 4
 MAX_PACKED_SETTINGS = 64      # bsb_create_packed: settings per handle
@@ -124,6 +124,9 @@ EXPORTS = {
                                          ctypes.c_void_p]),
     'bsb_rollout': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_uint64,
                                      ctypes.POINTER(Outputs), ctypes.c_void_p, ctypes.c_void_p]),
+    'bsb_rollout_masked': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p, ctypes.c_uint64,
+                                            ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Outputs), ctypes.c_void_p,
+                                            ctypes.c_void_p]),
     'bsb_random_actions': (ctypes.c_int32, [ctypes.c_uint64, ctypes.c_uint64, ctypes.c_int64, ctypes.c_int64,
                                             ctypes.c_int64, ctypes.c_int32, ctypes.c_void_p]),
     'bsb_steps_done': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64)]),

@@ -39,10 +39,12 @@ template <> struct HostEmit<Mnist> {
 // element by element with obs_cast, the function the kernels use.  kSameStep: a lane whose step returned LAST is reset
 // in the same call, and its final observation goes to a.final_obs when that is given.  kPacked: every lane runs with
 // its setting's parameters (pack_lane_params), as the packed kernels do.  kRagged: the same with ragged_setting_params,
-// and lane j of setting k writes row j of the setting's observation block.  `mask` (masked calls, T = 1): lane i acts
-// only where mask[i] != 0; the others sit the call out (lane_sit_out) and their outputs are not written.
+// and lane j of setting k writes row j of the setting's observation block.  `mask` (masked calls and rollouts): lane i
+// acts only while mask[i] != 0 and its budget episodes_left[i] (when given) is positive; each LAST it returns takes one
+// from the budget, so its active steps are a prefix of the T.  The calls it sits out come after them
+// (lane_sit_out_calls), and their outputs are not written.
 template <class V, int RK>
-void host_run(const EnvParams& p, const LaunchArgs& a, const uint8_t* mask = nullptr) {
+void host_run(const EnvParams& p, const LaunchArgs& a, const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr) {
   typedef typename V::Fam F;
   typedef typename V::Obs O;
   constexpr bool kSameStep = V::kSameStep, kPacked = V::kPacked, kRagged = V::kRagged;
@@ -66,8 +68,10 @@ void host_run(const EnvParams& p, const LaunchArgs& a, const uint8_t* mask = nul
     }
   };
   for (int64_t lane = 0; lane < B; ++lane) {
-    if (mask && !mask[lane]) {
-      if (track) lane_sit_out(p, lane);
+    const bool budgeted = mask && mask[lane] && episodes_left;
+    int64_t left = budgeted ? episodes_left[lane] : 0;
+    if ((mask && !mask[lane]) || (budgeted && left <= 0)) {
+      if (track) lane_sit_out_calls(p, lane, a.T);
       continue;
     }
     if constexpr (kPacked) { setting_p = p; pack_lane_params(setting_p, lane); }
@@ -92,6 +96,7 @@ void host_run(const EnvParams& p, const LaunchArgs& a, const uint8_t* mask = nul
     MergedReset<F, R> merged;
     F::init(p, merged.last);
     merged.done = false;
+    int64_t acted = 0;
     for (int64_t t = 0; t < a.T; ++t) {
       const int64_t off = t * B + lane;
       int32_t action = 0;
@@ -103,8 +108,13 @@ void host_run(const EnvParams& p, const LaunchArgs& a, const uint8_t* mask = nul
       lane_step<F, R, kSameStep>(lp, lane, L, rng, wrng, ep, action, a.mode, noise, track, a.step0 + t, out, off, &merged);
       if constexpr (kSameStep) { if (merged.done && fin) render(lp, merged.last, merged.rng, fin + off * (int64_t)K); }
       render(lp, L, rng, lane_obs + t * step_elems);
+      ++acted;
+      // the step's LAST: a same-step lane's merged reset, else the _reset_next_step flag the step left set
+      if (budgeted && (kSameStep ? merged.done : L.nr != 0) && --left == 0) break;
     }
     lane_close<F>(lp, lane, L, rng, wrng, ep, noise, track);
+    if (mask && track && acted < a.T) lane_sit_out_calls(p, lane, a.T - acted);
+    if (budgeted) episodes_left[lane] = left;
   }
 }
 
@@ -367,21 +377,23 @@ int run_variant(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoP
   });
 }
 
-// Masked calls of variant V (bsb_reset_masked / bsb_step_masked): the host path, or one launch of masked_kernel with
-// one chunk of 32 lanes per warp.
+// Masked calls of variant V (bsb_reset_masked / bsb_step_masked, and bsb_rollout_masked when `rollout`): the host
+// path, or one launch of masked_kernel / masked_rollout_kernel with one chunk of 32 lanes per warp.
 template <class V>
-int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, cudaStream_t stream) {
+int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* episodes_left, bool rollout,
+               cudaStream_t stream) {
   constexpr bool kMt = Compiled<V>::kMt;
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
   if (e->device < 0) {
-    if constexpr (kMt) { if (mt) { host_run<V, 1>(e->p, a, mask); return BSB_OK; } }
-    host_run<V, 0>(e->p, a, mask);
+    if constexpr (kMt) { if (mt) { host_run<V, 1>(e->p, a, mask, episodes_left); return BSB_OK; } }
+    host_run<V, 0>(e->p, a, mask, episodes_left);
     return BSB_OK;
   }
   MaskArgs m;
   m.mask = mask;
   m.noise = e->p.wrapper == BSB_WRAP_REWARD_NOISE ? 1 : 0;
   m.track = e->p.ep != nullptr ? 1 : 0;
+  m.episodes_left = episodes_left;
   LaunchArgs la = a;
   la.bad_action = e->bad_action_dev;
   la.use_pdl = 0;
@@ -391,6 +403,10 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, cudaStream_
   g.smem = 0;
   g.n_chunks = V::kRagged ? (int64_t)e->n_settings * ((e->lanes_per_setting + 31) / 32) : (e->p.batch + 31) / 32;
   g.grid = (g.n_chunks + g.threads / 32 - 1) / (g.threads / 32);
+  if (rollout) {
+    if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_rollout_kernel<V, 1>, e->p, la, m); }
+    return launch(e, la, g, stream, masked_rollout_kernel<V, 0>, e->p, la, m);
+  }
   if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_kernel<V, 1>, e->p, la, m); }
   return launch(e, la, g, stream, masked_kernel<V, 0>, e->p, la, m);
 }

@@ -83,9 +83,10 @@ template <class T> int env_alloc_t(bsb_env* e, T** out, size_t count, bool snaps
   return rc;
 }
 
-// `two_phase`: a two-phase host step (mailbox_launch; deep_sea and catch only).  `mask`: a masked call.
+// `two_phase`: a two-phase host step (mailbox_launch; deep_sea and catch only).  `mask`: a masked call, or with
+// `rollout` a masked rollout (`episodes_left`: its budgets, nullable).
 int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr,
-        const uint8_t* mask = nullptr) {
+        const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr, bool rollout = false) {
   DeviceGuard guard(e->device);
   LaunchArgs a = args;
   if (e->device >= 0) {
@@ -94,7 +95,7 @@ int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseA
     if (capture != cudaStreamCaptureStatusNone) e->graph_safe = true;
     if (e->graph_safe) a.clock = e->clock;      // a.step0 == e->steps_done, which no longer moves
   }
-  if (mask) return e->variant->run_masked(e, a, mask, stream);
+  if (mask) return e->variant->run_masked(e, a, mask, episodes_left, rollout, stream);
   return e->variant->run(e, a, stream, two_phase);
 }
 
@@ -832,22 +833,28 @@ int32_t bsb_step(bsb_env* env, const int32_t* actions, const bsb_outputs* out, v
   return rc;
 }
 
-// bsb_reset_masked / bsb_step_masked: lane i makes the call only where mask[i] != 0 (run_masked).  Host handles
-// validate the actions of active lanes only: an inactive lane's action is never read.
+// bsb_reset_masked / bsb_step_masked / bsb_rollout_masked: lane i makes the calls only where mask[i] != 0
+// (run_masked), a rollout's lanes only while their budgets last.  Host handles validate the actions of masked-in
+// lanes only, at every step of a rollout: an inactive lane's action is never read.
 static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask, const bsb_outputs* out, void* stream,
-                       int mode) {
+                       int mode, int64_t T = 1, bool rollout = false, uint64_t action_seed = 0,
+                       int32_t* actions_out = nullptr, int64_t* episodes_left = nullptr) {
   { int crc = check_final_observation(env, out); if (crc != BSB_OK) return crc; }
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
-  if (env->device < 0 && mode == MODE_STEP) {
+  if (env->device < 0 && mode == MODE_STEP && actions) {
     const uint32_t n = (uint32_t)env->p.num_actions;
-    for (int64_t k = 0; k < env->p.batch; ++k)
-      if (mask[k] && (uint32_t)actions[k] >= n)
-        return fail(BSB_INVALID_ARGUMENT, "action " + std::to_string(actions[k]) + " of active lane " + std::to_string(k) +
-                                              " is outside [0, " + std::to_string(n) + ")");
+    const int64_t B = env->p.batch;
+    for (int64_t t = 0; t < T; ++t)
+      for (int64_t k = 0; k < B; ++k)
+        if (mask[k] && (uint32_t)actions[t * B + k] >= n)
+          return fail(BSB_INVALID_ARGUMENT, "action " + std::to_string(actions[t * B + k]) + " of active lane " +
+                                                std::to_string(k) + (rollout ? " at step " + std::to_string(t) : "") +
+                                                " is outside [0, " + std::to_string(n) + ")");
   }
-  LaunchArgs a = make_args(env, out, mode == MODE_STEP ? actions : nullptr, 1, mode);
-  int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask);
-  if (rc == BSB_OK) advance_steps(env, 1);
+  LaunchArgs a = make_args(env, out, mode == MODE_STEP ? actions : nullptr, T, mode);
+  a.action_seed = action_seed; a.actions_out = actions_out;
+  int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask, episodes_left, rollout);
+  if (rc == BSB_OK) advance_steps(env, T);
   return rc;
 }
 
@@ -875,6 +882,15 @@ int32_t bsb_rollout(bsb_env* env, int64_t num_steps, const int32_t* actions, uin
   int rc = run(env, a, static_cast<cudaStream_t>(stream));
   if (rc == BSB_OK) advance_steps(env, num_steps);
   return rc;
+}
+
+int32_t bsb_rollout_masked(bsb_env* env, int64_t num_steps, const int32_t* actions, uint64_t action_seed,
+                           const uint8_t* mask, int64_t* episodes_left, const bsb_outputs* out, int32_t* actions_out,
+                           void* stream) {
+  if (!env || !mask || !out || !out->observation)
+    return fail(BSB_INVALID_ARGUMENT, "bsb_rollout_masked needs a mask and outputs with an observation buffer");
+  if (num_steps <= 0) return fail(BSB_INVALID_ARGUMENT, "num_steps must be positive");
+  return masked_call(env, actions, mask, out, stream, MODE_STEP, num_steps, true, action_seed, actions_out, episodes_left);
 }
 
 int32_t bsb_random_actions(uint64_t action_seed, uint64_t lane_offset, int64_t batch, int64_t first_step,

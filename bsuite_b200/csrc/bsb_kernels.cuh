@@ -357,6 +357,14 @@ BSB_HD void lane_sit_out(const EnvParams& p, int64_t lane) {
   if (*first_count != 0.0) *start_call += 1.0;
   *first_count += 1.0;
 }
+// d >= 1 consecutive calls of lane_sit_out at once (masked rollouts: a lane's sit-outs all follow its last active
+// call): first_count gains d, start_call d, or d - 1 when the first of them met first_count == 0.
+BSB_HD void lane_sit_out_calls(const EnvParams& p, int64_t lane, int64_t d) {
+  double* first_count = p.ep + 3 * p.batch + lane;
+  double* start_call = p.ep + 4 * p.batch + lane;
+  *start_call += (double)(*first_count != 0.0 ? d : d - 1);
+  *first_count += (double)d;
+}
 
 // Observation emitter of each family.
 static const int EMIT_ROWS = 0, EMIT_ONEHOT = 1, EMIT_TWOHOT = 2, EMIT_IMAGE = 3;
@@ -1469,6 +1477,7 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
 struct MaskArgs {
   const uint8_t* mask;      // [B], device memory
   int32_t noise, track;     // the RewardNoise stream is live / the Logging accumulators are tracked
+  int64_t* episodes_left;   // masked rollouts: [B] episode budgets, counted down at each LAST (nullable)
 };
 
 // Writes lane j's observation `val(e)` (element e of K) with the whole warp: 16-byte streaming stores when `vec`
@@ -1594,6 +1603,116 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(c
         *sub = 0ull;
         if (atomicAdd(a.clock + CLOCK_TOP, 1ull) == (unsigned long long)groups - 1ull) {
           const unsigned long long steps = (unsigned long long)(step0 - a.step0) + 1ull;
+          for (int r = 0; r < CLOCK_GROUPS; ++r) a.clock[16 * r] = steps;
+          a.clock[CLOCK_TOP] = 0ull;
+        }
+      }
+    }
+  }
+}
+
+// bsb_rollout_masked: T masked steps in one launch, laid out as masked_kernel (one chunk of 32 lanes per warp, ragged
+// chunks within one setting, rows through emit_lane_subset) with transition_kernel's T loop.  Lane i is active at step
+// t while mask[i] != 0 and its budget (m.episodes_left, when given) is positive; each LAST of an active step takes one
+// from the budget.  So a lane's active steps are a prefix of the launch: its state, RNG streams, accumulators and
+// budget stay in registers over them, and the calls it sits out all come after its last active one
+// (lane_sit_out_calls, once, after lane_close).  A warp whose lanes are all inactive stops stepping.  Graph-safe mode
+// advances the call count by T; the mask and the budgets are read (and the budgets written) at every launch, so
+// graph replays keep counting the budgets down.  A kernel of its own rather than a T loop in masked_kernel: a shared
+// body (a __device__ function, or a compile-time flag on masked_kernel) changed masked_kernel's register allocation.
+template <class V, int RK>
+__global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_rollout_kernel(const EnvParams p, const LaunchArgs a, const MaskArgs m) {
+  typedef typename V::Fam Fam;
+  typedef typename V::Obs O;
+  typedef typename RngOf<RK>::type R;
+  const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
+  int64_t step0 = a.step0;
+  if (a.clock) step0 += (int64_t)*reinterpret_cast<volatile unsigned long long*>(a.clock + 16 * (blockIdx.x % CLOCK_GROUPS));
+  const MailFields out = {a.reward, a.reward_f64, a.discount, a.step_type};
+  const bool noise = m.noise != 0, track = m.track != 0;
+  const RaggedTable* table = V::kRagged ? reinterpret_cast<const RaggedTable*>(p.pack) : nullptr;
+  const int64_t lanes = V::kRagged ? table->pack.lanes_per_setting : p.batch;      // lanes per setting block
+  const int64_t per_setting = (lanes + 31) / 32;
+  const int64_t n_chunks = (V::kRagged ? table->pack.n_settings : 1) * per_setting;
+  const int64_t chunk = (int64_t)blockIdx.x * warps_per_cta + warp;
+  const int64_t T = a.T;
+
+  if (chunk < n_chunks) {
+    const int64_t k = chunk / per_setting;
+    const int64_t local_base = (chunk - k * per_setting) * 32;         // the chunk's first row within its block
+    const int64_t lane = k * lanes + local_base + tid;
+    const bool in = local_base + tid < lanes;
+    EnvParams lp = p;
+    O* block = reinterpret_cast<O*>(a.obs);
+    if constexpr (V::kRagged) {
+      const RaggedSetting& s = ragged_setting(table, k);
+      ragged_setting_params(lp, s, table->mapping_bits);
+      block += s.obs_offset;
+    } else if constexpr (V::kPacked) {
+      if (in) pack_lane_params(lp, lane);
+    }
+    const int64_t step_elems = V::kRagged ? table->step_elems : p.batch * (int64_t)p.obs_numel;
+    const bool selected = in && m.mask[lane] != 0;
+    int64_t left = selected && m.episodes_left ? m.episodes_left[lane] : 0;
+    bool on = selected && (!m.episodes_left || left > 0);
+    const bool opened = on;
+
+    typename Fam::Lane L;
+    R rng, wrng;
+    EpisodeStats ep;
+    ActionStream action_stream;
+    action_stream.open();
+    Fam::init(p, L);
+    MergedReset<Fam, R> merged;            // same-step kernels only
+    if constexpr (V::kSameStep) { Fam::init(p, merged.last); merged.done = false; }
+    if (on) lane_open<Fam>(lp, lane, L, rng, wrng, ep, a.mode, noise, track);
+    int64_t acted = 0;                     // the lane's active steps
+    for (int64_t t = 0; t < T && __any_sync(0xffffffffu, on); ++t) {
+      const int64_t off = t * p.batch + lane;
+      if (on) {
+        int32_t action;
+        if (a.actions) {
+          action = a.actions[off];
+          if ((uint32_t)action >= (uint32_t)p.num_actions) {
+            if (a.bad_action) *a.bad_action = 1;
+            action = action < 0 ? 0 : p.num_actions - 1;
+          }
+        } else {
+          action = action_stream.sample(a.action_seed, lp.lane_offset + (uint64_t)lane, (uint64_t)(step0 + t), p.num_actions);
+        }
+        if (a.actions_out) a.actions_out[off] = action;
+        if constexpr (V::kSameStep) lane_step<Fam, R, true>(p, lane, L, rng, wrng, ep, action, MODE_STEP, noise, track, step0 + t, out, off, &merged);
+        else lane_step<Fam>(lp, lane, L, rng, wrng, ep, action, MODE_STEP, noise, track, step0 + t, out, off);
+      }
+      if constexpr (V::kSameStep) {
+        if (a.final_obs)
+          emit_lane_subset<Fam>(lp, merged.last, merged.rng, reinterpret_cast<O*>(a.final_obs) + t * p.batch * (int64_t)p.obs_numel,
+                                lp.obs_numel, local_base, on && merged.done, a.final_vec_ok != 0);
+      }
+      emit_lane_subset<Fam>(lp, L, rng, block + t * step_elems, lp.obs_numel, local_base, on, a.obs_vec_ok != 0);
+      if (on) {
+        ++acted;
+        // the step's LAST: a same-step lane's merged reset, else the _reset_next_step flag the step left set
+        const bool last = V::kSameStep ? merged.done : L.nr != 0;
+        if (m.episodes_left && last && --left == 0) on = false;
+      }
+    }
+    if (opened) lane_close<Fam>(lp, lane, L, rng, wrng, ep, noise, track);
+    if (in && track && acted < T) lane_sit_out_calls(p, lane, T - acted);
+    if (selected && m.episodes_left) m.episodes_left[lane] = left;
+  }
+
+  if (a.clock) {        // graph-safe mode: the last CTA advances the call count by T (transition_kernel's epilogue)
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      const unsigned groups = gridDim.x < (unsigned)CLOCK_GROUPS ? gridDim.x : (unsigned)CLOCK_GROUPS;
+      const unsigned g = blockIdx.x % groups;
+      const unsigned members = gridDim.x / groups + (g < gridDim.x % groups ? 1u : 0u);
+      unsigned long long* sub = a.clock + CLOCK_SUB0 + 16 * g;
+      if (atomicAdd(sub, 1ull) == (unsigned long long)members - 1ull) {
+        *sub = 0ull;
+        if (atomicAdd(a.clock + CLOCK_TOP, 1ull) == (unsigned long long)groups - 1ull) {
+          const unsigned long long steps = (unsigned long long)(step0 - a.step0) + (unsigned long long)T;
           for (int r = 0; r < CLOCK_GROUPS; ++r) a.clock[16 * r] = steps;
           a.clock[CLOCK_TOP] = 0ull;
         }

@@ -589,12 +589,33 @@ class BatchedEnvironment:
     _lib.check(self._lib.bsb_invalid_actions(self._handle.ptr, ctypes.byref(seen)))
     return bool(seen.value)
 
-  def rollout(self, num_steps: int, actions=None, action_seed: int = 0, out: Optional[StepBuffers] = None):
+  def rollout(self, num_steps: int, actions=None, action_seed: int = 0, out: Optional[StepBuffers] = None,
+              mask=None, episodes_left=None):
     """`num_steps` fused step() calls; actions [T,B] or None for on-device uniform random actions.
 
     Returns a TimeStep with a leading T axis; when `out.actions` is set it receives the actions used.
-    """
+
+    `mask` (bool or uint8 tensor [B] on the environment's device; needs `out`): a masked rollout
+    (`bsb_rollout_masked`), the same as `num_steps` masked steps.  Lane i steps while its mask is set and, when
+    `episodes_left` (int64 [B] contiguous tensor on the device) is given, while its entry is positive; each LAST
+    it returns takes one from that entry, in place.  The (t, lane) entries of `out` at steps a lane sits out keep what
+    they held.  Every step counts once in `steps_done`."""
     num_steps = int(num_steps)
+    if episodes_left is not None and mask is None:
+      raise ValueError('episodes_left needs mask=: the lanes whose budgets count down')
+    if mask is not None:
+      mask = self._mask(mask, out)
+      if episodes_left is not None:
+        torch = self._torch
+        if not isinstance(episodes_left, torch.Tensor) or episodes_left.dtype is not torch.int64:
+          raise ValueError(f'episodes_left must be an int64 tensor, got '
+                           f'{getattr(episodes_left, "dtype", type(episodes_left).__name__)}')
+        if tuple(episodes_left.shape) != (self._batch,):
+          raise ValueError(f'episodes_left must have shape ({self._batch},), got {tuple(episodes_left.shape)}')
+        if episodes_left.device != self._device:
+          raise ValueError(f'episodes_left must live on {self._device}, got {episodes_left.device}')
+        if not episodes_left.is_contiguous():
+          raise ValueError('episodes_left must be contiguous: it is updated in place')
     out = out or self.make_buffers(num_steps, with_actions=actions is None)
     act_ptr = None
     if actions is not None:
@@ -603,8 +624,14 @@ class BatchedEnvironment:
     outputs = out.bind(self._obs_dtype)
     act_out = ctypes.c_void_p(out.actions.data_ptr()) if out.actions is not None else None
     self._async_work = True
-    _lib.check(self._lib.bsb_rollout(self._handle.ptr, num_steps, act_ptr, int(action_seed) & _MASK64,
-                                     ctypes.byref(outputs), act_out, self._stream()))
+    if mask is not None:
+      left_ptr = ctypes.c_void_p(episodes_left.data_ptr()) if episodes_left is not None else None
+      _lib.check(self._lib.bsb_rollout_masked(self._handle.ptr, num_steps, act_ptr, int(action_seed) & _MASK64,
+                                              ctypes.c_void_p(mask.data_ptr()), left_ptr, ctypes.byref(outputs),
+                                              act_out, self._stream()))
+    else:
+      _lib.check(self._lib.bsb_rollout(self._handle.ptr, num_steps, act_ptr, int(action_seed) & _MASK64,
+                                       ctypes.byref(outputs), act_out, self._stream()))
     return out.timestep()
 
   def capture(self, num_steps: int = 1, sample_actions: bool = False, fused: bool = False,

@@ -5,6 +5,8 @@
     new_timestep)`); lanes reset themselves, so the loop is over steps, not episodes.  The reference loop itself
     runs unchanged on the B = 1 face (`DmEnvAdapter`): it only calls `reset()` / `step()`.
   * `RandomAgent` -- `bsuite/baselines/random/agent.py:26-45` with one generator call per step for the whole batch.
+  * `run_episodes` / `run_random_episodes` -- `experiment.run` to each lane's episode budget, with any agent through
+    masked steps, or with the random agent's actions sampled on the device through fused masked rollouts.
   * `Trajectory` / `collect` -- the `[T + 1]` observations / `[T]` actions, rewards, discounts layout of
     `bsuite/baselines/utils/sequence.py:26-35`, as device tensors with a lane axis, filled by ONE fused rollout
     (`bsb_rollout`: on-device uniform random actions) instead of T appends.
@@ -77,6 +79,20 @@ def run(agent, environment, num_steps: int) -> None:
     timestep = new_timestep
 
 
+def episode_budget(environment, num_episodes: Optional[int] = None):
+  """Every lane's episode budget as an int64 tensor [B] on the environment's device: `num_episodes`, or by default
+  the lane's `bsuite_num_episodes` (per setting on a packed environment)."""
+  torch = environment._torch
+  B, device = environment.batch, environment.device
+  if num_episodes is not None:
+    return torch.full((B,), int(num_episodes), dtype=torch.int64, device=device)
+  if environment.bsuite_ids is not None:
+    lanes = environment.lanes_per_setting
+    per_setting = [spec.bsuite_num_episodes for spec in environment._pack[1]]
+    return torch.tensor(per_setting, dtype=torch.int64).repeat_interleave(lanes).to(device)
+  return torch.full((B,), int(environment.bsuite_num_episodes), dtype=torch.int64, device=device)
+
+
 def run_episodes(agent, environment, num_episodes: Optional[int] = None, check_every: int = 16):
   """`experiment.run` (baselines/experiment.py:24-57) for B lanes: every lane plays exactly its episode budget and
   then stops, as the reference's loop stops after `num_episodes` episodes.
@@ -90,14 +106,7 @@ def run_episodes(agent, environment, num_episodes: Optional[int] = None, check_e
   is still running once every `check_every` calls.  Returns the number of calls made after the first reset."""
   torch = environment._torch
   B, device = environment.batch, environment.device
-  if num_episodes is not None:
-    budget = torch.full((B,), int(num_episodes), dtype=torch.int64, device=device)
-  elif environment.bsuite_ids is not None:
-    lanes = environment.lanes_per_setting
-    per_setting = [spec.bsuite_num_episodes for spec in environment._pack[1]]
-    budget = torch.tensor(per_setting, dtype=torch.int64).repeat_interleave(lanes).to(device)
-  else:
-    budget = torch.full((B,), int(environment.bsuite_num_episodes), dtype=torch.int64, device=device)
+  budget = episode_budget(environment, num_episodes)
   finished = torch.zeros(B, dtype=torch.int64, device=device)
   active = budget > 0
   out = environment.make_buffers()
@@ -120,6 +129,31 @@ def run_episodes(agent, environment, num_episodes: Optional[int] = None, check_e
     finished += ((new_timestep.step_type == 2) & active).to(torch.int64)
     active = finished < budget
     timestep = new_timestep
+
+
+def run_random_episodes(environment, num_episodes: Optional[int] = None, action_seed: int = 0,
+                        steps_per_launch: int = 64):
+  """`run_episodes` for the reference's random agent (baselines/random/agent.py:35-37) with the actions sampled on
+  the device: every lane plays exactly its episode budget (`episode_budget`) in fused masked rollouts
+  (`rollout(..., mask=..., episodes_left=...)`), `steps_per_launch` calls per launch.
+
+  One masked reset of the lanes with a positive budget, then rollouts until no lane has episodes left; the host
+  syncs once per launch to ask.  Per lane, `bsuite_info()`, episode statistics, log rows and scores equal those of
+  `run_episodes` with an agent whose actions are `environment.random_actions(1, action_seed,
+  first_step=environment.steps_done)`; only `steps_done` may differ.  Returns the number of calls made after the
+  reset."""
+  T = int(steps_per_launch)
+  if T <= 0:
+    raise ValueError(f'steps_per_launch must be positive, got {steps_per_launch}')
+  left = episode_budget(environment, num_episodes)
+  mask = left > 0
+  environment.reset(out=environment.make_buffers(), mask=mask)
+  out = environment.make_buffers(T)
+  calls = 0
+  while bool((left > 0).any()):
+    environment.rollout(T, action_seed=action_seed, out=out, mask=mask, episodes_left=left)
+    calls += T
+  return calls
 
 
 class Replay:

@@ -37,7 +37,7 @@
 extern "C" {
 #endif
 
-#define BSB_ABI_VERSION 14
+#define BSB_ABI_VERSION 15
 #define BSB_DEVICE_HOST (-1)
 #define BSB_MAX_INFO 4
 #define BSB_MAX_PACKED_SETTINGS 64 /* bsb_create_packed: settings per handle */
@@ -360,6 +360,35 @@ int32_t bsb_rollout(bsb_env* env, int64_t num_steps, const int32_t* actions,
                     uint64_t action_seed, const bsb_outputs* out,
                     int32_t* actions_out, void* stream);
 
+/*
+ * Masked rollout: T masked steps fused in one launch, each lane stopping at
+ * its own episode budget.  num_steps, actions (int32 [T,B] or NULL to sample
+ * as bsb_rollout does at global step steps_done + t), action_seed, out
+ * (leading T axis; final_observation on same-step handles) and actions_out
+ * mean what they mean for bsb_rollout.  mask (uint8 [B], required) and
+ * episodes_left (int64 [B], nullable) live in the handle's memory space.
+ * Lane i is active at step t when mask[i] != 0 and episodes_left is NULL or
+ * its budget left_i(t) > 0, where left_i(0) = episodes_left[i] and each LAST
+ * timestep of an active step (a same-step handle's merged LAST included)
+ * takes one from it; episodes_left[i] receives left_i(T).  A lane's active
+ * steps are therefore a prefix of the T.  The call equals, bit for bit, T
+ * calls of bsb_step_masked with mask_t[i] = active(i, t): every output entry
+ * written, actions_out, lane state, RNG streams, info fields, Logging
+ * columns, log rows, bsb_steps_done (+T) and the invalid-action flag.  The
+ * (lane, t) entries of inactive steps -- in every output and in actions_out
+ * -- are not written, and their actions are never read.  A host handle
+ * refuses (BSB_INVALID_ARGUMENT, before anything moves) an out-of-range
+ * action of any lane whose mask is set at ANY of the T steps, including
+ * steps after its budget would have stopped it.  Works in graph-safe mode
+ * and may be captured: a replay reads mask and episodes_left as they are
+ * then and writes episodes_left back, so replays keep counting budgets down.
+ */
+int32_t bsb_rollout_masked(bsb_env* env, int64_t num_steps,
+                           const int32_t* actions, uint64_t action_seed,
+                           const uint8_t* mask, int64_t* episodes_left,
+                           const bsb_outputs* out, int32_t* actions_out,
+                           void* stream);
+
 /* Host mirror of the on-device action sampler: out int32 [T,B] (host). */
 int32_t bsb_random_actions(uint64_t action_seed, uint64_t lane_offset,
                            int64_t batch, int64_t first_step, int64_t num_steps,
@@ -390,7 +419,8 @@ int32_t bsb_read_episode_stats(bsb_env* env, int32_t field, double* dst,
                                void* stream);
 
 /*
- * CUDA graphs.  bsb_step / bsb_reset / bsb_rollout / bsb_read_* / bsb_sum_episode_stats may be called on a stream
+ * CUDA graphs.  bsb_step / bsb_reset / bsb_rollout / the masked calls (bsb_reset_masked / bsb_step_masked /
+ * bsb_rollout_masked) / bsb_read_* / bsb_sum_episode_stats may be called on a stream
  * that is being captured.  A graph freezes launch arguments, so the first captured launch moves the handle's step
  * counter (it indexes the on-device action stream and the Logging columns) and its chunk scheduler into device
  * memory, for good: replays and eager calls can then be mixed in any order, and bsb_steps_done / bsb_get_state

@@ -145,6 +145,27 @@ for bsuite_id, batch, kw in (('deep_sea/11', 1001, {}), ('catch/0', 997, dict(au
     env.close()
   assert all(torch.equal(a, b) for a, b in zip(*got))
   print(bsuite_id, batch, 'masked calls == host path: True', flush=True)
+# Masked rollouts (masked_rollout_kernel): the same workloads as T steps per launch, lanes stopping at their own
+# budgets mid-launch, sampled actions written to actions_out, against the host path.
+for bsuite_id, batch, kw in (('deep_sea/11', 1001, {}), ('catch/0', 997, dict(autoreset='same_step')),
+                             ('umbrella_distract/3', 501, {}), ('mnist/0', 333, dict(obs_dtype='bfloat16'))):
+  gen = torch.Generator().manual_seed(4)
+  mask = torch.rand(batch, generator=gen) < 0.7
+  budgets = torch.randint(0, 3, (batch,), generator=gen, dtype=torch.int64)
+  got = []
+  for device in ('cuda', 'cpu'):
+    env = bsuite_b200.load_from_id(bsuite_id, batch=batch, device=device, seed=3, track_episodes=True, **kw)
+    out = env.make_buffers(12, with_actions=True, final_observation='autoreset' in kw)
+    for buf in (out.observation, out.reward, out.discount, out.step_type, out.actions):
+      buf.fill_(5)                           # entries of steps a lane sits out are never written
+    left = budgets.clone().to(device)
+    for _ in range(3):
+      env.rollout(12, action_seed=1, out=out, mask=mask.to(device), episodes_left=left)
+    got.append([out.observation.cpu(), out.reward.cpu(), out.actions.cpu(), left.cpu()] +
+               [v.cpu() for v in env.episode_stats().values()])      # per lane: sums over lanes may round differently
+    env.close()
+  assert all(torch.equal(a, b) for a, b in zip(*got))
+  print(bsuite_id, batch, 'masked rollouts == host path: True', flush=True)
 # One-launch reduction over several environments and a whole lock-step in one graph.
 from bsuite_b200 import suite
 ids = ['catch/0', 'deep_sea/0', 'bandit_noise/0', 'cartpole/0', 'mnist/0', 'umbrella_length/0']
