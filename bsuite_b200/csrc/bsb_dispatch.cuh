@@ -122,11 +122,24 @@ void host_run(const EnvParams& p, const LaunchArgs& a, const uint8_t* mask = nul
 // Launch geometry, shared by the launchers of both kernels.
 struct Geometry { int threads = 0; size_t smem = 0; int64_t n_chunks = 0, grid = 0; int extra_blocks = 0; };
 
+// The chunks of `cl` lanes a launch deals: a ragged pack's setting k owns ceil(L / cl) of them, so no chunk straddles
+// two settings; every other handle is one block of B lanes.
+inline int64_t launch_chunks(const bsb_env* e, bool ragged, int cl) {
+  const int64_t lanes = ragged ? e->lanes_per_setting : e->p.batch;
+  return (ragged ? (int64_t)e->n_settings : 1) * ((lanes + cl - 1) / cl);
+}
+
 // Chunk lanes, emitter plan (group lanes, stage rows), CTA size, shared memory and grid of a launch; fills a's
 // emitter fields and, for a persistent grid (the deep_sea and mnist bulk paths, once the grid exceeds what is
 // resident), its chunk counter.  `extra_threads` > 0 (the copiers of two-phase host steps) puts g.extra_blocks
 // blocks of that many threads in all (at least one) in front of the chunk owners.
-template <class F, class O>
+// kRagged (float32 observations, the settings' shapes in e->obs_rows / obs_cols, their deep_sea group sizes in
+// e->group_lanes): the same rules with the chunks of ragged_chunks.  Row stages are sized for the largest K.  deep_sea
+// tiles keep the grouped bulk store and its persistent grid, each setting with its own group size; the stage holds two
+// of the largest group (a.group_lanes * p.obs_numel elements each, p.obs_numel being the largest K).  On compressible
+// memory, where a batch of the same size would turn to compare-then-store or streaming stores, every chunk uses the
+// streaming stores.
+template <class F, class O, bool kRagged = false>
 int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int extra_threads = 0) {
   const int K = e->p.obs_numel;
   const bool is_onehot = EmitKind<F>::value == EMIT_ONEHOT;
@@ -154,7 +167,7 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int extra_threads = 0) {
   if (is_image)
     while (chunk > 8 && (B + chunk - 1) / chunk < 4 * (int64_t)e->num_sms) chunk >>= 1;
   a.chunk_lanes = chunk;
-  g.n_chunks = (B + chunk - 1) / chunk;
+  g.n_chunks = launch_chunks(e, kRagged, chunk);
   int threads = 64;         // one chunk per warp: small CTAs spread evenly over the SMs (transition_kernel)
   bool persistent = false;
   const size_t tile = (size_t)K * elem;
@@ -167,16 +180,21 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int extra_threads = 0) {
   a.emit_reuse = 0;
   if (is_onehot && a.emit_bulk && g.n_chunks >= 4 * (int64_t)e->num_sms && in_compressed_block(a.obs)) {
     a.emit_bulk = 0;
-    a.emit_reuse = a.T == 1 ? 1 : 0;
+    a.emit_reuse = a.T == 1 && !kRagged ? 1 : 0;
   }
   if (is_onehot && a.emit_bulk) {
-    // Lanes per bulk store: the largest power of two <= 16 with one store <= 40 KB, so a group never spans a
-    // 32-lane chunk.  N = 32 -> 8 lanes (32 KB stores; 88.8 us per headline step against 91.9 with 4 lanes, DESIGN.md
-    // §3), N = 50 -> 4 lanes (40 KB).  Narrow tiles reach the 16-lane cap first: N = 32 in bfloat16 -> 16 lanes
-    // (32 KB), in uint8 -> 16 lanes (16 KB).
-    int m = 1;
-    while (m < 16 && (size_t)(2 * m) * tile <= 40 * 1024) m <<= 1;
-    if (((size_t)m * tile) % 16 != 0 || (size_t)TILE_STAGES * m * tile > 100 * 1024) {
+    int m;                                  // lanes per bulk store
+    if constexpr (kRagged) {
+      int64_t largest = 0;
+      for (int32_t k = 0; k < e->n_settings; ++k) {
+        const int64_t elems = (int64_t)e->group_lanes[k] * e->obs_rows[k] * e->obs_cols[k];
+        largest = elems > largest ? elems : largest;
+      }
+      m = (int)((largest + K - 1) / K);
+    } else {
+      m = tile_group_lanes(tile);
+    }
+    if (m == 0) {
       a.emit_bulk = 0;                      // tiles too large (or misaligned) for the staged path: vector stores
     } else {
       a.group_lanes = m; threads = 32; persistent = true;
@@ -233,65 +251,6 @@ int plan_launch(bsb_env* e, LaunchArgs& a, Geometry& g, int extra_threads = 0) {
   return BSB_OK;
 }
 
-// The plan of a ragged pack's launch (float32 observations, the settings' shapes in e->obs_rows / obs_cols, their
-// deep_sea group sizes in e->group_lanes): plan_launch's rules with the chunk count of ragged_chunks.  Row stages are
-// sized for the largest K.  deep_sea tiles keep the grouped bulk store and its persistent grid, each setting with its
-// own group size; the stage holds two of the largest group (a.group_lanes * p.obs_numel elements each, p.obs_numel
-// being the largest K).  On compressible memory, where plan_launch would turn a batch of the same size to
-// compare-then-store or streaming stores, every chunk uses the streaming stores.
-template <class F>
-int plan_ragged_launch(bsb_env* e, LaunchArgs& a, Geometry& g) {
-  const int64_t K = e->p.obs_numel;
-  const bool is_onehot = EmitKind<F>::value == EMIT_ONEHOT;
-  a.emit_bulk = 1;
-  a.emit_reuse = 0;
-  a.group_lanes = 1;
-  a.work_counter = nullptr;
-  a.work_base = 0;
-  a.stage_rows = ((size_t)2 * 32 * (size_t)K * sizeof(float) <= 14 * 1024) ? 2 : 1;
-  if (a.T == 1 && EmitKind<F>::value == EMIT_ROWS) a.stage_rows = 1;
-  a.cta_extra_elems = 0;
-  a.bad_action = e->bad_action_dev;
-  a.chunk_lanes = 32;
-  g.n_chunks = (int64_t)e->n_settings * ((e->lanes_per_setting + 31) / 32);
-  int threads = 64;
-  bool persistent = false;
-  if (is_onehot && g.n_chunks >= 4 * (int64_t)e->num_sms && in_compressed_block(a.obs)) a.emit_bulk = 0;
-  if (is_onehot && a.emit_bulk) {
-    int64_t largest = 0;
-    for (int32_t k = 0; k < e->n_settings; ++k) {
-      const int64_t elems = (int64_t)e->group_lanes[k] * e->obs_rows[k] * e->obs_cols[k];
-      largest = elems > largest ? elems : largest;
-    }
-    if (largest == 0) {
-      a.emit_bulk = 0;
-    } else {
-      a.group_lanes = (int)((largest + K - 1) / K); threads = 32; persistent = true;
-    }
-  }
-  a.use_pdl = (a.mode == MODE_STEP && a.T == 1) ? 1 : 0;
-  size_t per_warp = smem_elems_per_warp<F, float>((int)K, a.emit_bulk != 0, false, a.group_lanes, a.stage_rows) * sizeof(float);
-  if (EmitKind<F>::value == EMIT_ROWS && per_warp > 96 * 1024) { a.emit_bulk = 0; a.stage_rows = 0; per_warp = 0; }
-  size_t smem = per_warp * (size_t)(threads / 32);
-  while (smem > 96 * 1024 && threads > 32) { threads >>= 1; smem = per_warp * (size_t)(threads / 32); }
-  if (smem > 200 * 1024) return fail(BSB_UNSUPPORTED, "observation too large for the staged emitter");
-  g.threads = threads;
-  g.smem = smem;
-  g.extra_blocks = 0;
-  g.grid = (g.n_chunks + threads / 32 - 1) / (threads / 32);
-  if (persistent) {
-    int64_t per_sm = (int64_t)((227 * 1024) / (smem + 1024));
-    per_sm = per_sm < 1 ? 1 : (per_sm > 16 ? 16 : per_sm);
-    const int64_t resident = (int64_t)e->num_sms * per_sm;
-    if (g.grid > resident) {
-      g.grid = resident;
-      a.work_counter = a.clock ? a.clock + CLOCK_CHUNK : e->work_counter;
-      a.work_base = a.clock ? 0ull : e->work_base;
-    }
-  }
-  return BSB_OK;
-}
-
 template <class Kernel, class... Args>
 int launch(bsb_env* e, const LaunchArgs& a, const Geometry& g, cudaStream_t stream, Kernel kernel, const Args&... args) {
   if (g.smem > 48 * 1024) BSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
@@ -337,6 +296,15 @@ int with_flags(const bsb_env* e, const LaunchArgs& a, Launch launch) {
   return track ? launch(std::false_type(), std::true_type()) : launch(std::false_type(), std::false_type());
 }
 
+// The host path of variant V with the handle's bit source (unmasked calls: no mask, no budgets).
+template <class V>
+void run_host(const bsb_env* e, const LaunchArgs& a, const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr) {
+  if constexpr (Compiled<V>::kMt) {
+    if (e->p.rng_kind == BSB_RNG_MT19937) return host_run<V, 1>(e->p, a, mask, episodes_left);
+  }
+  host_run<V, 0>(e->p, a, mask, episodes_left);
+}
+
 // Kernels and host path of variant V, the runner bsb_create stores in the handle.  The bit sources and kernels are
 // those the variant list (BSB_VARIANTS) compiles for V: bsb_create picks no runner for an MT19937 handle whose variant
 // lacks MT19937, and only a variant with two_phase_host_kernel is given `two_phase` (a two-phase host step).
@@ -344,11 +312,7 @@ template <class V>
 int run_variant(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoPhaseArgs* two_phase) {
   constexpr bool kMt = Compiled<V>::kMt;
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
-  if (e->device < 0) {
-    if constexpr (kMt) { if (mt) { host_run<V, 1>(e->p, a); return BSB_OK; } }
-    host_run<V, 0>(e->p, a);
-    return BSB_OK;
-  }
+  if (e->device < 0) { run_host<V>(e, a); return BSB_OK; }
   return with_flags(e, a, [&](auto noise, auto track) {
     constexpr bool kNoise = decltype(noise)::value, kTrack = decltype(track)::value;
     if constexpr (Compiled<V>::kTwoPhase) {
@@ -357,19 +321,13 @@ int run_variant(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoP
         return two_phase_launch<V, 0, kNoise, kTrack>(e, a, *two_phase, stream);
       }
     }
-    LaunchArgs la = a;
-    Geometry g;
-    if constexpr (V::kRagged) {
+    if constexpr (V::kRagged && kNoise) {
       // ragged packs take no reward wrapper (bsb_create_ragged): Logging off / on are their only kernels
-      if constexpr (kNoise) {
-        return fail(BSB_INTERNAL, "a ragged pack reached the RewardNoise kernel");
-      } else {
-        const int rc = plan_ragged_launch<typename V::Fam>(e, la, g);
-        if (rc != BSB_OK) return rc;
-        return launch(e, la, g, stream, transition_kernel<V, 0, false, kTrack>, e->p, la);
-      }
+      return fail(BSB_INTERNAL, "a ragged pack reached the RewardNoise kernel");
     } else {
-      const int rc = plan_launch<typename V::Fam, typename V::Obs>(e, la, g);
+      LaunchArgs la = a;
+      Geometry g;
+      const int rc = plan_launch<typename V::Fam, typename V::Obs, V::kRagged>(e, la, g);
       if (rc != BSB_OK) return rc;
       if constexpr (kMt) { if (mt) return launch(e, la, g, stream, transition_kernel<V, 1, kNoise, kTrack>, e->p, la); }
       return launch(e, la, g, stream, transition_kernel<V, 0, kNoise, kTrack>, e->p, la);
@@ -384,11 +342,7 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
                cudaStream_t stream) {
   constexpr bool kMt = Compiled<V>::kMt;
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
-  if (e->device < 0) {
-    if constexpr (kMt) { if (mt) { host_run<V, 1>(e->p, a, mask, episodes_left); return BSB_OK; } }
-    host_run<V, 0>(e->p, a, mask, episodes_left);
-    return BSB_OK;
-  }
+  if (e->device < 0) { run_host<V>(e, a, mask, episodes_left); return BSB_OK; }
   MaskArgs m;
   m.mask = mask;
   m.noise = e->p.wrapper == BSB_WRAP_REWARD_NOISE ? 1 : 0;
@@ -401,7 +355,7 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
   Geometry g;
   g.threads = 64;
   g.smem = 0;
-  g.n_chunks = V::kRagged ? (int64_t)e->n_settings * ((e->lanes_per_setting + 31) / 32) : (e->p.batch + 31) / 32;
+  g.n_chunks = launch_chunks(e, V::kRagged, 32);
   g.grid = (g.n_chunks + g.threads / 32 - 1) / (g.threads / 32);
   if (rollout) {
     if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_rollout_kernel<V, 1>, e->p, la, m); }

@@ -610,12 +610,7 @@ static int32_t create_env(const bsb_config* config, int64_t batch, int32_t devic
       if (c.family == BSB_DEEP_SEA) { s[k].inv_size = 1.0 / (double)ck.size; s[k].move_cost_step = ck.unscaled_move_cost / (double)ck.size; }
       s[k].num_bits = ck.num_bits; s[k].n_distractor = ck.n_distractor; s[k].obs_numel = K;
       s[k].memory_length = ck.memory_length; s[k].chain_length = ck.chain_length;
-      // deep_sea: lanes per bulk store by plan_launch's rule (the largest power of two <= 16 whose store is <= 40 KB),
-      // or 0 where that store is not a whole number of 16-byte words or two groups exceed 100 KB
-      int32_t m = 1;
-      const size_t tile = (size_t)K * sizeof(float);
-      while (m < 16 && (size_t)(2 * m) * tile <= 40 * 1024) m <<= 1;
-      s[k].group_lanes = (((size_t)m * tile) % 16 != 0 || (size_t)TILE_STAGES * m * tile > 100 * 1024) ? 0 : m;
+      s[k].group_lanes = tile_group_lanes((size_t)K * sizeof(float));      // deep_sea: lanes per bulk store
       e->group_lanes.push_back(c.family == BSB_DEEP_SEA ? s[k].group_lanes : 0);
     }
     void* d = nullptr;

@@ -397,6 +397,17 @@ size_t smem_elems_per_warp(int K, bool emit_bulk, bool emit_reuse, int group_lan
   return 0;
 }
 
+// deep_sea bulk path: lanes per bulk store of tiles of `tile` bytes, the largest power of two <= 16 with one store
+// <= 40 KB, so a group never spans a 32-lane chunk.  N = 32 -> 8 lanes (32 KB stores; 88.8 us per headline step
+// against 91.9 with 4 lanes, DESIGN.md §3), N = 50 -> 4 lanes (40 KB).  Narrow tiles reach the 16-lane cap first:
+// N = 32 in bfloat16 -> 16 lanes (32 KB), in uint8 -> 16 lanes (16 KB).  0: no bulk path, the store is not a whole
+// number of 16-byte words or the two staged groups exceed 100 KB.
+inline int tile_group_lanes(size_t tile) {
+  int m = 1;
+  while (m < 16 && (size_t)(2 * m) * tile <= 40 * 1024) m <<= 1;
+  return (((size_t)m * tile) % 16 != 0 || (size_t)TILE_STAGES * m * tile > 100 * 1024) ? 0 : m;
+}
+
 #if defined(__CUDACC__)
 
 __device__ __forceinline__ void st_stream(float4* dst, float4 v) { __stcs(dst, v); }
