@@ -335,11 +335,11 @@ int run_variant(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoP
   });
 }
 
-// Masked calls of variant V (bsb_reset_masked / bsb_step_masked, and bsb_rollout_masked when `rollout`): the host
-// path, or one launch of masked_kernel / masked_rollout_kernel with one chunk of 32 lanes per warp.
+// Masked calls of variant V (bsb_reset_masked / bsb_step_masked / bsb_rollout_masked): the host path, or one launch of
+// masked_kernel with one chunk of 32 lanes per warp.  A call with nothing for the T loop, the action stream or the
+// budgets to do (every masked reset and step) takes the kOneCall instantiation.
 template <class V>
-int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* episodes_left, bool rollout,
-               cudaStream_t stream) {
+int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* episodes_left, cudaStream_t stream) {
   constexpr bool kMt = Compiled<V>::kMt;
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
   if (e->device < 0) { run_host<V>(e, a, mask, episodes_left); return BSB_OK; }
@@ -357,12 +357,13 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
   g.smem = 0;
   g.n_chunks = launch_chunks(e, V::kRagged, 32);
   g.grid = (g.n_chunks + g.threads / 32 - 1) / (g.threads / 32);
-  if (rollout) {
-    if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_rollout_kernel<V, 1>, e->p, la, m); }
-    return launch(e, la, g, stream, masked_rollout_kernel<V, 0>, e->p, la, m);
-  }
-  if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_kernel<V, 1>, e->p, la, m); }
-  return launch(e, la, g, stream, masked_kernel<V, 0>, e->p, la, m);
+  const bool one_call = a.T == 1 && !episodes_left && !a.actions_out && (a.mode != MODE_STEP || a.actions);
+  auto go = [&](auto one) {
+    constexpr bool kOneCall = decltype(one)::value;
+    if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_kernel<V, 1, kOneCall>, e->p, la, m); }
+    return launch(e, la, g, stream, masked_kernel<V, 0, kOneCall>, e->p, la, m);
+  };
+  return one_call ? go(std::true_type()) : go(std::false_type());
 }
 
 }  // namespace bsb

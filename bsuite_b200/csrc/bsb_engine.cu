@@ -83,10 +83,10 @@ template <class T> int env_alloc_t(bsb_env* e, T** out, size_t count, bool snaps
   return rc;
 }
 
-// `two_phase`: a two-phase host step (mailbox_launch; deep_sea and catch only).  `mask`: a masked call, or with
-// `rollout` a masked rollout (`episodes_left`: its budgets, nullable).
+// `two_phase`: a two-phase host step (mailbox_launch; deep_sea and catch only).  `mask`: a masked call or rollout
+// (`episodes_left`: a rollout's budgets, nullable).
 int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr,
-        const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr, bool rollout = false) {
+        const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr) {
   DeviceGuard guard(e->device);
   LaunchArgs a = args;
   if (e->device >= 0) {
@@ -95,7 +95,7 @@ int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseA
     if (capture != cudaStreamCaptureStatusNone) e->graph_safe = true;
     if (e->graph_safe) a.clock = e->clock;      // a.step0 == e->steps_done, which no longer moves
   }
-  if (mask) return e->variant->run_masked(e, a, mask, episodes_left, rollout, stream);
+  if (mask) return e->variant->run_masked(e, a, mask, episodes_left, stream);
   return e->variant->run(e, a, stream, two_phase);
 }
 
@@ -848,7 +848,7 @@ static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask
   }
   LaunchArgs a = make_args(env, out, mode == MODE_STEP ? actions : nullptr, T, mode);
   a.action_seed = action_seed; a.actions_out = actions_out;
-  int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask, episodes_left, rollout);
+  int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask, episodes_left);
   if (rc == BSB_OK) advance_steps(env, T);
   return rc;
 }

@@ -26,16 +26,15 @@ int drain_log_rows(bsb_env* e);                         // waits out host steps 
 // Kernels and host path of kernel variant V (bsb_dispatch.cuh), explicitly instantiated for each entry of the variant
 // list (BSB_VARIANTS) in the translation unit the list gives it (bsb_variants.cu).  `two_phase`: a two-phase host step.
 template <class V> int run_variant(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs* two_phase);
-// Masked calls of variant V (bsb_reset_masked / bsb_step_masked; bsb_rollout_masked when `rollout`): `mask` [B] and
-// `episodes_left` [B] (nullable) live where the handle's state does.
-template <class V> int run_masked(bsb_env*, const LaunchArgs&, const uint8_t* mask, int64_t* episodes_left, bool rollout,
-                                  cudaStream_t);
+// Masked calls of variant V (bsb_reset_masked / bsb_step_masked / bsb_rollout_masked): `mask` [B] and `episodes_left`
+// [B] (nullable) live where the handle's state does.
+template <class V> int run_masked(bsb_env*, const LaunchArgs&, const uint8_t* mask, int64_t* episodes_left, cudaStream_t);
 // An entry of the variant list, as bsb_create looks it up (bsb_engine.cu).
 struct VariantEntry {
   int family, obs_dtype, mode;
   bool mt, two_phase;
   int (*run)(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs*);
-  int (*run_masked)(bsb_env*, const LaunchArgs&, const uint8_t*, int64_t*, bool, cudaStream_t);
+  int (*run_masked)(bsb_env*, const LaunchArgs&, const uint8_t*, int64_t*, cudaStream_t);
 };
 
 #define BSB_CUDA(expr)                                                                   \

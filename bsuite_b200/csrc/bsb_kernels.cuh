@@ -343,22 +343,16 @@ BSB_HD void lane_step(const EnvParams& p, int64_t lane, typename F::Lane& L, R& 
   }
 }
 
-// A lane that sits out a masked call (bsb_step_masked / bsb_reset_masked) makes no call, but the handle's call count
-// still advances, and episode_stat / log_row_write read the lane's Logging columns from that global count.  So the
-// lane's own counters move instead: first_count and start_call each gain the skipped call, and steps = calls -
-// first_count and episode_len = calls - 1 - start_call keep the values of the lane's own call sequence.  Before the
-// lane's first call (first_count == 0 means "no episode yet" to episode_len) the first skip sets first_count to 1 and
-// leaves start_call at 0: after d skips first_count = d and start_call = d - 1, which read steps = episode_len = 0, and
-// the lane's first call overwrites start_call (it follows the constructor's _reset_next_step, as after a LAST).  The
-// same-step marker ep[5] waits for the lane's next call and is left alone.
-BSB_HD void lane_sit_out(const EnvParams& p, int64_t lane) {
-  double* first_count = p.ep + 3 * p.batch + lane;
-  double* start_call = p.ep + 4 * p.batch + lane;
-  if (*first_count != 0.0) *start_call += 1.0;
-  *first_count += 1.0;
-}
-// d >= 1 consecutive calls of lane_sit_out at once (masked rollouts: a lane's sit-outs all follow its last active
-// call): first_count gains d, start_call d, or d - 1 when the first of them met first_count == 0.
+// A lane that sits out a masked call (bsb_step_masked / bsb_reset_masked, or a step of bsb_rollout_masked) makes no
+// call, but the handle's call count still advances, and episode_stat / log_row_write read the lane's Logging columns
+// from that global count.  So the lane's own counters move instead: first_count and start_call each gain the skipped
+// call, and steps = calls - first_count and episode_len = calls - 1 - start_call keep the values of the lane's own call
+// sequence.  Before the lane's first call (first_count == 0 means "no episode yet" to episode_len) the first skip sets
+// first_count to 1 and leaves start_call at 0: after d skips first_count = d and start_call = d - 1, which read steps =
+// episode_len = 0, and the lane's first call overwrites start_call (it follows the constructor's _reset_next_step, as
+// after a LAST).  The same-step marker ep[5] waits for the lane's next call and is left alone.
+// d >= 1 consecutive sit-outs at once (a masked rollout's sit-outs all follow the lane's last active call):
+// first_count gains d, start_call d, or d - 1 when the first of them met first_count == 0.
 BSB_HD void lane_sit_out_calls(const EnvParams& p, int64_t lane, int64_t d) {
   double* first_count = p.ep + 3 * p.batch + lane;
   double* start_call = p.ep + 4 * p.batch + lane;
@@ -1482,9 +1476,9 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
 
 // ----- masked calls -----------------------------------------------------------------------------------------------
 // bsb_step_masked / bsb_reset_masked: one call in which lane i acts only where mask[i] != 0.  An active lane makes the
-// call an unmasked reset / step would make; an inactive lane makes none (lane_sit_out) and none of its output entries
-// is written.  Noise and Logging are runtime flags here (lane_open / lane_step take them as arguments), so each
-// variant compiles one masked kernel per bit source.
+// call an unmasked reset / step would make; an inactive lane makes none (lane_sit_out_calls) and none of its output
+// entries is written.  Noise and Logging are runtime flags here (lane_open / lane_step take them as arguments), so
+// each variant compiles one masked kernel per bit source.
 struct MaskArgs {
   const uint8_t* mask;      // [B], device memory
   int32_t noise, track;     // the RewardNoise stream is live / the Logging accumulators are tracked
@@ -1537,11 +1531,18 @@ __device__ __forceinline__ void emit_lane_subset(const EnvParams& lp, const type
   }
 }
 
-// One masked call, T = 1.  One chunk of 32 lanes per warp; a ragged pack's chunks never straddle two settings (as in
-// ragged_chunks), and row j of setting k goes to the setting's block.  Graph-safe mode reads the call index from the
-// device clock and advances it by one, as transition_kernel does; the mask is read on every launch, so a graph
-// replays with whatever the mask buffer holds.
-template <class V, int RK>
+// Every masked call: a masked reset or step (T = 1, no budgets) or bsb_rollout_masked's T masked steps, in one launch.
+// One chunk of 32 lanes per warp; a ragged pack's chunks never straddle two settings, and row j of setting k goes to
+// the setting's block (emit_lane_subset).  Lane i is active at step t while mask[i] != 0 and its budget
+// (m.episodes_left, when given) is positive; each LAST of an active step takes one from the budget.  So a lane's
+// active steps are a prefix of the launch: its state, RNG streams, accumulators and budget stay in registers over
+// them, and the calls it sits out all come after its last active one (lane_sit_out_calls, once, after lane_close).  A
+// warp whose lanes are all inactive stops stepping.  Graph-safe mode reads the call index from the device clock and
+// advances it by T, as transition_kernel does; the mask and the budgets are read (and the budgets written) at every
+// launch, so a graph replays with whatever the mask buffer holds and keeps counting the budgets down.  kOneCall: a
+// masked reset or step (T = 1, the caller's actions, no budgets, no actions_out), for which the T loop, the action
+// stream and the budget compile out; with them live, masked steps of catch and cartpole took 11-21 % longer.
+template <class V, int RK, bool kOneCall>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(const EnvParams p, const LaunchArgs a, const MaskArgs m) {
   typedef typename V::Fam Fam;
   typedef typename V::Obs O;
@@ -1556,97 +1557,8 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(c
   const int64_t per_setting = (lanes + 31) / 32;
   const int64_t n_chunks = (V::kRagged ? table->pack.n_settings : 1) * per_setting;
   const int64_t chunk = (int64_t)blockIdx.x * warps_per_cta + warp;
-
-  if (chunk < n_chunks) {
-    const int64_t k = chunk / per_setting;
-    const int64_t local_base = (chunk - k * per_setting) * 32;         // the chunk's first row within its block
-    const int64_t lane = k * lanes + local_base + tid;
-    const bool in = local_base + tid < lanes;
-    EnvParams lp = p;
-    O* block = reinterpret_cast<O*>(a.obs);
-    if constexpr (V::kRagged) {
-      const RaggedSetting& s = ragged_setting(table, k);
-      ragged_setting_params(lp, s, table->mapping_bits);
-      block += s.obs_offset;
-    } else if constexpr (V::kPacked) {
-      if (in) pack_lane_params(lp, lane);
-    }
-    const bool on = in && m.mask[lane] != 0;
-
-    typename Fam::Lane L;
-    R rng, wrng;
-    EpisodeStats ep;
-    Fam::init(p, L);
-    MergedReset<Fam, R> merged;            // same-step kernels only
-    if constexpr (V::kSameStep) { Fam::init(p, merged.last); merged.done = false; }
-    if (on) {
-      lane_open<Fam>(lp, lane, L, rng, wrng, ep, a.mode, noise, track);
-      int32_t action = 0;
-      if (a.mode == MODE_STEP) {
-        action = a.actions[lane];
-        if ((uint32_t)action >= (uint32_t)p.num_actions) {
-          if (a.bad_action) *a.bad_action = 1;
-          action = action < 0 ? 0 : p.num_actions - 1;
-        }
-      }
-      if constexpr (V::kSameStep) lane_step<Fam, R, true>(p, lane, L, rng, wrng, ep, action, a.mode, noise, track, step0, out, lane, &merged);
-      else lane_step<Fam>(lp, lane, L, rng, wrng, ep, action, a.mode, noise, track, step0, out, lane);
-    } else if (in && track) {
-      lane_sit_out(p, lane);
-    }
-    if constexpr (V::kSameStep) {
-      if (a.final_obs)
-        emit_lane_subset<Fam>(lp, merged.last, merged.rng, reinterpret_cast<O*>(a.final_obs), lp.obs_numel, local_base,
-                              on && merged.done, a.final_vec_ok != 0);
-    }
-    emit_lane_subset<Fam>(lp, L, rng, block, lp.obs_numel, local_base, on, a.obs_vec_ok != 0);
-    if (on) lane_close<Fam>(lp, lane, L, rng, wrng, ep, noise, track);
-  }
-
-  if (a.clock) {        // graph-safe mode: the last CTA advances the call count by one (transition_kernel's epilogue)
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      const unsigned groups = gridDim.x < (unsigned)CLOCK_GROUPS ? gridDim.x : (unsigned)CLOCK_GROUPS;
-      const unsigned g = blockIdx.x % groups;
-      const unsigned members = gridDim.x / groups + (g < gridDim.x % groups ? 1u : 0u);
-      unsigned long long* sub = a.clock + CLOCK_SUB0 + 16 * g;
-      if (atomicAdd(sub, 1ull) == (unsigned long long)members - 1ull) {
-        *sub = 0ull;
-        if (atomicAdd(a.clock + CLOCK_TOP, 1ull) == (unsigned long long)groups - 1ull) {
-          const unsigned long long steps = (unsigned long long)(step0 - a.step0) + 1ull;
-          for (int r = 0; r < CLOCK_GROUPS; ++r) a.clock[16 * r] = steps;
-          a.clock[CLOCK_TOP] = 0ull;
-        }
-      }
-    }
-  }
-}
-
-// bsb_rollout_masked: T masked steps in one launch, laid out as masked_kernel (one chunk of 32 lanes per warp, ragged
-// chunks within one setting, rows through emit_lane_subset) with transition_kernel's T loop.  Lane i is active at step
-// t while mask[i] != 0 and its budget (m.episodes_left, when given) is positive; each LAST of an active step takes one
-// from the budget.  So a lane's active steps are a prefix of the launch: its state, RNG streams, accumulators and
-// budget stay in registers over them, and the calls it sits out all come after its last active one
-// (lane_sit_out_calls, once, after lane_close).  A warp whose lanes are all inactive stops stepping.  Graph-safe mode
-// advances the call count by T; the mask and the budgets are read (and the budgets written) at every launch, so
-// graph replays keep counting the budgets down.  A kernel of its own rather than a T loop in masked_kernel: a shared
-// body (a __device__ function, or a compile-time flag on masked_kernel) changed masked_kernel's register allocation.
-template <class V, int RK>
-__global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_rollout_kernel(const EnvParams p, const LaunchArgs a, const MaskArgs m) {
-  typedef typename V::Fam Fam;
-  typedef typename V::Obs O;
-  typedef typename RngOf<RK>::type R;
-  const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
-  int64_t step0 = a.step0;
-  if (a.clock) step0 += (int64_t)*reinterpret_cast<volatile unsigned long long*>(a.clock + 16 * (blockIdx.x % CLOCK_GROUPS));
-  const MailFields out = {a.reward, a.reward_f64, a.discount, a.step_type};
-  const bool noise = m.noise != 0, track = m.track != 0;
-  const RaggedTable* table = V::kRagged ? reinterpret_cast<const RaggedTable*>(p.pack) : nullptr;
-  const int64_t lanes = V::kRagged ? table->pack.lanes_per_setting : p.batch;      // lanes per setting block
-  const int64_t per_setting = (lanes + 31) / 32;
-  const int64_t n_chunks = (V::kRagged ? table->pack.n_settings : 1) * per_setting;
-  const int64_t chunk = (int64_t)blockIdx.x * warps_per_cta + warp;
-  const int64_t T = a.T;
+  const int64_t T = kOneCall ? 1 : a.T;
+  int64_t* const budgets = kOneCall ? nullptr : m.episodes_left;
 
   if (chunk < n_chunks) {
     const int64_t k = chunk / per_setting;
@@ -1664,8 +1576,8 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_rollout_
     }
     const int64_t step_elems = V::kRagged ? table->step_elems : p.batch * (int64_t)p.obs_numel;
     const bool selected = in && m.mask[lane] != 0;
-    int64_t left = selected && m.episodes_left ? m.episodes_left[lane] : 0;
-    bool on = selected && (!m.episodes_left || left > 0);
+    int64_t left = selected && budgets ? budgets[lane] : 0;
+    bool on = selected && (!budgets || left > 0);
     const bool opened = on;
 
     typename Fam::Lane L;
@@ -1678,22 +1590,24 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_rollout_
     if constexpr (V::kSameStep) { Fam::init(p, merged.last); merged.done = false; }
     if (on) lane_open<Fam>(lp, lane, L, rng, wrng, ep, a.mode, noise, track);
     int64_t acted = 0;                     // the lane's active steps
-    for (int64_t t = 0; t < T && __any_sync(0xffffffffu, on); ++t) {
+    for (int64_t t = 0; t < T && (kOneCall || __any_sync(0xffffffffu, on)); ++t) {
       const int64_t off = t * p.batch + lane;
       if (on) {
-        int32_t action;
-        if (a.actions) {
-          action = a.actions[off];
-          if ((uint32_t)action >= (uint32_t)p.num_actions) {
-            if (a.bad_action) *a.bad_action = 1;
-            action = action < 0 ? 0 : p.num_actions - 1;
+        int32_t action = 0;
+        if (a.mode == MODE_STEP) {
+          if (kOneCall || a.actions) {
+            action = a.actions[off];
+            if ((uint32_t)action >= (uint32_t)p.num_actions) {
+              if (a.bad_action) *a.bad_action = 1;
+              action = action < 0 ? 0 : p.num_actions - 1;
+            }
+          } else {
+            action = action_stream.sample(a.action_seed, lp.lane_offset + (uint64_t)lane, (uint64_t)(step0 + t), p.num_actions);
           }
-        } else {
-          action = action_stream.sample(a.action_seed, lp.lane_offset + (uint64_t)lane, (uint64_t)(step0 + t), p.num_actions);
+          if (!kOneCall && a.actions_out) a.actions_out[off] = action;
         }
-        if (a.actions_out) a.actions_out[off] = action;
-        if constexpr (V::kSameStep) lane_step<Fam, R, true>(p, lane, L, rng, wrng, ep, action, MODE_STEP, noise, track, step0 + t, out, off, &merged);
-        else lane_step<Fam>(lp, lane, L, rng, wrng, ep, action, MODE_STEP, noise, track, step0 + t, out, off);
+        if constexpr (V::kSameStep) lane_step<Fam, R, true>(p, lane, L, rng, wrng, ep, action, a.mode, noise, track, step0 + t, out, off, &merged);
+        else lane_step<Fam>(lp, lane, L, rng, wrng, ep, action, a.mode, noise, track, step0 + t, out, off);
       }
       if constexpr (V::kSameStep) {
         if (a.final_obs)
@@ -1705,12 +1619,12 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_rollout_
         ++acted;
         // the step's LAST: a same-step lane's merged reset, else the _reset_next_step flag the step left set
         const bool last = V::kSameStep ? merged.done : L.nr != 0;
-        if (m.episodes_left && last && --left == 0) on = false;
+        if (budgets && last && --left == 0) on = false;
       }
     }
     if (opened) lane_close<Fam>(lp, lane, L, rng, wrng, ep, noise, track);
     if (in && track && acted < T) lane_sit_out_calls(p, lane, T - acted);
-    if (selected && m.episodes_left) m.episodes_left[lane] = left;
+    if (selected && budgets) budgets[lane] = left;
   }
 
   if (a.clock) {        // graph-safe mode: the last CTA advances the call count by T (transition_kernel's epilogue)

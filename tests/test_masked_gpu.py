@@ -1,4 +1,5 @@
-"""Masked calls on the device (masked_kernel): against the host path and against separate device handles."""
+"""Masked resets and steps on the device (masked_kernel): against the host path and against separate device
+handles."""
 import numpy as np
 import pytest
 import torch
@@ -23,7 +24,8 @@ OBS = {'float': 'float32', 'Bf16': 'bfloat16', 'uint8_t': 'uint8'}
 
 
 def masked_kernel_cases():
-  """One case per masked_kernel instantiation of the variant list: (family, O, mode, bit source)."""
+  """One case per variant of the list and bit source, (family, O, mode, bit source): its masked_kernel instantiations
+  (masked resets and steps here, masked rollouts in test_masked_rollout_gpu)."""
   cases = []
   for variants in bsb_build.variant_list().values():
     for family, obs, mode, mt, _ in variants:
@@ -85,7 +87,7 @@ def test_every_masked_kernel_matches_the_host_path(case, mnist_dir):
 
 
 def test_gpu_cases_cover_every_masked_kernel_of_the_list():
-  """Each masked_kernel instantiation (a variant of the list, times its bit sources) has a case above."""
+  """Each variant of the list, times its bit sources, has a case above, and with it both masked_kernel instantiations."""
   cases = masked_kernel_cases()
   want = sum(1 + int(mt) for variants in bsb_build.variant_list().values() for _, _, _, mt, _ in variants)
   assert len(set(cases)) == len(cases) == want

@@ -1,4 +1,4 @@
-"""Masked rollouts on the device (masked_rollout_kernel) against the host path."""
+"""Masked rollouts on the device (masked_kernel, T steps per launch) against the host path."""
 import numpy as np
 import pytest
 import torch

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Masked rollouts (`rollout(..., mask=..., episodes_left=...)`, masked_rollout_kernel) on one GPU, in two legs.
+"""Masked rollouts (`rollout(..., mask=..., episodes_left=...)`, masked_kernel) on one GPU, in two legs.
 
     python tools/bench_masked_rollout.py [--out out/masked_rollout.jsonl] [--repeats 5] [--lanes 64] [--episodes 20]
 

@@ -145,7 +145,7 @@ for bsuite_id, batch, kw in (('deep_sea/11', 1001, {}), ('catch/0', 997, dict(au
     env.close()
   assert all(torch.equal(a, b) for a, b in zip(*got))
   print(bsuite_id, batch, 'masked calls == host path: True', flush=True)
-# Masked rollouts (masked_rollout_kernel): the same workloads as T steps per launch, lanes stopping at their own
+# Masked rollouts (masked_kernel again): the same workloads as T steps per launch, lanes stopping at their own
 # budgets mid-launch, sampled actions written to actions_out, against the host path.
 for bsuite_id, batch, kw in (('deep_sea/11', 1001, {}), ('catch/0', 997, dict(autoreset='same_step')),
                              ('umbrella_distract/3', 501, {}), ('mnist/0', 333, dict(obs_dtype='bfloat16'))):
