@@ -160,15 +160,15 @@ def bsuite_score(source) -> Scores:
   return _run(sources, lanes, envs[0].device, envs[0]._stream())   # pylint: disable=protected-access
 
 
-def score_rows(rows: Mapping[str, Mapping[str, Any]], stream=None) -> Scores:
+def score_rows(rows: Mapping[str, Mapping[str, Any]], stream=None, lanes: Optional[int] = None) -> Scores:
   """Scores caller-owned rows: `{bsuite_id: logged}` where `logged` has the keys of `logged_rows()` -- `columns`,
   `rows` float64 [n_points, n_columns, B] and `counts` int32 [B] -- as torch tensors (all on one device) or numpy
-  arrays, and optionally `first_lane`: the lanes scored are [first_lane, first_lane + L), with L the same for
-  every id (default: all lanes of the first id)."""
+  arrays, and optionally `first_lane`: the lanes scored are [first_lane, first_lane + L), with L = `lanes` the
+  same for every id (default: all lanes of the first id from its first_lane on)."""
   import torch  # pylint: disable=import-outside-toplevel
   if not rows:
     raise ValueError('nothing to score')
-  held, sources, lanes = [], [], None
+  held, sources = [], []
   for bsuite_id, logged in rows.items():
     data = torch.as_tensor(logged['rows'], dtype=torch.float64)
     counts = torch.as_tensor(logged['counts'], dtype=torch.int32)

@@ -974,6 +974,14 @@ int32_t bsb_sum_episode_stats_many(bsb_env* const* envs, int32_t count, double* 
     if (!envs[k]->p.ep) return fail(BSB_INVALID_ARGUMENT, "environment was created without BSB_FLAG_TRACK_EPISODES");
     if (envs[k]->device != envs[0]->device) return fail(BSB_INVALID_ARGUMENT, "environments live on different devices");
   }
+  // Two grid rows of one handle would share its partials and its ticket: the last-block test could then fire before
+  // every block of either row has written.  Refused on both paths, so they answer alike.
+  {
+    std::vector<bsb_env*> seen(envs, envs + count);
+    std::sort(seen.begin(), seen.end());
+    if (std::adjacent_find(seen.begin(), seen.end()) != seen.end())
+      return fail(BSB_INVALID_ARGUMENT, "the same environment is given twice");
+  }
   if (envs[0]->device < 0 || count > kSumManyMax) {       // host path / oversized lists: one environment at a time
     for (int32_t k = 0; k < count; ++k) { int rc = bsb_sum_episode_stats(envs[k], dst + 5 * k, stream); if (rc != BSB_OK) return rc; }
     return BSB_OK;

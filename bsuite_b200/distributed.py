@@ -62,6 +62,19 @@ def gather_episode_returns(env, group=None) -> Dict[str, Any]:
   return dict(steps=gathered[:, 0], episode=gathered[:, 1], total_return=gathered[:, 2], lanes=gathered[:, 5])
 
 
+def _distinct(envs):
+  """`envs` as a list in which no handle appears twice: one reduction launch keeps a handle's partial sums in that
+  handle's own scratch, so `bsb_sum_episode_stats_many` refuses a repeated handle (a log point would fail later)."""
+  envs = list(envs) if isinstance(envs, (list, tuple)) else [envs]
+  seen = set()
+  for env in envs:
+    ptr = env._handle.ptr.value  # pylint: disable=protected-access
+    if ptr in seen:
+      raise ValueError('an environment appears twice in one log point')
+    seen.add(ptr)
+  return envs
+
+
 class LogPoint:
   """Asynchronous log point for one or more tracked environments (SURVEY.md 8e: "off the critical path").
 
@@ -82,7 +95,7 @@ class LogPoint:
     import torch
     import torch.distributed as dist
     self._torch, self._dist, self._group = torch, dist, group
-    self.envs = list(envs) if isinstance(envs, (list, tuple)) else [envs]
+    self.envs = _distinct(envs)
     self._device = self.envs[0].device
     self._cuda = self._device.type == 'cuda'
     self.world = dist.get_world_size(group) if (dist.is_available() and dist.is_initialized()) else 1
@@ -160,7 +173,7 @@ class NativeLogPoint:
     import torch
     import torch.distributed as dist
     self._torch = torch
-    self.envs = list(envs) if isinstance(envs, (list, tuple)) else [envs]
+    self.envs = _distinct(envs)
     self._device = self.envs[0].device
     if self._device.type != 'cuda':
       raise RuntimeError('NativeLogPoint needs CUDA environments')

@@ -440,7 +440,9 @@ int32_t bsb_sum_episode_stats(bsb_env* env, double* dst5, void* stream);
 
 /* The same reduction for `count` environments of one device in ONE kernel launch:
  * dst receives [count][5].  A log point of a whole sweep (bsuite/sweep.py:134-150:
- * 23 experiments) is then one launch and one all-gather. */
+ * 23 experiments) is then one launch and one all-gather.  Each handle may appear
+ * once: a repeated handle returns BSB_INVALID_ARGUMENT on the host and the device
+ * path alike (the launch keeps its partial sums in per-handle scratch). */
 int32_t bsb_sum_episode_stats_many(bsb_env* const* envs, int32_t count,
                                    double* dst, void* stream);
 
@@ -649,7 +651,9 @@ int32_t bsb_invalid_actions(bsb_env* env, int32_t* seen);
  * log rows at log-spaced episodes only: utils/wrappers.py:99-110).  local and
  * gathered are caller-owned device buffers that must stay valid until
  * bsb_comm_wait(comm, s), which makes stream `s` wait (on the device) for the
- * latest gather.  Replaces the process pool's result collection of
+ * latest gather.  As for bsb_sum_episode_stats_many, a handle repeated in `envs`
+ * returns BSB_INVALID_ARGUMENT before any reduction or gather is enqueued.
+ * Replaces the process pool's result collection of
  * bsuite/baselines/utils/pool.py:28-54.
  */
 #define BSB_COMM_ID_BYTES 128
