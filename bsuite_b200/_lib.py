@@ -137,6 +137,8 @@ EXPORTS = {
     'bsb_sum_episode_stats': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     'bsb_sum_episode_stats_many': (ctypes.c_int32, [ctypes.POINTER(ctypes.c_void_p), ctypes.c_int32, ctypes.c_void_p,
                                                     ctypes.c_void_p]),
+    'bsb_sum_setting_stats': (ctypes.c_int32, [ctypes.POINTER(ctypes.c_void_p), ctypes.c_int32, ctypes.c_void_p,
+                                               ctypes.c_void_p]),
     'bsb_log_layout': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32)]),
     'bsb_read_log_rows': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     'bsb_state_bytes': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64)]),
@@ -155,6 +157,8 @@ EXPORTS = {
     'bsb_comm_world': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32)]),
     'bsb_log_point': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_void_p), ctypes.c_int32, ctypes.c_void_p,
                                        ctypes.c_void_p, ctypes.c_void_p]),
+    'bsb_log_point_settings': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_void_p), ctypes.c_int32,
+                                                ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]),
     'bsb_comm_wait': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p]),
     'bsb_launch_count': (ctypes.c_int64, []),
     'bsb_image_plan_create': (ctypes.c_int32, [ctypes.POINTER(ImageDesc), ctypes.c_int32, ctypes.POINTER(ctypes.c_void_p)]),

@@ -3,8 +3,9 @@
 // with dlopen (no link-time dependency: single-GPU users never load it); the five entry points used are declared
 // here from NCCL's public, stable C API.
 //
-// A log point = one reduction kernel on the caller's stream (bsb_sum_episode_stats_many) + ncclAllGather on a side
-// stream the communicator owns, fenced by events in both directions, so the caller's stream goes on stepping.
+// A log point = one reduction kernel on the caller's stream (bsb_sum_episode_stats_many, or bsb_sum_setting_stats for
+// one row per setting) + ncclAllGather on a side stream the communicator owns, fenced by events in both directions,
+// so the caller's stream goes on stepping.
 #include <dlfcn.h>
 
 #include <cstdlib>
@@ -127,19 +128,34 @@ int32_t bsb_comm_world(const bsb_comm* comm, int32_t* rank, int32_t* world) {
   return BSB_OK;
 }
 
-int32_t bsb_log_point(bsb_comm* comm, bsb_env* const* envs, int32_t count, double* local, double* gathered, void* stream) {
+// bsb_log_point (one row per handle) and bsb_log_point_settings (one row per setting).
+static int32_t log_point(bsb_comm* comm, bsb_env* const* envs, int32_t count, bool per_setting, double* local,
+                         double* gathered, void* stream) {
   if (!comm || !envs || !local || !gathered || count <= 0) return fail(BSB_INVALID_ARGUMENT, "bad arguments");
   DeviceScope scope(comm->device);
   cudaStream_t caller = static_cast<cudaStream_t>(stream);
   // the previous gather may still be reading `local` / writing `gathered`: the reduction must not overtake it
   if (comm->issued) BSB_CUDA(cudaStreamWaitEvent(caller, comm->done, 0));
-  { int rc = bsb_sum_episode_stats_many(envs, count, local, stream); if (rc != BSB_OK) return rc; }
+  int rc = per_setting ? bsb_sum_setting_stats(envs, count, local, stream)
+                       : bsb_sum_episode_stats_many(envs, count, local, stream);
+  if (rc != BSB_OK) return rc;
+  size_t rows = 0;                      // the reduction has checked every handle
+  for (int32_t k = 0; k < count; ++k) rows += per_setting ? (size_t)envs[k]->n_settings : 1;
   BSB_CUDA(cudaEventRecord(comm->ready, caller));
   BSB_CUDA(cudaStreamWaitEvent(comm->side, comm->ready, 0));
-  BSB_NCCL(g_nccl.AllGather(local, gathered, (size_t)count * 5, kNcclFloat64, comm->comm, comm->side));
+  BSB_NCCL(g_nccl.AllGather(local, gathered, rows * 5, kNcclFloat64, comm->comm, comm->side));
   BSB_CUDA(cudaEventRecord(comm->done, comm->side));
   comm->issued = true;
   return BSB_OK;
+}
+
+int32_t bsb_log_point(bsb_comm* comm, bsb_env* const* envs, int32_t count, double* local, double* gathered, void* stream) {
+  return log_point(comm, envs, count, false, local, gathered, stream);
+}
+
+int32_t bsb_log_point_settings(bsb_comm* comm, bsb_env* const* envs, int32_t count, double* local, double* gathered,
+                               void* stream) {
+  return log_point(comm, envs, count, true, local, gathered, stream);
 }
 
 int32_t bsb_comm_wait(bsb_comm* comm, void* stream) {

@@ -364,16 +364,30 @@ __global__ void episode_stat_kernel(const EnvParams p, int field, int64_t calls,
   if (i < p.batch) dst[i] = episode_stat(p, i, field, calls);
 }
 
-// Sums of the five Logging columns over the lanes of up to kSumManyMax environments in ONE launch (blockIdx.y =
-// environment: a log point of the 23-experiment sweep is one kernel instead of 23).  Deterministic: a fixed grid (a
-// function of the batch only) of block-strided partial sums lands in the environment's scratch[block][5]; the block
-// that finishes last adds the partials in block order and re-arms the ticket.  (No floating-point atomics: the result
-// must not depend on scheduling -- a graph replay and an eager call must agree to the bit.)
+// Sums of the five Logging columns over the lanes of up to kSumManyMax environments in ONE launch (blockIdx.y = row:
+// a log point of the 23-experiment sweep is one kernel instead of 23).  A row sums the contiguous lane range
+// [first, first + lanes) of a handle whose per-lane arrays have stride `batch`: the whole handle is the range
+// (0, batch), setting k of a pack is (k * lanes, lanes).  A job covers `n_settings` consecutive rows; row_start[j] is
+// the first row of job j.  Deterministic: a fixed grid of block-strided partial sums, counted from `first`, lands in
+// the row's own scratch[block][5]; the block that finishes last adds the partials in block order and re-arms the
+// row's ticket.  So a row's order is the one a standalone handle of `lanes` lanes sums in.  (No floating-point
+// atomics: the result must not depend on scheduling -- a graph replay and an eager call must agree to the bit.)
 constexpr int kSumBlocks = 64, kSumThreads = 256, kSumManyMax = 64;
-struct SumJob { const double* ep; int64_t batch; int64_t calls; const unsigned long long* clock; double* scratch; };
-struct SumJobs { SumJob job[kSumManyMax]; };
+constexpr int kSumScratch = kSumBlocks * 5 + 1;      // doubles per row: the partials, then the ticket
+struct SumJob {
+  const double* ep; int64_t batch; int64_t lanes; int64_t calls; const unsigned long long* clock; double* scratch;
+  int32_t n_settings;
+};
+struct SumJobs { SumJob job[kSumManyMax]; int32_t row_start[kSumManyMax]; int32_t count; };
+static_assert(sizeof(SumJobs) + sizeof(double*) <= 4096, "kernel parameters must stay within 4 KB");
 __global__ void episode_sum_many_kernel(const SumJobs jobs, double* dst) {
-  const SumJob j = jobs.job[blockIdx.y];
+  const int row = (int)blockIdx.y;
+  int h = 0;
+  while (h + 1 < jobs.count && jobs.row_start[h + 1] <= row) ++h;
+  const SumJob j = jobs.job[h];
+  const int setting = row - jobs.row_start[h];
+  const int64_t first = (int64_t)setting * j.lanes;
+  double* scratch = j.scratch + (int64_t)setting * kSumScratch;
   EnvParams p;
   p.ep = const_cast<double*>(j.ep); p.batch = j.batch;
   int64_t calls = j.calls;
@@ -381,32 +395,32 @@ __global__ void episode_sum_many_kernel(const SumJobs jobs, double* dst) {
   __shared__ double partial[5][kSumThreads / 32];
   __shared__ bool is_last;
   double v[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.batch; i += (int64_t)gridDim.x * blockDim.x)
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < j.lanes; i += (int64_t)gridDim.x * blockDim.x)
 #pragma unroll
-    for (int f = 0; f < 5; ++f) v[f] += episode_stat(p, i, f, calls);
+    for (int f = 0; f < 5; ++f) v[f] += episode_stat(p, first + i, f, calls);
 #pragma unroll
   for (int f = 0; f < 5; ++f)
     for (int o = 16; o > 0; o >>= 1) v[f] += __shfl_down_sync(0xffffffffu, v[f], o);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (lane == 0) for (int f = 0; f < 5; ++f) partial[f][warp] = v[f];
   __syncthreads();
-  // blocks that own no lanes of this environment contribute exact zeros, so the block-order sum below equals the
-  // one a grid of min(blocks, ceil(batch / threads)) blocks forms (bsb_sum_episode_stats launches that many)
+  // blocks that own no lanes of this row contribute exact zeros, so the block-order sum below equals the one a grid
+  // of min(blocks, ceil(lanes / threads)) blocks forms (bsb_sum_episode_stats launches that many)
   if (threadIdx.x < 5) {
     double s = 0.0;
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += partial[threadIdx.x][w];
-    j.scratch[blockIdx.x * 5 + threadIdx.x] = s;
+    scratch[blockIdx.x * 5 + threadIdx.x] = s;
     __threadfence();
   }
   __syncthreads();
-  unsigned long long* ticket = reinterpret_cast<unsigned long long*>(j.scratch + kSumBlocks * 5);
+  unsigned long long* ticket = reinterpret_cast<unsigned long long*>(scratch + kSumBlocks * 5);
   if (threadIdx.x == 0) is_last = atomicAdd(ticket, 1ull) == (unsigned long long)gridDim.x - 1ull;
   __syncthreads();
   if (!is_last) return;
   __threadfence();
   if (threadIdx.x < 5) {
     double s = 0.0;
-    for (unsigned b = 0; b < gridDim.x; ++b) s += __ldcg(j.scratch + b * 5 + threadIdx.x);
+    for (unsigned b = 0; b < gridDim.x; ++b) s += __ldcg(scratch + b * 5 + threadIdx.x);
     dst[blockIdx.y * 5 + threadIdx.x] = s;
   }
   if (threadIdx.x == 0) *ticket = 0ull;
@@ -541,7 +555,8 @@ static int32_t create_env(const bsb_config* config, int64_t batch, int32_t devic
   if (device >= 0) {
     BSB_TRY(env_alloc_t(e, &e->work_counter, 1, false));
     BSB_TRY(env_alloc_t(e, &e->clock, CLOCK_WORDS, false));
-    BSB_TRY(env_alloc_t(e, &e->sum_scratch, kSumBlocks * 5 + 1, false));
+    // every setting's own partials and ticket, so the rows of one per-setting launch never share them
+    BSB_TRY(env_alloc_t(e, &e->sum_scratch, (size_t)e->n_settings * kSumScratch, false));
     void* flag = nullptr; void* flag_dev = nullptr;
     if (cudaHostAlloc(&flag, sizeof(int32_t), cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess ||
         cudaHostGetDevicePointer(&flag_dev, flag, 0) != cudaSuccess) {
@@ -941,33 +956,32 @@ int32_t bsb_read_episode_stats(bsb_env* env, int32_t field, double* dst, void* s
   return BSB_OK;
 }
 
-int32_t bsb_sum_episode_stats(bsb_env* env, double* dst5, void* stream) {
-  if (!env || !dst5) return fail(BSB_INVALID_ARGUMENT, "null argument");
-  if (!env->p.ep) return fail(BSB_INVALID_ARGUMENT, "environment was created without BSB_FLAG_TRACK_EPISODES");
-  { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
-  const int64_t B = env->p.batch;
-  if (env->device >= 0) {
-    DeviceGuard guard(env->device);
-    int64_t blocks = (B + kSumThreads - 1) / kSumThreads;
-    if (blocks > kSumBlocks) blocks = kSumBlocks;
-    SumJobs jobs;
-    memset(&jobs, 0, sizeof(jobs));
-    jobs.job[0].ep = env->p.ep; jobs.job[0].batch = B; jobs.job[0].calls = env->steps_done;
-    jobs.job[0].clock = env->graph_safe ? env->clock : nullptr; jobs.job[0].scratch = env->sum_scratch;
-    episode_sum_many_kernel<<<dim3((unsigned)blocks, 1), kSumThreads, 0, static_cast<cudaStream_t>(stream)>>>(jobs, dst5);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    BSB_CUDA(cudaGetLastError());
-  } else {
-    for (int f = 0; f < 5; ++f) {
-      double s = 0.0;
-      for (int64_t i = 0; i < B; ++i) s += episode_stat(env->p, i, f, env->steps_done);
-      dst5[f] = s;
-    }
-  }
-  return BSB_OK;
+// The rows of `env`: one for the whole handle, or one per setting (an ordinary handle has one setting).
+static int32_t sum_rows(const bsb_env* env, bool per_setting) { return per_setting ? env->n_settings : 1; }
+
+// Fills the job of `env` (whole handle or per setting) at jobs.job[k], its first row at `row`.
+static void put_sum_job(SumJobs& jobs, int32_t k, int32_t row, const bsb_env* env, bool per_setting) {
+  SumJob& j = jobs.job[k];
+  j.ep = env->p.ep; j.batch = env->p.batch; j.calls = env->steps_done;
+  j.lanes = per_setting ? env->lanes_per_setting : env->p.batch;
+  j.n_settings = sum_rows(env, per_setting);
+  j.clock = env->graph_safe ? env->clock : nullptr; j.scratch = env->sum_scratch;
+  jobs.row_start[k] = row;
 }
 
-int32_t bsb_sum_episode_stats_many(bsb_env* const* envs, int32_t count, double* dst, void* stream) {
+// The host path: each row's lanes in order from 0.0.
+static void host_sums(const bsb_env* env, bool per_setting, double* dst) {
+  const int64_t lanes = per_setting ? env->lanes_per_setting : env->p.batch;
+  for (int32_t r = 0; r < sum_rows(env, per_setting); ++r)
+    for (int f = 0; f < 5; ++f) {
+      double s = 0.0;
+      for (int64_t i = r * lanes; i < (r + 1) * lanes; ++i) s += episode_stat(env->p, i, f, env->steps_done);
+      dst[5 * r + f] = s;
+    }
+}
+
+// Shared validation of the list calls: null handles, untracked handles, mixed devices, a repeated handle.
+static int32_t check_sum_list(bsb_env* const* envs, int32_t count, const double* dst) {
   if (!envs || !dst || count <= 0) return fail(BSB_INVALID_ARGUMENT, "bad arguments");
   for (int32_t k = 0; k < count; ++k) {
     if (!envs[k]) return fail(BSB_INVALID_ARGUMENT, "null environment");
@@ -976,28 +990,67 @@ int32_t bsb_sum_episode_stats_many(bsb_env* const* envs, int32_t count, double* 
   }
   // Two grid rows of one handle would share its partials and its ticket: the last-block test could then fire before
   // every block of either row has written.  Refused on both paths, so they answer alike.
-  {
-    std::vector<bsb_env*> seen(envs, envs + count);
-    std::sort(seen.begin(), seen.end());
-    if (std::adjacent_find(seen.begin(), seen.end()) != seen.end())
-      return fail(BSB_INVALID_ARGUMENT, "the same environment is given twice");
-  }
-  if (envs[0]->device < 0 || count > kSumManyMax) {       // host path / oversized lists: one environment at a time
-    for (int32_t k = 0; k < count; ++k) { int rc = bsb_sum_episode_stats(envs[k], dst + 5 * k, stream); if (rc != BSB_OK) return rc; }
-    return BSB_OK;
-  }
-  DeviceGuard guard(envs[0]->device);
+  std::vector<bsb_env*> seen(envs, envs + count);
+  std::sort(seen.begin(), seen.end());
+  if (std::adjacent_find(seen.begin(), seen.end()) != seen.end())
+    return fail(BSB_INVALID_ARGUMENT, "the same environment is given twice");
+  return BSB_OK;
+}
+
+// The rows of up to kSumManyMax validated handles of one device in ONE launch of `blocks` x rows blocks.
+static int32_t launch_sums(bsb_env* const* envs, int32_t count, bool per_setting, int64_t blocks, double* dst,
+                           void* stream) {
   SumJobs jobs;
   memset(&jobs, 0, sizeof(jobs));
+  int32_t rows = 0;
   for (int32_t k = 0; k < count; ++k) {
     { int frc = drain_host_steps(envs[k]); if (frc != BSB_OK) return frc; }
-    jobs.job[k].ep = envs[k]->p.ep; jobs.job[k].batch = envs[k]->p.batch; jobs.job[k].calls = envs[k]->steps_done;
-    jobs.job[k].clock = envs[k]->graph_safe ? envs[k]->clock : nullptr; jobs.job[k].scratch = envs[k]->sum_scratch;
+    put_sum_job(jobs, k, rows, envs[k], per_setting);
+    rows += sum_rows(envs[k], per_setting);
   }
-  episode_sum_many_kernel<<<dim3(kSumBlocks, (unsigned)count), kSumThreads, 0, static_cast<cudaStream_t>(stream)>>>(jobs, dst);
+  jobs.count = count;
+  DeviceGuard guard(envs[0]->device);
+  episode_sum_many_kernel<<<dim3((unsigned)blocks, (unsigned)rows), kSumThreads, 0, static_cast<cudaStream_t>(stream)>>>(jobs, dst);
   g_launches.fetch_add(1, std::memory_order_relaxed);
   BSB_CUDA(cudaGetLastError());
   return BSB_OK;
+}
+
+int32_t bsb_sum_episode_stats(bsb_env* env, double* dst5, void* stream) {
+  if (!env || !dst5) return fail(BSB_INVALID_ARGUMENT, "null argument");
+  if (!env->p.ep) return fail(BSB_INVALID_ARGUMENT, "environment was created without BSB_FLAG_TRACK_EPISODES");
+  if (env->device >= 0) {
+    int64_t blocks = (env->p.batch + kSumThreads - 1) / kSumThreads;
+    if (blocks > kSumBlocks) blocks = kSumBlocks;
+    return launch_sums(&env, 1, false, blocks, dst5, stream);
+  }
+  { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
+  host_sums(env, false, dst5);
+  return BSB_OK;
+}
+
+// bsb_sum_episode_stats_many (per_setting false) and bsb_sum_setting_stats (true).
+static int32_t sum_list(bsb_env* const* envs, int32_t count, bool per_setting, double* dst, void* stream) {
+  { int rc = check_sum_list(envs, count, dst); if (rc != BSB_OK) return rc; }
+  if (envs[0]->device < 0 || count > kSumManyMax) {       // host path / oversized lists: one environment at a time
+    for (int32_t k = 0; k < count; ++k) {
+      int rc = envs[k]->device < 0 ? drain_host_steps(envs[k])
+                                    : launch_sums(envs + k, 1, per_setting, kSumBlocks, dst, stream);
+      if (rc != BSB_OK) return rc;
+      if (envs[k]->device < 0) host_sums(envs[k], per_setting, dst);
+      dst += 5 * sum_rows(envs[k], per_setting);
+    }
+    return BSB_OK;
+  }
+  return launch_sums(envs, count, per_setting, kSumBlocks, dst, stream);
+}
+
+int32_t bsb_sum_episode_stats_many(bsb_env* const* envs, int32_t count, double* dst, void* stream) {
+  return sum_list(envs, count, false, dst, stream);
+}
+
+int32_t bsb_sum_setting_stats(bsb_env* const* envs, int32_t count, double* dst, void* stream) {
+  return sum_list(envs, count, true, dst, stream);
 }
 
 int32_t bsb_log_layout(const bsb_env* env, int32_t* n_points, int32_t* n_columns) {

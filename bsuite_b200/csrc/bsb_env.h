@@ -71,7 +71,7 @@ struct bsb_env {
   // then on the device clock counts the steps (kernel comment in bsb_kernels.cuh) and steps = steps_done + clock[0].
   bool graph_safe;
   unsigned long long* clock;         // device, CLOCK_WORDS words: step count (replicated), chunk counter, finished-CTA counters
-  double* sum_scratch;               // device: bsb_sum_episode_stats partials [64][5] + the ticket
+  double* sum_scratch;               // device: per setting, the sum kernel's partials [64][5] + the ticket
   unsigned long long* work_counter;  // device counter of the dynamic chunk scheduler
   unsigned long long work_base;      // its value when the next launch starts
   int num_sms;

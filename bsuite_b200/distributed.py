@@ -40,6 +40,29 @@ def load_sharded(bsuite_id: str, global_batch: int, rank: Optional[int] = None, 
   return registry.load_from_id(bsuite_id, batch=count, device=device, seed=seed, lane_offset=first, **engine_kwargs)
 
 
+def load_experiment_sharded(experiment_name: str, lanes_per_setting: int, rank: Optional[int] = None,
+                            world: Optional[int] = None, **kwargs):
+  """This rank's shard of `registry.load_experiment(experiment_name, lanes_per_setting, ...)`: every setting keeps
+  the global lanes `shard_range(lanes_per_setting, rank, world)` (passed on as `lane_offset`), as `load_sharded`
+  shards one id, so a setting's lanes do not depend on how the pack is sharded."""
+  rank, world = _rank_world(rank, world)
+  first, count = shard_range(lanes_per_setting, rank, world)
+  if count == 0:
+    raise ValueError(f'rank {rank} would own no lanes (lanes_per_setting {lanes_per_setting} < world {world})')
+  if 'lane_offset' in kwargs:
+    raise ValueError('lane_offset follows from rank and world')
+  return registry.load_experiment(experiment_name, count, lane_offset=first, **kwargs)
+
+
+def _rank_world(rank, world):
+  if rank is None or world is None:
+    import torch.distributed as dist
+    if dist.is_available() and dist.is_initialized():
+      return dist.get_rank(), dist.get_world_size()
+    return 0, 1
+  return rank, world
+
+
 def gather_episode_returns(env, group=None) -> Dict[str, Any]:
   """One all-gather of the per-rank reduction of the Logging columns (utils/wrappers.py:113-125), synchronous on
   the current stream (`LogPoint` is the asynchronous form).
@@ -60,6 +83,18 @@ def gather_episode_returns(env, group=None) -> Dict[str, Any]:
   else:
     gathered = block.view(1, -1)
   return dict(steps=gathered[:, 0], episode=gathered[:, 1], total_return=gathered[:, 2], lanes=gathered[:, 5])
+
+
+def _row_ids(envs, per_setting):
+  """The bsuite_id of every row of a log point: per setting, or per environment (None where it is not known)."""
+  ids = []
+  for env in envs:
+    packed = getattr(env, 'bsuite_ids', None)
+    if per_setting and packed is not None:
+      ids.extend(packed)
+    else:
+      ids.append(None if packed is not None else getattr(env, 'bsuite_id', None))
+  return tuple(ids)
 
 
 def _distinct(envs):
@@ -87,11 +122,16 @@ class LogPoint:
   so the caller's stream goes on launching steps k+1... immediately.  `issue()` returns a ticket; `result(ticket)`
   makes the caller's stream (default) or the host wait for that gather and returns `[world, n_envs, 5]` with the
   columns (steps, episode, total_return, episode_len, episode_return).  `slots` tickets can be in flight.
+
+  `per_setting=True`: one row per setting of every packed environment (an ordinary one keeps its one row), still one
+  reduction launch (`bsb_sum_setting_stats`); results are `[world, rows, 5]`.  Each row equals what a standalone
+  environment of that setting would report.  `row_ids` names each row's bsuite_id (None for an ordinary environment
+  not loaded by id, or for a whole pack without `per_setting`).
   """
 
   COLUMNS = ('steps', 'episode', 'total_return', 'episode_len', 'episode_return')
 
-  def __init__(self, envs, group=None, slots: int = 2):
+  def __init__(self, envs, group=None, slots: int = 2, per_setting: bool = False):
     import torch
     import torch.distributed as dist
     self._torch, self._dist, self._group = torch, dist, group
@@ -99,7 +139,9 @@ class LogPoint:
     self._device = self.envs[0].device
     self._cuda = self._device.type == 'cuda'
     self.world = dist.get_world_size(group) if (dist.is_available() and dist.is_initialized()) else 1
-    n = len(self.envs)
+    self.per_setting = bool(per_setting)
+    self.row_ids = _row_ids(self.envs, self.per_setting)
+    n = len(self.row_ids)
     self._slots = int(slots)
     self._local = torch.zeros((self._slots, n, 5), dtype=torch.float64, device=self._device)
     self._gathered = (torch.zeros((self._slots, self.world, n, 5), dtype=torch.float64, device=self._device)
@@ -122,10 +164,12 @@ class LogPoint:
     if self._side is not None and ticket >= self._slots:
       current.wait_event(self._done[slot])          # the gather that last read this slot's block has finished
     block = self._local[slot]
-    if len(self.envs) == 1:
-      self.envs[0].episode_stat_sums(out=block[0])
+    first = self.envs[0]
+    if self.per_setting:                             # every setting of every environment in ONE reduction launch
+      _lib.check(first._lib.bsb_sum_setting_stats(self._handles, len(self.envs), block.data_ptr(), first._stream()))  # pylint: disable=protected-access
+    elif len(self.envs) == 1:
+      first.episode_stat_sums(out=block[0])
     else:                                            # every environment in ONE reduction launch
-      first = self.envs[0]
       _lib.check(first._lib.bsb_sum_episode_stats_many(self._handles, len(self.envs), block.data_ptr(), first._stream()))  # pylint: disable=protected-access
     if self.world == 1:
       if self._cuda:
@@ -143,7 +187,8 @@ class LogPoint:
     return ticket
 
   def result(self, ticket: int, host_sync: bool = False):
-    """`[world, n_envs, 5]` of `ticket` (valid until `slots` further tickets have been issued)."""
+    """`[world, rows, 5]` of `ticket` (valid until `slots` further tickets have been issued); rows are the
+    environments, or their settings with `per_setting`."""
     if not self._issued - self._slots <= ticket < self._issued:
       raise ValueError(f'ticket {ticket} is not in flight (issued {self._issued}, slots {self._slots})')
     slot = ticket % self._slots
@@ -166,14 +211,18 @@ class NativeLogPoint:
   """`LogPoint` without torch.distributed on the data path: the C ABI's own communicator (`bsb_comm_*`, NCCL
   loaded by the library at run time) -- what a non-Python FFI host uses.  The 128-byte NCCL id still has to reach
   every rank once; here it travels through `torch.distributed` if that is initialised (any backend), else pass
-  `unique_id` / `rank` / `world` yourself.  One ticket in flight: `issue()` then `result()`.
+  `unique_id` / `rank` / `world` yourself.  One ticket in flight: `issue()` then `result()`.  `per_setting` and
+  `row_ids` as for `LogPoint` (`bsb_log_point_settings`).
   """
 
-  def __init__(self, envs, unique_id: Optional[bytes] = None, rank: Optional[int] = None, world: Optional[int] = None):
+  def __init__(self, envs, unique_id: Optional[bytes] = None, rank: Optional[int] = None, world: Optional[int] = None,
+               per_setting: bool = False):
     import torch
     import torch.distributed as dist
     self._torch = torch
     self.envs = _distinct(envs)
+    self.per_setting = bool(per_setting)
+    self.row_ids = _row_ids(self.envs, self.per_setting)
     self._device = self.envs[0].device
     if self._device.type != 'cuda':
       raise RuntimeError('NativeLogPoint needs CUDA environments')
@@ -194,18 +243,18 @@ class NativeLogPoint:
     buf = (ctypes.c_uint8 * _lib.COMM_ID_BYTES).from_buffer_copy(unique_id)
     _lib.check(self._lib.bsb_comm_create(buf, rank, world, self._device.index, ctypes.byref(handle)))
     self._comm = handle
-    n = len(self.envs)
+    n = len(self.row_ids)
     self._local = torch.zeros((n, 5), dtype=torch.float64, device=self._device)
     self._gathered = torch.zeros((world, n, 5), dtype=torch.float64, device=self._device)
-    self._handles = (ctypes.c_void_p * n)(*[env._handle.ptr.value for env in self.envs])  # pylint: disable=protected-access
+    self._handles = (ctypes.c_void_p * len(self.envs))(*[env._handle.ptr.value for env in self.envs])  # pylint: disable=protected-access
 
   def issue(self):
     stream = self.envs[0]._stream()  # pylint: disable=protected-access
-    _lib.check(self._lib.bsb_log_point(self._comm, self._handles, len(self.envs), self._local.data_ptr(),
-                                       self._gathered.data_ptr(), stream))
+    call = self._lib.bsb_log_point_settings if self.per_setting else self._lib.bsb_log_point
+    _lib.check(call(self._comm, self._handles, len(self.envs), self._local.data_ptr(), self._gathered.data_ptr(), stream))
 
   def result(self):
-    """`[world, n_envs, 5]`; the caller's current stream is fenced behind the gather (the host does not block)."""
+    """`[world, rows, 5]`; the caller's current stream is fenced behind the gather (the host does not block)."""
     _lib.check(self._lib.bsb_comm_wait(self._comm, self.envs[0]._stream()))  # pylint: disable=protected-access
     return self._gathered
 

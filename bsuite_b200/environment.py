@@ -336,6 +336,7 @@ class BatchedEnvironment:
   bsuite_id = property(lambda self: self._bsuite_id)
   setting_seeds = property(lambda self: None if self._pack is None else self._pack[2])
   lanes_per_setting = property(lambda self: self._batch if self._pack is None else self._pack[3])
+  n_settings = property(lambda self: 1 if self._pack is None else len(self._pack[0]))
 
   def lanes_of(self, bsuite_id: str) -> slice:
     """The slice of the lane axis that holds setting `bsuite_id` of a packed environment."""
@@ -724,19 +725,30 @@ class BatchedEnvironment:
     return dict(columns=_lib.EPISODE_STAT_FIELDS + self._info_names, rows=rows, counts=counts,
                 schedule=np.asarray(self._log_schedule))
 
-  def episode_stat_sums(self, out=None):
+  def episode_stat_sums(self, out=None, per_setting: bool = False):
     """Sums over this environment's lanes of (steps, episode, total_return, episode_len, episode_return): a float64
     tensor [5] on the environment's device, produced by ONE reduction kernel (`bsb_sum_episode_stats`).  `out`
     (contiguous float64 [5] on the same device, e.g. a row of a preallocated log-point block) receives the sums
-    in place, so a log point allocates nothing."""
+    in place, so a log point allocates nothing.
+
+    `per_setting=True`: one row per setting, float64 [n_settings, 5] in `bsuite_ids` order ([1, 5] for an ordinary
+    environment), still one launch (`bsb_sum_setting_stats`).  Row k equals, bit for bit, `episode_stat_sums()` of
+    `load_from_id(bsuite_ids[k], batch=lanes_per_setting, seed=setting_seeds[k], lane_offset=lane_offset,
+    track_episodes=True)` after the same calls.  `out` then takes that shape."""
     if not self._track:
       raise RuntimeError('create the environment with track_episodes=True')
     torch = self._torch
+    shape = (self.n_settings, 5) if per_setting else (5,)
     if out is None:
-      out = torch.empty(5, dtype=torch.float64, device=self._device)
-    elif not (out.dtype is torch.float64 and out.numel() == 5 and out.is_contiguous() and out.device == self._device):
-      raise ValueError('out must be a contiguous float64 tensor of 5 elements on the environment\'s device')
-    _lib.check(self._lib.bsb_sum_episode_stats(self._handle.ptr, out.data_ptr(), self._stream()))
+      out = torch.empty(shape, dtype=torch.float64, device=self._device)
+    elif not (out.dtype is torch.float64 and out.numel() == 5 * (self.n_settings if per_setting else 1) and
+              out.is_contiguous() and out.device == self._device):
+      raise ValueError(f'out must be a contiguous float64 tensor of shape {shape} on the environment\'s device')
+    if per_setting:
+      handles = (ctypes.c_void_p * 1)(self._handle.ptr.value)
+      _lib.check(self._lib.bsb_sum_setting_stats(handles, 1, out.data_ptr(), self._stream()))
+    else:
+      _lib.check(self._lib.bsb_sum_episode_stats(self._handle.ptr, out.data_ptr(), self._stream()))
     return out
 
   # ---- checkpoint ------------------------------------------------------------

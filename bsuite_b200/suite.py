@@ -6,10 +6,16 @@ stream, so the 23 small kernels of a full-sweep step overlap on the GPU instead 
 Across GPUs every id's lanes are sharded evenly (rank r owns lanes [r*lanes/W, (r+1)*lanes/W) of EVERY id), so the
 observation-heavy families (deep_sea, mnist) do not imbalance the ranks; the only collective is the all-gather of
 per-rank return statistics at log points.
+
+`SweepBatch(..., packed=True)` holds one packed environment per experiment instead (`registry.load_experiment`, ragged
+where the settings differ in shape): the full 468-id sweep is 23 handles, a lock-step 23 launches, and a log point
+one per-setting reduction launch whose rows equal, bit for bit, what one handle per id would report.
 """
 
+import ctypes
 from typing import Dict, List, Optional, Sequence
 
+from bsuite_b200 import _lib
 from bsuite_b200 import distributed
 from bsuite_b200 import registry
 from bsuite_b200 import sweep
@@ -25,9 +31,10 @@ def one_per_experiment(setting: int = 0) -> List[str]:
 _STATE_BYTES = {0: 8, 1: 8, 2: 80, 3: 80, 4: 48}
 
 
-def algorithmic_bytes_per_lane_step(env) -> int:
+def algorithmic_bytes_per_lane_step(env, obs_shape=None) -> int:
+  """`obs_shape`: the shape of one setting of a packed environment (default: `env.obs_shape`)."""
   numel = 1
-  for d in env.obs_shape:
+  for d in (env.obs_shape if obs_shape is None else obs_shape):
     numel *= d
   return 4 * numel + 16 + _STATE_BYTES.get(env.family, 16)
 
@@ -46,22 +53,53 @@ class GraphedSweep:
 
 
 class SweepBatch:
+  """Many bsuite_ids advanced in lock-step, `lanes` lanes each (this rank's shard of them).
+
+  `packed=False` (default): `envs` maps each bsuite_id to its own environment.  `packed=True`: the ids (default: all
+  468 of the sweep) are grouped by experiment into one `load_experiment(..., ragged=True)` pack each; `envs` maps
+  experiment name to pack and `pack_of(bsuite_id)` finds a setting's pack.  `rollout`, `capture`, `last_buffers`,
+  the log points and `local_returns` answer per bsuite_id in both modes, with the same values lane for lane; packs
+  are next-step only, so `autoreset='same_step'` raises ValueError."""
 
   def __init__(self, bsuite_ids: Optional[Sequence[str]] = None, lanes: int = 4096, device='cuda', seed: int = 0,
                rank: int = 0, world: int = 1, track_episodes: bool = True, ring: int = 1,
-               autoreset: str = 'next_step', record_rows: bool = False):
+               autoreset: str = 'next_step', record_rows: bool = False, packed: bool = False):
     import torch
     self._torch = torch
-    self.bsuite_ids = list(bsuite_ids) if bsuite_ids is not None else one_per_experiment()
+    self.packed = bool(packed)
+    if bsuite_ids is None:
+      bsuite_ids = sweep.SWEEP if self.packed else one_per_experiment()
+    self.bsuite_ids = list(bsuite_ids)
     first, count = distributed.shard_range(lanes, rank, world)
     self.lanes, self.local_lanes, self.lane_offset = lanes, count, first
-    self.envs = {
-        bsuite_id: registry.load_from_id(bsuite_id, batch=count, device=device, seed=seed, lane_offset=first,
-                                         track_episodes=track_episodes, autoreset=autoreset,
-                                         record_rows=record_rows)
-        for bsuite_id in self.bsuite_ids
-    }
+    if self.packed:
+      if autoreset != 'next_step':
+        raise ValueError("a packed SweepBatch takes autoreset='next_step' only (packs are next-step environments)")
+      if len(set(self.bsuite_ids)) != len(self.bsuite_ids):
+        raise ValueError('bsuite_ids must not repeat an id')
+      groups: Dict[str, List[int]] = {}
+      for bsuite_id in self.bsuite_ids:
+        name, _ = registry.unpack_bsuite_id(bsuite_id)
+        groups.setdefault(name, []).append(sweep.BY_EXPERIMENT[name].index(bsuite_id))
+      self.envs = {
+          name: registry.load_experiment(name, count, settings=settings, device=device, seed=seed, lane_offset=first,
+                                         ragged=True, track_episodes=track_episodes, record_rows=record_rows)
+          for name, settings in groups.items()
+      }
+      self._pack_of = {i: name for name, env in self.envs.items() for i in env.bsuite_ids}
+      # row r of a per-setting reduction over `envs` (pack order, then setting order) -> position in bsuite_ids
+      rows = [i for env in self.envs.values() for i in env.bsuite_ids]
+      self._row_order = torch.tensor([rows.index(i) for i in self.bsuite_ids], dtype=torch.int64)
+    else:
+      self.envs = {
+          bsuite_id: registry.load_from_id(bsuite_id, batch=count, device=device, seed=seed, lane_offset=first,
+                                           track_episodes=track_episodes, autoreset=autoreset,
+                                           record_rows=record_rows)
+          for bsuite_id in self.bsuite_ids
+      }
     self._device = next(iter(self.envs.values())).device
+    if self.packed:
+      self._row_order = self._row_order.to(self._device)
     self._cuda = self._device.type == 'cuda'
     self._streams = {k: torch.cuda.Stream(device=self._device) for k in self.envs} if self._cuda else {}
     self._ring = max(1, int(ring))      # output buffer sets cycled through by successive rollouts (> L2 when timing)
@@ -70,6 +108,13 @@ class SweepBatch:
     self._buffer_steps = None
     self._lp = None
     self._cols = None
+    self._views: Dict[str, object] = {}      # packed: bsuite_id -> per-slot StepBuffers views of its pack's buffers
+
+  def pack_of(self, bsuite_id: str):
+    """The packed environment that holds setting `bsuite_id` (`packed=True`)."""
+    if not self.packed:
+      raise ValueError('pack_of needs SweepBatch(..., packed=True)')
+    return self.envs[self._pack_of[bsuite_id]]
 
   def _ensure_buffers(self, num_steps: int):
     if self._buffer_steps != num_steps:
@@ -77,6 +122,22 @@ class SweepBatch:
       self._buffers = {k: [env.make_buffers(num_steps, with_actions=True) for _ in range(self._ring)]
                        for k, env in self.envs.items()}
       self._buffer_steps = num_steps
+      if self.packed:
+        self._views = {i: [self._setting_view(i, slot) for slot in range(self._ring)] for i in self.bsuite_ids}
+
+  def _setting_view(self, bsuite_id: str, slot: int):
+    """StepBuffers of views (no copies) of setting `bsuite_id`'s lanes in its pack's buffers of `slot`."""
+    from bsuite_b200.environment import StepBuffers  # pylint: disable=import-outside-toplevel
+    env = self.pack_of(bsuite_id)
+    buffers = self._buffers[self._pack_of[bsuite_id]][slot]
+    k, lanes = env.bsuite_ids.index(bsuite_id), env.lanes_of(bsuite_id)
+    return StepBuffers(observation=env.split_observation(buffers.observation)[k], reward=buffers.reward[:, lanes],
+                       discount=buffers.discount[:, lanes], step_type=buffers.step_type[:, lanes],
+                       actions=buffers.actions[:, lanes])
+
+  def _per_id(self, slot: int):
+    """id -> TimeStep of the latest rollout into `slot`, in bsuite_ids order."""
+    return {i: self._views[i][slot].timestep() for i in self.bsuite_ids}
 
   def rollout(self, num_steps: int, action_seed: int = 0):
     """`num_steps` fused steps of every environment (on-device uniform random actions); returns id -> TimeStep.
@@ -92,7 +153,7 @@ class SweepBatch:
     if not self._cuda or len(self.envs) == 1:      # nothing to overlap: stay on the caller's stream
       for k, env in self.envs.items():
         result[k] = env.rollout(num_steps, action_seed=action_seed, out=self._buffers[k][slot])
-      return result
+      return self._per_id(slot) if self.packed else result
     current = torch.cuda.current_stream(self._device)
     for k, env in self.envs.items():
       stream = self._streams[k]
@@ -101,7 +162,7 @@ class SweepBatch:
         result[k] = env.rollout(num_steps, action_seed=action_seed, out=self._buffers[k][slot])
     for stream in self._streams.values():
       current.wait_stream(stream)
-    return result
+    return self._per_id(slot) if self.packed else result
 
   def capture(self, num_steps: int = 1, action_seed: int = 0, lock_steps: int = 1) -> 'GraphedSweep':
     """Records `lock_steps` successive lock-steps of every id (a `num_steps`-step rollout each, on-device actions)
@@ -133,14 +194,20 @@ class SweepBatch:
     self._buffers, self._buffer_steps = {}, None
 
   def last_buffers(self, bsuite_id: str):
-    """The `StepBuffers` (outputs + the actions sampled on the device) the latest rollout of `bsuite_id` wrote."""
-    return self._buffers[bsuite_id][(self._turn - 1) % self._ring]
+    """The `StepBuffers` (outputs + the actions sampled on the device) the latest rollout of `bsuite_id` wrote
+    (packed: views of that setting's lanes)."""
+    slot = (self._turn - 1) % self._ring
+    return self._views[bsuite_id][slot] if self.packed else self._buffers[bsuite_id][slot]
 
   def _log_point(self):
     if self._lp is None:
-      self._lp = distributed.LogPoint(list(self.envs.values()))
+      self._lp = distributed.LogPoint(list(self.envs.values()), per_setting=self.packed)
       self._cols = self._torch.tensor([2, 1, 0], device=self._device)     # (total_return, episode, steps)
     return self._lp
+
+  def _in_id_order(self, rows):
+    """Rows [..., n_rows, 5] of a per-setting reduction, in bsuite_ids order (unpacked rows already are)."""
+    return rows.index_select(-2, self._row_order) if self.packed else rows
 
   def issue_log_point(self) -> int:
     """Asynchronous log point (`distributed.LogPoint`): one reduction kernel per id on the current stream, writing
@@ -149,7 +216,7 @@ class SweepBatch:
 
   def log_point_result(self, ticket: int, host_sync: bool = False):
     """float64 [world, n_ids, 3]: per-rank, per-id sums of (total_return, episode, steps) of `ticket`."""
-    return self._log_point().result(ticket, host_sync=host_sync).index_select(-1, self._cols)
+    return self._in_id_order(self._log_point().result(ticket, host_sync=host_sync)).index_select(-1, self._cols)
 
   def join_log_points(self):
     """Makes the caller's stream wait (on the device) for every log point still in flight."""
@@ -159,10 +226,15 @@ class SweepBatch:
   def local_returns(self):
     """float64 [n_ids, 3] on the device: per-id sums of (total_return, episode, steps) over this rank's lanes."""
     torch = self._torch
-    block = torch.empty((len(self.envs), 5), dtype=torch.float64, device=self._device)
-    for i, env in enumerate(self.envs.values()):
-      env.episode_stat_sums(out=block[i])                     # one reduction kernel per id, written in place
-    return block.index_select(-1, self._log_point() and self._cols)
+    block = torch.empty((len(self.bsuite_ids), 5), dtype=torch.float64, device=self._device)
+    if self.packed:                                           # every setting of every pack in one reduction launch
+      envs = list(self.envs.values())
+      handles = (ctypes.c_void_p * len(envs))(*[env._handle.ptr.value for env in envs])  # pylint: disable=protected-access
+      _lib.check(envs[0]._lib.bsb_sum_setting_stats(handles, len(envs), block.data_ptr(), envs[0]._stream()))  # pylint: disable=protected-access
+    else:
+      for i, env in enumerate(self.envs.values()):
+        env.episode_stat_sums(out=block[i])                   # one reduction kernel per id, written in place
+    return self._in_id_order(block).index_select(-1, self._log_point() and self._cols)
 
   def gather_returns(self):
     """The one collective of the path, synchronous form: returns [world, n_ids, 3] (see `issue_log_point`)."""
@@ -171,6 +243,9 @@ class SweepBatch:
   def bytes_per_step(self) -> int:
     """Algorithmic bytes of one lock-step of the whole local batch (SURVEY.md 8d: dense observation + action +
     reward + discount + step_type + compact lane state read and written)."""
+    if self.packed:                                           # each setting with its own observation shape
+      return sum(env.lanes_per_setting * algorithmic_bytes_per_lane_step(env, shape)
+                 for env in self.envs.values() for shape in env.obs_shapes)
     return sum(env.batch * algorithmic_bytes_per_lane_step(env) for env in self.envs.values())
 
   def close(self):

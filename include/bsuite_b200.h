@@ -420,7 +420,7 @@ int32_t bsb_read_episode_stats(bsb_env* env, int32_t field, double* dst,
 
 /*
  * CUDA graphs.  bsb_step / bsb_reset / bsb_rollout / the masked calls (bsb_reset_masked / bsb_step_masked /
- * bsb_rollout_masked) / bsb_read_* / bsb_sum_episode_stats may be called on a stream
+ * bsb_rollout_masked) / bsb_read_* / bsb_sum_* may be called on a stream
  * that is being captured.  A graph freezes launch arguments, so the first captured launch moves the handle's step
  * counter (it indexes the on-device action stream and the Logging columns) and its chunk scheduler into device
  * memory, for good: replays and eager calls can then be mixed in any order, and bsb_steps_done / bsb_get_state
@@ -445,6 +445,22 @@ int32_t bsb_sum_episode_stats(bsb_env* env, double* dst5, void* stream);
  * path alike (the launch keeps its partial sums in per-handle scratch). */
 int32_t bsb_sum_episode_stats_many(bsb_env* const* envs, int32_t count,
                                    double* dst, void* stream);
+
+/* Per-setting rows of the same reduction: dst receives [rows][5] (steps, episode,
+ * total_return, episode_len, episode_return), rows in handle order and, within a
+ * packed or ragged handle (bsb_create_packed / bsb_create_ragged), in setting
+ * order; an ordinary handle gives one row, equal to bsb_sum_episode_stats.
+ * Row k of a pack of L lanes per setting sums lanes [k*L, (k+1)*L) in the order a
+ * standalone L-lane handle sums its own, so it equals, bit for bit,
+ * bsb_sum_episode_stats of a standalone handle of that setting (its seed, L lanes,
+ * the pack's lane_offset) after the same calls -- on the device and on the host
+ * path alike.  Up to 64 handles (and every setting in them) take ONE launch; a
+ * longer list takes one launch per handle.  Every setting has its own partials and
+ * ticket, allocated with the handle.  Refusals as for bsb_sum_episode_stats_many.
+ * May be captured in a CUDA graph; graph-safe handles read their step counter on
+ * the device. */
+int32_t bsb_sum_setting_stats(bsb_env* const* envs, int32_t count,
+                              double* dst, void* stream);
 
 /*
  * Per-lane log rows (see bsb_config.log_schedule): row k of lane i holds the
@@ -665,6 +681,10 @@ int32_t bsb_comm_destroy(bsb_comm* comm);
 int32_t bsb_comm_world(const bsb_comm* comm, int32_t* rank, int32_t* world);
 int32_t bsb_log_point(bsb_comm* comm, bsb_env* const* envs, int32_t count,
                       double* local, double* gathered, void* stream);
+/* bsb_log_point over the rows of bsb_sum_setting_stats: local [rows][5],
+ * gathered [world][rows][5]. */
+int32_t bsb_log_point_settings(bsb_comm* comm, bsb_env* const* envs, int32_t count,
+                               double* local, double* gathered, void* stream);
 int32_t bsb_comm_wait(bsb_comm* comm, void* stream);
 
 /* Number of kernels this library has launched in this process (bench evidence). */
