@@ -48,7 +48,7 @@ def blob_sections(env):
   mt = env._rng_kind == _lib.RNG_MT19937                            # pylint: disable=protected-access
   order = [('steps_done', np.int64, ()), ('st_word', np.uint32, (B,))]
   if fam == _lib.MEMORY_CHAIN:
-    order.append(('st_ctx', np.uint32, (B,)))
+    order.append(('st_ctx', np.uint64, (B,)))
   if fam in (_lib.CARTPOLE, _lib.CARTPOLE_SWINGUP):
     order.append(('st_f64', np.float64, (6, B)))
   if fam == _lib.MOUNTAIN_CAR:
