@@ -146,6 +146,9 @@ EXPORTS = {
     'bsb_set_state': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p]),
     'bsb_step_host': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Outputs), ctypes.c_void_p,
                                        ctypes.c_void_p, ctypes.c_uint32]),
+    'bsb_step_host_masked': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                              ctypes.POINTER(Outputs), ctypes.c_void_p, ctypes.c_void_p,
+                                              ctypes.c_uint32]),
     'bsb_host_flush': (ctypes.c_int32, [ctypes.c_void_p]),
     'bsb_host_wait': (ctypes.c_int32, [ctypes.c_void_p]),
     'bsb_host_timing': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p]),

@@ -335,11 +335,13 @@ int run_variant(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoP
   });
 }
 
-// Masked calls of variant V (bsb_reset_masked / bsb_step_masked / bsb_rollout_masked): the host path, or one launch of
-// masked_kernel with one chunk of 32 lanes per warp.  A call with nothing for the T loop, the action stream or the
-// budgets to do (every masked reset and step) takes the kOneCall instantiation.
+// Masked calls of variant V (bsb_reset_masked / bsb_step_masked / bsb_rollout_masked / bsb_step_host_masked): the host
+// path, or one launch of masked_kernel with one chunk of 32 lanes per warp.  A masked host step (a launch that
+// carries the mailbox, or a `mask_out` to clear spent lanes in) takes the CALL_HOST instantiation; any other call with
+// nothing for the T loop, the action stream or the budgets to do (every masked reset and step) takes CALL_ONE.
 template <class V>
-int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* episodes_left, cudaStream_t stream) {
+int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* episodes_left, uint8_t* mask_out,
+               cudaStream_t stream) {
   constexpr bool kMt = Compiled<V>::kMt;
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
   if (e->device < 0) { run_host<V>(e, a, mask, episodes_left); return BSB_OK; }
@@ -348,6 +350,7 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
   m.noise = e->p.wrapper == BSB_WRAP_REWARD_NOISE ? 1 : 0;
   m.track = e->p.ep != nullptr ? 1 : 0;
   m.episodes_left = episodes_left;
+  m.mask_out = mask_out;
   LaunchArgs la = a;
   la.bad_action = e->bad_action_dev;
   la.use_pdl = 0;
@@ -357,13 +360,19 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
   g.smem = 0;
   g.n_chunks = launch_chunks(e, V::kRagged, 32);
   g.grid = (g.n_chunks + g.threads / 32 - 1) / (g.threads / 32);
+  const bool host_call = a.mailbox || mask_out;
   const bool one_call = a.T == 1 && !episodes_left && !a.actions_out && (a.mode != MODE_STEP || a.actions);
-  auto go = [&](auto one) {
-    constexpr bool kOneCall = decltype(one)::value;
-    if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_kernel<V, 1, kOneCall>, e->p, la, m); }
-    return launch(e, la, g, stream, masked_kernel<V, 0, kOneCall>, e->p, la, m);
+  auto go = [&](auto kind) {
+    constexpr int kCall = decltype(kind)::value;
+    if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_kernel<V, 1, kCall>, e->p, la, m); }
+    return launch(e, la, g, stream, masked_kernel<V, 0, kCall>, e->p, la, m);
   };
-  return one_call ? go(std::true_type()) : go(std::false_type());
+  if (host_call) {
+    if (a.T != 1 || a.mode != MODE_STEP || !a.actions || a.actions_out)
+      return fail(BSB_INTERNAL, "a masked host step must be one step of the caller's actions");
+    return go(std::integral_constant<int, CALL_HOST>());
+  }
+  return one_call ? go(std::integral_constant<int, CALL_ONE>()) : go(std::integral_constant<int, CALL_ROLLOUT>());
 }
 
 }  // namespace bsb

@@ -83,10 +83,10 @@ template <class T> int env_alloc_t(bsb_env* e, T** out, size_t count, bool snaps
   return rc;
 }
 
-// `two_phase`: a two-phase host step (mailbox_launch; deep_sea and catch only).  `mask`: a masked call or rollout
-// (`episodes_left`: a rollout's budgets, nullable).
+// `two_phase`: a two-phase host step (mailbox_launch; deep_sea and catch only).  `mask`: a masked call, rollout or
+// host step (`episodes_left`: the budgets, nullable; `mask_out`: a budgeted host step's mask write-back, nullable).
 int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr,
-        const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr) {
+        const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr) {
   DeviceGuard guard(e->device);
   LaunchArgs a = args;
   if (e->device >= 0) {
@@ -95,7 +95,7 @@ int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseA
     if (capture != cudaStreamCaptureStatusNone) e->graph_safe = true;
     if (e->graph_safe) a.clock = e->clock;      // a.step0 == e->steps_done, which no longer moves
   }
-  if (mask) return e->variant->run_masked(e, a, mask, episodes_left, stream);
+  if (mask) return e->variant->run_masked(e, a, mask, episodes_left, mask_out, stream);
   return e->variant->run(e, a, stream, two_phase);
 }
 
@@ -274,11 +274,14 @@ bool scalars_back_to_back(const bsb_outputs& out, size_t B) {
 }
 
 // Enqueues the step of `actions` into the device-addressable buffers `out`, which signals `ticket` through the
-// mailbox.
-int mailbox_launch(bsb_env* e, unsigned long long ticket, const int32_t* actions, const bsb_outputs& out) {
+// mailbox.  `mask` (a masked host step; `episodes_left` and `mask_out` nullable): one masked_kernel launch, whose
+// observations are written when it signals, so it never takes the two-phase kernel.
+int mailbox_launch(bsb_env* e, unsigned long long ticket, const int32_t* actions, const bsb_outputs& out,
+                   const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr) {
   LaunchArgs a = make_args(e, &out, actions, 1, MODE_STEP);
   a.mailbox = e->mailbox_dev; a.mail = e->mail; a.ticket = ticket;
   { static const int timing = getenv("BSB_HOST_TIMING") ? atoi(getenv("BSB_HOST_TIMING")) : 0; a.timing = timing; }
+  if (mask) return run(e, a, e->copy_stream, nullptr, mask, episodes_left, mask_out);
   if (!family_obs_from_state(e)) return run(e, a, e->copy_stream);
   { int src = alloc_scalar_staging(e, true); if (src != BSB_OK) return src; }
   TwoPhaseArgs h;
@@ -340,6 +343,7 @@ void destroy_env(bsb_env* e) {
     if (e->d_reward) cudaFree(e->d_reward);      // also owns d_discount / d_step_type
     if (e->d_reward64) cudaFree(e->d_reward64);
     if (e->d_obs) cudaFree(e->d_obs);
+    if (e->d_mask) cudaFree(e->d_mask);
     if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
     if (e->order_event) cudaEventDestroy(e->order_event);
     if (e->fence_event) cudaEventDestroy(e->fence_event);
@@ -492,6 +496,7 @@ static int32_t create_env(const bsb_config* config, int64_t batch, int32_t devic
   e->h2d_stream = nullptr; e->h2d_event = nullptr;
   e->early_inflight = false;
   e->h2d_actions = nullptr; e->d_reward = nullptr; e->d_reward64 = nullptr; e->d_discount = nullptr; e->d_step_type = nullptr; e->d_obs = nullptr;
+  e->d_mask = nullptr;
   e->copy_stream = nullptr;
   DeviceGuard guard(device);
 
@@ -843,12 +848,13 @@ int32_t bsb_step(bsb_env* env, const int32_t* actions, const bsb_outputs* out, v
   return rc;
 }
 
-// bsb_reset_masked / bsb_step_masked / bsb_rollout_masked: lane i makes the calls only where mask[i] != 0
-// (run_masked), a rollout's lanes only while their budgets last.  Host handles validate the actions of masked-in
-// lanes only, at every step of a rollout: an inactive lane's action is never read.
+// bsb_reset_masked / bsb_step_masked / bsb_rollout_masked / bsb_step_host_masked: lane i makes the calls only where
+// mask[i] != 0 (run_masked), a rollout's or host step's lanes only while their budgets last.  Host handles validate
+// the actions of masked-in lanes only, at every step of a rollout (a host step: of lanes with budget left): an
+// inactive lane's action is never read.  `mask_out`: a budgeted host step's write-back (run_masked).
 static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask, const bsb_outputs* out, void* stream,
                        int mode, int64_t T = 1, bool rollout = false, uint64_t action_seed = 0,
-                       int32_t* actions_out = nullptr, int64_t* episodes_left = nullptr) {
+                       int32_t* actions_out = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr) {
   { int crc = check_final_observation(env, out); if (crc != BSB_OK) return crc; }
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
   if (env->device < 0 && mode == MODE_STEP && actions) {
@@ -856,14 +862,14 @@ static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask
     const int64_t B = env->p.batch;
     for (int64_t t = 0; t < T; ++t)
       for (int64_t k = 0; k < B; ++k)
-        if (mask[k] && (uint32_t)actions[t * B + k] >= n)
+        if (mask[k] && (rollout || !episodes_left || episodes_left[k] > 0) && (uint32_t)actions[t * B + k] >= n)
           return fail(BSB_INVALID_ARGUMENT, "action " + std::to_string(actions[t * B + k]) + " of active lane " +
                                                 std::to_string(k) + (rollout ? " at step " + std::to_string(t) : "") +
                                                 " is outside [0, " + std::to_string(n) + ")");
   }
   LaunchArgs a = make_args(env, out, mode == MODE_STEP ? actions : nullptr, T, mode);
   a.action_seed = action_seed; a.actions_out = actions_out;
-  int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask, episodes_left);
+  int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask, episodes_left, mask_out);
   if (rc == BSB_OK) advance_steps(env, T);
   return rc;
 }
@@ -1163,13 +1169,22 @@ static int report_bad_actions(bsb_env* env) {
   return BSB_OK;
 }
 
-int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* host_out, float* device_obs,
-                      void* caller_stream, uint32_t flags) {
+// bsb_step_host (mask null) and bsb_step_host_masked.  A masked step is masked_call's step on the caller's host
+// buffers: zero-copy with the mailbox when they are pinned, staged otherwise; with `episodes_left`, a lane whose budget
+// is spent after the step has its mask byte cleared (run_masked's `mask_out`, or the loop below on host handles).
+static int32_t host_step(bsb_env* env, const int32_t* actions, uint8_t* mask, int64_t* episodes_left,
+                         const bsb_outputs* host_out, float* device_obs, void* caller_stream, uint32_t flags) {
   if (!env || !actions || !host_out) return fail(BSB_INVALID_ARGUMENT, "null argument");
-  if (host_out->final_observation) return fail(BSB_UNSUPPORTED, "bsb_step_host does not deliver final_observation");
+  const std::string name = mask ? "bsb_step_host_masked" : "bsb_step_host";
+  if (host_out->final_observation) return fail(BSB_UNSUPPORTED, name + " does not deliver final_observation");
   if (env->device < 0) {
     if (!host_out->observation) return fail(BSB_INVALID_ARGUMENT, "a host environment writes observations to host_out->observation");
-    return bsb_step(env, actions, host_out, nullptr);
+    if (!mask) return bsb_step(env, actions, host_out, nullptr);
+    const int rc = masked_call(env, actions, mask, host_out, nullptr, MODE_STEP, 1, false, 0, nullptr, episodes_left);
+    if (rc == BSB_OK && episodes_left)
+      for (int64_t k = 0; k < env->p.batch; ++k)
+        if (mask[k] && episodes_left[k] <= 0) mask[k] = 0;
+    return rc;
   }
   if (!host_out->observation && !device_obs) return fail(BSB_INVALID_ARGUMENT, "need host_out->observation or device_obs");
   if ((flags & BSB_HOST_NO_WAIT) && (flags & BSB_HOST_PRELAUNCH)) return fail(BSB_INVALID_ARGUMENT, "BSB_HOST_NO_WAIT and BSB_HOST_PRELAUNCH exclude each other");
@@ -1190,8 +1205,10 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
   // Zero-copy path: when the caller's action and scalar buffers are PINNED host memory (device-addressable under
   // unified addressing), the transition kernel reads the actions from and writes reward / discount / step_type to
   // host memory directly over PCIe -- 1 MB per step, overlapped with the observation stream -- instead of three
-  // separate copies with their launch and DMA latencies before and after the kernel.
+  // separate copies with their launch and DMA latencies before and after the kernel.  A masked step also reads (and
+  // writes back) the mask there.
   void* d_actions = mapped_device_pointer(env, actions);
+  uint8_t* d_mask = mask ? static_cast<uint8_t*>(mapped_device_pointer(env, mask)) : nullptr;
   void* d_reward = host_out->reward ? mapped_device_pointer(env, host_out->reward) : nullptr;
   void* d_reward64 = host_out->reward_f64 ? mapped_device_pointer(env, host_out->reward_f64) : nullptr;
   void *d_discount = nullptr, *d_step_type = nullptr;
@@ -1202,8 +1219,9 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
     d_discount = host_out->discount ? mapped_device_pointer(env, host_out->discount) : nullptr;
     d_step_type = host_out->step_type ? mapped_device_pointer(env, host_out->step_type) : nullptr;
   }
-  const bool all_mapped = d_actions && (!host_out->reward || d_reward) && (!host_out->reward_f64 || d_reward64) &&
-                          (!host_out->discount || d_discount) && (!host_out->step_type || d_step_type);
+  const bool all_mapped = d_actions && (!mask || d_mask) && (!host_out->reward || d_reward) &&
+                          (!host_out->reward_f64 || d_reward64) && (!host_out->discount || d_discount) &&
+                          (!host_out->step_type || d_step_type);
   if (all_mapped) {
     if (!device_obs && !env->d_obs) BSB_CUDA(cudaMalloc(&env->d_obs, obs_bytes));
     bsb_outputs dev;
@@ -1215,13 +1233,15 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
     dev.final_observation = nullptr;
     const int32_t* dev_actions = static_cast<const int32_t*>(d_actions);
     cudaStream_t zs = env->copy_stream;
+    uint8_t* mask_out = episodes_left ? d_mask : nullptr;
     // Completion through the mailbox: the kernel's last CTA stores the ticket into pinned host memory after a
     // system-scope fence and the host spins on that word -- a stream synchronise costs a wake-up per step.
     // Observations copied to the host, graph-safe handles and unaligned observation buffers keep the synchronise.
     const bool spin = !env->graph_safe && !host_out->observation && reinterpret_cast<uintptr_t>(dev.observation) % 16 == 0;
     if (!spin) {
       { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
-      int zrc = bsb_step(env, dev_actions, &dev, zs);
+      int zrc = mask ? masked_call(env, dev_actions, d_mask, &dev, zs, MODE_STEP, 1, false, 0, nullptr, episodes_left, mask_out)
+                     : bsb_step(env, dev_actions, &dev, zs);
       if (zrc != BSB_OK) return zrc;
       if (host_out->observation) BSB_CUDA(cudaMemcpyAsync(host_out->observation, dev.observation, obs_bytes, cudaMemcpyDeviceToHost, zs));
       BSB_CUDA(cudaStreamSynchronize(zs));
@@ -1229,7 +1249,7 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
     }
     { int mrc = mailbox_open(env); if (mrc != BSB_OK) return mrc; }
     const unsigned long long ticket = ++env->next_ticket;
-    if (family_obs_from_state(env)) {
+    if (!mask && family_obs_from_state(env)) {
       // Two-phase step: phase 1 (the transitions of every lane) is all that stands between this launch and the
       // observation stream, and reading 4 B per lane over PCIe from inside the kernel is most of it.  The DMA
       // engine brings the actions over NOW, on a side stream, while the previous step's kernel is still
@@ -1245,7 +1265,7 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
       BSB_CUDA(cudaStreamWaitEvent(zs, env->h2d_event, 0));
       dev_actions = env->h2d_actions;
     }
-    { int lrc = mailbox_launch(env, ticket, dev_actions, dev); if (lrc != BSB_OK) return lrc; }
+    { int lrc = mailbox_launch(env, ticket, dev_actions, dev, d_mask, episodes_left, mask_out); if (lrc != BSB_OK) return lrc; }
     if ((flags & BSB_HOST_FENCE_CALLER) && env->early_inflight) {
       // Two-phase step: the observation stores outlive this call.  Fence the caller's stream behind the kernel:
       // whatever the caller enqueues there afterwards sees complete observations.
@@ -1263,12 +1283,15 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
     env->steps_done += 1;
     return report_bad_actions(env);
   }
-  // Staged copies (a pageable buffer among them): actions in, bsb_step on device scratch, scalars out.
+  // Staged copies (a pageable buffer among them): actions in, bsb_step on device scratch, scalars out.  A masked step
+  // also takes the mask in (and back, with budgets) and the scalars in first, so that the entries of inactive lanes
+  // come back as they were; its actions are clamped and reported as on the zero-copy path.
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
   if (!env->h2d_actions) BSB_CUDA(cudaMalloc(&env->h2d_actions, B * 4));
   { int src = alloc_scalar_staging(env, host_out->reward_f64 != nullptr); if (src != BSB_OK) return src; }
   if (!device_obs && !env->d_obs) BSB_CUDA(cudaMalloc(&env->d_obs, obs_bytes));
-  { int vrc = check_host_actions(env, actions, (int64_t)B); if (vrc != BSB_OK) return vrc; }
+  if (mask && !env->d_mask) BSB_CUDA(cudaMalloc(&env->d_mask, B));
+  if (!mask) { int vrc = check_host_actions(env, actions, (int64_t)B); if (vrc != BSB_OK) return vrc; }
   cudaStream_t s = env->copy_stream;
   BSB_CUDA(cudaMemcpyAsync(env->h2d_actions, actions, B * 4, cudaMemcpyHostToDevice, s));
   bsb_outputs dev;
@@ -1278,9 +1301,25 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
   dev.reward_f64 = host_out->reward_f64 ? env->d_reward64 : nullptr;
   dev.discount = host_out->discount ? env->d_discount : nullptr;
   dev.step_type = host_out->step_type ? env->d_step_type : nullptr;
-  int rc = bsb_step(env, env->h2d_actions, &dev, s);
+  const bool b2b = scalars_back_to_back(*host_out, B);
+  int rc;
+  if (mask) {
+    BSB_CUDA(cudaMemcpyAsync(env->d_mask, mask, B, cudaMemcpyHostToDevice, s));
+    if (b2b) {
+      BSB_CUDA(cudaMemcpyAsync(env->d_reward, host_out->reward, 3 * B * 4, cudaMemcpyHostToDevice, s));
+    } else {
+      if (host_out->reward) BSB_CUDA(cudaMemcpyAsync(dev.reward, host_out->reward, B * 4, cudaMemcpyHostToDevice, s));
+      if (host_out->discount) BSB_CUDA(cudaMemcpyAsync(dev.discount, host_out->discount, B * 4, cudaMemcpyHostToDevice, s));
+      if (host_out->step_type) BSB_CUDA(cudaMemcpyAsync(dev.step_type, host_out->step_type, B * 4, cudaMemcpyHostToDevice, s));
+    }
+    if (host_out->reward_f64) BSB_CUDA(cudaMemcpyAsync(dev.reward_f64, host_out->reward_f64, B * 8, cudaMemcpyHostToDevice, s));
+    rc = masked_call(env, env->h2d_actions, env->d_mask, &dev, s, MODE_STEP, 1, false, 0, nullptr, episodes_left,
+                     episodes_left ? env->d_mask : nullptr);
+  } else {
+    rc = bsb_step(env, env->h2d_actions, &dev, s);
+  }
   if (rc != BSB_OK) return rc;
-  if (scalars_back_to_back(*host_out, B)) {
+  if (b2b) {
     BSB_CUDA(cudaMemcpyAsync(host_out->reward, env->d_reward, 3 * B * 4, cudaMemcpyDeviceToHost, s));
   } else {
     if (host_out->reward) BSB_CUDA(cudaMemcpyAsync(host_out->reward, dev.reward, B * 4, cudaMemcpyDeviceToHost, s));
@@ -1289,8 +1328,20 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* h
   }
   if (host_out->reward_f64) BSB_CUDA(cudaMemcpyAsync(host_out->reward_f64, dev.reward_f64, B * 8, cudaMemcpyDeviceToHost, s));
   if (host_out->observation) BSB_CUDA(cudaMemcpyAsync(host_out->observation, dev.observation, obs_bytes, cudaMemcpyDeviceToHost, s));
+  if (mask && episodes_left) BSB_CUDA(cudaMemcpyAsync(mask, env->d_mask, B, cudaMemcpyDeviceToHost, s));
   BSB_CUDA(cudaStreamSynchronize(s));
-  return BSB_OK;
+  return mask ? report_bad_actions(env) : BSB_OK;
+}
+
+int32_t bsb_step_host(bsb_env* env, const int32_t* actions, const bsb_outputs* host_out, float* device_obs,
+                      void* caller_stream, uint32_t flags) {
+  return host_step(env, actions, nullptr, nullptr, host_out, device_obs, caller_stream, flags);
+}
+
+int32_t bsb_step_host_masked(bsb_env* env, const int32_t* actions, uint8_t* mask, int64_t* episodes_left,
+                             const bsb_outputs* host_out, float* device_obs, void* caller_stream, uint32_t flags) {
+  if (env && !mask) return fail(BSB_INVALID_ARGUMENT, "bsb_step_host_masked needs a mask");
+  return host_step(env, actions, mask, episodes_left, host_out, device_obs, caller_stream, flags);
 }
 
 

@@ -26,15 +26,17 @@ int drain_log_rows(bsb_env* e);                         // waits out host steps 
 // Kernels and host path of kernel variant V (bsb_dispatch.cuh), explicitly instantiated for each entry of the variant
 // list (BSB_VARIANTS) in the translation unit the list gives it (bsb_variants.cu).  `two_phase`: a two-phase host step.
 template <class V> int run_variant(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs* two_phase);
-// Masked calls of variant V (bsb_reset_masked / bsb_step_masked / bsb_rollout_masked): `mask` [B] and `episodes_left`
-// [B] (nullable) live where the handle's state does.
-template <class V> int run_masked(bsb_env*, const LaunchArgs&, const uint8_t* mask, int64_t* episodes_left, cudaStream_t);
+// Masked calls of variant V (bsb_reset_masked / bsb_step_masked / bsb_rollout_masked / bsb_step_host_masked): `mask`
+// [B] and `episodes_left` [B] (nullable) live where the handle's state does, or `mask` is a pinned host buffer's
+// device alias.  `mask_out` (masked host steps with budgets, else null): where spent lanes' mask bytes are cleared.
+template <class V> int run_masked(bsb_env*, const LaunchArgs&, const uint8_t* mask, int64_t* episodes_left,
+                                  uint8_t* mask_out, cudaStream_t);
 // An entry of the variant list, as bsb_create looks it up (bsb_engine.cu).
 struct VariantEntry {
   int family, obs_dtype, mode;
   bool mt, two_phase;
   int (*run)(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs*);
-  int (*run_masked)(bsb_env*, const LaunchArgs&, const uint8_t*, int64_t*, cudaStream_t);
+  int (*run_masked)(bsb_env*, const LaunchArgs&, const uint8_t*, int64_t*, uint8_t*, cudaStream_t);
 };
 
 #define BSB_CUDA(expr)                                                                   \
@@ -80,6 +82,7 @@ struct bsb_env {
   std::vector<std::pair<void*, size_t> > state_blocks;  // snapshot layout
   // bsb_step_host scratch (device)
   int32_t* h2d_actions; float* d_reward; double* d_reward64; float* d_discount; int32_t* d_step_type; float* d_obs;
+  uint8_t* d_mask;                    // bsb_step_host_masked on a pageable mask: its device staging
   cudaStream_t copy_stream;
   cudaEvent_t order_event;            // BSB_HOST_ORDER_AFTER_STREAM: fences copy_stream behind the caller's stream
   cudaEvent_t fence_event;            // BSB_HOST_FENCE_CALLER: fences the caller's stream behind a two-phase host step

@@ -1480,10 +1480,17 @@ two_phase_host_kernel(const EnvParams p, const LaunchArgs a, const TwoPhaseArgs 
 // entries is written.  Noise and Logging are runtime flags here (lane_open / lane_step take them as arguments), so
 // each variant compiles one masked kernel per bit source.
 struct MaskArgs {
-  const uint8_t* mask;      // [B], device memory
+  const uint8_t* mask;      // [B], device memory (host steps: pinned host memory's device alias, or device staging)
   int32_t noise, track;     // the RewardNoise stream is live / the Logging accumulators are tracked
-  int64_t* episodes_left;   // masked rollouts: [B] episode budgets, counted down at each LAST (nullable)
+  int64_t* episodes_left;   // masked rollouts and host steps: [B] episode budgets, counted down at each LAST (nullable)
+  uint8_t* mask_out;        // host steps with budgets: mask[i] is cleared here once lane i's budget is spent (null
+                            // for every other call)
 };
+
+// What one masked_kernel instantiation runs.  CALL_ROLLOUT: bsb_rollout_masked (T steps, sampled or given actions,
+// budgets, actions_out).  CALL_ONE: a masked reset or step (T = 1, the caller's actions, no budgets).  CALL_HOST:
+// bsb_step_host_masked (T = 1, the caller's actions, optional budgets, the mask write-back, the mailbox signal).
+enum CallKind { CALL_ROLLOUT = 0, CALL_ONE = 1, CALL_HOST = 2 };
 
 // Writes lane j's observation `val(e)` (element e of K) with the whole warp: 16-byte streaming stores when `vec`
 // (the row starts 16-byte aligned and is a whole number of 16-byte words), else one element per store.
@@ -1539,11 +1546,16 @@ __device__ __forceinline__ void emit_lane_subset(const EnvParams& lp, const type
 // them, and the calls it sits out all come after its last active one (lane_sit_out_calls, once, after lane_close).  A
 // warp whose lanes are all inactive stops stepping.  Graph-safe mode reads the call index from the device clock and
 // advances it by T, as transition_kernel does; the mask and the budgets are read (and the budgets written) at every
-// launch, so a graph replays with whatever the mask buffer holds and keeps counting the budgets down.  kOneCall: a
-// masked reset or step (T = 1, the caller's actions, no budgets, no actions_out), for which the T loop, the action
-// stream and the budget compile out; with them live, masked steps of catch and cartpole took 11-21 % longer.
-template <class V, int RK, bool kOneCall>
+// launch, so a graph replays with whatever the mask buffer holds and keeps counting the budgets down.  kCall ==
+// CALL_ONE: a masked reset or step (T = 1, the caller's actions, no budgets, no actions_out), for which the T loop,
+// the action stream and the budget compile out; with them live, masked steps of catch and cartpole took 11-21 %
+// longer.  kCall == CALL_HOST: a masked host step, CALL_ONE with the budgets kept, mask[i] cleared in m.mask_out for
+// a budgeted lane whose budget is spent after the step, and completion signalled through the mailbox when the launch
+// carries one.  No store here is a bulk store, so once every thread has fenced (signal_done) the observations are
+// written too: a masked host step is always single-phase.
+template <class V, int RK, int kCall>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(const EnvParams p, const LaunchArgs a, const MaskArgs m) {
+  constexpr bool kOneCall = kCall != CALL_ROLLOUT;      // one call: T = 1 and the caller's actions
   typedef typename V::Fam Fam;
   typedef typename V::Obs O;
   typedef typename RngOf<RK>::type R;
@@ -1558,7 +1570,7 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(c
   const int64_t n_chunks = (V::kRagged ? table->pack.n_settings : 1) * per_setting;
   const int64_t chunk = (int64_t)blockIdx.x * warps_per_cta + warp;
   const int64_t T = kOneCall ? 1 : a.T;
-  int64_t* const budgets = kOneCall ? nullptr : m.episodes_left;
+  int64_t* const budgets = kCall == CALL_ONE ? nullptr : m.episodes_left;
 
   if (chunk < n_chunks) {
     const int64_t k = chunk / per_setting;
@@ -1625,8 +1637,11 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(c
     if (opened) lane_close<Fam>(lp, lane, L, rng, wrng, ep, noise, track);
     if (in && track && acted < T) lane_sit_out_calls(p, lane, T - acted);
     if (selected && budgets) budgets[lane] = left;
+    // the host's view of the lanes still running: only a lane whose budget is spent writes its byte
+    if constexpr (kCall == CALL_HOST) { if (selected && budgets && left <= 0 && m.mask_out) m.mask_out[lane] = 0; }
   }
 
+  if constexpr (kCall == CALL_HOST) { if (a.mailbox) signal_done(a); }
   if (a.clock) {        // graph-safe mode: the last CTA advances the call count by T (transition_kernel's epilogue)
     __syncthreads();
     if (threadIdx.x == 0) {

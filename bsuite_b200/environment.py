@@ -432,6 +432,20 @@ class BatchedEnvironment:
     mask = mask.contiguous()
     return mask.view(torch.uint8) if mask.dtype is torch.bool else mask
 
+  def _episodes_left(self, episodes_left):
+    """Checks an `episodes_left` argument: an int64 [B] contiguous tensor on the environment's device."""
+    torch = self._torch
+    if not isinstance(episodes_left, torch.Tensor) or episodes_left.dtype is not torch.int64:
+      raise ValueError(f'episodes_left must be an int64 tensor, got '
+                       f'{getattr(episodes_left, "dtype", type(episodes_left).__name__)}')
+    if tuple(episodes_left.shape) != (self._batch,):
+      raise ValueError(f'episodes_left must have shape ({self._batch},), got {tuple(episodes_left.shape)}')
+    if episodes_left.device != self._device:
+      raise ValueError(f'episodes_left must live on {self._device}, got {episodes_left.device}')
+    if not episodes_left.is_contiguous():
+      raise ValueError('episodes_left must be contiguous: it is updated in place')
+    return episodes_left
+
   def reset(self, out: Optional[StepBuffers] = None, mask=None):
     """base.Environment.reset for every lane (base.py:54-57).
 
@@ -515,7 +529,7 @@ class BatchedEnvironment:
     return StepBuffers(observation=observation, reward=reward, discount=discount, step_type=step_type)
 
   def step_host(self, actions, host: StepBuffers, out: Optional[StepBuffers] = None, prelaunch: bool = False,
-                wait: bool = True):
+                wait: bool = True, mask=None, episodes_left=None):
     """One step driven from HOST memory through `bsb_step_host`: the reference's call pattern, one
     `env.step(action)` per decision (baselines/experiment.py:45-57), for agents whose policy runs on the host.
 
@@ -532,8 +546,30 @@ class BatchedEnvironment:
 
     `wait=False` (pinned buffers, CUDA): returns once the step is enqueued; `host` holds the results after
     `host_wait()`.  `rollouts.HostHalves` uses it to drive two half-batches alternately (`BSB_HOST_NO_WAIT`).
+
+    `mask` (CPU bool or uint8 contiguous tensor [B], ideally pinned: read in place): only the lanes where it is set
+    step (`bsb_step_host_masked`); the others make no call, their actions are never read and their entries of `host`
+    (scalars) and `out.observation` are left as they are.  `episodes_left` (int64 [B] contiguous tensor on the
+    environment's device; needs `mask`): a lane with a mask set steps only while its entry is positive, each LAST
+    takes one from it in place, and `mask` is cleared in place for every lane whose budget is spent after the step
+    (a bool mask is viewed, not copied, so the caller's tensor is updated; with `wait=False`, after `host_wait()`).
+    The call equals `rollout(1, actions, mask=..., episodes_left=...)`.  A masked step always runs in one phase.
     """
     torch = self._torch
+    if episodes_left is not None and mask is None:
+      raise ValueError('episodes_left needs mask=: the lanes whose budgets count down')
+    if mask is not None:
+      if not isinstance(mask, torch.Tensor) or mask.dtype not in (torch.bool, torch.uint8):
+        raise ValueError(f'mask must be a bool or uint8 tensor, got {getattr(mask, "dtype", type(mask).__name__)}')
+      if tuple(mask.shape) != (self._batch,):
+        raise ValueError(f'mask must have shape ({self._batch},), got {tuple(mask.shape)}')
+      if mask.device.type != 'cpu':
+        raise ValueError(f'step_host takes its mask in host memory (a CPU tensor), got {mask.device}')
+      if not mask.is_contiguous():
+        raise ValueError('mask must be contiguous: it is updated in place')
+      mask = mask.view(torch.uint8) if mask.dtype is torch.bool else mask
+      if episodes_left is not None:
+        self._episodes_left(episodes_left)
     if not (type(actions) is torch.Tensor and actions.dtype is torch.int32 and actions.device.type == 'cpu'
             and actions.dim() == 1 and actions.shape[0] == self._batch and actions.is_contiguous()):
       if not isinstance(actions, torch.Tensor):
@@ -562,7 +598,12 @@ class BatchedEnvironment:
       if self._async_work:
         flags |= _lib.HOST_ORDER_AFTER_STREAM
         self._async_work = False
-    status = self._lib.bsb_step_host(self._handle.ptr, actions.data_ptr(), ctypes.byref(houts), dev_obs, stream, flags)
+    if mask is None:
+      status = self._lib.bsb_step_host(self._handle.ptr, actions.data_ptr(), ctypes.byref(houts), dev_obs, stream, flags)
+    else:
+      left_ptr = None if episodes_left is None else episodes_left.data_ptr()
+      status = self._lib.bsb_step_host_masked(self._handle.ptr, actions.data_ptr(), mask.data_ptr(), left_ptr,
+                                              ctypes.byref(houts), dev_obs, stream, flags)
     if status:
       _lib.check(status)
     if self._ordinal < 0 and host.observation is not None:
@@ -607,16 +648,7 @@ class BatchedEnvironment:
     if mask is not None:
       mask = self._mask(mask, out)
       if episodes_left is not None:
-        torch = self._torch
-        if not isinstance(episodes_left, torch.Tensor) or episodes_left.dtype is not torch.int64:
-          raise ValueError(f'episodes_left must be an int64 tensor, got '
-                           f'{getattr(episodes_left, "dtype", type(episodes_left).__name__)}')
-        if tuple(episodes_left.shape) != (self._batch,):
-          raise ValueError(f'episodes_left must have shape ({self._batch},), got {tuple(episodes_left.shape)}')
-        if episodes_left.device != self._device:
-          raise ValueError(f'episodes_left must live on {self._device}, got {episodes_left.device}')
-        if not episodes_left.is_contiguous():
-          raise ValueError('episodes_left must be contiguous: it is updated in place')
+        self._episodes_left(episodes_left)
     out = out or self.make_buffers(num_steps, with_actions=actions is None)
     act_ptr = None
     if actions is not None:

@@ -7,6 +7,8 @@
   * `RandomAgent` -- `bsuite/baselines/random/agent.py:26-45` with one generator call per step for the whole batch.
   * `run_episodes` / `run_random_episodes` -- `experiment.run` to each lane's episode budget, with any agent through
     masked steps, or with the random agent's actions sampled on the device through fused masked rollouts.
+  * `run_host_episodes` / `HostParts.run_episodes` -- the same for a HOST-side policy, through masked host steps
+    (`step_host(..., mask=..., episodes_left=...)`), on one handle or over part-batches.
   * `Trajectory` / `collect` -- the `[T + 1]` observations / `[T]` actions, rewards, discounts layout of
     `bsuite/baselines/utils/sequence.py:26-35`, as device tensors with a lane axis, filled by ONE fused rollout
     (`bsb_rollout`: on-device uniform random actions) instead of T appends.
@@ -156,6 +158,41 @@ def run_random_episodes(environment, num_episodes: Optional[int] = None, action_
   return calls
 
 
+def _start_budgeted(environment, num_episodes, out, host):
+  """Budgets (device), the host mask of the lanes that have episodes to play (pinned on CUDA), and one masked reset of
+  those lanes into `out`, whose scalars are copied into `host` for the first decision."""
+  torch = environment._torch
+  left = episode_budget(environment, num_episodes)
+  running = left > 0
+  mask = torch.empty(environment.batch, dtype=torch.bool, pin_memory=environment.device.type == 'cuda')
+  mask.copy_(running.cpu())
+  environment.reset(out=out, mask=running)
+  for name in ('reward', 'discount', 'step_type'):
+    getattr(host, name).copy_(getattr(out, name))
+  return left, mask
+
+
+def run_host_episodes(policy, environment, num_episodes: Optional[int] = None) -> int:
+  """`run_episodes` for a HOST-side policy through masked `step_host`: every lane plays exactly its episode budget
+  (`episode_budget`) on the host step's fast path (pinned actions, scalars and mask).
+
+  One masked reset of the lanes with a positive budget on the device, then `step_host(..., mask=mask,
+  episodes_left=budgets)` until the pinned mask is empty: each step clears the mask of the lanes whose budget it
+  spent, so `mask` is always the set of lanes still running.  `policy(call, host_timestep, device_observation, mask)
+  -> CPU int32 [B]` (ideally pinned) is asked once per call with the latest timestep (the reset's before the first
+  step); the actions of lanes whose mask is clear are never read.  Per lane, `bsuite_info()`, episode statistics, log
+  rows and scores equal those of `run_episodes` with an agent that makes the same actions; only `steps_done` may
+  differ.  Returns the number of calls made after the reset."""
+  out, host = environment.make_buffers(), environment.make_host_buffers()
+  left, mask = _start_budgeted(environment, num_episodes, out, host)
+  timestep, calls = host.timestep(), 0
+  while bool(mask.any()):
+    actions = policy(calls, timestep, out.observation, mask)
+    timestep, _ = environment.step_host(actions, host, out, mask=mask, episodes_left=left)
+    calls += 1
+  return calls
+
+
 class Replay:
   """Uniform replay of flat item tuples as device tensors (`bsuite/baselines/utils/replay.py:24-88`): a ring of
   `capacity` slots per item, `add(items)` writes one tuple, `sample(size)` returns a list of `[size, ...]` tensors
@@ -286,11 +323,13 @@ class HostParts:
     self.drain()
     return [e.reset(out=o) for e, o in zip(self.envs, self.out)]
 
-  def submit(self, part: int, actions):
-    """Enqueues one step of `part` with `actions` (pinned CPU int32 [sizes[part]]); returns at once."""
+  def submit(self, part: int, actions, mask=None, episodes_left=None):
+    """Enqueues one step of `part` with `actions` (pinned CPU int32 [sizes[part]]); returns at once.  `mask` /
+    `episodes_left`: a masked step (`step_host`); the mask is written back when the step is collected."""
     if self._in_flight[part]:
       raise RuntimeError(f'part {part} already has a step in flight: collect() it first')
-    self.envs[part].step_host(actions, self.host[part], self.out[part], wait=False)
+    self.envs[part].step_host(actions, self.host[part], self.out[part], wait=False, mask=mask,
+                              episodes_left=episodes_left)
     self._in_flight[part] = True
 
   def collect(self, part: int):
@@ -318,6 +357,30 @@ class HostParts:
     for part in range(self.parts):
       last[part] = self.collect(part)[0]
     return last
+
+  def run_episodes(self, policy, num_episodes: Optional[int] = None):
+    """`run_host_episodes` over the parts: one budget tensor and one pinned mask per part, one masked reset each,
+    then masked steps driven round-robin with `wait=False`; a part leaves the rotation when its mask empties.
+    `policy(part, call, host_timestep, device_observation, mask) -> CPU int32 [sizes[part]]` is asked with that
+    part's latest timestep and mask.  Per lane, the result equals one-handle `run_host_episodes` over all `batch`
+    lanes (lane keys continue across parts).  Returns the number of calls made on each part after its reset."""
+    self.drain()
+    budgets = [_start_budgeted(env, num_episodes, out, host) for env, out, host in zip(self.envs, self.out, self.host)]
+    calls = [0] * self.parts
+    rotation = [part for part in range(self.parts) if bool(budgets[part][1].any())]
+    for part in rotation:
+      left, mask = budgets[part]
+      self.submit(part, policy(part, 0, self.host[part].timestep(), self.out[part].observation, mask), mask, left)
+    while rotation:
+      for part in list(rotation):
+        timestep, observation = self.collect(part)
+        calls[part] += 1
+        left, mask = budgets[part]
+        if not bool(mask.any()):
+          rotation.remove(part)
+          continue
+        self.submit(part, policy(part, calls[part], timestep, observation, mask), mask, left)
+    return calls
 
   def close(self):
     self.drain()

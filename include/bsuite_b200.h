@@ -628,6 +628,49 @@ int32_t bsb_step_host(bsb_env* env, const int32_t* actions,
                       const bsb_outputs* host_out, float* device_obs,
                       void* caller_stream, uint32_t flags);
 
+/*
+ * Masked host-driven step: bsb_step_host for a chosen subset of lanes, each
+ * stopping at its own episode budget, so that a host-side agent can play every
+ * lane to exactly its budget on the host step's fast path.  actions, host_out,
+ * device_obs, caller_stream and flags mean what they mean for bsb_step_host
+ * (BSB_HOST_NO_WAIT with bsb_host_wait / bsb_host_flush included; one step in
+ * flight per handle; masked and unmasked host steps may be interleaved).
+ *
+ * mask (uint8 [B], required) lives in HOST memory, like actions: pinned memory
+ * is read in place, pageable memory is staged.  episodes_left (int64 [B],
+ * nullable) lives in the handle's memory space, as for bsb_rollout_masked
+ * (device memory for a CUDA handle: budgets never cross PCIe).  Lane i is
+ * active when mask[i] != 0 and episodes_left is NULL or episodes_left[i] > 0.
+ * The call equals, bit for bit, bsb_rollout_masked(env, 1, actions, 0, mask',
+ * episodes_left, out, NULL) with mask' a device copy of mask taken before the
+ * call (without episodes_left: bsb_step_masked): every output entry written,
+ * lane state, RNG streams, info fields, Logging columns, log rows,
+ * episodes_left, bsb_steps_done (+1) and the invalid-action flag.  Inactive
+ * lanes' entries of host_out's scalars and of device_obs are not written and
+ * their actions are never read.  host_out->observation, when set, receives the
+ * whole device observation buffer after the step.
+ *
+ * Mask write-back: with episodes_left, the call clears mask[i] in place for
+ * every lane whose budget is <= 0 after the step, so that afterwards
+ * mask[i] == old_mask[i] && episodes_left[i] > 0: the host always holds the set
+ * of lanes still running.  Only lanes that just ran out (or whose budget was
+ * already spent) write their byte, before the completion word (with
+ * BSB_HOST_NO_WAIT: read the mask after bsb_host_wait).  Without
+ * episodes_left the mask is only read.
+ *
+ * A masked host step always runs in one phase (its kernel has no bulk stores,
+ * so completion means the observations are written), on deep_sea from size 16
+ * up and catch too.  An out-of-range action of an active lane is refused before
+ * anything moves on a host handle (BSB_INVALID_ARGUMENT); on a CUDA handle it is
+ * clamped and reported after the step (BSB_INVALID_ARGUMENT, or by
+ * bsb_host_wait), as bsb_step_host's zero-copy path does.  Refused:
+ * final_observation (BSB_UNSUPPORTED) and a NULL mask.
+ */
+int32_t bsb_step_host_masked(bsb_env* env, const int32_t* actions,
+                             uint8_t* mask, int64_t* episodes_left,
+                             const bsb_outputs* host_out, float* device_obs,
+                             void* caller_stream, uint32_t flags);
+
 /* Collects a BSB_HOST_NO_WAIT step nobody waited for (no-op otherwise).  Unlike
  * bsb_host_wait it does not report an out-of-range action of that step. */
 int32_t bsb_host_flush(bsb_env* env);
