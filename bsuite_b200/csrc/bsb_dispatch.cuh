@@ -42,7 +42,8 @@ template <> struct HostEmit<Mnist> {
 // and lane j of setting k writes row j of the setting's observation block.  `mask` (masked calls and rollouts): lane i
 // acts only while mask[i] != 0 and its budget episodes_left[i] (when given) is positive; each LAST it returns takes one
 // from the budget, so its active steps are a prefix of the T.  The calls it sits out come after them
-// (lane_sit_out_calls), and their outputs are not written.
+// (lane_sit_out_calls), and their outputs are not written.  No observation buffer (bsb_advance_masked): nothing is
+// rendered, and each observation's random draws are made without it (ObsDraws::skip), as the kernel does.
 template <class V, int RK>
 void host_run(const EnvParams& p, const LaunchArgs& a, const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr) {
   typedef typename V::Fam F;
@@ -75,14 +76,14 @@ void host_run(const EnvParams& p, const LaunchArgs& a, const uint8_t* mask = nul
       continue;
     }
     if constexpr (kPacked) { setting_p = p; pack_lane_params(setting_p, lane); }
-    O* lane_obs = obs + lane * (int64_t)K;      // step 0's observation row of this lane
+    O* lane_obs = obs ? obs + lane * (int64_t)K : nullptr;      // step 0's observation row of this lane
     int64_t step_elems = B * (int64_t)K;
     if constexpr (kRagged) {
       const int64_t k = lane / ragged->pack.lanes_per_setting;
       const RaggedSetting& s = ragged_setting(ragged, k);
       setting_p = p;
       ragged_setting_params(setting_p, s, ragged->mapping_bits);
-      lane_obs = obs + s.obs_offset + (lane - s.lane_shift) * (int64_t)s.obs_numel;
+      if (obs) lane_obs = obs + s.obs_offset + (lane - s.lane_shift) * (int64_t)s.obs_numel;
       step_elems = ragged->step_elems;
     }
     const EnvParams& lp = (kPacked || kRagged) ? setting_p : p;
@@ -107,7 +108,8 @@ void host_run(const EnvParams& p, const LaunchArgs& a, const uint8_t* mask = nul
       }
       lane_step<F, R, kSameStep>(lp, lane, L, rng, wrng, ep, action, a.mode, noise, track, a.step0 + t, out, off, &merged);
       if constexpr (kSameStep) { if (merged.done && fin) render(lp, merged.last, merged.rng, fin + off * (int64_t)K); }
-      render(lp, L, rng, lane_obs + t * step_elems);
+      if (obs) render(lp, L, rng, lane_obs + t * step_elems);
+      else ObsDraws<F>::skip(lp, rng);      // bsb_advance_masked: the observation's draws, not the observation
       ++acted;
       // the step's LAST: a same-step lane's merged reset, else the _reset_next_step flag the step left set
       if (budgeted && (kSameStep ? merged.done : L.nr != 0) && --left == 0) break;
@@ -335,9 +337,10 @@ int run_variant(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoP
   });
 }
 
-// Masked calls of variant V (bsb_reset_masked / bsb_step_masked / bsb_rollout_masked / bsb_step_host_masked): the host
-// path, or one launch of masked_kernel with one chunk of 32 lanes per warp.  A masked host step (a launch that
-// carries the mailbox, or a `mask_out` to clear spent lanes in) takes the CALL_HOST instantiation; any other call with
+// Masked calls of variant V (bsb_reset_masked / bsb_step_masked / bsb_rollout_masked / bsb_step_host_masked /
+// bsb_advance_masked): the host path, or one launch of masked_kernel with one chunk of 32 lanes per warp.  A masked
+// host step (a launch that carries the mailbox, or a `mask_out` to clear spent lanes in) takes the CALL_HOST
+// instantiation; a launch with no observation buffer (bsb_advance_masked) takes CALL_ADVANCE; any other call with
 // nothing for the T loop, the action stream or the budgets to do (every masked reset and step) takes CALL_ONE.
 template <class V>
 int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* episodes_left, uint8_t* mask_out,
@@ -371,6 +374,12 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
     if (a.T != 1 || a.mode != MODE_STEP || !a.actions || a.actions_out)
       return fail(BSB_INTERNAL, "a masked host step must be one step of the caller's actions");
     return go(std::integral_constant<int, CALL_HOST>());
+  }
+  if (!a.obs) {
+    if (a.mode != MODE_STEP || a.actions || a.actions_out || a.final_obs || a.reward || a.reward_f64 || a.discount ||
+        a.step_type)
+      return fail(BSB_INTERNAL, "a launch without observations must be an advance: sampled actions, no outputs");
+    return go(std::integral_constant<int, CALL_ADVANCE>());
   }
   return one_call ? go(std::integral_constant<int, CALL_ONE>()) : go(std::integral_constant<int, CALL_ROLLOUT>());
 }

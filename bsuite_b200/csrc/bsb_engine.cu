@@ -909,6 +909,17 @@ int32_t bsb_rollout_masked(bsb_env* env, int64_t num_steps, const int32_t* actio
   return masked_call(env, actions, mask, out, stream, MODE_STEP, num_steps, true, action_seed, actions_out, episodes_left);
 }
 
+// bsb_rollout_masked of sampled actions with no outputs: a launch without an observation buffer takes masked_kernel's
+// CALL_ADVANCE instantiation (run_masked), and the host path renders nothing.
+int32_t bsb_advance_masked(bsb_env* env, int64_t num_steps, uint64_t action_seed, const uint8_t* mask,
+                           int64_t* episodes_left, void* stream) {
+  if (!env || !mask) return fail(BSB_INVALID_ARGUMENT, "bsb_advance_masked needs a handle and a mask");
+  if (num_steps <= 0) return fail(BSB_INVALID_ARGUMENT, "num_steps must be positive");
+  bsb_outputs none;
+  memset(&none, 0, sizeof(none));
+  return masked_call(env, nullptr, mask, &none, stream, MODE_STEP, num_steps, true, action_seed, nullptr, episodes_left);
+}
+
 int32_t bsb_random_actions(uint64_t action_seed, uint64_t lane_offset, int64_t batch, int64_t first_step,
                            int64_t num_steps, int32_t num_actions, int32_t* out) {
   if (!out || batch <= 0 || num_steps <= 0 || num_actions <= 0) return fail(BSB_INVALID_ARGUMENT, "bad arguments");

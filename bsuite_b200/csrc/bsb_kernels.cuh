@@ -1490,7 +1490,8 @@ struct MaskArgs {
 // What one masked_kernel instantiation runs.  CALL_ROLLOUT: bsb_rollout_masked (T steps, sampled or given actions,
 // budgets, actions_out).  CALL_ONE: a masked reset or step (T = 1, the caller's actions, no budgets).  CALL_HOST:
 // bsb_step_host_masked (T = 1, the caller's actions, optional budgets, the mask write-back, the mailbox signal).
-enum CallKind { CALL_ROLLOUT = 0, CALL_ONE = 1, CALL_HOST = 2 };
+// CALL_ADVANCE: bsb_advance_masked (T steps of sampled actions, optional budgets, no per-step output at all).
+enum CallKind { CALL_ROLLOUT = 0, CALL_ONE = 1, CALL_HOST = 2, CALL_ADVANCE = 3 };
 
 // Writes lane j's observation `val(e)` (element e of K) with the whole warp: 16-byte streaming stores when `vec`
 // (the row starts 16-byte aligned and is a whole number of 16-byte words), else one element per store.
@@ -1552,17 +1553,22 @@ __device__ __forceinline__ void emit_lane_subset(const EnvParams& lp, const type
 // longer.  kCall == CALL_HOST: a masked host step, CALL_ONE with the budgets kept, mask[i] cleared in m.mask_out for
 // a budgeted lane whose budget is spent after the step, and completion signalled through the mailbox when the launch
 // carries one.  No store here is a bulk store, so once every thread has fenced (signal_done) the observations are
-// written too: a masked host step is always single-phase.
+// written too: a masked host step is always single-phase.  kCall == CALL_ADVANCE: CALL_ROLLOUT with sampled actions
+// and every per-step output compiled out (observations, final observations, scalars, actions_out); where an
+// observation would be rendered the lane makes the draws rendering makes (ObsDraws::skip), so its streams end where
+// CALL_ROLLOUT's do.  A same-step final observation is rendered from a copy of the stream and is simply not rendered.
 template <class V, int RK, int kCall>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(const EnvParams p, const LaunchArgs a, const MaskArgs m) {
-  constexpr bool kOneCall = kCall != CALL_ROLLOUT;      // one call: T = 1 and the caller's actions
+  constexpr bool kOneCall = kCall == CALL_ONE || kCall == CALL_HOST;      // one call: T = 1 and the caller's actions
+  constexpr bool kEmit = kCall != CALL_ADVANCE;                           // the call writes per-step outputs
   typedef typename V::Fam Fam;
   typedef typename V::Obs O;
   typedef typename RngOf<RK>::type R;
   const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
   int64_t step0 = a.step0;
   if (a.clock) step0 += (int64_t)*reinterpret_cast<volatile unsigned long long*>(a.clock + 16 * (blockIdx.x % CLOCK_GROUPS));
-  const MailFields out = {a.reward, a.reward_f64, a.discount, a.step_type};
+  const MailFields out = kEmit ? MailFields{a.reward, a.reward_f64, a.discount, a.step_type} : MailFields{};
+  const int32_t mode = kEmit ? a.mode : (int32_t)MODE_STEP;
   const bool noise = m.noise != 0, track = m.track != 0;
   const RaggedTable* table = V::kRagged ? reinterpret_cast<const RaggedTable*>(p.pack) : nullptr;
   const int64_t lanes = V::kRagged ? table->pack.lanes_per_setting : p.batch;      // lanes per setting block
@@ -1600,14 +1606,14 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(c
     Fam::init(p, L);
     MergedReset<Fam, R> merged;            // same-step kernels only
     if constexpr (V::kSameStep) { Fam::init(p, merged.last); merged.done = false; }
-    if (on) lane_open<Fam>(lp, lane, L, rng, wrng, ep, a.mode, noise, track);
+    if (on) lane_open<Fam>(lp, lane, L, rng, wrng, ep, mode, noise, track);
     int64_t acted = 0;                     // the lane's active steps
     for (int64_t t = 0; t < T && (kOneCall || __any_sync(0xffffffffu, on)); ++t) {
       const int64_t off = t * p.batch + lane;
       if (on) {
         int32_t action = 0;
-        if (a.mode == MODE_STEP) {
-          if (kOneCall || a.actions) {
+        if (mode == MODE_STEP) {
+          if (kCall != CALL_ADVANCE && (kOneCall || a.actions)) {
             action = a.actions[off];
             if ((uint32_t)action >= (uint32_t)p.num_actions) {
               if (a.bad_action) *a.bad_action = 1;
@@ -1616,17 +1622,21 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(c
           } else {
             action = action_stream.sample(a.action_seed, lp.lane_offset + (uint64_t)lane, (uint64_t)(step0 + t), p.num_actions);
           }
-          if (!kOneCall && a.actions_out) a.actions_out[off] = action;
+          if (kCall == CALL_ROLLOUT && a.actions_out) a.actions_out[off] = action;
         }
-        if constexpr (V::kSameStep) lane_step<Fam, R, true>(p, lane, L, rng, wrng, ep, action, a.mode, noise, track, step0 + t, out, off, &merged);
-        else lane_step<Fam>(lp, lane, L, rng, wrng, ep, action, a.mode, noise, track, step0 + t, out, off);
+        if constexpr (V::kSameStep) lane_step<Fam, R, true>(p, lane, L, rng, wrng, ep, action, mode, noise, track, step0 + t, out, off, &merged);
+        else lane_step<Fam>(lp, lane, L, rng, wrng, ep, action, mode, noise, track, step0 + t, out, off);
       }
-      if constexpr (V::kSameStep) {
-        if (a.final_obs)
-          emit_lane_subset<Fam>(lp, merged.last, merged.rng, reinterpret_cast<O*>(a.final_obs) + t * p.batch * (int64_t)p.obs_numel,
-                                lp.obs_numel, local_base, on && merged.done, a.final_vec_ok != 0);
+      if constexpr (!kEmit) {
+        if (on) ObsDraws<Fam>::skip(lp, rng);    // the draws of the observation CALL_ROLLOUT would render here
+      } else {
+        if constexpr (V::kSameStep) {
+          if (a.final_obs)
+            emit_lane_subset<Fam>(lp, merged.last, merged.rng, reinterpret_cast<O*>(a.final_obs) + t * p.batch * (int64_t)p.obs_numel,
+                                  lp.obs_numel, local_base, on && merged.done, a.final_vec_ok != 0);
+        }
+        emit_lane_subset<Fam>(lp, L, rng, block + t * step_elems, lp.obs_numel, local_base, on, a.obs_vec_ok != 0);
       }
-      emit_lane_subset<Fam>(lp, L, rng, block + t * step_elems, lp.obs_numel, local_base, on, a.obs_vec_ok != 0);
       if (on) {
         ++acted;
         // the step's LAST: a same-step lane's merged reset, else the _reset_next_step flag the step left set

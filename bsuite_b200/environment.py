@@ -417,10 +417,10 @@ class BatchedEnvironment:
     return actions
 
   # ---- dynamics ------------------------------------------------------------
-  def _mask(self, mask, out):
+  def _mask(self, mask, out, needs_out: bool = True):
     """The uint8 [B] tensor of a `mask` argument on the environment's device (a bool tensor is viewed, not copied)."""
     torch = self._torch
-    if out is None:
+    if needs_out and out is None:
       raise ValueError('a masked call needs out=: the buffers that hold every lane\'s latest timestep (inactive '
                        'lanes leave their entries as they are)')
     if not isinstance(mask, torch.Tensor) or mask.dtype not in (torch.bool, torch.uint8):
@@ -666,6 +666,27 @@ class BatchedEnvironment:
       _lib.check(self._lib.bsb_rollout(self._handle.ptr, num_steps, act_ptr, int(action_seed) & _MASK64,
                                        ctypes.byref(outputs), act_out, self._stream()))
     return out.timestep()
+
+  def advance(self, num_steps: int, action_seed: int = 0, mask=None, episodes_left=None) -> None:
+    """`rollout(num_steps, action_seed=..., mask=..., episodes_left=...)` with on-device random actions and no
+    outputs (`bsb_advance_masked`): the lanes move exactly as that masked rollout moves them -- lane state, RNG
+    streams, `bsuite_info()`, episode statistics, log rows, `episodes_left` and `steps_done` -- but no observation,
+    scalar or action is written anywhere.  For runs whose results are the accumulators, log rows and scores, such as
+    `rollouts.run_random_episodes`.
+
+    `mask` (bool or uint8 tensor [B] on the environment's device; None: every lane) and `episodes_left` (int64 [B]
+    contiguous tensor on the device, counted down in place; None: no budgets) mean what they mean for `rollout`.
+    `num_steps` <= 0 raises `EngineError`."""
+    num_steps = int(num_steps)
+    if mask is None:
+      mask = self._torch.ones(self._batch, dtype=self._torch.uint8, device=self._device)
+    mask = self._mask(mask, None, needs_out=False)
+    if episodes_left is not None:
+      self._episodes_left(episodes_left)
+    self._async_work = True
+    left_ptr = ctypes.c_void_p(episodes_left.data_ptr()) if episodes_left is not None else None
+    _lib.check(self._lib.bsb_advance_masked(self._handle.ptr, num_steps, int(action_seed) & _MASK64,
+                                            ctypes.c_void_p(mask.data_ptr()), left_ptr, self._stream()))
 
   def capture(self, num_steps: int = 1, sample_actions: bool = False, fused: bool = False,
               action_seed: int = 0, final_observation: bool = False) -> GraphedSteps:

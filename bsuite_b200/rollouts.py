@@ -6,7 +6,8 @@
     runs unchanged on the B = 1 face (`DmEnvAdapter`): it only calls `reset()` / `step()`.
   * `RandomAgent` -- `bsuite/baselines/random/agent.py:26-45` with one generator call per step for the whole batch.
   * `run_episodes` / `run_random_episodes` -- `experiment.run` to each lane's episode budget, with any agent through
-    masked steps, or with the random agent's actions sampled on the device through fused masked rollouts.
+    masked steps, or with the random agent's actions sampled on the device through fused masked launches that write
+    no per-step output (`advance`); `suite.SweepBatch.run_random_episodes` does the latter for a whole sweep.
   * `run_host_episodes` / `HostParts.run_episodes` -- the same for a HOST-side policy, through masked host steps
     (`step_host(..., mask=..., episodes_left=...)`), on one handle or over part-batches.
   * `Trajectory` / `collect` -- the `[T + 1]` observations / `[T]` actions, rewards, discounts layout of
@@ -136,10 +137,10 @@ def run_episodes(agent, environment, num_episodes: Optional[int] = None, check_e
 def run_random_episodes(environment, num_episodes: Optional[int] = None, action_seed: int = 0,
                         steps_per_launch: int = 64):
   """`run_episodes` for the reference's random agent (baselines/random/agent.py:35-37) with the actions sampled on
-  the device: every lane plays exactly its episode budget (`episode_budget`) in fused masked rollouts
-  (`rollout(..., mask=..., episodes_left=...)`), `steps_per_launch` calls per launch.
+  the device: every lane plays exactly its episode budget (`episode_budget`) in fused masked launches that write no
+  per-step output (`advance(..., mask=..., episodes_left=...)`), `steps_per_launch` calls per launch.
 
-  One masked reset of the lanes with a positive budget, then rollouts until no lane has episodes left; the host
+  One masked reset of the lanes with a positive budget, then launches until no lane has episodes left; the host
   syncs once per launch to ask.  Per lane, `bsuite_info()`, episode statistics, log rows and scores equal those of
   `run_episodes` with an agent whose actions are `environment.random_actions(1, action_seed,
   first_step=environment.steps_done)`; only `steps_done` may differ.  Returns the number of calls made after the
@@ -150,10 +151,9 @@ def run_random_episodes(environment, num_episodes: Optional[int] = None, action_
   left = episode_budget(environment, num_episodes)
   mask = left > 0
   environment.reset(out=environment.make_buffers(), mask=mask)
-  out = environment.make_buffers(T)
   calls = 0
   while bool((left > 0).any()):
-    environment.rollout(T, action_seed=action_seed, out=out, mask=mask, episodes_left=left)
+    environment.advance(T, action_seed=action_seed, mask=mask, episodes_left=left)
     calls += T
   return calls
 

@@ -30,6 +30,9 @@ def one_per_experiment(setting: int = 0) -> List[str]:
 # cartpole / swingup 5 x f64, mountain_car 2 x f64 + the step word, the rest a word + an 8-byte RNG position).
 _STATE_BYTES = {0: 8, 1: 8, 2: 80, 3: 80, 4: 48}
 
+# `SweepBatch.run_random_episodes`' calls per launch (DESIGN.md §7, "Advancing to the budgets").
+RUN_STEPS_PER_LAUNCH = 1024
+
 
 def algorithmic_bytes_per_lane_step(env, obs_shape=None) -> int:
   """`obs_shape`: the shape of one setting of a packed environment (default: `env.obs_shape`)."""
@@ -163,6 +166,57 @@ class SweepBatch:
     for stream in self._streams.values():
       current.wait_stream(stream)
     return self._per_id(slot) if self.packed else result
+
+  def run_random_episodes(self, num_episodes: Optional[int] = None, action_seed: int = 0,
+                          steps_per_launch: int = RUN_STEPS_PER_LAUNCH) -> Dict[str, int]:
+    """Plays every lane of every environment to its episode budget with the reference's random agent: the sweep's
+    real workload, after which `local_returns`, the log rows and `analysis.bsuite_score(self)` hold its results.
+
+    Per environment this is `rollouts.run_random_episodes(env, num_episodes, action_seed, steps_per_launch)`: one
+    masked reset of the lanes with a positive budget (`rollouts.episode_budget`: `num_episodes`, or each setting's
+    `bsuite_num_episodes`), then output-free launches of `steps_per_launch` calls (`advance`) until none of its lanes
+    has episodes left, so every lane ends exactly as it would there.  Environments run in rounds, each on its own
+    stream on CUDA; after each round the host reads every environment's "any lane left" flag with one device-to-host
+    copy, and an environment leaves the rotation once its lanes are done.  The caller's current stream waits for all
+    of them before this returns.  Returns the calls made after the reset per environment, keyed like `envs`."""
+    import contextlib  # pylint: disable=import-outside-toplevel
+    from bsuite_b200 import rollouts  # pylint: disable=import-outside-toplevel
+    torch = self._torch
+    T = int(steps_per_launch)
+    if T <= 0:
+      raise ValueError(f'steps_per_launch must be positive, got {steps_per_launch}')
+    keys = list(self.envs)
+    current = torch.cuda.current_stream(self._device) if self._cuda else None
+    on_stream = lambda k: torch.cuda.stream(self._streams[k]) if self._cuda else contextlib.nullcontext()
+    left = {k: rollouts.episode_budget(env, num_episodes) for k, env in self.envs.items()}
+    masks = {k: value > 0 for k, value in left.items()}
+    running = torch.zeros(len(keys), dtype=torch.bool, device=self._device)      # any lane left, per environment
+    if self._cuda:                     # the budgets, masks and flags are made on the caller's stream
+      for k in keys:
+        self._streams[k].wait_stream(current)
+    reset_out = {}                     # the resets' buffers, kept until every stream has joined the caller's
+    calls = {k: 0 for k in keys}
+    rotation = list(range(len(keys)))
+    first = True
+    while rotation:
+      for i in rotation:
+        k = keys[i]
+        with on_stream(k):
+          if first:
+            reset_out[k] = self.envs[k].make_buffers()
+            self.envs[k].reset(out=reset_out[k], mask=masks[k])
+          else:
+            self.envs[k].advance(T, action_seed=action_seed, mask=masks[k], episodes_left=left[k])
+            calls[k] += T
+          running[i] = (left[k] > 0).any()
+      if self._cuda:
+        for i in rotation:
+          current.wait_stream(self._streams[keys[i]])
+      flags = running.tolist()         # the round's one device-to-host read
+      rotation = [i for i in rotation if flags[i]]
+      first = False
+    del reset_out
+    return calls
 
   def capture(self, num_steps: int = 1, action_seed: int = 0, lock_steps: int = 1) -> 'GraphedSweep':
     """Records `lock_steps` successive lock-steps of every id (a `num_steps`-step rollout each, on-device actions)

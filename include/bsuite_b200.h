@@ -389,6 +389,27 @@ int32_t bsb_rollout_masked(bsb_env* env, int64_t num_steps,
                            const bsb_outputs* out, int32_t* actions_out,
                            void* stream);
 
+/*
+ * Advance: a masked rollout of sampled actions that writes no per-step
+ * output, for runs whose results live in the lanes' accumulators, log rows
+ * and scores (playing every lane to its episode budget).  The call equals,
+ * bit for bit, bsb_rollout_masked(env, num_steps, NULL, action_seed, mask,
+ * episodes_left, out, NULL, stream) for any out, in everything but the
+ * outputs: lane state, RNG streams (an observation's own draws, such as
+ * umbrella_chain's distractors, are still made), info fields, Logging
+ * columns, log rows, episodes_left and bsb_steps_done (+T).  Nothing per step
+ * is written: no observation, final observation, scalar or action.  mask
+ * (uint8 [B], required) and episodes_left (int64 [B], nullable) live in the
+ * handle's memory space.  Refused (BSB_INVALID_ARGUMENT): a NULL env or mask,
+ * num_steps <= 0.  Accepts every handle bsb_rollout_masked accepts, collects
+ * an uncollected BSB_HOST_NO_WAIT step first, works in graph-safe mode and may
+ * be captured: a replay reads mask and episodes_left as they are then and
+ * writes episodes_left back.
+ */
+int32_t bsb_advance_masked(bsb_env* env, int64_t num_steps,
+                           uint64_t action_seed, const uint8_t* mask,
+                           int64_t* episodes_left, void* stream);
+
 /* Host mirror of the on-device action sampler: out int32 [T,B] (host). */
 int32_t bsb_random_actions(uint64_t action_seed, uint64_t lane_offset,
                            int64_t batch, int64_t first_step, int64_t num_steps,
@@ -420,7 +441,7 @@ int32_t bsb_read_episode_stats(bsb_env* env, int32_t field, double* dst,
 
 /*
  * CUDA graphs.  bsb_step / bsb_reset / bsb_rollout / the masked calls (bsb_reset_masked / bsb_step_masked /
- * bsb_rollout_masked) / bsb_read_* / bsb_sum_* may be called on a stream
+ * bsb_rollout_masked / bsb_advance_masked) / bsb_read_* / bsb_sum_* may be called on a stream
  * that is being captured.  A graph freezes launch arguments, so the first captured launch moves the handle's step
  * counter (it indexes the on-device action stream and the Logging columns) and its chunk scheduler into device
  * memory, for good: replays and eager calls can then be mixed in any order, and bsb_steps_done / bsb_get_state
