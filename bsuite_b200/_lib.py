@@ -129,6 +129,8 @@ EXPORTS = {
                                             ctypes.c_void_p]),
     'bsb_advance_masked': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_uint64, ctypes.c_void_p,
                                             ctypes.c_void_p, ctypes.c_void_p]),
+    'bsb_step_budgeted': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                           ctypes.POINTER(Outputs), ctypes.POINTER(Outputs), ctypes.c_void_p]),
     'bsb_random_actions': (ctypes.c_int32, [ctypes.c_uint64, ctypes.c_uint64, ctypes.c_int64, ctypes.c_int64,
                                             ctypes.c_int64, ctypes.c_int32, ctypes.c_void_p]),
     'bsb_steps_done': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64)]),

@@ -1,6 +1,7 @@
 // Host path and kernel launch, instantiated once per kernel variant in the translation unit the variant list gives it
 // (bsb_variants.cu).
 #pragma once
+#include <cstring>
 #include <type_traits>
 #include <vector>
 
@@ -307,6 +308,42 @@ void run_host(const bsb_env* e, const LaunchArgs& a, const uint8_t* mask = nullp
   host_run<V, 0>(e->p, a, mask, episodes_left);
 }
 
+// bsb_step_budgeted on a host handle, as masked_kernel's CALL_BUDGETED runs it: every masked-in lane's current
+// entries of a's outputs go to `previous` (observation rows as raw bytes), then the masked step with budgets, then the
+// mask is cleared for the masked-in lanes whose budget was spent before the call.
+template <class V>
+void host_budgeted(const bsb_env* e, const LaunchArgs& a, uint8_t* mask, int64_t* episodes_left,
+                   const bsb_outputs* previous) {
+  typedef typename V::Obs O;
+  const EnvParams& p = e->p;
+  const int64_t B = p.batch;
+  const RaggedTable* ragged = V::kRagged ? reinterpret_cast<const RaggedTable*>(p.pack) : nullptr;
+  const O* obs = reinterpret_cast<const O*>(a.obs);
+  O* prev_obs = reinterpret_cast<O*>(previous->observation);
+  const O* fin = reinterpret_cast<const O*>(a.final_obs);
+  O* prev_fin = reinterpret_cast<O*>(previous->final_observation);
+  std::vector<uint8_t> spent((size_t)B, 0);
+  for (int64_t lane = 0; lane < B; ++lane) {
+    if (!mask[lane]) continue;
+    spent[(size_t)lane] = episodes_left[lane] <= 0;
+    int64_t row = lane * (int64_t)p.obs_numel, K = p.obs_numel;
+    if constexpr (V::kRagged) {
+      const RaggedSetting& s = ragged_setting(ragged, lane / ragged->pack.lanes_per_setting);
+      row = s.obs_offset + (lane - s.lane_shift) * (int64_t)s.obs_numel;
+      K = s.obs_numel;
+    }
+    memcpy(prev_obs + row, obs + row, (size_t)K * sizeof(O));
+    if (fin && prev_fin) memcpy(prev_fin + lane * (int64_t)p.obs_numel, fin + lane * (int64_t)p.obs_numel, (size_t)p.obs_numel * sizeof(O));
+    if (a.reward && previous->reward) previous->reward[lane] = a.reward[lane];
+    if (a.reward_f64 && previous->reward_f64) previous->reward_f64[lane] = a.reward_f64[lane];
+    if (a.discount && previous->discount) previous->discount[lane] = a.discount[lane];
+    if (a.step_type && previous->step_type) previous->step_type[lane] = a.step_type[lane];
+  }
+  run_host<V>(e, a, mask, episodes_left);
+  for (int64_t lane = 0; lane < B; ++lane)
+    if (spent[(size_t)lane]) mask[lane] = 0;
+}
+
 // Kernels and host path of variant V, the runner bsb_create stores in the handle.  The bit sources and kernels are
 // those the variant list (BSB_VARIANTS) compiles for V: bsb_create picks no runner for an MT19937 handle whose variant
 // lacks MT19937, and only a variant with two_phase_host_kernel is given `two_phase` (a two-phase host step).
@@ -341,14 +378,23 @@ int run_variant(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoP
 // bsb_advance_masked): the host path, or one launch of masked_kernel with one chunk of 32 lanes per warp.  A masked
 // host step (a launch that carries the mailbox, or a `mask_out` to clear spent lanes in) takes the CALL_HOST
 // instantiation; a launch with no observation buffer (bsb_advance_masked) takes CALL_ADVANCE; any other call with
-// nothing for the T loop, the action stream or the budgets to do (every masked reset and step) takes CALL_ONE.
+// nothing for the T loop, the action stream or the budgets to do (every masked reset and step) takes CALL_ONE.  A
+// budgeted step (`previous` given: bsb_step_budgeted, whose `mask_out` is the mask) takes CALL_BUDGETED.
 template <class V>
 int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* episodes_left, uint8_t* mask_out,
-               cudaStream_t stream) {
+               const bsb_outputs* previous, cudaStream_t stream) {
   constexpr bool kMt = Compiled<V>::kMt;
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
-  if (e->device < 0) { run_host<V>(e, a, mask, episodes_left); return BSB_OK; }
+  if (previous && (a.T != 1 || a.mode != MODE_STEP || !a.actions || a.actions_out || a.mailbox || !episodes_left ||
+                   mask_out != mask))
+    return fail(BSB_INTERNAL, "a budgeted step must be one step of the caller's actions, with budgets, clearing its mask");
+  if (e->device < 0) {
+    if (previous) host_budgeted<V>(e, a, mask_out, episodes_left, previous);
+    else run_host<V>(e, a, mask, episodes_left);
+    return BSB_OK;
+  }
   MaskArgs m;
+  memset(&m, 0, sizeof(m));
   m.mask = mask;
   m.noise = e->p.wrapper == BSB_WRAP_REWARD_NOISE ? 1 : 0;
   m.track = e->p.ep != nullptr ? 1 : 0;
@@ -370,6 +416,17 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
     if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_kernel<V, 1, kCall>, e->p, la, m); }
     return launch(e, la, g, stream, masked_kernel<V, 0, kCall>, e->p, la, m);
   };
+  if (previous) {
+    m.prev_obs = previous->observation;
+    m.prev_reward = previous->reward;
+    m.prev_reward_f64 = previous->reward_f64;
+    m.prev_discount = previous->discount;
+    m.prev_step_type = previous->step_type;
+    m.prev_final_obs = previous->final_observation;
+    m.prev_vec_ok = reinterpret_cast<uintptr_t>(previous->observation) % 16 == 0 ? 1 : 0;
+    m.prev_final_vec_ok = reinterpret_cast<uintptr_t>(previous->final_observation) % 16 == 0 ? 1 : 0;
+    return go(std::integral_constant<int, CALL_BUDGETED>());
+  }
   if (host_call) {
     if (a.T != 1 || a.mode != MODE_STEP || !a.actions || a.actions_out)
       return fail(BSB_INTERNAL, "a masked host step must be one step of the caller's actions");

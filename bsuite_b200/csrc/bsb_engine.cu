@@ -84,9 +84,11 @@ template <class T> int env_alloc_t(bsb_env* e, T** out, size_t count, bool snaps
 }
 
 // `two_phase`: a two-phase host step (mailbox_launch; deep_sea and catch only).  `mask`: a masked call, rollout or
-// host step (`episodes_left`: the budgets, nullable; `mask_out`: a budgeted host step's mask write-back, nullable).
+// host step (`episodes_left`: the budgets, nullable; `mask_out`: a budgeted host step's mask write-back, nullable;
+// `previous`: a budgeted step's previous outputs, nullable).
 int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr,
-        const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr) {
+        const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr,
+        const bsb_outputs* previous = nullptr) {
   DeviceGuard guard(e->device);
   LaunchArgs a = args;
   if (e->device >= 0) {
@@ -95,7 +97,7 @@ int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseA
     if (capture != cudaStreamCaptureStatusNone) e->graph_safe = true;
     if (e->graph_safe) a.clock = e->clock;      // a.step0 == e->steps_done, which no longer moves
   }
-  if (mask) return e->variant->run_masked(e, a, mask, episodes_left, mask_out, stream);
+  if (mask) return e->variant->run_masked(e, a, mask, episodes_left, mask_out, previous, stream);
   return e->variant->run(e, a, stream, two_phase);
 }
 
@@ -851,10 +853,12 @@ int32_t bsb_step(bsb_env* env, const int32_t* actions, const bsb_outputs* out, v
 // bsb_reset_masked / bsb_step_masked / bsb_rollout_masked / bsb_step_host_masked: lane i makes the calls only where
 // mask[i] != 0 (run_masked), a rollout's or host step's lanes only while their budgets last.  Host handles validate
 // the actions of masked-in lanes only, at every step of a rollout (a host step: of lanes with budget left): an
-// inactive lane's action is never read.  `mask_out`: a budgeted host step's write-back (run_masked).
+// inactive lane's action is never read.  `mask_out`: a budgeted host step's write-back, or a budgeted step's mask;
+// `previous`: a budgeted step's previous outputs (run_masked).
 static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask, const bsb_outputs* out, void* stream,
                        int mode, int64_t T = 1, bool rollout = false, uint64_t action_seed = 0,
-                       int32_t* actions_out = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr) {
+                       int32_t* actions_out = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr,
+                       const bsb_outputs* previous = nullptr) {
   { int crc = check_final_observation(env, out); if (crc != BSB_OK) return crc; }
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
   if (env->device < 0 && mode == MODE_STEP && actions) {
@@ -869,7 +873,7 @@ static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask
   }
   LaunchArgs a = make_args(env, out, mode == MODE_STEP ? actions : nullptr, T, mode);
   a.action_seed = action_seed; a.actions_out = actions_out;
-  int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask, episodes_left, mask_out);
+  int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask, episodes_left, mask_out, previous);
   if (rc == BSB_OK) advance_steps(env, T);
   return rc;
 }
@@ -918,6 +922,22 @@ int32_t bsb_advance_masked(bsb_env* env, int64_t num_steps, uint64_t action_seed
   bsb_outputs none;
   memset(&none, 0, sizeof(none));
   return masked_call(env, nullptr, mask, &none, stream, MODE_STEP, num_steps, true, action_seed, nullptr, episodes_left);
+}
+
+// One masked step with budgets that first keeps the masked-in lanes' current outputs in `previous`: masked_kernel's
+// CALL_BUDGETED instantiation (run_masked), or host_budgeted on a host handle.  The mask is cleared in place one call
+// after a lane's budget is spent.
+int32_t bsb_step_budgeted(bsb_env* env, const int32_t* actions, uint8_t* mask, int64_t* episodes_left,
+                          const bsb_outputs* out, const bsb_outputs* previous, void* stream) {
+  if (!env || !actions || !mask || !episodes_left || !out || !previous || !out->observation || !previous->observation)
+    return fail(BSB_INVALID_ARGUMENT, "bsb_step_budgeted needs actions, a mask, budgets and two output sets with "
+                                      "observation buffers");
+  if (previous->observation == out->observation)
+    return fail(BSB_INVALID_ARGUMENT, "bsb_step_budgeted needs `previous` to have its own observation buffer");
+  if (!out->final_observation != !previous->final_observation)
+    return fail(BSB_INVALID_ARGUMENT, "final_observation must be set in both output sets or in neither");
+  { int crc = check_final_observation(env, previous); if (crc != BSB_OK) return crc; }
+  return masked_call(env, actions, mask, out, stream, MODE_STEP, 1, false, 0, nullptr, episodes_left, mask, previous);
 }
 
 int32_t bsb_random_actions(uint64_t action_seed, uint64_t lane_offset, int64_t batch, int64_t first_step,

@@ -26,17 +26,19 @@ int drain_log_rows(bsb_env* e);                         // waits out host steps 
 // Kernels and host path of kernel variant V (bsb_dispatch.cuh), explicitly instantiated for each entry of the variant
 // list (BSB_VARIANTS) in the translation unit the list gives it (bsb_variants.cu).  `two_phase`: a two-phase host step.
 template <class V> int run_variant(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs* two_phase);
-// Masked calls of variant V (bsb_reset_masked / bsb_step_masked / bsb_rollout_masked / bsb_step_host_masked): `mask`
-// [B] and `episodes_left` [B] (nullable) live where the handle's state does, or `mask` is a pinned host buffer's
-// device alias.  `mask_out` (masked host steps with budgets, else null): where spent lanes' mask bytes are cleared.
+// Masked calls of variant V (bsb_reset_masked / bsb_step_masked / bsb_rollout_masked / bsb_step_host_masked /
+// bsb_advance_masked / bsb_step_budgeted): `mask` [B] and `episodes_left` [B] (nullable) live where the handle's
+// state does, or `mask` is a pinned host buffer's device alias.  `mask_out` (masked host steps with budgets and
+// budgeted steps, else null): where spent lanes' mask bytes are cleared.  `previous` (budgeted steps, else null): the
+// outputs that receive the masked-in lanes' current entries before the step.
 template <class V> int run_masked(bsb_env*, const LaunchArgs&, const uint8_t* mask, int64_t* episodes_left,
-                                  uint8_t* mask_out, cudaStream_t);
+                                  uint8_t* mask_out, const bsb_outputs* previous, cudaStream_t);
 // An entry of the variant list, as bsb_create looks it up (bsb_engine.cu).
 struct VariantEntry {
   int family, obs_dtype, mode;
   bool mt, two_phase;
   int (*run)(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs*);
-  int (*run_masked)(bsb_env*, const LaunchArgs&, const uint8_t*, int64_t*, uint8_t*, cudaStream_t);
+  int (*run_masked)(bsb_env*, const LaunchArgs&, const uint8_t*, int64_t*, uint8_t*, const bsb_outputs*, cudaStream_t);
 };
 
 #define BSB_CUDA(expr)                                                                   \

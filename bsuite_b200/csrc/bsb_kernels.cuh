@@ -1483,15 +1483,28 @@ struct MaskArgs {
   const uint8_t* mask;      // [B], device memory (host steps: pinned host memory's device alias, or device staging)
   int32_t noise, track;     // the RewardNoise stream is live / the Logging accumulators are tracked
   int64_t* episodes_left;   // masked rollouts and host steps: [B] episode budgets, counted down at each LAST (nullable)
-  uint8_t* mask_out;        // host steps with budgets: mask[i] is cleared here once lane i's budget is spent (null
-                            // for every other call)
+  uint8_t* mask_out;        // host steps with budgets: mask[i] is cleared here once lane i's budget is spent;
+                            // budgeted steps: the mask itself, cleared for lanes whose budget was spent before the
+                            // call (null for every other call)
+  // bsb_step_budgeted: the `previous` outputs, which receive the masked-in lanes' current entries of the launch's
+  // outputs before the step (null for every other call); prev_vec_ok / prev_final_vec_ok: both observation (final
+  // observation) buffers start 16-byte aligned
+  float* prev_obs;
+  float* prev_reward;
+  double* prev_reward_f64;
+  float* prev_discount;
+  int32_t* prev_step_type;
+  float* prev_final_obs;
+  int32_t prev_vec_ok, prev_final_vec_ok;
 };
 
 // What one masked_kernel instantiation runs.  CALL_ROLLOUT: bsb_rollout_masked (T steps, sampled or given actions,
 // budgets, actions_out).  CALL_ONE: a masked reset or step (T = 1, the caller's actions, no budgets).  CALL_HOST:
 // bsb_step_host_masked (T = 1, the caller's actions, optional budgets, the mask write-back, the mailbox signal).
 // CALL_ADVANCE: bsb_advance_masked (T steps of sampled actions, optional budgets, no per-step output at all).
-enum CallKind { CALL_ROLLOUT = 0, CALL_ONE = 1, CALL_HOST = 2, CALL_ADVANCE = 3 };
+// CALL_BUDGETED: bsb_step_budgeted (CALL_HOST without the mailbox: T = 1, the caller's actions, budgets, the masked-in
+// lanes' outputs copied to `previous` first, and the mask cleared for lanes whose budget was spent before the call).
+enum CallKind { CALL_ROLLOUT = 0, CALL_ONE = 1, CALL_HOST = 2, CALL_ADVANCE = 3, CALL_BUDGETED = 4 };
 
 // Writes lane j's observation `val(e)` (element e of K) with the whole warp: 16-byte streaming stores when `vec`
 // (the row starts 16-byte aligned and is a whole number of 16-byte words), else one element per store.
@@ -1539,6 +1552,36 @@ __device__ __forceinline__ void emit_lane_subset(const EnvParams& lp, const type
   }
 }
 
+// Copies the rows row0 + tid of `src` to `dst` ([rows, K] elements of O, as raw bytes: no cast) for the warp's lanes
+// for which `on` holds; the other rows are not touched.  Rows: each lane's thread copies its own row.  Tiles, boards
+// and images: the warp walks the lanes __ballot_sync selects and copies each row, with 16-byte loads and stores when
+// `vec_base` (both buffers start 16-byte aligned) and the row is a whole number of 16-byte words, as emit_lane_subset
+// writes it.
+template <class F, class O>
+__device__ __forceinline__ void copy_lane_subset(const O* src, O* dst, int K, int64_t row0, bool on, bool vec_base) {
+  const int tid = threadIdx.x & 31;
+  if (EmitKind<F>::value == EMIT_ROWS) {
+    if (on) {
+      const O* s = src + (row0 + tid) * (int64_t)K;
+      O* d = dst + (row0 + tid) * (int64_t)K;
+      for (int e = 0; e < K; ++e) d[e] = s[e];
+    }
+    return;
+  }
+  const bool vec = vec_base && ((int64_t)K * (int64_t)sizeof(O)) % 16 == 0;
+  for (unsigned rest = __ballot_sync(0xffffffffu, on); rest != 0u; rest &= rest - 1u) {
+    const int j = __ffs(rest) - 1;
+    const O* s = src + (row0 + j) * (int64_t)K;
+    O* d = dst + (row0 + j) * (int64_t)K;
+    if (vec) {
+      const int words = (int)(((int64_t)K * (int64_t)sizeof(O)) >> 4);
+      for (int q = tid; q < words; q += 32) __stcs(reinterpret_cast<uint4*>(d) + q, reinterpret_cast<const uint4*>(s)[q]);
+    } else {
+      for (int e = tid; e < K; e += 32) d[e] = s[e];
+    }
+  }
+}
+
 // Every masked call: a masked reset or step (T = 1, no budgets) or bsb_rollout_masked's T masked steps, in one launch.
 // One chunk of 32 lanes per warp; a ragged pack's chunks never straddle two settings, and row j of setting k goes to
 // the setting's block (emit_lane_subset).  Lane i is active at step t while mask[i] != 0 and its budget
@@ -1557,9 +1600,14 @@ __device__ __forceinline__ void emit_lane_subset(const EnvParams& lp, const type
 // and every per-step output compiled out (observations, final observations, scalars, actions_out); where an
 // observation would be rendered the lane makes the draws rendering makes (ObsDraws::skip), so its streams end where
 // CALL_ROLLOUT's do.  A same-step final observation is rendered from a copy of the stream and is simply not rendered.
+// kCall == CALL_BUDGETED: CALL_HOST without the mailbox, where every masked-in lane (budget left or not) first copies
+// its current entries of the outputs -- observation row, scalars, final observation -- to `previous`
+// (copy_lane_subset; the warp syncs before any new row is written), and a masked-in lane whose budget was spent before
+// the call clears its mask byte instead of stepping.
 template <class V, int RK, int kCall>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(const EnvParams p, const LaunchArgs a, const MaskArgs m) {
-  constexpr bool kOneCall = kCall == CALL_ONE || kCall == CALL_HOST;      // one call: T = 1 and the caller's actions
+  // one call: T = 1 and the caller's actions
+  constexpr bool kOneCall = kCall == CALL_ONE || kCall == CALL_HOST || kCall == CALL_BUDGETED;
   constexpr bool kEmit = kCall != CALL_ADVANCE;                           // the call writes per-step outputs
   typedef typename V::Fam Fam;
   typedef typename V::Obs O;
@@ -1597,6 +1645,22 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(c
     int64_t left = selected && budgets ? budgets[lane] : 0;
     bool on = selected && (!budgets || left > 0);
     const bool opened = on;
+    if constexpr (kCall == CALL_BUDGETED) {      // the outputs of the call before this one, for the agent (T = 1)
+      O* prev_block = reinterpret_cast<O*>(m.prev_obs) + (block - reinterpret_cast<O*>(a.obs));
+      copy_lane_subset<Fam>(block, prev_block, lp.obs_numel, local_base, selected, a.obs_vec_ok != 0 && m.prev_vec_ok != 0);
+      if constexpr (V::kSameStep) {
+        if (a.final_obs && m.prev_final_obs)
+          copy_lane_subset<Fam>(reinterpret_cast<const O*>(a.final_obs), reinterpret_cast<O*>(m.prev_final_obs), lp.obs_numel,
+                                local_base, selected, a.final_vec_ok != 0 && m.prev_final_vec_ok != 0);
+      }
+      if (selected) {
+        if (a.reward && m.prev_reward) m.prev_reward[lane] = a.reward[lane];
+        if (a.reward_f64 && m.prev_reward_f64) m.prev_reward_f64[lane] = a.reward_f64[lane];
+        if (a.discount && m.prev_discount) m.prev_discount[lane] = a.discount[lane];
+        if (a.step_type && m.prev_step_type) m.prev_step_type[lane] = a.step_type[lane];
+      }
+      __syncwarp();
+    }
 
     typename Fam::Lane L;
     R rng, wrng;
@@ -1649,6 +1713,9 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(c
     if (selected && budgets) budgets[lane] = left;
     // the host's view of the lanes still running: only a lane whose budget is spent writes its byte
     if constexpr (kCall == CALL_HOST) { if (selected && budgets && left <= 0 && m.mask_out) m.mask_out[lane] = 0; }
+    // a budgeted step clears the mask one call after the budget is spent: on the call that returns the lane's last
+    // LAST `previous` still holds the timestep before it, on the next one both buffers hold the LAST
+    if constexpr (kCall == CALL_BUDGETED) { if (selected && !opened) m.mask_out[lane] = 0; }
   }
 
   if constexpr (kCall == CALL_HOST) { if (a.mailbox) signal_done(a); }

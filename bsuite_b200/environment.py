@@ -462,13 +462,24 @@ class BatchedEnvironment:
       _lib.check(self._lib.bsb_reset(self._handle.ptr, ctypes.byref(outputs), self._stream()))
     return out.timestep()
 
-  def step(self, actions, out: Optional[StepBuffers] = None, mask=None):
+  def step(self, actions, out: Optional[StepBuffers] = None, mask=None, episodes_left=None,
+           previous: Optional[StepBuffers] = None):
     """base.Environment.step for every lane (base.py:59-65); actions int [B].
 
     `mask` (bool or uint8 tensor [B] on the environment's device; needs `out`): only the lanes where it is set step;
     the others make no call, their actions are ignored (never validated) and their entries of `out` are left as they
-    are (`bsb_step_masked`).  Every call, masked or not, counts once in `steps_done`."""
+    are (`bsb_step_masked`).  Every call, masked or not, counts once in `steps_done`.
+
+    `episodes_left` (int64 [B] contiguous tensor on the device) and `previous` (StepBuffers like `out`, with their
+    own tensors) go together and need `mask` and `out`: a budgeted step (`bsb_step_budgeted`).  Every lane whose mask
+    is set first copies its entries of `out` into `previous`; then it steps if its budget is positive (each LAST
+    takes one from it in place), else it sits out and its mask is cleared in place (a bool mask is viewed, not
+    copied, so the caller's tensor is updated).  So on the call that returns a lane's last LAST, `previous` holds the
+    timestep before it, and on the next call both hold the LAST.  An agent loop that passes `previous` to its update
+    needs no copies of its own (`rollouts.run_episodes`)."""
     torch = self._torch
+    if episodes_left is not None or previous is not None:
+      return self._step_budgeted(actions, out, mask, episodes_left, previous)
     if mask is not None:
       return self._step_masked(actions, out, mask)
     if not (type(actions) is torch.Tensor and actions.dtype is torch.int32 and actions.dim() == 1
@@ -495,6 +506,27 @@ class BatchedEnvironment:
     self._async_work = True
     _lib.check(self._lib.bsb_step_masked(self._handle.ptr, actions.data_ptr(), mask.data_ptr(), ctypes.byref(outputs),
                                          self._stream()))
+    return out.timestep()
+
+  def _step_budgeted(self, actions, out, mask, episodes_left, previous):
+    if episodes_left is None or previous is None:
+      raise ValueError('episodes_left and previous go together: a budgeted step needs both')
+    if mask is None:
+      raise ValueError('a budgeted step needs mask=: the lanes that play, cleared in place once their budget is spent')
+    if not isinstance(previous, StepBuffers):
+      raise ValueError(f'previous must be StepBuffers, got {type(previous).__name__}')
+    if isinstance(mask, self._torch.Tensor) and not mask.is_contiguous():
+      raise ValueError('mask must be contiguous: it is updated in place')
+    mask = self._mask(mask, out)
+    self._episodes_left(episodes_left)
+    actions = self._device_actions(actions, (self._batch,))
+    outputs = out._outputs if out._bound is self._obs_dtype else out.bind(self._obs_dtype)
+    prev = previous._outputs if previous._bound is self._obs_dtype else previous.bind(self._obs_dtype)
+    self._async_work = True
+    status = self._lib.bsb_step_budgeted(self._handle.ptr, actions.data_ptr(), mask.data_ptr(), episodes_left.data_ptr(),
+                                         ctypes.byref(outputs), ctypes.byref(prev), self._stream())
+    if status:
+      _lib.check(status)
     return out.timestep()
 
   def make_mixed_buffers(self) -> StepBuffers:

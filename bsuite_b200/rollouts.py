@@ -6,8 +6,9 @@
     runs unchanged on the B = 1 face (`DmEnvAdapter`): it only calls `reset()` / `step()`.
   * `RandomAgent` -- `bsuite/baselines/random/agent.py:26-45` with one generator call per step for the whole batch.
   * `run_episodes` / `run_random_episodes` -- `experiment.run` to each lane's episode budget, with any agent through
-    masked steps, or with the random agent's actions sampled on the device through fused masked launches that write
-    no per-step output (`advance`); `suite.SweepBatch.run_random_episodes` does the latter for a whole sweep.
+    budgeted steps (one launch per call), or with the random agent's actions sampled on the device through fused
+    masked launches that write no per-step output (`advance`); `suite.SweepBatch.run_episodes` and
+    `run_random_episodes` do the same for a whole sweep.
   * `run_host_episodes` / `HostParts.run_episodes` -- the same for a HOST-side policy, through masked host steps
     (`step_host(..., mask=..., episodes_left=...)`), on one handle or over part-batches.
   * `Trajectory` / `collect` -- the `[T + 1]` observations / `[T]` actions, rewards, discounts layout of
@@ -96,42 +97,53 @@ def episode_budget(environment, num_episodes: Optional[int] = None):
   return torch.full((B,), int(environment.bsuite_num_episodes), dtype=torch.int64, device=device)
 
 
+class EpisodeLoop:
+  """One environment's side of `run_episodes`, for loops that drive several environments in turn
+  (`suite.SweepBatch.run_episodes`): the budgets (`episode_budget`), the mask of the lanes still playing, the output
+  buffers and the `previous` buffers the agent's update reads, and one masked reset of the lanes with a positive
+  budget.  `step()` is one call of the agent and one budgeted step (`step(..., mask=, episodes_left=, previous=)`);
+  `any_left()` is the device flag "some lane has episodes left"."""
+
+  def __init__(self, agent, environment, num_episodes: Optional[int] = None):
+    self.agent, self.environment = agent, environment
+    self.left = episode_budget(environment, num_episodes)
+    self.mask = self.left > 0
+    self.out, self.previous = environment.make_buffers(), environment.make_buffers()
+    self.timestep = environment.reset(out=self.out, mask=self.mask)
+    # lanes without a budget are never stepped: their entries of `previous` show what `out` holds, as every other
+    # lane's do from its first call on
+    for name in ('observation', 'reward', 'discount', 'step_type'):
+      getattr(self.previous, name).copy_(getattr(self.out, name))
+    self.calls = 0
+
+  def any_left(self):
+    return (self.left > 0).any()
+
+  def step(self) -> None:
+    actions = self.agent.select_action(self.timestep)
+    self.timestep = self.environment.step(actions, out=self.out, mask=self.mask, episodes_left=self.left,
+                                          previous=self.previous)
+    self.calls += 1
+    self.agent.update(self.previous.timestep(), actions, self.timestep)
+
+
 def run_episodes(agent, environment, num_episodes: Optional[int] = None, check_every: int = 16):
   """`experiment.run` (baselines/experiment.py:24-57) for B lanes: every lane plays exactly its episode budget and
   then stops, as the reference's loop stops after `num_episodes` episodes.
 
   The budget is `num_episodes` for every lane, or by default each lane's `bsuite_num_episodes` (per setting on a
   packed environment).  Lanes run in lock-step, so they reach their budgets at different calls; a lane that has
-  finished is masked out of the following calls (`step(..., mask=...)`), so its `bsuite_info()`, episode statistics
-  and log rows describe exactly the budget's episodes.  The agent sees the whole batch every call
-  (`select_action(timestep) -> int tensor [B]`, `update(timestep, actions, new_timestep)`); a finished lane's
-  entries of the timestep keep its final LAST.  The LAST counts stay on the device; the loop asks whether any lane
-  is still running once every `check_every` calls.  Returns the number of calls made after the first reset."""
-  torch = environment._torch
-  B, device = environment.batch, environment.device
-  budget = episode_budget(environment, num_episodes)
-  finished = torch.zeros(B, dtype=torch.int64, device=device)
-  active = budget > 0
-  out = environment.make_buffers()
-  timestep = environment.reset(out=out, mask=active)
-  # the agent keeps the previous timestep while the same buffers receive the next one
-  spare = environment.make_buffers()
-  calls = 0
-  while True:
-    if calls % max(int(check_every), 1) == 0 and not bool(active.any()):
-      return calls
-    actions = agent.select_action(timestep)
-    spare.observation.copy_(out.observation)
-    spare.reward.copy_(out.reward)
-    spare.discount.copy_(out.discount)
-    spare.step_type.copy_(out.step_type)
-    previous = spare.timestep()
-    new_timestep = environment.step(actions, out=out, mask=active)
-    calls += 1
-    agent.update(previous, actions, new_timestep)
-    finished += ((new_timestep.step_type == 2) & active).to(torch.int64)
-    active = finished < budget
-    timestep = new_timestep
+  finished is masked out of the following calls, so its `bsuite_info()`, episode statistics and log rows describe
+  exactly the budget's episodes.  The agent sees the whole batch every call (`select_action(timestep) -> int tensor
+  [B]`, `update(timestep, actions, new_timestep)`); a finished lane's entries of the timestep keep its final LAST.
+  Each call is one budgeted step (`step(..., mask=, episodes_left=, previous=)`, `EpisodeLoop`), which counts the
+  budgets down and keeps the timestep the agent acted on on the device; the loop asks whether any lane is still
+  running once every `check_every` calls.  Returns the number of calls made after the first reset."""
+  loop = EpisodeLoop(agent, environment, num_episodes)
+  check_every = max(int(check_every), 1)
+  while loop.calls % check_every != 0 or bool(loop.any_left()):
+    loop.step()
+  return loop.calls
 
 
 def run_random_episodes(environment, num_episodes: Optional[int] = None, action_seed: int = 0,

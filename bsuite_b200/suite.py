@@ -218,6 +218,99 @@ class SweepBatch:
     del reset_out
     return calls
 
+  def run_episodes(self, agents, num_episodes: Optional[int] = None, check_every: int = 16) -> Dict[str, int]:
+    """Plays every lane of every environment to its episode budget with the caller's agents; afterwards
+    `local_returns`, the log rows and `analysis.bsuite_score(self)` hold the agents' results.
+
+    `agents` is keyed like `envs` (experiment name when packed, bsuite_id otherwise); each has the interface
+    `rollouts.run_episodes` takes (`select_action(timestep) -> int tensor [B]`, `update(timestep, actions,
+    new_timestep)`) and sees its environment's whole batch (a ragged pack's agent reads it with `split_observation`).
+    Per environment this is `rollouts.run_episodes(agents[k], env, num_episodes, check_every)` -- the same
+    `rollouts.EpisodeLoop`, one budgeted step per call -- so every lane, every value an agent is passed and the call
+    counts equal that loop's.  Environments take lock-steps in rotation, each on its own stream on CUDA, with the
+    agent's `select_action` and `update` on that stream too, so different agents' kernels can overlap.  Every
+    `check_every` lock-steps the host reads every remaining environment's "any lane left" flag with one
+    device-to-host copy; an environment leaves the rotation once its lanes are done.  The caller's current stream
+    waits for all of them before this returns.  Returns the calls made after the reset per environment."""
+    import contextlib  # pylint: disable=import-outside-toplevel
+    from bsuite_b200 import rollouts  # pylint: disable=import-outside-toplevel
+    torch = self._torch
+    keys = list(self.envs)
+    missing = [k for k in keys if k not in agents]
+    if missing:
+      raise ValueError(f'agents must be keyed like envs; no agent for {", ".join(missing)}')
+    check_every = max(int(check_every), 1)
+    current = torch.cuda.current_stream(self._device) if self._cuda else None
+    on_stream = lambda k: torch.cuda.stream(self._streams[k]) if self._cuda else contextlib.nullcontext()
+    running = torch.zeros(len(keys), dtype=torch.bool, device=self._device)      # any lane left, per environment
+    if self._cuda:                     # the agents' state was made on the caller's stream
+      for k in keys:
+        self._streams[k].wait_stream(current)
+    loops = {}                         # kept until every stream has joined the caller's
+    for k in keys:
+      with on_stream(k):
+        loops[k] = rollouts.EpisodeLoop(agents[k], self.envs[k], num_episodes)
+    rotation = list(range(len(keys)))
+    lock_steps = 0
+    while rotation:
+      if lock_steps % check_every == 0:
+        for i in rotation:
+          with on_stream(keys[i]):
+            running[i] = loops[keys[i]].any_left()
+        if self._cuda:
+          for i in rotation:
+            current.wait_stream(self._streams[keys[i]])
+        flags = running.tolist()       # one device-to-host read per check
+        rotation = [i for i in rotation if flags[i]]
+      for i in rotation:
+        with on_stream(keys[i]):
+          loops[keys[i]].step()
+      lock_steps += 1
+    if self._cuda:
+      for k in keys:
+        current.wait_stream(self._streams[k])
+    return {k: loop.calls for k, loop in loops.items()}
+
+  def run_host_episodes(self, policies, num_episodes: Optional[int] = None) -> Dict[str, int]:
+    """`run_episodes` for HOST-side policies, keyed like `envs`: per environment this is
+    `rollouts.run_host_episodes(policies[k], env, num_episodes)` -- one budget tensor and one pinned mask, one masked
+    reset, then masked host steps (`step_host(..., mask=, episodes_left=)`) until the mask is empty -- with the
+    environments' steps driven round-robin with `wait=False`, as `rollouts.HostParts.run_episodes` drives its parts,
+    so one environment's PCIe round trip and decision hide behind the other environments' kernels.
+    `policy(call, host_timestep, device_observation, mask) -> CPU int32 [B]` (ideally pinned) is asked with its
+    environment's latest timestep and mask.  CUDA environments only.  Returns the calls made after the reset per
+    environment."""
+    from bsuite_b200 import rollouts  # pylint: disable=import-outside-toplevel
+    if not self._cuda:
+      raise ValueError('run_host_episodes drives CUDA environments from pinned host buffers')
+    keys = list(self.envs)
+    missing = [k for k in keys if k not in policies]
+    if missing:
+      raise ValueError(f'policies must be keyed like envs; no policy for {", ".join(missing)}')
+    out = {k: env.make_buffers() for k, env in self.envs.items()}
+    host = {k: env.make_host_buffers() for k, env in self.envs.items()}
+    budgets = {k: rollouts._start_budgeted(env, num_episodes, out[k], host[k])  # pylint: disable=protected-access
+               for k, env in self.envs.items()}
+    calls = {k: 0 for k in keys}
+
+    def submit(k):
+      left, mask = budgets[k]
+      actions = policies[k](calls[k], host[k].timestep(), out[k].observation, mask)
+      self.envs[k].step_host(actions, host[k], out[k], wait=False, mask=mask, episodes_left=left)
+
+    rotation = [k for k in keys if bool(budgets[k][1].any())]
+    for k in rotation:
+      submit(k)
+    while rotation:
+      for k in list(rotation):
+        self.envs[k].host_wait()
+        calls[k] += 1
+        if not bool(budgets[k][1].any()):
+          rotation.remove(k)
+          continue
+        submit(k)
+    return calls
+
   def capture(self, num_steps: int = 1, action_seed: int = 0, lock_steps: int = 1) -> 'GraphedSweep':
     """Records `lock_steps` successive lock-steps of every id (a `num_steps`-step rollout each, on-device actions)
     into a single CUDA graph: the per-id launches fork from the capturing stream onto the ids' streams and join

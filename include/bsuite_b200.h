@@ -410,6 +410,38 @@ int32_t bsb_advance_masked(bsb_env* env, int64_t num_steps,
                            uint64_t action_seed, const uint8_t* mask,
                            int64_t* episodes_left, void* stream);
 
+/*
+ * Budgeted step: one masked step with episode budgets that first keeps the
+ * outputs the agent acted on, so an agent loop needs one call per step.
+ * For each lane i with mask[i] != 0: (1) lane i's current entries of `out`
+ * -- observation row, reward, reward_f64, discount, step_type, and
+ * final_observation when both output sets carry it -- are copied (as raw
+ * bytes) to the same entries of `previous`, for each scalar both carry;
+ * (2) if episodes_left[i] > 0 the lane makes exactly the call
+ * bsb_rollout_masked(env, 1, actions, 0, mask, episodes_left, out, NULL,
+ * stream) makes for it (a LAST takes one from its budget); (3) otherwise it
+ * sits out and mask[i] is cleared.  Lanes whose mask is clear are not
+ * touched.  So the call equals: copy out -> previous where mask; then that
+ * bsb_rollout_masked; then mask[i] &= (episodes_left[i] > 0 before the
+ * call) -- in outputs, previous, mask, budgets, lane state, RNG streams,
+ * info fields, Logging columns, log rows, bsb_steps_done (+1) and the
+ * invalid-action flag.  The mask is cleared one call AFTER the budget is
+ * spent: on the call that returns a lane's last LAST, `previous` still holds
+ * the timestep before it; on the next call both hold the LAST.  Actions of
+ * lanes that sit out are never read.  actions (int32 [B]), mask (uint8 [B],
+ * updated in place), episodes_left (int64 [B], counted down in place), out
+ * and previous all live in the handle's memory space and are required.
+ * Refused (BSB_INVALID_ARGUMENT): a NULL pointer (or observation buffer),
+ * `previous` whose observation buffer is out's, final_observation set in one
+ * output set and not the other, final_observation on a next-step handle.
+ * Accepts every handle bsb_step_masked accepts, collects an uncollected
+ * BSB_HOST_NO_WAIT step first, works in graph-safe mode and may be captured:
+ * a replay reads and writes mask and episodes_left as they are then.
+ */
+int32_t bsb_step_budgeted(bsb_env* env, const int32_t* actions, uint8_t* mask,
+                          int64_t* episodes_left, const bsb_outputs* out,
+                          const bsb_outputs* previous, void* stream);
+
 /* Host mirror of the on-device action sampler: out int32 [T,B] (host). */
 int32_t bsb_random_actions(uint64_t action_seed, uint64_t lane_offset,
                            int64_t batch, int64_t first_step, int64_t num_steps,
@@ -441,7 +473,7 @@ int32_t bsb_read_episode_stats(bsb_env* env, int32_t field, double* dst,
 
 /*
  * CUDA graphs.  bsb_step / bsb_reset / bsb_rollout / the masked calls (bsb_reset_masked / bsb_step_masked /
- * bsb_rollout_masked / bsb_advance_masked) / bsb_read_* / bsb_sum_* may be called on a stream
+ * bsb_rollout_masked / bsb_advance_masked / bsb_step_budgeted) / bsb_read_* / bsb_sum_* may be called on a stream
  * that is being captured.  A graph freezes launch arguments, so the first captured launch moves the handle's step
  * counter (it indexes the on-device action stream and the Logging columns) and its chunk scheduler into device
  * memory, for good: replays and eager calls can then be mixed in any order, and bsb_steps_done / bsb_get_state
