@@ -79,6 +79,16 @@ class Outputs(ctypes.Structure):
               ('discount', ctypes.c_void_p), ('step_type', ctypes.c_void_p), ('final_observation', ctypes.c_void_p)]
 
 
+# enum bsb_policy_kind
+POLICY_EPSILON_GREEDY, POLICY_SOFTMAX = range(2)
+
+
+class Policy(ctypes.Structure):
+  """struct bsb_policy."""
+  _fields_ = [('kind', ctypes.c_int32), ('reserved', ctypes.c_int32), ('values', ctypes.c_void_p),
+              ('epsilon', ctypes.c_double), ('seed', ctypes.c_uint64)]
+
+
 SCORE_MAX_SOURCES = 512      # bsb_score: sources per call
 # enum bsb_score_quantity: the row columns a score reads
 SCORE_QUANTITIES = ('episode', 'total_return', 'total_regret', 'raw_return', 'best_episode', 'total_perfect',
@@ -131,6 +141,9 @@ EXPORTS = {
                                             ctypes.c_void_p, ctypes.c_void_p]),
     'bsb_step_budgeted': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
                                            ctypes.POINTER(Outputs), ctypes.POINTER(Outputs), ctypes.c_void_p]),
+    'bsb_step_budgeted_policy': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(Policy), ctypes.c_void_p,
+                                                  ctypes.c_void_p, ctypes.POINTER(Outputs), ctypes.POINTER(Outputs),
+                                                  ctypes.c_void_p, ctypes.c_void_p]),
     'bsb_random_actions': (ctypes.c_int32, [ctypes.c_uint64, ctypes.c_uint64, ctypes.c_int64, ctypes.c_int64,
                                             ctypes.c_int64, ctypes.c_int32, ctypes.c_void_p]),
     'bsb_steps_done': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64)]),

@@ -344,6 +344,38 @@ void host_budgeted(const bsb_env* e, const LaunchArgs& a, uint8_t* mask, int64_t
     if (spent[(size_t)lane]) mask[lane] = 0;
 }
 
+// bsb_step_budgeted_policy on a host handle, as masked_kernel's CALL_POLICY runs it: every masked-in lane with budget
+// left picks its action from its row of the policy's values (select_action; an invalid row raises the invalid-action
+// flag) and writes it to a.actions_out, then host_budgeted steps with those actions.  Rows of other lanes are not read.
+template <class V>
+void host_policy(const bsb_env* e, const LaunchArgs& a, uint8_t* mask, int64_t* episodes_left,
+                 const bsb_outputs* previous, const bsb_policy& policy) {
+  const EnvParams& p = e->p;
+  const int64_t B = p.batch;
+  const RaggedTable* ragged = V::kRagged ? reinterpret_cast<const RaggedTable*>(p.pack) : nullptr;
+  std::vector<int32_t> actions((size_t)B, 0);
+  for (int64_t lane = 0; lane < B; ++lane) {
+    if (!mask[lane] || episodes_left[lane] <= 0) continue;
+    EnvParams lp = p;                     // the lane's setting: its lane_offset keys the stream as the kernel's does
+    if constexpr (V::kRagged) {
+      ragged_setting_params(lp, ragged_setting(ragged, lane / ragged->pack.lanes_per_setting), ragged->mapping_bits);
+    } else if constexpr (V::kPacked) {
+      pack_lane_params(lp, lane);
+    }
+    bool invalid = false;
+    const int32_t action = select_action(policy.kind, policy.values + lane * (int64_t)p.num_actions, p.num_actions,
+                                         policy.epsilon, policy.seed, lp.lane_offset + (uint64_t)lane,
+                                         (uint64_t)a.step0, invalid);
+    if (invalid && e->bad_action_host) *e->bad_action_host = 1;
+    actions[(size_t)lane] = action;
+    if (a.actions_out) a.actions_out[lane] = action;
+  }
+  LaunchArgs chosen = a;
+  chosen.actions = actions.data();
+  chosen.actions_out = nullptr;
+  host_budgeted<V>(e, chosen, mask, episodes_left, previous);
+}
+
 // Kernels and host path of variant V, the runner bsb_create stores in the handle.  The bit sources and kernels are
 // those the variant list (BSB_VARIANTS) compiles for V: bsb_create picks no runner for an MT19937 handle whose variant
 // lacks MT19937, and only a variant with two_phase_host_kernel is given `two_phase` (a two-phase host step).
@@ -379,17 +411,21 @@ int run_variant(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoP
 // host step (a launch that carries the mailbox, or a `mask_out` to clear spent lanes in) takes the CALL_HOST
 // instantiation; a launch with no observation buffer (bsb_advance_masked) takes CALL_ADVANCE; any other call with
 // nothing for the T loop, the action stream or the budgets to do (every masked reset and step) takes CALL_ONE.  A
-// budgeted step (`previous` given: bsb_step_budgeted, whose `mask_out` is the mask) takes CALL_BUDGETED.
+// budgeted step (`previous` given: bsb_step_budgeted, whose `mask_out` is the mask) takes CALL_BUDGETED, and one with a
+// `policy` (bsb_step_budgeted_policy: no actions, the picks to a.actions_out) takes CALL_POLICY.
 template <class V>
 int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* episodes_left, uint8_t* mask_out,
-               const bsb_outputs* previous, cudaStream_t stream) {
+               const bsb_outputs* previous, const bsb_policy* policy, cudaStream_t stream) {
   constexpr bool kMt = Compiled<V>::kMt;
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
-  if (previous && (a.T != 1 || a.mode != MODE_STEP || !a.actions || a.actions_out || a.mailbox || !episodes_left ||
-                   mask_out != mask))
-    return fail(BSB_INTERNAL, "a budgeted step must be one step of the caller's actions, with budgets, clearing its mask");
+  if (previous && (a.T != 1 || a.mode != MODE_STEP || !a.actions == !policy || (a.actions_out && !policy) ||
+                   a.mailbox || !episodes_left || mask_out != mask))
+    return fail(BSB_INTERNAL, "a budgeted step must be one step of the caller's actions or policy, with budgets, "
+                              "clearing its mask");
+  if (policy && !previous) return fail(BSB_INTERNAL, "a policy step must be a budgeted step");
   if (e->device < 0) {
-    if (previous) host_budgeted<V>(e, a, mask_out, episodes_left, previous);
+    if (policy) host_policy<V>(e, a, mask_out, episodes_left, previous, *policy);
+    else if (previous) host_budgeted<V>(e, a, mask_out, episodes_left, previous);
     else run_host<V>(e, a, mask, episodes_left);
     return BSB_OK;
   }
@@ -425,6 +461,13 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
     m.prev_final_obs = previous->final_observation;
     m.prev_vec_ok = reinterpret_cast<uintptr_t>(previous->observation) % 16 == 0 ? 1 : 0;
     m.prev_final_vec_ok = reinterpret_cast<uintptr_t>(previous->final_observation) % 16 == 0 ? 1 : 0;
+    if (policy) {
+      m.policy_values = policy->values;
+      m.policy_epsilon = policy->epsilon;
+      m.policy_seed = policy->seed;
+      m.policy_kind = policy->kind;
+      return go(std::integral_constant<int, CALL_POLICY>());
+    }
     return go(std::integral_constant<int, CALL_BUDGETED>());
   }
   if (host_call) {

@@ -85,10 +85,10 @@ template <class T> int env_alloc_t(bsb_env* e, T** out, size_t count, bool snaps
 
 // `two_phase`: a two-phase host step (mailbox_launch; deep_sea and catch only).  `mask`: a masked call, rollout or
 // host step (`episodes_left`: the budgets, nullable; `mask_out`: a budgeted host step's mask write-back, nullable;
-// `previous`: a budgeted step's previous outputs, nullable).
+// `previous`: a budgeted step's previous outputs, nullable; `policy`: a budgeted step's selection rule, nullable).
 int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr,
         const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr,
-        const bsb_outputs* previous = nullptr) {
+        const bsb_outputs* previous = nullptr, const bsb_policy* policy = nullptr) {
   DeviceGuard guard(e->device);
   LaunchArgs a = args;
   if (e->device >= 0) {
@@ -97,7 +97,7 @@ int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseA
     if (capture != cudaStreamCaptureStatusNone) e->graph_safe = true;
     if (e->graph_safe) a.clock = e->clock;      // a.step0 == e->steps_done, which no longer moves
   }
-  if (mask) return e->variant->run_masked(e, a, mask, episodes_left, mask_out, previous, stream);
+  if (mask) return e->variant->run_masked(e, a, mask, episodes_left, mask_out, previous, policy, stream);
   return e->variant->run(e, a, stream, two_phase);
 }
 
@@ -571,6 +571,9 @@ static int32_t create_env(const bsb_config* config, int64_t batch, int32_t devic
     }
     e->bad_action_host = static_cast<int32_t*>(flag); *e->bad_action_host = 0;
     e->bad_action_dev = static_cast<int32_t*>(flag_dev);
+  } else {
+    e->bad_action_flag = 0;
+    e->bad_action_host = &e->bad_action_flag;
   }
   // lane state
   BSB_TRY(env_alloc_t(e, &p.st_word, B, true));
@@ -854,11 +857,11 @@ int32_t bsb_step(bsb_env* env, const int32_t* actions, const bsb_outputs* out, v
 // mask[i] != 0 (run_masked), a rollout's or host step's lanes only while their budgets last.  Host handles validate
 // the actions of masked-in lanes only, at every step of a rollout (a host step: of lanes with budget left): an
 // inactive lane's action is never read.  `mask_out`: a budgeted host step's write-back, or a budgeted step's mask;
-// `previous`: a budgeted step's previous outputs (run_masked).
+// `previous`: a budgeted step's previous outputs; `policy`: the rule that picks a budgeted step's actions (run_masked).
 static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask, const bsb_outputs* out, void* stream,
                        int mode, int64_t T = 1, bool rollout = false, uint64_t action_seed = 0,
                        int32_t* actions_out = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr,
-                       const bsb_outputs* previous = nullptr) {
+                       const bsb_outputs* previous = nullptr, const bsb_policy* policy = nullptr) {
   { int crc = check_final_observation(env, out); if (crc != BSB_OK) return crc; }
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
   if (env->device < 0 && mode == MODE_STEP && actions) {
@@ -873,7 +876,7 @@ static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask
   }
   LaunchArgs a = make_args(env, out, mode == MODE_STEP ? actions : nullptr, T, mode);
   a.action_seed = action_seed; a.actions_out = actions_out;
-  int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask, episodes_left, mask_out, previous);
+  int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask, episodes_left, mask_out, previous, policy);
   if (rc == BSB_OK) advance_steps(env, T);
   return rc;
 }
@@ -927,17 +930,43 @@ int32_t bsb_advance_masked(bsb_env* env, int64_t num_steps, uint64_t action_seed
 // One masked step with budgets that first keeps the masked-in lanes' current outputs in `previous`: masked_kernel's
 // CALL_BUDGETED instantiation (run_masked), or host_budgeted on a host handle.  The mask is cleared in place one call
 // after a lane's budget is spent.
-int32_t bsb_step_budgeted(bsb_env* env, const int32_t* actions, uint8_t* mask, int64_t* episodes_left,
-                          const bsb_outputs* out, const bsb_outputs* previous, void* stream) {
-  if (!env || !actions || !mask || !episodes_left || !out || !previous || !out->observation || !previous->observation)
-    return fail(BSB_INVALID_ARGUMENT, "bsb_step_budgeted needs actions, a mask, budgets and two output sets with "
+// The refusals bsb_step_budgeted and bsb_step_budgeted_policy share (`choice`: the actions or the policy).
+static int check_budgeted(const bsb_env* env, const void* choice, const uint8_t* mask, const int64_t* episodes_left,
+                          const bsb_outputs* out, const bsb_outputs* previous, const std::string& name,
+                          const char* what) {
+  if (!env || !choice || !mask || !episodes_left || !out || !previous || !out->observation || !previous->observation)
+    return fail(BSB_INVALID_ARGUMENT, name + " needs " + what + ", a mask, budgets and two output sets with "
                                       "observation buffers");
   if (previous->observation == out->observation)
-    return fail(BSB_INVALID_ARGUMENT, "bsb_step_budgeted needs `previous` to have its own observation buffer");
+    return fail(BSB_INVALID_ARGUMENT, name + " needs `previous` to have its own observation buffer");
   if (!out->final_observation != !previous->final_observation)
     return fail(BSB_INVALID_ARGUMENT, "final_observation must be set in both output sets or in neither");
-  { int crc = check_final_observation(env, previous); if (crc != BSB_OK) return crc; }
+  return check_final_observation(env, previous);
+}
+
+int32_t bsb_step_budgeted(bsb_env* env, const int32_t* actions, uint8_t* mask, int64_t* episodes_left,
+                          const bsb_outputs* out, const bsb_outputs* previous, void* stream) {
+  { int rc = check_budgeted(env, actions, mask, episodes_left, out, previous, "bsb_step_budgeted", "actions"); if (rc != BSB_OK) return rc; }
   return masked_call(env, actions, mask, out, stream, MODE_STEP, 1, false, 0, nullptr, episodes_left, mask, previous);
+}
+
+// bsb_step_budgeted with each stepping lane's action chosen from its row of policy->values on the policy stream:
+// masked_kernel's CALL_POLICY instantiation (run_masked), or host_policy on a host handle.
+int32_t bsb_step_budgeted_policy(bsb_env* env, const bsb_policy* policy, uint8_t* mask, int64_t* episodes_left,
+                                 const bsb_outputs* out, const bsb_outputs* previous, int32_t* actions_out,
+                                 void* stream) {
+  const std::string name = "bsb_step_budgeted_policy";
+  { int rc = check_budgeted(env, policy, mask, episodes_left, out, previous, name, "a policy"); if (rc != BSB_OK) return rc; }
+  if (!policy->values) return fail(BSB_INVALID_ARGUMENT, name + " needs the policy's values");
+  if (policy->kind != BSB_POLICY_EPSILON_GREEDY && policy->kind != BSB_POLICY_SOFTMAX)
+    return fail(BSB_INVALID_ARGUMENT, "unknown policy kind " + std::to_string(policy->kind));
+  if (policy->reserved != 0) return fail(BSB_INVALID_ARGUMENT, "bsb_policy.reserved must be 0");
+  if (policy->kind == BSB_POLICY_EPSILON_GREEDY && !(policy->epsilon >= 0.0 && policy->epsilon <= 1.0))
+    return fail(BSB_INVALID_ARGUMENT, "epsilon must lie in [0, 1], got " + std::to_string(policy->epsilon));
+  if (policy->kind == BSB_POLICY_SOFTMAX && policy->epsilon != 0.0)
+    return fail(BSB_INVALID_ARGUMENT, "a softmax policy takes no epsilon: it must be 0");
+  return masked_call(env, nullptr, mask, out, stream, MODE_STEP, 1, false, 0, actions_out, episodes_left, mask, previous,
+                     policy);
 }
 
 int32_t bsb_random_actions(uint64_t action_seed, uint64_t lane_offset, int64_t batch, int64_t first_step,

@@ -30,15 +30,17 @@ template <class V> int run_variant(bsb_env*, const LaunchArgs&, cudaStream_t, co
 // bsb_advance_masked / bsb_step_budgeted): `mask` [B] and `episodes_left` [B] (nullable) live where the handle's
 // state does, or `mask` is a pinned host buffer's device alias.  `mask_out` (masked host steps with budgets and
 // budgeted steps, else null): where spent lanes' mask bytes are cleared.  `previous` (budgeted steps, else null): the
-// outputs that receive the masked-in lanes' current entries before the step.
+// outputs that receive the masked-in lanes' current entries before the step.  `policy` (bsb_step_budgeted_policy,
+// else null): the rule that chooses a budgeted step's actions.
 template <class V> int run_masked(bsb_env*, const LaunchArgs&, const uint8_t* mask, int64_t* episodes_left,
-                                  uint8_t* mask_out, const bsb_outputs* previous, cudaStream_t);
+                                  uint8_t* mask_out, const bsb_outputs* previous, const bsb_policy* policy, cudaStream_t);
 // An entry of the variant list, as bsb_create looks it up (bsb_engine.cu).
 struct VariantEntry {
   int family, obs_dtype, mode;
   bool mt, two_phase;
   int (*run)(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs*);
-  int (*run_masked)(bsb_env*, const LaunchArgs&, const uint8_t*, int64_t*, uint8_t*, const bsb_outputs*, cudaStream_t);
+  int (*run_masked)(bsb_env*, const LaunchArgs&, const uint8_t*, int64_t*, uint8_t*, const bsb_outputs*, const bsb_policy*,
+                    cudaStream_t);
 };
 
 #define BSB_CUDA(expr)                                                                   \
@@ -89,8 +91,10 @@ struct bsb_env {
   cudaEvent_t order_event;            // BSB_HOST_ORDER_AFTER_STREAM: fences copy_stream behind the caller's stream
   cudaEvent_t fence_event;            // BSB_HOST_FENCE_CALLER: fences the caller's stream behind a two-phase host step
   // Out-of-range actions (ADVICE r01): the kernels clamp them before any table index or state packing and raise
-  // this pinned flag; bsb_step_host / bsb_invalid_actions report it.
+  // this pinned flag; bsb_step_host / bsb_invalid_actions report it.  A host handle's flag is bad_action_flag, which
+  // only bsb_step_budgeted_policy raises (for invalid value rows): its actions are validated before anything moves.
   int32_t* bad_action_host; int32_t* bad_action_dev;
+  int32_t bad_action_flag;
   // Host-driven steps without a stream synchronise (bsb_step_host on pinned buffers): the kernel signals completion
   // through a pinned mailbox the host spins on (bsb_kernels.cuh, HostMailbox).
   bsb::HostMailbox* mailbox; bsb::HostMailbox* mailbox_dev; bsb::DeviceMail* mail;

@@ -1496,6 +1496,12 @@ struct MaskArgs {
   int32_t* prev_step_type;
   float* prev_final_obs;
   int32_t prev_vec_ok, prev_final_vec_ok;
+  // bsb_step_budgeted_policy: the agent's values [B, num_actions] (action values or logits), the selection rule
+  // (POLICY_*), epsilon and the policy stream's seed (null / 0 for every other call)
+  const float* policy_values;
+  double policy_epsilon;
+  uint64_t policy_seed;
+  int32_t policy_kind;
 };
 
 // What one masked_kernel instantiation runs.  CALL_ROLLOUT: bsb_rollout_masked (T steps, sampled or given actions,
@@ -1504,7 +1510,9 @@ struct MaskArgs {
 // CALL_ADVANCE: bsb_advance_masked (T steps of sampled actions, optional budgets, no per-step output at all).
 // CALL_BUDGETED: bsb_step_budgeted (CALL_HOST without the mailbox: T = 1, the caller's actions, budgets, the masked-in
 // lanes' outputs copied to `previous` first, and the mask cleared for lanes whose budget was spent before the call).
-enum CallKind { CALL_ROLLOUT = 0, CALL_ONE = 1, CALL_HOST = 2, CALL_ADVANCE = 3, CALL_BUDGETED = 4 };
+// CALL_POLICY: bsb_step_budgeted_policy (CALL_BUDGETED with each stepping lane's action chosen from its row of the
+// policy's values by select_action, and written to actions_out).
+enum CallKind { CALL_ROLLOUT = 0, CALL_ONE = 1, CALL_HOST = 2, CALL_ADVANCE = 3, CALL_BUDGETED = 4, CALL_POLICY = 5 };
 
 // Writes lane j's observation `val(e)` (element e of K) with the whole warp: 16-byte streaming stores when `vec`
 // (the row starts 16-byte aligned and is a whole number of 16-byte words), else one element per store.
@@ -1603,11 +1611,14 @@ __device__ __forceinline__ void copy_lane_subset(const O* src, O* dst, int K, in
 // kCall == CALL_BUDGETED: CALL_HOST without the mailbox, where every masked-in lane (budget left or not) first copies
 // its current entries of the outputs -- observation row, scalars, final observation -- to `previous`
 // (copy_lane_subset; the warp syncs before any new row is written), and a masked-in lane whose budget was spent before
-// the call clears its mask byte instead of stepping.
+// the call clears its mask byte instead of stepping.  kCall == CALL_POLICY: CALL_BUDGETED where a stepping lane reads
+// its row of m.policy_values instead of an action and picks with select_action, keyed by (m.policy_seed, global lane)
+// at the call's step index; the pick goes to a.actions_out (nullable) and an invalid row raises a.bad_action.
 template <class V, int RK, int kCall>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(const EnvParams p, const LaunchArgs a, const MaskArgs m) {
   // one call: T = 1 and the caller's actions
-  constexpr bool kOneCall = kCall == CALL_ONE || kCall == CALL_HOST || kCall == CALL_BUDGETED;
+  constexpr bool kOneCall = kCall == CALL_ONE || kCall == CALL_HOST || kCall == CALL_BUDGETED || kCall == CALL_POLICY;
+  constexpr bool kKeepPrevious = kCall == CALL_BUDGETED || kCall == CALL_POLICY;     // a budgeted step
   constexpr bool kEmit = kCall != CALL_ADVANCE;                           // the call writes per-step outputs
   typedef typename V::Fam Fam;
   typedef typename V::Obs O;
@@ -1645,7 +1656,7 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(c
     int64_t left = selected && budgets ? budgets[lane] : 0;
     bool on = selected && (!budgets || left > 0);
     const bool opened = on;
-    if constexpr (kCall == CALL_BUDGETED) {      // the outputs of the call before this one, for the agent (T = 1)
+    if constexpr (kKeepPrevious) {      // the outputs of the call before this one, for the agent (T = 1)
       O* prev_block = reinterpret_cast<O*>(m.prev_obs) + (block - reinterpret_cast<O*>(a.obs));
       copy_lane_subset<Fam>(block, prev_block, lp.obs_numel, local_base, selected, a.obs_vec_ok != 0 && m.prev_vec_ok != 0);
       if constexpr (V::kSameStep) {
@@ -1677,16 +1688,24 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(c
       if (on) {
         int32_t action = 0;
         if (mode == MODE_STEP) {
-          if (kCall != CALL_ADVANCE && (kOneCall || a.actions)) {
-            action = a.actions[off];
-            if ((uint32_t)action >= (uint32_t)p.num_actions) {
-              if (a.bad_action) *a.bad_action = 1;
-              action = action < 0 ? 0 : p.num_actions - 1;
-            }
+          if constexpr (kCall == CALL_POLICY) {
+            bool invalid = false;
+            action = select_action(m.policy_kind, m.policy_values + lane * (int64_t)p.num_actions, p.num_actions,
+                                   m.policy_epsilon, m.policy_seed, lp.lane_offset + (uint64_t)lane, (uint64_t)step0, invalid);
+            if (invalid && a.bad_action) *a.bad_action = 1;
+            if (a.actions_out) a.actions_out[lane] = action;
           } else {
-            action = action_stream.sample(a.action_seed, lp.lane_offset + (uint64_t)lane, (uint64_t)(step0 + t), p.num_actions);
+            if (kCall != CALL_ADVANCE && (kOneCall || a.actions)) {
+              action = a.actions[off];
+              if ((uint32_t)action >= (uint32_t)p.num_actions) {
+                if (a.bad_action) *a.bad_action = 1;
+                action = action < 0 ? 0 : p.num_actions - 1;
+              }
+            } else {
+              action = action_stream.sample(a.action_seed, lp.lane_offset + (uint64_t)lane, (uint64_t)(step0 + t), p.num_actions);
+            }
+            if (kCall == CALL_ROLLOUT && a.actions_out) a.actions_out[off] = action;
           }
-          if (kCall == CALL_ROLLOUT && a.actions_out) a.actions_out[off] = action;
         }
         if constexpr (V::kSameStep) lane_step<Fam, R, true>(p, lane, L, rng, wrng, ep, action, mode, noise, track, step0 + t, out, off, &merged);
         else lane_step<Fam>(lp, lane, L, rng, wrng, ep, action, mode, noise, track, step0 + t, out, off);
@@ -1715,7 +1734,7 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(c
     if constexpr (kCall == CALL_HOST) { if (selected && budgets && left <= 0 && m.mask_out) m.mask_out[lane] = 0; }
     // a budgeted step clears the mask one call after the budget is spent: on the call that returns the lane's last
     // LAST `previous` still holds the timestep before it, on the next one both buffers hold the LAST
-    if constexpr (kCall == CALL_BUDGETED) { if (selected && !opened) m.mask_out[lane] = 0; }
+    if constexpr (kKeepPrevious) { if (selected && !opened) m.mask_out[lane] = 0; }
   }
 
   if constexpr (kCall == CALL_HOST) { if (a.mailbox) signal_done(a); }

@@ -61,7 +61,7 @@ BSB_HD PhiloxBlock philox4x64_10(u64 c0, u64 c1, u64 c2, u64 c3, u64 k0, u64 k1)
 }
 
 // Stream ids carried in counter word 3.
-enum : u64 { STREAM_ENV = 0, STREAM_WRAPPER = 1, STREAM_ACTIONS = 2 };
+enum : u64 { STREAM_ENV = 0, STREAM_WRAPPER = 1, STREAM_ACTIONS = 2, STREAM_POLICY = 3 };
 
 // On-device uniform random actions (the workload of baselines/random/agent.py:35-37).
 // The action stream of a lane is the Philox stream (key = (action_seed, global lane), counter word 3 =
@@ -84,6 +84,84 @@ struct ActionStream {
 BSB_HD int32_t sample_action(u64 action_seed, u64 global_lane, u64 step, int32_t n) {
   ActionStream s; s.open();
   return s.sample(action_seed, global_lane, step, n);
+}
+
+// exp(x) built from + - * and ldexp alone, so the host path and the kernels (compiled with --fmad=false /
+// -ffp-contract=off) compute the same bits, which libm's and libdevice's exp do not.  x = k ln2 + r with k the nearest
+// integer to x / ln2 (the 1.5 * 2^52 shift) and ln2 split Cody-Waite style (k * hi is exact), |r| <= ln2 / 2; exp(r)
+// is its Taylor series to r^13 (truncation below 2^-57), evaluated as 1 + (r + r^2 q(r)).  Results in [-745, 0]
+// are within one ulp of the exact value (DESIGN.md §3, "Policy steps").  A subnormal result is scaled in two steps,
+// the last one a multiplication, so it is rounded once as IEEE rounds it.  x <= -746 (and -inf) gives 0.
+BSB_HD double bsb_exp(double x) {
+  if (!(x > -746.0)) return x != x ? x : 0.0;
+  if (x > 709.8) return INFINITY;
+  const double shift = 6755399441055744.0;
+  const double kd = (x * 1.4426950408889634 + shift) - shift;
+  const double r = (x - kd * 0.6931471803691238) - kd * 1.9082149292705877e-10;
+  double q = 1.6059043836821613e-10;
+  q = q * r + 2.08767569878681e-09;
+  q = q * r + 2.505210838544172e-08;
+  q = q * r + 2.755731922398589e-07;
+  q = q * r + 2.7557319223985893e-06;
+  q = q * r + 2.48015873015873e-05;
+  q = q * r + 0.0001984126984126984;
+  q = q * r + 0.001388888888888889;
+  q = q * r + 0.008333333333333333;
+  q = q * r + 0.041666666666666664;
+  q = q * r + 0.16666666666666666;
+  q = q * r + 0.5;
+  const double p = 1.0 + (r + (r * r) * q);
+  const int k = (int)kd;
+  if (k < -1021) return ldexp(p, k + 600) * 2.409919865102884e-181;      // 2^-600
+  return ldexp(p, k);
+}
+
+// Agents' action selection inside a budgeted step (bsb_step_budgeted_policy).  Lane g's draw at global step s is the
+// Philox block at counter (s, 0, 0, STREAM_POLICY) with key (seed, g); w0 decides exploration, lo32(w1) picks among
+// actions (multiply-shift, as ActionStream maps a chunk) and w1 >> 11 places softmax's target.
+enum : int32_t { POLICY_EPSILON_GREEDY = 0, POLICY_SOFTMAX = 1 };
+
+// The action `kind` picks from `row` (n floats: action values or logits).  A row with NaN, or for softmax a row with
+// +inf or without a finite entry, sets `invalid` and gets a uniform pick.  Epsilon-greedy: with u = (w0 >> 11) 2^-53,
+// u < epsilon explores uniformly; otherwise the pick is among the k entries equal to the row's maximum (±inf are
+// ordinary values), in ascending order.  Softmax: weights bsb_exp(l_a - max) (-inf weighs 0), the first action whose
+// running sum exceeds u' * sum with u' = (w1 >> 11) 2^-53, or the last action of positive weight when rounding leaves
+// none.  The weights are computed twice rather than stored, since a row may be of any length.
+BSB_HD int32_t select_action(int32_t kind, const float* row, int32_t n, double epsilon, u64 seed, u64 global_lane,
+                             u64 step, bool& invalid) {
+  const PhiloxBlock b = philox4x64_10(step, 0, 0, STREAM_POLICY, seed, global_lane);
+  const u32 pick = (u32)b.v1;
+  float m = -INFINITY;
+  bool nan = false;
+  for (int32_t a = 0; a < n; ++a) {
+    const float v = row[a];
+    if (v != v) nan = true;
+    else if (v > m) m = v;
+  }
+  const int32_t uniform = (int32_t)(((u64)pick * (u64)(u32)n) >> 32);
+  if (nan || (kind == POLICY_SOFTMAX && (m == INFINITY || m == -INFINITY))) { invalid = true; return uniform; }
+  if (kind == POLICY_EPSILON_GREEDY) {
+    if ((double)(b.v0 >> 11) * 1.1102230246251565e-16 < epsilon) return uniform;      // 2^-53
+    u32 k = 0;
+    for (int32_t a = 0; a < n; ++a) k += row[a] == m ? 1u : 0u;
+    u32 j = (u32)(((u64)pick * (u64)k) >> 32);
+    for (int32_t a = 0; a < n; ++a)
+      if (row[a] == m && j-- == 0u) return a;
+    return n - 1;
+  }
+  const double top = (double)m;
+  double total = 0.0;
+  for (int32_t a = 0; a < n; ++a) total += bsb_exp((double)row[a] - top);
+  const double target = ((double)(b.v1 >> 11) * 1.1102230246251565e-16) * total;
+  double run = 0.0;
+  int32_t last = 0;
+  for (int32_t a = 0; a < n; ++a) {
+    const double w = bsb_exp((double)row[a] - top);
+    run += w;
+    if (w > 0.0) last = a;
+    if (run > target) return a;
+  }
+  return last;
 }
 
 // ---------------------------------------------------------------------------

@@ -21,6 +21,7 @@ import numpy as np
 from bsuite_b200 import _lib
 from bsuite_b200 import dm_env
 from bsuite_b200 import obs_memory
+from bsuite_b200 import rollouts
 from bsuite_b200.experiments import EnvSpec
 
 specs = dm_env.specs
@@ -462,8 +463,8 @@ class BatchedEnvironment:
       _lib.check(self._lib.bsb_reset(self._handle.ptr, ctypes.byref(outputs), self._stream()))
     return out.timestep()
 
-  def step(self, actions, out: Optional[StepBuffers] = None, mask=None, episodes_left=None,
-           previous: Optional[StepBuffers] = None):
+  def step(self, actions=None, out: Optional[StepBuffers] = None, mask=None, episodes_left=None,
+           previous: Optional[StepBuffers] = None, policy=None, policy_seed: int = 0):
     """base.Environment.step for every lane (base.py:59-65); actions int [B].
 
     `mask` (bool or uint8 tensor [B] on the environment's device; needs `out`): only the lanes where it is set step;
@@ -476,8 +477,17 @@ class BatchedEnvironment:
     takes one from it in place), else it sits out and its mask is cleared in place (a bool mask is viewed, not
     copied, so the caller's tensor is updated).  So on the call that returns a lane's last LAST, `previous` holds the
     timestep before it, and on the next call both hold the LAST.  An agent loop that passes `previous` to its update
-    needs no copies of its own (`rollouts.run_episodes`)."""
+    needs no copies of its own (`rollouts.run_episodes`).
+
+    `policy` (`rollouts.EpsilonGreedy(values, epsilon)` or `rollouts.Softmax(logits)`, float32 [B, num_actions]
+    contiguous on the device) replaces `actions` in a budgeted step (`bsb_step_budgeted_policy`): each lane that steps
+    picks its action from its row, drawing on the policy stream keyed by (`policy_seed`, global lane) at the call's
+    step index, and the picks land in `out.actions` (`make_buffers(with_actions=True)`); entries of lanes that sit out
+    are left as they are.  The call equals a budgeted step given those actions, bit for bit.  A row with NaN (softmax:
+    or +inf, or no finite entry) gets a uniform pick and raises `invalid_actions_seen()`."""
     torch = self._torch
+    if policy is not None:
+      return self._step_policy(actions, out, mask, episodes_left, previous, policy, policy_seed)
     if episodes_left is not None or previous is not None:
       return self._step_budgeted(actions, out, mask, episodes_left, previous)
     if mask is not None:
@@ -508,7 +518,8 @@ class BatchedEnvironment:
                                          self._stream()))
     return out.timestep()
 
-  def _step_budgeted(self, actions, out, mask, episodes_left, previous):
+  def _budgeted_args(self, out, mask, episodes_left, previous):
+    """The checked mask and bound output structs of a budgeted step."""
     if episodes_left is None or previous is None:
       raise ValueError('episodes_left and previous go together: a budgeted step needs both')
     if mask is None:
@@ -519,12 +530,51 @@ class BatchedEnvironment:
       raise ValueError('mask must be contiguous: it is updated in place')
     mask = self._mask(mask, out)
     self._episodes_left(episodes_left)
-    actions = self._device_actions(actions, (self._batch,))
     outputs = out._outputs if out._bound is self._obs_dtype else out.bind(self._obs_dtype)
     prev = previous._outputs if previous._bound is self._obs_dtype else previous.bind(self._obs_dtype)
+    return mask, outputs, prev
+
+  def _step_budgeted(self, actions, out, mask, episodes_left, previous):
+    mask, outputs, prev = self._budgeted_args(out, mask, episodes_left, previous)
+    actions = self._device_actions(actions, (self._batch,))
     self._async_work = True
     status = self._lib.bsb_step_budgeted(self._handle.ptr, actions.data_ptr(), mask.data_ptr(), episodes_left.data_ptr(),
                                          ctypes.byref(outputs), ctypes.byref(prev), self._stream())
+    if status:
+      _lib.check(status)
+    return out.timestep()
+
+  def _step_policy(self, actions, out, mask, episodes_left, previous, policy, policy_seed):
+    torch = self._torch
+    if actions is not None:
+      raise ValueError('policy replaces actions: pass one or the other')
+    if isinstance(policy, rollouts.EpsilonGreedy):
+      kind, values, epsilon = _lib.POLICY_EPSILON_GREEDY, policy.values, float(policy.epsilon)
+    elif isinstance(policy, rollouts.Softmax):
+      kind, values, epsilon = _lib.POLICY_SOFTMAX, policy.logits, 0.0
+    else:
+      raise ValueError(f'policy must be rollouts.EpsilonGreedy or rollouts.Softmax, got {type(policy).__name__}')
+    if episodes_left is None or previous is None:
+      raise ValueError('a policy step is a budgeted step: it needs episodes_left= and previous=')
+    shape = (self._batch, self._spec.num_actions)
+    if not (isinstance(values, torch.Tensor) and values.dtype is torch.float32 and tuple(values.shape) == shape
+            and values.device == self._device and values.is_contiguous()):
+      raise ValueError(f'policy values must be a contiguous float32 tensor of shape {shape} on {self._device}, got '
+                       f'{getattr(values, "dtype", type(values).__name__)} {tuple(getattr(values, "shape", ()))} on '
+                       f'{getattr(values, "device", None)}')
+    if out is not None and out.actions is None:
+      raise ValueError('a policy step writes the chosen actions to out.actions: make out with '
+                       'make_buffers(with_actions=True)')
+    mask, outputs, prev = self._budgeted_args(out, mask, episodes_left, previous)
+    chosen = out.actions
+    if not (chosen.dtype is torch.int32 and tuple(chosen.shape) == (self._batch,) and chosen.device == self._device
+            and chosen.is_contiguous()):
+      raise ValueError(f'out.actions must be a contiguous int32 tensor of shape ({self._batch},) on {self._device}')
+    spec = _lib.Policy(kind, 0, values.data_ptr(), epsilon, int(policy_seed) % (1 << 64))
+    self._async_work = True
+    status = self._lib.bsb_step_budgeted_policy(self._handle.ptr, ctypes.byref(spec), mask.data_ptr(),
+                                                episodes_left.data_ptr(), ctypes.byref(outputs), ctypes.byref(prev),
+                                                chosen.data_ptr(), self._stream())
     if status:
       _lib.check(status)
     return out.timestep()
@@ -656,7 +706,8 @@ class BatchedEnvironment:
   def invalid_actions_seen(self) -> bool:
     """True if a DEVICE-resident action tensor passed to `step()` / `rollout()` since the last call held a value
     outside [0, num_actions): the kernels clamp such actions before any table lookup and raise a flag (host
-    actions are rejected up front instead).  Synchronises the current stream."""
+    actions are rejected up front instead), or a policy step (`step(policy=...)`, on any device) met an invalid value
+    row.  Synchronises the current stream."""
     if self._ordinal >= 0:
       self._torch.cuda.current_stream(self._device).synchronize()
     seen = ctypes.c_int32()

@@ -5,6 +5,8 @@
     new_timestep)`); lanes reset themselves, so the loop is over steps, not episodes.  The reference loop itself
     runs unchanged on the B = 1 face (`DmEnvAdapter`): it only calls `reset()` / `step()`.
   * `RandomAgent` -- `bsuite/baselines/random/agent.py:26-45` with one generator call per step for the whole batch.
+  * `EpsilonGreedy` / `Softmax` -- the selection rules of the reference's dqn / boot_dqn and actor_critic agents,
+    which an agent's `select_policy` returns so that the budgeted step picks its actions on the device.
   * `run_episodes` / `run_random_episodes` -- `experiment.run` to each lane's episode budget, with any agent through
     budgeted steps (one launch per call), or with the random agent's actions sampled on the device through fused
     masked launches that write no per-step output (`advance`); `suite.SweepBatch.run_episodes` and
@@ -20,6 +22,18 @@
 """
 
 from typing import Any, NamedTuple, Optional
+
+
+class EpsilonGreedy(NamedTuple):
+  """Epsilon-greedy selection over action values (baselines/jax/dqn/agent.py:118-127): with probability `epsilon` a
+  uniform action, else the greedy one with ties broken uniformly.  `values`: float32 [B, num_actions]."""
+  values: Any
+  epsilon: float
+
+
+class Softmax(NamedTuple):
+  """A categorical sample over `logits` (baselines/jax/actor_critic/agent.py:102-108): float32 [B, num_actions]."""
+  logits: Any
 
 
 class Trajectory(NamedTuple):
@@ -102,13 +116,21 @@ class EpisodeLoop:
   (`suite.SweepBatch.run_episodes`): the budgets (`episode_budget`), the mask of the lanes still playing, the output
   buffers and the `previous` buffers the agent's update reads, and one masked reset of the lanes with a positive
   budget.  `step()` is one call of the agent and one budgeted step (`step(..., mask=, episodes_left=, previous=)`);
-  `any_left()` is the device flag "some lane has episodes left"."""
+  `any_left()` is the device flag "some lane has episodes left".
 
-  def __init__(self, agent, environment, num_episodes: Optional[int] = None):
+  An agent that defines `select_policy(timestep)` (returning `EpsilonGreedy` or `Softmax`) instead of
+  `select_action` has its actions chosen inside the step (`step(policy=..., policy_seed=...)`); its `update` receives
+  `out.actions`, where a lane that sat out keeps its last pick (0 before its first)."""
+
+  def __init__(self, agent, environment, num_episodes: Optional[int] = None, policy_seed: int = 0):
     self.agent, self.environment = agent, environment
+    self.uses_policy = not hasattr(agent, 'select_action') and hasattr(agent, 'select_policy')
+    self.policy_seed = int(policy_seed)
     self.left = episode_budget(environment, num_episodes)
     self.mask = self.left > 0
-    self.out, self.previous = environment.make_buffers(), environment.make_buffers()
+    self.out, self.previous = environment.make_buffers(with_actions=self.uses_policy), environment.make_buffers()
+    if self.uses_policy:
+      self.out.actions.zero_()
     self.timestep = environment.reset(out=self.out, mask=self.mask)
     # lanes without a budget are never stepped: their entries of `previous` show what `out` holds, as every other
     # lane's do from its first call on
@@ -120,14 +142,20 @@ class EpisodeLoop:
     return (self.left > 0).any()
 
   def step(self) -> None:
-    actions = self.agent.select_action(self.timestep)
-    self.timestep = self.environment.step(actions, out=self.out, mask=self.mask, episodes_left=self.left,
-                                          previous=self.previous)
+    if self.uses_policy:
+      policy = self.agent.select_policy(self.timestep)
+      self.timestep = self.environment.step(out=self.out, mask=self.mask, episodes_left=self.left,
+                                            previous=self.previous, policy=policy, policy_seed=self.policy_seed)
+      actions = self.out.actions
+    else:
+      actions = self.agent.select_action(self.timestep)
+      self.timestep = self.environment.step(actions, out=self.out, mask=self.mask, episodes_left=self.left,
+                                            previous=self.previous)
     self.calls += 1
     self.agent.update(self.previous.timestep(), actions, self.timestep)
 
 
-def run_episodes(agent, environment, num_episodes: Optional[int] = None, check_every: int = 16):
+def run_episodes(agent, environment, num_episodes: Optional[int] = None, check_every: int = 16, policy_seed: int = 0):
   """`experiment.run` (baselines/experiment.py:24-57) for B lanes: every lane plays exactly its episode budget and
   then stops, as the reference's loop stops after `num_episodes` episodes.
 
@@ -138,8 +166,11 @@ def run_episodes(agent, environment, num_episodes: Optional[int] = None, check_e
   [B]`, `update(timestep, actions, new_timestep)`); a finished lane's entries of the timestep keep its final LAST.
   Each call is one budgeted step (`step(..., mask=, episodes_left=, previous=)`, `EpisodeLoop`), which counts the
   budgets down and keeps the timestep the agent acted on on the device; the loop asks whether any lane is still
-  running once every `check_every` calls.  Returns the number of calls made after the first reset."""
-  loop = EpisodeLoop(agent, environment, num_episodes)
+  running once every `check_every` calls.  An agent with `select_policy(timestep)` instead of `select_action` returns
+  `EpsilonGreedy` / `Softmax` and has its actions chosen inside the step, on the policy stream keyed by
+  (`policy_seed`, global lane), so its exploration does not depend on how lanes are sharded or packed
+  (`EpisodeLoop`).  Returns the number of calls made after the first reset."""
+  loop = EpisodeLoop(agent, environment, num_episodes, policy_seed)
   check_every = max(int(check_every), 1)
   while loop.calls % check_every != 0 or bool(loop.any_left()):
     loop.step()

@@ -218,7 +218,8 @@ class SweepBatch:
     del reset_out
     return calls
 
-  def run_episodes(self, agents, num_episodes: Optional[int] = None, check_every: int = 16) -> Dict[str, int]:
+  def run_episodes(self, agents, num_episodes: Optional[int] = None, check_every: int = 16,
+                   policy_seed: int = 0) -> Dict[str, int]:
     """Plays every lane of every environment to its episode budget with the caller's agents; afterwards
     `local_returns`, the log rows and `analysis.bsuite_score(self)` hold the agents' results.
 
@@ -231,7 +232,10 @@ class SweepBatch:
     agent's `select_action` and `update` on that stream too, so different agents' kernels can overlap.  Every
     `check_every` lock-steps the host reads every remaining environment's "any lane left" flag with one
     device-to-host copy; an environment leaves the rotation once its lanes are done.  The caller's current stream
-    waits for all of them before this returns.  Returns the calls made after the reset per environment."""
+    waits for all of them before this returns.  Agents may define `select_policy` instead of `select_action`
+    (`rollouts.EpisodeLoop`); their policy streams are keyed by (`policy_seed`, lane within the setting), so a pack,
+    a per-id sweep and every shard pick the same actions for the same values.  Returns the calls made after the reset
+    per environment."""
     import contextlib  # pylint: disable=import-outside-toplevel
     from bsuite_b200 import rollouts  # pylint: disable=import-outside-toplevel
     torch = self._torch
@@ -249,7 +253,7 @@ class SweepBatch:
     loops = {}                         # kept until every stream has joined the caller's
     for k in keys:
       with on_stream(k):
-        loops[k] = rollouts.EpisodeLoop(agents[k], self.envs[k], num_episodes)
+        loops[k] = rollouts.EpisodeLoop(agents[k], self.envs[k], num_episodes, policy_seed)
     rotation = list(range(len(keys)))
     lock_steps = 0
     while rotation:

@@ -442,6 +442,55 @@ int32_t bsb_step_budgeted(bsb_env* env, const int32_t* actions, uint8_t* mask,
                           int64_t* episodes_left, const bsb_outputs* out,
                           const bsb_outputs* previous, void* stream);
 
+/*
+ * Policy step: bsb_step_budgeted where the engine chooses each lane's action
+ * from the agent's network output, so a learning agent's epsilon-greedy or
+ * softmax selection needs no kernels of its own.  The call equals
+ * bsb_step_budgeted(env, A, mask, episodes_left, out, previous, stream), bit
+ * for bit, where A holds the actions the policy picks; actions_out (int32
+ * [B], nullable) receives A[i] for every lane that stepped (mask set, budget
+ * left).  Other lanes' entries are not written and their value rows are
+ * never read.
+ *
+ * The policy stream: lane i's draw is the Philox4x64-10 block at counter
+ * (s, 0, 0, 3), s being the call's global step index (the step0 bsb_rollout
+ * samples at), with key (seed, global lane) -- keyed as bsb_rollout keys its
+ * sampled actions, so in a pack it is the lane within its setting.  Its words
+ * w0, w1 are all a lane uses.  It is stateless: nothing enters the state
+ * snapshot.
+ *   EPSILON_GREEDY: u = (w0 >> 11) * 2^-53; u < epsilon explores and picks
+ *     (lo32(w1) * A) >> 32.  Otherwise, with k entries equal (float ==) to
+ *     the row's maximum, the pick is the ((lo32(w1) * k) >> 32)-th of them in
+ *     ascending order.  +-inf are ordinary values.
+ *   SOFTMAX: w_a = exp((double)l_a - max) (-inf weighs 0), computed by an
+ *     exp the host path and the kernels share; target = ((w1 >> 11) *
+ *     2^-53) * sum(w).  The pick is the first a whose running double sum
+ *     exceeds the target, or the last a of positive weight if none does.
+ * A row containing NaN, or for SOFTMAX a row containing +inf or without a
+ * finite entry, raises the invalid-action flag (bsb_invalid_actions; host
+ * handles too) and that lane picks (lo32(w1) * A) >> 32.
+ * Refused (BSB_INVALID_ARGUMENT, before anything moves): whatever
+ * bsb_step_budgeted refuses, a NULL policy or values, an unknown kind, a
+ * non-zero `reserved`, epsilon outside [0, 1] or NaN, a non-zero epsilon for
+ * SOFTMAX.  values (float32 [B, A], contiguous) and actions_out live in the
+ * handle's memory space.  Accepts every handle bsb_step_budgeted accepts and
+ * may be captured: a replay reads values, mask and budgets as they are then,
+ * while kind, epsilon and seed replay as captured.
+ */
+typedef enum bsb_policy_kind { BSB_POLICY_EPSILON_GREEDY = 0, BSB_POLICY_SOFTMAX = 1 } bsb_policy_kind;
+typedef struct bsb_policy {
+  int32_t kind;          /* bsb_policy_kind */
+  int32_t reserved;      /* 0 */
+  const float* values;   /* float32 [B, num_actions], contiguous, in the handle's memory space:
+                            action values (EPSILON_GREEDY) or logits (SOFTMAX) */
+  double epsilon;        /* EPSILON_GREEDY: in [0, 1]; SOFTMAX: must be 0 */
+  uint64_t seed;         /* key of the policy stream */
+} bsb_policy;
+
+int32_t bsb_step_budgeted_policy(bsb_env* env, const bsb_policy* policy, uint8_t* mask,
+                                 int64_t* episodes_left, const bsb_outputs* out,
+                                 const bsb_outputs* previous, int32_t* actions_out, void* stream);
+
 /* Host mirror of the on-device action sampler: out int32 [T,B] (host). */
 int32_t bsb_random_actions(uint64_t action_seed, uint64_t lane_offset,
                            int64_t batch, int64_t first_step, int64_t num_steps,
@@ -473,8 +522,8 @@ int32_t bsb_read_episode_stats(bsb_env* env, int32_t field, double* dst,
 
 /*
  * CUDA graphs.  bsb_step / bsb_reset / bsb_rollout / the masked calls (bsb_reset_masked / bsb_step_masked /
- * bsb_rollout_masked / bsb_advance_masked / bsb_step_budgeted) / bsb_read_* / bsb_sum_* may be called on a stream
- * that is being captured.  A graph freezes launch arguments, so the first captured launch moves the handle's step
+ * bsb_rollout_masked / bsb_advance_masked / bsb_step_budgeted / bsb_step_budgeted_policy) / bsb_read_* / bsb_sum_* may
+ * be called on a stream that is being captured.  A graph freezes launch arguments, so the first captured launch moves the handle's step
  * counter (it indexes the on-device action stream and the Logging columns) and its chunk scheduler into device
  * memory, for good: replays and eager calls can then be mixed in any order, and bsb_steps_done / bsb_get_state
  * synchronise the device to read the counter back.  Consecutive captured steps keep their programmatic dependent
