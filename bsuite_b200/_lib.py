@@ -89,6 +89,12 @@ class Policy(ctypes.Structure):
               ('epsilon', ctypes.c_double), ('seed', ctypes.c_uint64)]
 
 
+class Replay(ctypes.Structure):
+  """struct bsb_replay: per-lane rings, or a sample's batch (num_added NULL)."""
+  _fields_ = [('capacity', ctypes.c_int64), ('num_added', ctypes.c_void_p), ('obs_tm1', ctypes.c_void_p),
+              ('action', ctypes.c_void_p), ('next', Outputs)]
+
+
 SCORE_MAX_SOURCES = 512      # bsb_score: sources per call
 # enum bsb_score_quantity: the row columns a score reads
 SCORE_QUANTITIES = ('episode', 'total_return', 'total_regret', 'raw_return', 'best_episode', 'total_perfect',
@@ -144,6 +150,13 @@ EXPORTS = {
     'bsb_step_budgeted_policy': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(Policy), ctypes.c_void_p,
                                                   ctypes.c_void_p, ctypes.POINTER(Outputs), ctypes.POINTER(Outputs),
                                                   ctypes.c_void_p, ctypes.c_void_p]),
+    'bsb_step_budgeted_record': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Policy),
+                                                  ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Outputs),
+                                                  ctypes.POINTER(Outputs), ctypes.c_void_p, ctypes.POINTER(Replay),
+                                                  ctypes.c_void_p]),
+    'bsb_replay_sample': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(Replay), ctypes.c_int64, ctypes.c_int64,
+                                           ctypes.c_uint64, ctypes.c_uint64, ctypes.POINTER(Replay), ctypes.c_void_p,
+                                           ctypes.c_void_p]),
     'bsb_random_actions': (ctypes.c_int32, [ctypes.c_uint64, ctypes.c_uint64, ctypes.c_int64, ctypes.c_int64,
                                             ctypes.c_int64, ctypes.c_int32, ctypes.c_void_p]),
     'bsb_steps_done': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64)]),

@@ -37,8 +37,8 @@ def variant_list():
 # bsb_variants.cu once per unit of the variant list, with its slice of the list.
 UNITS = [(os.path.basename(src)[:-3], src, []) for src in SOURCES if src != VARIANTS] + [
     (unit, VARIANTS, [f'-DBSB_UNIT=BSB_UNIT_{unit}']) for unit in variant_list()]
-HEADERS = [os.path.join(CSRC, f) for f in ('bsb_obs_dtype.h', 'bsb_rng.cuh', 'bsb_families.cuh', 'bsb_kernels.cuh', 'bsb_env.h',
-                                           'bsb_dispatch.cuh', 'bsb_score.cuh')] + [
+HEADERS = [os.path.join(CSRC, f) for f in ('bsb_obs_dtype.h', 'bsb_rng.cuh', 'bsb_families.cuh', 'bsb_kernels.cuh',
+                                           'bsb_masked_body.inc', 'bsb_env.h', 'bsb_dispatch.cuh', 'bsb_score.cuh')] + [
     os.path.join(os.path.dirname(HERE), 'include', 'bsuite_b200.h')]
 OUTPUT = os.path.join(HERE, 'libbsuite_b200.so')
 OBJ_DIR = os.path.join(HERE, 'build')

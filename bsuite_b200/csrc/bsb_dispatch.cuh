@@ -376,6 +376,66 @@ void host_policy(const bsb_env* e, const LaunchArgs& a, uint8_t* mask, int64_t* 
   host_budgeted<V>(e, chosen, mask, episodes_left, previous);
 }
 
+// bsb_step_budgeted_record on a host handle, as masked_kernel's CALL_RECORD runs it: host_policy (a policy) or
+// host_budgeted (the caller's actions), then every lane that stepped (mask set, budget left before the call) and whose
+// new step type is not FIRST appends its transition to slot num_added % capacity of its ring: o_tm1 from `previous`,
+// o_t from the new observation row (a same-step LAST: the final observation row), as raw bytes.
+template <class V>
+void host_record(const bsb_env* e, const LaunchArgs& a, uint8_t* mask, int64_t* episodes_left,
+                 const bsb_outputs* previous, const bsb_policy* policy, const bsb_replay& r) {
+  typedef typename V::Obs O;
+  const EnvParams& p = e->p;
+  const int64_t B = p.batch;
+  const RaggedTable* ragged = V::kRagged ? reinterpret_cast<const RaggedTable*>(p.pack) : nullptr;
+  const int64_t step_elems = V::kRagged ? ragged->step_elems : B * (int64_t)p.obs_numel;
+  std::vector<uint8_t> stepped((size_t)B, 0);
+  std::vector<int32_t> used((size_t)B, 0);
+  for (int64_t lane = 0; lane < B; ++lane) {
+    stepped[(size_t)lane] = mask[lane] && episodes_left[lane] > 0;
+    if (stepped[(size_t)lane] && !policy) {
+      const int32_t action = a.actions[lane];
+      used[(size_t)lane] = (uint32_t)action < (uint32_t)p.num_actions ? action : (action < 0 ? 0 : p.num_actions - 1);
+    }
+  }
+  if (policy) {
+    LaunchArgs picked = a;
+    picked.actions_out = used.data();
+    host_policy<V>(e, picked, mask, episodes_left, previous, *policy);
+    if (a.actions_out)
+      for (int64_t lane = 0; lane < B; ++lane)
+        if (stepped[(size_t)lane]) a.actions_out[lane] = used[(size_t)lane];
+  } else {
+    host_budgeted<V>(e, a, mask, episodes_left, previous);
+  }
+  const O* prev_obs = reinterpret_cast<const O*>(previous->observation);
+  const O* obs = reinterpret_cast<const O*>(a.obs);
+  const O* fin = reinterpret_cast<const O*>(a.final_obs);
+  O* ring_tm1 = reinterpret_cast<O*>(r.obs_tm1);
+  O* ring_obs = reinterpret_cast<O*>(r.next.observation);
+  for (int64_t lane = 0; lane < B; ++lane) {
+    const int32_t type = a.step_type[lane];
+    if (!stepped[(size_t)lane] || type == FIRST) continue;
+    const int64_t n = r.num_added[lane];
+    const int64_t slot = n % r.capacity;
+    r.num_added[lane] = n + 1;
+    const int64_t at = slot * B + lane;
+    r.action[at] = used[(size_t)lane];
+    if (r.next.reward) r.next.reward[at] = a.reward ? a.reward[lane] : (float)a.reward_f64[lane];
+    if (r.next.reward_f64) r.next.reward_f64[at] = a.reward_f64 ? a.reward_f64[lane] : (double)a.reward[lane];
+    if (r.next.discount) r.next.discount[at] = a.discount[lane];
+    if (r.next.step_type) r.next.step_type[at] = type;
+    int64_t row = lane * (int64_t)p.obs_numel, K = p.obs_numel;
+    if constexpr (V::kRagged) {
+      const RaggedSetting& s = ragged_setting(ragged, lane / ragged->pack.lanes_per_setting);
+      row = s.obs_offset + (lane - s.lane_shift) * (int64_t)s.obs_numel;
+      K = s.obs_numel;
+    }
+    const bool final_row = V::kSameStep && type == LAST;
+    memcpy(ring_tm1 + slot * step_elems + row, prev_obs + row, (size_t)K * sizeof(O));
+    memcpy(ring_obs + slot * step_elems + row, (final_row ? fin : obs) + row, (size_t)K * sizeof(O));
+  }
+}
+
 // Kernels and host path of variant V, the runner bsb_create stores in the handle.  The bit sources and kernels are
 // those the variant list (BSB_VARIANTS) compiles for V: bsb_create picks no runner for an MT19937 handle whose variant
 // lacks MT19937, and only a variant with two_phase_host_kernel is given `two_phase` (a two-phase host step).
@@ -412,10 +472,11 @@ int run_variant(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoP
 // instantiation; a launch with no observation buffer (bsb_advance_masked) takes CALL_ADVANCE; any other call with
 // nothing for the T loop, the action stream or the budgets to do (every masked reset and step) takes CALL_ONE.  A
 // budgeted step (`previous` given: bsb_step_budgeted, whose `mask_out` is the mask) takes CALL_BUDGETED, and one with a
-// `policy` (bsb_step_budgeted_policy: no actions, the picks to a.actions_out) takes CALL_POLICY.
+// `policy` (bsb_step_budgeted_policy: no actions, the picks to a.actions_out) takes CALL_POLICY.  A budgeted step with
+// a `replay` (bsb_step_budgeted_record, actions or a policy) takes CALL_RECORD.
 template <class V>
 int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* episodes_left, uint8_t* mask_out,
-               const bsb_outputs* previous, const bsb_policy* policy, cudaStream_t stream) {
+               const bsb_outputs* previous, const bsb_policy* policy, const bsb_replay* replay, cudaStream_t stream) {
   constexpr bool kMt = Compiled<V>::kMt;
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
   if (previous && (a.T != 1 || a.mode != MODE_STEP || !a.actions == !policy || (a.actions_out && !policy) ||
@@ -423,13 +484,15 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
     return fail(BSB_INTERNAL, "a budgeted step must be one step of the caller's actions or policy, with budgets, "
                               "clearing its mask");
   if (policy && !previous) return fail(BSB_INTERNAL, "a policy step must be a budgeted step");
+  if (replay && (!previous || !a.step_type)) return fail(BSB_INTERNAL, "a recorded step must be a budgeted step with step types");
   if (e->device < 0) {
-    if (policy) host_policy<V>(e, a, mask_out, episodes_left, previous, *policy);
+    if (replay) host_record<V>(e, a, mask_out, episodes_left, previous, policy, *replay);
+    else if (policy) host_policy<V>(e, a, mask_out, episodes_left, previous, *policy);
     else if (previous) host_budgeted<V>(e, a, mask_out, episodes_left, previous);
     else run_host<V>(e, a, mask, episodes_left);
     return BSB_OK;
   }
-  MaskArgs m;
+  RecordArgs m;                          // a MaskArgs for every kind but CALL_RECORD
   memset(&m, 0, sizeof(m));
   m.mask = mask;
   m.noise = e->p.wrapper == BSB_WRAP_REWARD_NOISE ? 1 : 0;
@@ -449,8 +512,14 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
   const bool one_call = a.T == 1 && !episodes_left && !a.actions_out && (a.mode != MODE_STEP || a.actions);
   auto go = [&](auto kind) {
     constexpr int kCall = decltype(kind)::value;
-    if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_kernel<V, 1, kCall>, e->p, la, m); }
-    return launch(e, la, g, stream, masked_kernel<V, 0, kCall>, e->p, la, m);
+    if constexpr (kCall == CALL_RECORD) {
+      if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_record_kernel<V, 1>, e->p, la, m); }
+      return launch(e, la, g, stream, masked_record_kernel<V, 0>, e->p, la, m);
+    } else {
+      const MaskArgs& base = m;
+      if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_kernel<V, 1, kCall>, e->p, la, base); }
+      return launch(e, la, g, stream, masked_kernel<V, 0, kCall>, e->p, la, base);
+    }
   };
   if (previous) {
     m.prev_obs = previous->observation;
@@ -466,8 +535,23 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
       m.policy_epsilon = policy->epsilon;
       m.policy_seed = policy->seed;
       m.policy_kind = policy->kind;
-      return go(std::integral_constant<int, CALL_POLICY>());
     }
+    if (replay) {
+      m.rec_capacity = replay->capacity;
+      m.rec_num_added = replay->num_added;
+      m.rec_obs_tm1 = replay->obs_tm1;
+      m.rec_action = replay->action;
+      m.rec_obs = replay->next.observation;
+      m.rec_reward = replay->next.reward;
+      m.rec_reward_f64 = replay->next.reward_f64;
+      m.rec_discount = replay->next.discount;
+      m.rec_step_type = replay->next.step_type;
+      m.rec_vec_ok = reinterpret_cast<uintptr_t>(replay->obs_tm1) % 16 == 0 &&
+                     reinterpret_cast<uintptr_t>(replay->next.observation) % 16 == 0 &&
+                     ((size_t)e->step_elems * (size_t)e->obs_elem_bytes) % 16 == 0 ? 1 : 0;
+      return go(std::integral_constant<int, CALL_RECORD>());
+    }
+    if (policy) return go(std::integral_constant<int, CALL_POLICY>());
     return go(std::integral_constant<int, CALL_BUDGETED>());
   }
   if (host_call) {

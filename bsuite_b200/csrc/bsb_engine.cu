@@ -85,10 +85,11 @@ template <class T> int env_alloc_t(bsb_env* e, T** out, size_t count, bool snaps
 
 // `two_phase`: a two-phase host step (mailbox_launch; deep_sea and catch only).  `mask`: a masked call, rollout or
 // host step (`episodes_left`: the budgets, nullable; `mask_out`: a budgeted host step's mask write-back, nullable;
-// `previous`: a budgeted step's previous outputs, nullable; `policy`: a budgeted step's selection rule, nullable).
+// `previous`: a budgeted step's previous outputs, nullable; `policy`: a budgeted step's selection rule, nullable;
+// `replay`: the rings a recorded step appends to, nullable).
 int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr,
         const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr,
-        const bsb_outputs* previous = nullptr, const bsb_policy* policy = nullptr) {
+        const bsb_outputs* previous = nullptr, const bsb_policy* policy = nullptr, const bsb_replay* replay = nullptr) {
   DeviceGuard guard(e->device);
   LaunchArgs a = args;
   if (e->device >= 0) {
@@ -97,7 +98,7 @@ int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseA
     if (capture != cudaStreamCaptureStatusNone) e->graph_safe = true;
     if (e->graph_safe) a.clock = e->clock;      // a.step0 == e->steps_done, which no longer moves
   }
-  if (mask) return e->variant->run_masked(e, a, mask, episodes_left, mask_out, previous, policy, stream);
+  if (mask) return e->variant->run_masked(e, a, mask, episodes_left, mask_out, previous, policy, replay, stream);
   return e->variant->run(e, a, stream, two_phase);
 }
 
@@ -857,11 +858,13 @@ int32_t bsb_step(bsb_env* env, const int32_t* actions, const bsb_outputs* out, v
 // mask[i] != 0 (run_masked), a rollout's or host step's lanes only while their budgets last.  Host handles validate
 // the actions of masked-in lanes only, at every step of a rollout (a host step: of lanes with budget left): an
 // inactive lane's action is never read.  `mask_out`: a budgeted host step's write-back, or a budgeted step's mask;
-// `previous`: a budgeted step's previous outputs; `policy`: the rule that picks a budgeted step's actions (run_masked).
+// `previous`: a budgeted step's previous outputs; `policy`: the rule that picks a budgeted step's actions; `replay`:
+// the rings a recorded step appends to (run_masked).
 static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask, const bsb_outputs* out, void* stream,
                        int mode, int64_t T = 1, bool rollout = false, uint64_t action_seed = 0,
                        int32_t* actions_out = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr,
-                       const bsb_outputs* previous = nullptr, const bsb_policy* policy = nullptr) {
+                       const bsb_outputs* previous = nullptr, const bsb_policy* policy = nullptr,
+                       const bsb_replay* replay = nullptr) {
   { int crc = check_final_observation(env, out); if (crc != BSB_OK) return crc; }
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
   if (env->device < 0 && mode == MODE_STEP && actions) {
@@ -876,7 +879,8 @@ static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask
   }
   LaunchArgs a = make_args(env, out, mode == MODE_STEP ? actions : nullptr, T, mode);
   a.action_seed = action_seed; a.actions_out = actions_out;
-  int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask, episodes_left, mask_out, previous, policy);
+  int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask, episodes_left, mask_out, previous, policy,
+               replay);
   if (rc == BSB_OK) advance_steps(env, T);
   return rc;
 }
@@ -930,7 +934,8 @@ int32_t bsb_advance_masked(bsb_env* env, int64_t num_steps, uint64_t action_seed
 // One masked step with budgets that first keeps the masked-in lanes' current outputs in `previous`: masked_kernel's
 // CALL_BUDGETED instantiation (run_masked), or host_budgeted on a host handle.  The mask is cleared in place one call
 // after a lane's budget is spent.
-// The refusals bsb_step_budgeted and bsb_step_budgeted_policy share (`choice`: the actions or the policy).
+// The refusals bsb_step_budgeted, bsb_step_budgeted_policy and bsb_step_budgeted_record share (`choice`: the actions or
+// the policy).
 static int check_budgeted(const bsb_env* env, const void* choice, const uint8_t* mask, const int64_t* episodes_left,
                           const bsb_outputs* out, const bsb_outputs* previous, const std::string& name,
                           const char* what) {
@@ -942,6 +947,19 @@ static int check_budgeted(const bsb_env* env, const void* choice, const uint8_t*
   if (!out->final_observation != !previous->final_observation)
     return fail(BSB_INVALID_ARGUMENT, "final_observation must be set in both output sets or in neither");
   return check_final_observation(env, previous);
+}
+
+// The refusals of a policy (bsb_step_budgeted_policy, bsb_step_budgeted_record).
+static int check_policy(const bsb_policy* policy, const std::string& name) {
+  if (!policy->values) return fail(BSB_INVALID_ARGUMENT, name + " needs the policy's values");
+  if (policy->kind != BSB_POLICY_EPSILON_GREEDY && policy->kind != BSB_POLICY_SOFTMAX)
+    return fail(BSB_INVALID_ARGUMENT, "unknown policy kind " + std::to_string(policy->kind));
+  if (policy->reserved != 0) return fail(BSB_INVALID_ARGUMENT, "bsb_policy.reserved must be 0");
+  if (policy->kind == BSB_POLICY_EPSILON_GREEDY && !(policy->epsilon >= 0.0 && policy->epsilon <= 1.0))
+    return fail(BSB_INVALID_ARGUMENT, "epsilon must lie in [0, 1], got " + std::to_string(policy->epsilon));
+  if (policy->kind == BSB_POLICY_SOFTMAX && policy->epsilon != 0.0)
+    return fail(BSB_INVALID_ARGUMENT, "a softmax policy takes no epsilon: it must be 0");
+  return BSB_OK;
 }
 
 int32_t bsb_step_budgeted(bsb_env* env, const int32_t* actions, uint8_t* mask, int64_t* episodes_left,
@@ -957,16 +975,208 @@ int32_t bsb_step_budgeted_policy(bsb_env* env, const bsb_policy* policy, uint8_t
                                  void* stream) {
   const std::string name = "bsb_step_budgeted_policy";
   { int rc = check_budgeted(env, policy, mask, episodes_left, out, previous, name, "a policy"); if (rc != BSB_OK) return rc; }
-  if (!policy->values) return fail(BSB_INVALID_ARGUMENT, name + " needs the policy's values");
-  if (policy->kind != BSB_POLICY_EPSILON_GREEDY && policy->kind != BSB_POLICY_SOFTMAX)
-    return fail(BSB_INVALID_ARGUMENT, "unknown policy kind " + std::to_string(policy->kind));
-  if (policy->reserved != 0) return fail(BSB_INVALID_ARGUMENT, "bsb_policy.reserved must be 0");
-  if (policy->kind == BSB_POLICY_EPSILON_GREEDY && !(policy->epsilon >= 0.0 && policy->epsilon <= 1.0))
-    return fail(BSB_INVALID_ARGUMENT, "epsilon must lie in [0, 1], got " + std::to_string(policy->epsilon));
-  if (policy->kind == BSB_POLICY_SOFTMAX && policy->epsilon != 0.0)
-    return fail(BSB_INVALID_ARGUMENT, "a softmax policy takes no epsilon: it must be 0");
+  { int rc = check_policy(policy, name); if (rc != BSB_OK) return rc; }
   return masked_call(env, nullptr, mask, out, stream, MODE_STEP, 1, false, 0, actions_out, episodes_left, mask, previous,
                      policy);
+}
+
+// The refusals a replay ring (`batch`: a sample's output, which has no counts) shares between the recorded step and
+// the sampler.
+static int check_ring(const bsb_replay* r, const std::string& name, const char* what, bool batch) {
+  if (!r || !r->obs_tm1 || !r->action || !r->next.observation || (!batch && !r->num_added))
+    return fail(BSB_INVALID_ARGUMENT, name + " needs " + what + " with obs_tm1, action, next.observation" +
+                                          (batch ? "" : " and num_added"));
+  if (batch && r->num_added) return fail(BSB_INVALID_ARGUMENT, name + ": a sample's batch has no num_added (NULL)");
+  if (r->capacity < 1 || r->capacity > INT32_MAX)
+    return fail(BSB_INVALID_ARGUMENT, name + ": capacity must lie in [1, 2^31 - 1], got " + std::to_string(r->capacity));
+  if (r->next.final_observation)
+    return fail(BSB_INVALID_ARGUMENT, name + ": a ring keeps no final observations (next.final_observation must be NULL)");
+  if (r->obs_tm1 == r->next.observation)
+    return fail(BSB_INVALID_ARGUMENT, name + ": obs_tm1 and next.observation must be separate buffers");
+  return BSB_OK;
+}
+
+// bsb_step_budgeted or bsb_step_budgeted_policy that appends each transition to its lane's ring: masked_kernel's
+// CALL_RECORD instantiation (run_masked), or host_record on a host handle.
+int32_t bsb_step_budgeted_record(bsb_env* env, const int32_t* actions, const bsb_policy* policy, uint8_t* mask,
+                                 int64_t* episodes_left, const bsb_outputs* out, const bsb_outputs* previous,
+                                 int32_t* actions_out, const bsb_replay* replay, void* stream) {
+  const std::string name = "bsb_step_budgeted_record";
+  if (!actions == !policy) return fail(BSB_INVALID_ARGUMENT, name + " takes actions or a policy: exactly one of them");
+  const void* choice = actions ? static_cast<const void*>(actions) : static_cast<const void*>(policy);
+  { int rc = check_budgeted(env, choice, mask, episodes_left, out, previous, name, actions ? "actions" : "a policy"); if (rc != BSB_OK) return rc; }
+  if (policy) { int rc = check_policy(policy, name); if (rc != BSB_OK) return rc; }
+  else if (actions_out) return fail(BSB_INVALID_ARGUMENT, name + ": actions_out reports a policy's picks: pass NULL with actions");
+  { int rc = check_ring(replay, name, "a replay", false); if (rc != BSB_OK) return rc; }
+  if (!out->step_type || !out->discount || (!out->reward && !out->reward_f64))
+    return fail(BSB_INVALID_ARGUMENT, name + " needs out's step_type, discount and reward (or reward_f64)");
+  for (const float* ring : {replay->obs_tm1, replay->next.observation})
+    if (ring == out->observation || ring == previous->observation || (out->final_observation && ring == out->final_observation))
+      return fail(BSB_INVALID_ARGUMENT, name + ": a ring observation buffer must not be out's or previous's");
+  if (env->same_step && !out->final_observation)
+    return fail(BSB_INVALID_ARGUMENT, name + " on a same-step handle needs out->final_observation: it is o_t of a LAST");
+  return masked_call(env, actions, mask, out, stream, MODE_STEP, 1, false, 0, actions_out, episodes_left, mask, previous,
+                     policy, replay);
+}
+
+// ----- replay sampling --------------------------------------------------------------------------------------------
+namespace bsb {
+namespace {
+
+// What one sample gathers (bsb_replay_sample).  Observation rows move as raw bytes: lane i's row is elements
+// [row_of(i), row_of(i) + K_i) of every slot of step_elems elements (a ragged pack: its setting's offset and length).
+struct SampleArgs {
+  const int64_t* num_added;
+  const uint8_t* obs_tm1; const uint8_t* obs;
+  const int32_t* action; const float* reward; const double* reward_f64; const float* discount; const int32_t* step_type;
+  uint8_t* out_tm1; uint8_t* out_obs;
+  int32_t* out_action; float* out_reward; double* out_reward_f64; float* out_discount; int32_t* out_step_type;
+  uint8_t* ready;
+  const RaggedTable* ragged;          // a ragged pack's settings (in the handle's memory space), else null
+  int64_t batch, lanes_per_setting, capacity, size, min_size, obs_numel, step_elems;
+  int32_t elem_bytes, vec_ok;         // vec_ok: the four observation buffers and every slot start 16-byte aligned
+  uint64_t seed, draw, lane_offset;
+  int64_t step0;                      // the call index; graph-safe mode adds the device clock
+  const unsigned long long* clock;
+};
+
+// (filled slots, ready) of lane i, and the first element and length of its observation row within a slot.
+BSB_HD void sample_lane(const SampleArgs& s, int64_t i, int64_t& n, bool& ok, int64_t& row, int64_t& K) {
+  n = s.num_added[i] < s.capacity ? s.num_added[i] : s.capacity;
+  ok = n >= (s.min_size > 1 ? s.min_size : 1);
+  row = i * s.obs_numel;
+  K = s.obs_numel;
+  if (s.ragged) {
+    const RaggedSetting& r = ragged_setting(s.ragged, i / s.ragged->pack.lanes_per_setting);
+    row = r.obs_offset + (i - r.lane_shift) * (int64_t)r.obs_numel;
+    K = r.obs_numel;
+  }
+}
+
+// The Philox block of samples 4 q .. 4 q + 3 of lane i at call index c: word j & 3 is sample j's.
+BSB_HD PhiloxBlock sample_block(const SampleArgs& s, int64_t c, int64_t i, int64_t q) {
+  return philox4x64_10((u64)c, s.draw, (u64)q, STREAM_REPLAY, s.seed, s.lane_offset + (u64)(i % s.lanes_per_setting));
+}
+
+// Sample j of lane i: slot `slot` of the ring to entry j of the batch.  `tid`, `threads`: this thread's share of the
+// row copy (the kernel's warp, or the whole row on the host).
+BSB_HD void sample_copy(const SampleArgs& s, int64_t i, int64_t j, int64_t slot, int64_t row, int64_t K, int tid,
+                        int threads) {
+  const int64_t from = slot * s.batch + i, to = j * s.batch + i;
+  if (tid == 0) {
+    s.out_action[to] = s.action[from];
+    if (s.out_reward) s.out_reward[to] = s.reward[from];
+    if (s.out_reward_f64) s.out_reward_f64[to] = s.reward_f64[from];
+    if (s.out_discount) s.out_discount[to] = s.discount[from];
+    if (s.out_step_type) s.out_step_type[to] = s.step_type[from];
+  }
+  const int64_t bytes = K * s.elem_bytes;
+  const int64_t src = (slot * s.step_elems + row) * s.elem_bytes, dst = (j * s.step_elems + row) * s.elem_bytes;
+  if (s.vec_ok && (row * s.elem_bytes) % 16 == 0 && bytes % 16 == 0) {
+    for (int64_t q = tid; q < bytes / 16; q += threads) {
+      reinterpret_cast<uint4*>(s.out_tm1 + dst)[q] = reinterpret_cast<const uint4*>(s.obs_tm1 + src)[q];
+      reinterpret_cast<uint4*>(s.out_obs + dst)[q] = reinterpret_cast<const uint4*>(s.obs + src)[q];
+    }
+  } else {
+    for (int64_t q = tid; q < bytes; q += threads) {
+      s.out_tm1[dst + q] = s.obs_tm1[src + q];
+      s.out_obs[dst + q] = s.obs[src + q];
+    }
+  }
+}
+
+// One warp per (group of four samples, lane i), lanes fastest: one Philox block for the group's four slots, then per
+// sample lane 0 moves the scalars and the warp both rows, with 16-byte loads and stores where the row and the buffers
+// allow.
+__global__ void __launch_bounds__(256) replay_sample_kernel(const SampleArgs s) {
+  const int tid = threadIdx.x & 31;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  const int64_t groups = (s.size + 3) / 4, items = groups * s.batch;
+  int64_t c = s.step0;
+  if (s.clock) c += (int64_t)*reinterpret_cast<const volatile unsigned long long*>(s.clock + 16 * (blockIdx.x % CLOCK_GROUPS));
+  for (int64_t item = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); item < items; item += warps) {
+    const int64_t q = item / s.batch, i = item - q * s.batch;
+    int64_t n, row, K;
+    bool ok;
+    sample_lane(s, i, n, ok, row, K);
+    if (q == 0 && tid == 0 && s.ready) s.ready[i] = ok ? 1 : 0;
+    if (!ok) continue;
+    const PhiloxBlock b = sample_block(s, c, i, q);
+    for (int64_t j = 4 * q; j < 4 * q + 4 && j < s.size; ++j)
+      sample_copy(s, i, j, replay_slot(replay_word(b, j), n), row, K, tid, 32);
+  }
+}
+
+// bsb_replay_sample on a host handle: the kernel's gather, lane by lane.
+void host_sample(const SampleArgs& s) {
+  for (int64_t i = 0; i < s.batch; ++i) {
+    int64_t n, row, K;
+    bool ok;
+    sample_lane(s, i, n, ok, row, K);
+    if (s.ready) s.ready[i] = ok ? 1 : 0;
+    if (!ok) continue;
+    for (int64_t q = 0; 4 * q < s.size; ++q) {
+      const PhiloxBlock b = sample_block(s, s.step0, i, q);
+      for (int64_t j = 4 * q; j < 4 * q + 4 && j < s.size; ++j)
+        sample_copy(s, i, j, replay_slot(replay_word(b, j), n), row, K, 0, 1);
+    }
+  }
+}
+
+}  // namespace
+}  // namespace bsb
+
+int32_t bsb_replay_sample(bsb_env* env, const bsb_replay* replay, int64_t size, int64_t min_size, uint64_t seed,
+                          uint64_t draw, const bsb_replay* batch, uint8_t* ready, void* stream) {
+  const std::string name = "bsb_replay_sample";
+  if (!env) return fail(BSB_INVALID_ARGUMENT, name + " needs a handle");
+  if (size <= 0) return fail(BSB_INVALID_ARGUMENT, name + ": size must be positive, got " + std::to_string(size));
+  if (min_size < 0) return fail(BSB_INVALID_ARGUMENT, name + ": min_size must not be negative, got " + std::to_string(min_size));
+  { int rc = check_ring(replay, name, "a replay", false); if (rc != BSB_OK) return rc; }
+  { int rc = check_ring(batch, name, "a batch", true); if (rc != BSB_OK) return rc; }
+  if (batch->capacity != size)
+    return fail(BSB_INVALID_ARGUMENT, name + ": the batch's capacity must equal size (" + std::to_string(size) + "), got " +
+                                          std::to_string(batch->capacity));
+  if ((batch->next.reward && !replay->next.reward) || (batch->next.reward_f64 && !replay->next.reward_f64) ||
+      (batch->next.discount && !replay->next.discount) || (batch->next.step_type && !replay->next.step_type))
+    return fail(BSB_INVALID_ARGUMENT, name + ": the batch asks for a scalar the ring does not carry");
+  { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
+  SampleArgs s;
+  memset(&s, 0, sizeof(s));
+  s.num_added = replay->num_added;
+  s.obs_tm1 = reinterpret_cast<const uint8_t*>(replay->obs_tm1);
+  s.obs = reinterpret_cast<const uint8_t*>(replay->next.observation);
+  s.action = replay->action; s.reward = replay->next.reward; s.reward_f64 = replay->next.reward_f64;
+  s.discount = replay->next.discount; s.step_type = replay->next.step_type;
+  s.out_tm1 = reinterpret_cast<uint8_t*>(batch->obs_tm1);
+  s.out_obs = reinterpret_cast<uint8_t*>(batch->next.observation);
+  s.out_action = batch->action; s.out_reward = batch->next.reward; s.out_reward_f64 = batch->next.reward_f64;
+  s.out_discount = batch->next.discount; s.out_step_type = batch->next.step_type;
+  s.ready = ready;
+  s.ragged = env->ragged ? reinterpret_cast<const RaggedTable*>(env->p.pack) : nullptr;
+  s.batch = env->p.batch; s.lanes_per_setting = env->lanes_per_setting;
+  s.capacity = replay->capacity; s.size = size; s.min_size = min_size;
+  s.obs_numel = env->p.obs_numel; s.step_elems = env->step_elems; s.elem_bytes = env->obs_elem_bytes;
+  s.vec_ok = ((size_t)env->step_elems * (size_t)env->obs_elem_bytes) % 16 == 0;
+  for (const float* buf : {replay->obs_tm1, replay->next.observation, batch->obs_tm1, batch->next.observation})
+    if (reinterpret_cast<uintptr_t>(buf) % 16 != 0) s.vec_ok = 0;
+  s.seed = seed; s.draw = draw; s.lane_offset = env->p.lane_offset;
+  s.step0 = env->steps_done;
+  if (env->device < 0) { host_sample(s); return BSB_OK; }
+  DeviceGuard guard(env->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+  BSB_CUDA(cudaStreamIsCapturing(st, &capture));
+  if (capture != cudaStreamCaptureStatusNone) env->graph_safe = true;
+  if (env->graph_safe) s.clock = env->clock;
+  const int64_t warps = (size + 3) / 4 * s.batch;
+  int64_t grid = (warps + 7) / 8;
+  const int64_t cap = (int64_t)env->num_sms * 64;
+  if (grid > cap) grid = cap;
+  replay_sample_kernel<<<(unsigned)grid, 256, 0, st>>>(s);
+  BSB_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return BSB_OK;
 }
 
 int32_t bsb_random_actions(uint64_t action_seed, uint64_t lane_offset, int64_t batch, int64_t first_step,

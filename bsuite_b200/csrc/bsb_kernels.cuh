@@ -1504,6 +1504,23 @@ struct MaskArgs {
   int32_t policy_kind;
 };
 
+// The arguments of a CALL_RECORD launch: MaskArgs grown at its end by the lanes' rings (bsb_replay).  The growth is a
+// struct of its own, passed to masked_record_kernel only: a larger MaskArgs changed the code ptxas emits for existing
+// masked kernels.  The action source is policy_values when non-null, else a.actions.  rec_vec_ok: both ring
+// observation buffers start 16-byte aligned and a slot is a whole number of 16-byte words.
+struct RecordArgs : MaskArgs {
+  int64_t rec_capacity;
+  int64_t* rec_num_added;
+  float* rec_obs_tm1;
+  int32_t* rec_action;
+  float* rec_obs;
+  float* rec_reward;
+  double* rec_reward_f64;
+  float* rec_discount;
+  int32_t* rec_step_type;
+  int32_t rec_vec_ok;
+};
+
 // What one masked_kernel instantiation runs.  CALL_ROLLOUT: bsb_rollout_masked (T steps, sampled or given actions,
 // budgets, actions_out).  CALL_ONE: a masked reset or step (T = 1, the caller's actions, no budgets).  CALL_HOST:
 // bsb_step_host_masked (T = 1, the caller's actions, optional budgets, the mask write-back, the mailbox signal).
@@ -1511,8 +1528,11 @@ struct MaskArgs {
 // CALL_BUDGETED: bsb_step_budgeted (CALL_HOST without the mailbox: T = 1, the caller's actions, budgets, the masked-in
 // lanes' outputs copied to `previous` first, and the mask cleared for lanes whose budget was spent before the call).
 // CALL_POLICY: bsb_step_budgeted_policy (CALL_BUDGETED with each stepping lane's action chosen from its row of the
-// policy's values by select_action, and written to actions_out).
-enum CallKind { CALL_ROLLOUT = 0, CALL_ONE = 1, CALL_HOST = 2, CALL_ADVANCE = 3, CALL_BUDGETED = 4, CALL_POLICY = 5 };
+// policy's values by select_action, and written to actions_out).  CALL_RECORD: bsb_step_budgeted_record
+// (CALL_BUDGETED or CALL_POLICY, chosen at run time by m.policy_values, with each transition appended to its lane's
+// ring).
+enum CallKind { CALL_ROLLOUT = 0, CALL_ONE = 1, CALL_HOST = 2, CALL_ADVANCE = 3, CALL_BUDGETED = 4, CALL_POLICY = 5,
+                CALL_RECORD = 6 };
 
 // Writes lane j's observation `val(e)` (element e of K) with the whole warp: 16-byte streaming stores when `vec`
 // (the row starts 16-byte aligned and is a whole number of 16-byte words), else one element per store.
@@ -1590,6 +1610,37 @@ __device__ __forceinline__ void copy_lane_subset(const O* src, O* dst, int K, in
   }
 }
 
+// Copies the rows row0 + tid of `src` ([rows, K] elements of O, raw bytes) into the same rows of slot `slot` of `ring`
+// (a slot is `stride` elements; `slot` is each lane's own) for the warp's lanes for which `on` holds, with streaming
+// stores: copy_lane_subset's walk, with each lane's slot taken from its thread.  `vec_base`: both buffers, and every
+// slot of `ring`, start 16-byte aligned.
+template <class F, class O>
+__device__ __forceinline__ void record_lane_rows(const O* src, O* ring, int64_t stride, int64_t slot, int K, int64_t row0,
+                                                 bool on, bool vec_base) {
+  const int tid = threadIdx.x & 31;
+  if (EmitKind<F>::value == EMIT_ROWS) {
+    if (on) {
+      const O* s = src + (row0 + tid) * (int64_t)K;
+      O* d = ring + slot * stride + (row0 + tid) * (int64_t)K;
+      for (int e = 0; e < K; ++e) st_stream(d + e, s[e]);
+    }
+    return;
+  }
+  const bool vec = vec_base && ((int64_t)K * (int64_t)sizeof(O)) % 16 == 0;
+  for (unsigned rest = __ballot_sync(0xffffffffu, on); rest != 0u; rest &= rest - 1u) {
+    const int j = __ffs(rest) - 1;
+    const int64_t c = __shfl_sync(0xffffffffu, (long long)slot, j);
+    const O* s = src + (row0 + j) * (int64_t)K;
+    O* d = ring + c * stride + (row0 + j) * (int64_t)K;
+    if (vec) {
+      const int words = (int)(((int64_t)K * (int64_t)sizeof(O)) >> 4);
+      for (int q = tid; q < words; q += 32) __stcs(reinterpret_cast<uint4*>(d) + q, reinterpret_cast<const uint4*>(s)[q]);
+    } else {
+      for (int e = tid; e < K; e += 32) st_stream(d + e, s[e]);
+    }
+  }
+}
+
 // Every masked call: a masked reset or step (T = 1, no budgets) or bsb_rollout_masked's T masked steps, in one launch.
 // One chunk of 32 lanes per warp; a ragged pack's chunks never straddle two settings, and row j of setting k goes to
 // the setting's block (emit_lane_subset).  Lane i is active at step t while mask[i] != 0 and its budget
@@ -1614,147 +1665,22 @@ __device__ __forceinline__ void copy_lane_subset(const O* src, O* dst, int K, in
 // the call clears its mask byte instead of stepping.  kCall == CALL_POLICY: CALL_BUDGETED where a stepping lane reads
 // its row of m.policy_values instead of an action and picks with select_action, keyed by (m.policy_seed, global lane)
 // at the call's step index; the pick goes to a.actions_out (nullable) and an invalid row raises a.bad_action.
+// kCall == CALL_RECORD: CALL_POLICY when m.policy_values is set, else CALL_BUDGETED; after the step every lane that
+// stepped and whose new step type is not FIRST appends (o_tm1, a_tm1, r_t, d_t, o_t) to slot num_added % capacity of
+// its ring and counts it.  The rows are copied, never rendered again (rendering draws for some families): o_tm1 from
+// the row the lane copied to `previous`, o_t from the row the warp has just emitted (a same-step LAST: the final
+// observation), after a __syncwarp.  The body (bsb_masked_body.inc) is shared with masked_record_kernel, which runs
+// CALL_RECORD.
 template <class V, int RK, int kCall>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(const EnvParams p, const LaunchArgs a, const MaskArgs m) {
-  // one call: T = 1 and the caller's actions
-  constexpr bool kOneCall = kCall == CALL_ONE || kCall == CALL_HOST || kCall == CALL_BUDGETED || kCall == CALL_POLICY;
-  constexpr bool kKeepPrevious = kCall == CALL_BUDGETED || kCall == CALL_POLICY;     // a budgeted step
-  constexpr bool kEmit = kCall != CALL_ADVANCE;                           // the call writes per-step outputs
-  typedef typename V::Fam Fam;
-  typedef typename V::Obs O;
-  typedef typename RngOf<RK>::type R;
-  const int tid = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_cta = blockDim.x >> 5;
-  int64_t step0 = a.step0;
-  if (a.clock) step0 += (int64_t)*reinterpret_cast<volatile unsigned long long*>(a.clock + 16 * (blockIdx.x % CLOCK_GROUPS));
-  const MailFields out = kEmit ? MailFields{a.reward, a.reward_f64, a.discount, a.step_type} : MailFields{};
-  const int32_t mode = kEmit ? a.mode : (int32_t)MODE_STEP;
-  const bool noise = m.noise != 0, track = m.track != 0;
-  const RaggedTable* table = V::kRagged ? reinterpret_cast<const RaggedTable*>(p.pack) : nullptr;
-  const int64_t lanes = V::kRagged ? table->pack.lanes_per_setting : p.batch;      // lanes per setting block
-  const int64_t per_setting = (lanes + 31) / 32;
-  const int64_t n_chunks = (V::kRagged ? table->pack.n_settings : 1) * per_setting;
-  const int64_t chunk = (int64_t)blockIdx.x * warps_per_cta + warp;
-  const int64_t T = kOneCall ? 1 : a.T;
-  int64_t* const budgets = kCall == CALL_ONE ? nullptr : m.episodes_left;
+#include "bsb_masked_body.inc"
+}
 
-  if (chunk < n_chunks) {
-    const int64_t k = chunk / per_setting;
-    const int64_t local_base = (chunk - k * per_setting) * 32;         // the chunk's first row within its block
-    const int64_t lane = k * lanes + local_base + tid;
-    const bool in = local_base + tid < lanes;
-    EnvParams lp = p;
-    O* block = reinterpret_cast<O*>(a.obs);
-    if constexpr (V::kRagged) {
-      const RaggedSetting& s = ragged_setting(table, k);
-      ragged_setting_params(lp, s, table->mapping_bits);
-      block += s.obs_offset;
-    } else if constexpr (V::kPacked) {
-      if (in) pack_lane_params(lp, lane);
-    }
-    const int64_t step_elems = V::kRagged ? table->step_elems : p.batch * (int64_t)p.obs_numel;
-    const bool selected = in && m.mask[lane] != 0;
-    int64_t left = selected && budgets ? budgets[lane] : 0;
-    bool on = selected && (!budgets || left > 0);
-    const bool opened = on;
-    if constexpr (kKeepPrevious) {      // the outputs of the call before this one, for the agent (T = 1)
-      O* prev_block = reinterpret_cast<O*>(m.prev_obs) + (block - reinterpret_cast<O*>(a.obs));
-      copy_lane_subset<Fam>(block, prev_block, lp.obs_numel, local_base, selected, a.obs_vec_ok != 0 && m.prev_vec_ok != 0);
-      if constexpr (V::kSameStep) {
-        if (a.final_obs && m.prev_final_obs)
-          copy_lane_subset<Fam>(reinterpret_cast<const O*>(a.final_obs), reinterpret_cast<O*>(m.prev_final_obs), lp.obs_numel,
-                                local_base, selected, a.final_vec_ok != 0 && m.prev_final_vec_ok != 0);
-      }
-      if (selected) {
-        if (a.reward && m.prev_reward) m.prev_reward[lane] = a.reward[lane];
-        if (a.reward_f64 && m.prev_reward_f64) m.prev_reward_f64[lane] = a.reward_f64[lane];
-        if (a.discount && m.prev_discount) m.prev_discount[lane] = a.discount[lane];
-        if (a.step_type && m.prev_step_type) m.prev_step_type[lane] = a.step_type[lane];
-      }
-      __syncwarp();
-    }
-
-    typename Fam::Lane L;
-    R rng, wrng;
-    EpisodeStats ep;
-    ActionStream action_stream;
-    action_stream.open();
-    Fam::init(p, L);
-    MergedReset<Fam, R> merged;            // same-step kernels only
-    if constexpr (V::kSameStep) { Fam::init(p, merged.last); merged.done = false; }
-    if (on) lane_open<Fam>(lp, lane, L, rng, wrng, ep, mode, noise, track);
-    int64_t acted = 0;                     // the lane's active steps
-    for (int64_t t = 0; t < T && (kOneCall || __any_sync(0xffffffffu, on)); ++t) {
-      const int64_t off = t * p.batch + lane;
-      if (on) {
-        int32_t action = 0;
-        if (mode == MODE_STEP) {
-          if constexpr (kCall == CALL_POLICY) {
-            bool invalid = false;
-            action = select_action(m.policy_kind, m.policy_values + lane * (int64_t)p.num_actions, p.num_actions,
-                                   m.policy_epsilon, m.policy_seed, lp.lane_offset + (uint64_t)lane, (uint64_t)step0, invalid);
-            if (invalid && a.bad_action) *a.bad_action = 1;
-            if (a.actions_out) a.actions_out[lane] = action;
-          } else {
-            if (kCall != CALL_ADVANCE && (kOneCall || a.actions)) {
-              action = a.actions[off];
-              if ((uint32_t)action >= (uint32_t)p.num_actions) {
-                if (a.bad_action) *a.bad_action = 1;
-                action = action < 0 ? 0 : p.num_actions - 1;
-              }
-            } else {
-              action = action_stream.sample(a.action_seed, lp.lane_offset + (uint64_t)lane, (uint64_t)(step0 + t), p.num_actions);
-            }
-            if (kCall == CALL_ROLLOUT && a.actions_out) a.actions_out[off] = action;
-          }
-        }
-        if constexpr (V::kSameStep) lane_step<Fam, R, true>(p, lane, L, rng, wrng, ep, action, mode, noise, track, step0 + t, out, off, &merged);
-        else lane_step<Fam>(lp, lane, L, rng, wrng, ep, action, mode, noise, track, step0 + t, out, off);
-      }
-      if constexpr (!kEmit) {
-        if (on) ObsDraws<Fam>::skip(lp, rng);    // the draws of the observation CALL_ROLLOUT would render here
-      } else {
-        if constexpr (V::kSameStep) {
-          if (a.final_obs)
-            emit_lane_subset<Fam>(lp, merged.last, merged.rng, reinterpret_cast<O*>(a.final_obs) + t * p.batch * (int64_t)p.obs_numel,
-                                  lp.obs_numel, local_base, on && merged.done, a.final_vec_ok != 0);
-        }
-        emit_lane_subset<Fam>(lp, L, rng, block + t * step_elems, lp.obs_numel, local_base, on, a.obs_vec_ok != 0);
-      }
-      if (on) {
-        ++acted;
-        // the step's LAST: a same-step lane's merged reset, else the _reset_next_step flag the step left set
-        const bool last = V::kSameStep ? merged.done : L.nr != 0;
-        if (budgets && last && --left == 0) on = false;
-      }
-    }
-    if (opened) lane_close<Fam>(lp, lane, L, rng, wrng, ep, noise, track);
-    if (in && track && acted < T) lane_sit_out_calls(p, lane, T - acted);
-    if (selected && budgets) budgets[lane] = left;
-    // the host's view of the lanes still running: only a lane whose budget is spent writes its byte
-    if constexpr (kCall == CALL_HOST) { if (selected && budgets && left <= 0 && m.mask_out) m.mask_out[lane] = 0; }
-    // a budgeted step clears the mask one call after the budget is spent: on the call that returns the lane's last
-    // LAST `previous` still holds the timestep before it, on the next one both buffers hold the LAST
-    if constexpr (kKeepPrevious) { if (selected && !opened) m.mask_out[lane] = 0; }
-  }
-
-  if constexpr (kCall == CALL_HOST) { if (a.mailbox) signal_done(a); }
-  if (a.clock) {        // graph-safe mode: the last CTA advances the call count by T (transition_kernel's epilogue)
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      const unsigned groups = gridDim.x < (unsigned)CLOCK_GROUPS ? gridDim.x : (unsigned)CLOCK_GROUPS;
-      const unsigned g = blockIdx.x % groups;
-      const unsigned members = gridDim.x / groups + (g < gridDim.x % groups ? 1u : 0u);
-      unsigned long long* sub = a.clock + CLOCK_SUB0 + 16 * g;
-      if (atomicAdd(sub, 1ull) == (unsigned long long)members - 1ull) {
-        *sub = 0ull;
-        if (atomicAdd(a.clock + CLOCK_TOP, 1ull) == (unsigned long long)groups - 1ull) {
-          const unsigned long long steps = (unsigned long long)(step0 - a.step0) + (unsigned long long)T;
-          for (int r = 0; r < CLOCK_GROUPS; ++r) a.clock[16 * r] = steps;
-          a.clock[CLOCK_TOP] = 0ull;
-        }
-      }
-    }
-  }
+// CALL_RECORD: masked_kernel's body with RecordArgs.
+template <class V, int RK>
+__global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_record_kernel(const EnvParams p, const LaunchArgs a, const RecordArgs m) {
+  constexpr int kCall = CALL_RECORD;
+#include "bsb_masked_body.inc"
 }
 
 #endif  // __CUDACC__

@@ -61,7 +61,7 @@ BSB_HD PhiloxBlock philox4x64_10(u64 c0, u64 c1, u64 c2, u64 c3, u64 k0, u64 k1)
 }
 
 // Stream ids carried in counter word 3.
-enum : u64 { STREAM_ENV = 0, STREAM_WRAPPER = 1, STREAM_ACTIONS = 2, STREAM_POLICY = 3 };
+enum : u64 { STREAM_ENV = 0, STREAM_WRAPPER = 1, STREAM_ACTIONS = 2, STREAM_POLICY = 3, STREAM_REPLAY = 4 };
 
 // On-device uniform random actions (the workload of baselines/random/agent.py:35-37).
 // The action stream of a lane is the Philox stream (key = (action_seed, global lane), counter word 3 =
@@ -163,6 +163,14 @@ BSB_HD int32_t select_action(int32_t kind, const float* row, int32_t n, double e
   }
   return last;
 }
+
+// Replay sampling (bsb_replay_sample): sample j of global lane g at call index s and draw d is word j & 3 of the Philox
+// block at counter (s, d, j >> 2, STREAM_REPLAY) with key (seed, g), mapped onto the n filled slots by multiply-shift
+// of its low 32 bits (n <= 2^31 - 1).  Stateless, like the policy stream.
+BSB_HD u64 replay_word(const PhiloxBlock& b, int64_t j) {
+  switch (j & 3) { case 0: return b.v0; case 1: return b.v1; case 2: return b.v2; default: return b.v3; }
+}
+BSB_HD int64_t replay_slot(u64 word, int64_t n) { return (int64_t)(((word & 0xffffffffull) * (u64)n) >> 32); }
 
 // ---------------------------------------------------------------------------
 // Bit source 1: Philox stream with numpy's buffering semantics.

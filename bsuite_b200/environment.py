@@ -464,7 +464,7 @@ class BatchedEnvironment:
     return out.timestep()
 
   def step(self, actions=None, out: Optional[StepBuffers] = None, mask=None, episodes_left=None,
-           previous: Optional[StepBuffers] = None, policy=None, policy_seed: int = 0):
+           previous: Optional[StepBuffers] = None, policy=None, policy_seed: int = 0, replay=None):
     """base.Environment.step for every lane (base.py:59-65); actions int [B].
 
     `mask` (bool or uint8 tensor [B] on the environment's device; needs `out`): only the lanes where it is set step;
@@ -484,12 +484,20 @@ class BatchedEnvironment:
     picks its action from its row, drawing on the policy stream keyed by (`policy_seed`, global lane) at the call's
     step index, and the picks land in `out.actions` (`make_buffers(with_actions=True)`); entries of lanes that sit out
     are left as they are.  The call equals a budgeted step given those actions, bit for bit.  A row with NaN (softmax:
-    or +inf, or no finite entry) gets a uniform pick and raises `invalid_actions_seen()`."""
+    or +inf, or no finite entry) gets a uniform pick and raises `invalid_actions_seen()`.
+
+    `replay` (a `rollouts.LaneReplay` of this environment) records a budgeted or policy step
+    (`bsb_step_budgeted_record`): the call is the same step, bit for bit, and every lane that stepped and whose new
+    step type is not FIRST appends (o_tm1, a_tm1, r_t, d_t, o_t) to its own ring in the same launch -- o_tm1 the row
+    copied to `previous`, o_t the new row (a same-step LAST: `out.final_observation`, which such an environment's
+    `out` must carry)."""
     torch = self._torch
+    if replay is not None and episodes_left is None and previous is None:
+      raise ValueError('replay= records a budgeted or policy step: it needs mask=, episodes_left= and previous=')
     if policy is not None:
-      return self._step_policy(actions, out, mask, episodes_left, previous, policy, policy_seed)
+      return self._step_policy(actions, out, mask, episodes_left, previous, policy, policy_seed, replay)
     if episodes_left is not None or previous is not None:
-      return self._step_budgeted(actions, out, mask, episodes_left, previous)
+      return self._step_budgeted(actions, out, mask, episodes_left, previous, replay)
     if mask is not None:
       return self._step_masked(actions, out, mask)
     if not (type(actions) is torch.Tensor and actions.dtype is torch.int32 and actions.dim() == 1
@@ -534,9 +542,27 @@ class BatchedEnvironment:
     prev = previous._outputs if previous._bound is self._obs_dtype else previous.bind(self._obs_dtype)
     return mask, outputs, prev
 
-  def _step_budgeted(self, actions, out, mask, episodes_left, previous):
+  def _ring(self, replay):
+    """The bsb_replay struct of a `rollouts.LaneReplay` argument."""
+    if not isinstance(replay, rollouts.LaneReplay):
+      raise ValueError(f'replay must be a rollouts.LaneReplay, got {type(replay).__name__}')
+    if replay.environment is not self:
+      raise ValueError('replay belongs to another environment: make it with LaneReplay(this environment, capacity)')
+    return replay._ring      # pylint: disable=protected-access
+
+  def _step_budgeted(self, actions, out, mask, episodes_left, previous, replay=None):
     mask, outputs, prev = self._budgeted_args(out, mask, episodes_left, previous)
     actions = self._device_actions(actions, (self._batch,))
+    if replay is not None:
+      ring = self._ring(replay)
+      self._async_work = True
+      status = self._lib.bsb_step_budgeted_record(self._handle.ptr, actions.data_ptr(), None, mask.data_ptr(),
+                                                  episodes_left.data_ptr(), ctypes.byref(outputs), ctypes.byref(prev),
+                                                  None, ctypes.byref(ring), self._stream())
+      if status:
+        _lib.check(status)
+      replay._draw = 0        # pylint: disable=protected-access
+      return out.timestep()
     self._async_work = True
     status = self._lib.bsb_step_budgeted(self._handle.ptr, actions.data_ptr(), mask.data_ptr(), episodes_left.data_ptr(),
                                          ctypes.byref(outputs), ctypes.byref(prev), self._stream())
@@ -544,7 +570,7 @@ class BatchedEnvironment:
       _lib.check(status)
     return out.timestep()
 
-  def _step_policy(self, actions, out, mask, episodes_left, previous, policy, policy_seed):
+  def _step_policy(self, actions, out, mask, episodes_left, previous, policy, policy_seed, replay=None):
     torch = self._torch
     if actions is not None:
       raise ValueError('policy replaces actions: pass one or the other')
@@ -571,6 +597,16 @@ class BatchedEnvironment:
             and chosen.is_contiguous()):
       raise ValueError(f'out.actions must be a contiguous int32 tensor of shape ({self._batch},) on {self._device}')
     spec = _lib.Policy(kind, 0, values.data_ptr(), epsilon, int(policy_seed) % (1 << 64))
+    if replay is not None:
+      ring = self._ring(replay)
+      self._async_work = True
+      status = self._lib.bsb_step_budgeted_record(self._handle.ptr, None, ctypes.byref(spec), mask.data_ptr(),
+                                                  episodes_left.data_ptr(), ctypes.byref(outputs), ctypes.byref(prev),
+                                                  chosen.data_ptr(), ctypes.byref(ring), self._stream())
+      if status:
+        _lib.check(status)
+      replay._draw = 0        # pylint: disable=protected-access
+      return out.timestep()
     self._async_work = True
     status = self._lib.bsb_step_budgeted_policy(self._handle.ptr, ctypes.byref(spec), mask.data_ptr(),
                                                 episodes_left.data_ptr(), ctypes.byref(outputs), ctypes.byref(prev),

@@ -13,6 +13,9 @@
     `run_random_episodes` do the same for a whole sweep.
   * `run_host_episodes` / `HostParts.run_episodes` -- the same for a HOST-side policy, through masked host steps
     (`step_host(..., mask=..., episodes_left=...)`), on one handle or over part-batches.
+  * `LaneReplay` -- one replay ring per lane (baselines/utils/replay.py, as each bsuite_id run of the reference owns
+    its own), filled by the budgeted step itself (`step(..., replay=...)`) and sampled on the device in one launch;
+    `run_episodes` records for an agent that carries one as `agent.replay`.
   * `Trajectory` / `collect` -- the `[T + 1]` observations / `[T]` actions, rewards, discounts layout of
     `bsuite/baselines/utils/sequence.py:26-35`, as device tensors with a lane axis, filled by ONE fused rollout
     (`bsb_rollout`: on-device uniform random actions) instead of T appends.
@@ -120,7 +123,9 @@ class EpisodeLoop:
 
   An agent that defines `select_policy(timestep)` (returning `EpsilonGreedy` or `Softmax`) instead of
   `select_action` has its actions chosen inside the step (`step(policy=..., policy_seed=...)`); its `update` receives
-  `out.actions`, where a lane that sat out keeps its last pick (0 before its first)."""
+  `out.actions`, where a lane that sat out keeps its last pick (0 before its first).  An agent whose `replay`
+  attribute is a `LaneReplay` of the environment has every transition recorded into it by the step
+  (`step(..., replay=...)`); its `update` is called as before and need only sample and learn."""
 
   def __init__(self, agent, environment, num_episodes: Optional[int] = None, policy_seed: int = 0):
     self.agent, self.environment = agent, environment
@@ -128,7 +133,12 @@ class EpisodeLoop:
     self.policy_seed = int(policy_seed)
     self.left = episode_budget(environment, num_episodes)
     self.mask = self.left > 0
-    self.out, self.previous = environment.make_buffers(with_actions=self.uses_policy), environment.make_buffers()
+    replay = getattr(agent, 'replay', None)
+    self.replay = replay if isinstance(replay, LaneReplay) else None
+    # a recorded same-step environment keeps the final observations: they are o_t of the LAST transitions
+    final = self.replay is not None and environment.autoreset == 'same_step'
+    self.out = environment.make_buffers(with_actions=self.uses_policy, final_observation=final)
+    self.previous = environment.make_buffers(final_observation=final)
     if self.uses_policy:
       self.out.actions.zero_()
     self.timestep = environment.reset(out=self.out, mask=self.mask)
@@ -145,12 +155,13 @@ class EpisodeLoop:
     if self.uses_policy:
       policy = self.agent.select_policy(self.timestep)
       self.timestep = self.environment.step(out=self.out, mask=self.mask, episodes_left=self.left,
-                                            previous=self.previous, policy=policy, policy_seed=self.policy_seed)
+                                            previous=self.previous, policy=policy, policy_seed=self.policy_seed,
+                                            replay=self.replay)
       actions = self.out.actions
     else:
       actions = self.agent.select_action(self.timestep)
       self.timestep = self.environment.step(actions, out=self.out, mask=self.mask, episodes_left=self.left,
-                                            previous=self.previous)
+                                            previous=self.previous, replay=self.replay)
     self.calls += 1
     self.agent.update(self.previous.timestep(), actions, self.timestep)
 
@@ -169,7 +180,8 @@ def run_episodes(agent, environment, num_episodes: Optional[int] = None, check_e
   running once every `check_every` calls.  An agent with `select_policy(timestep)` instead of `select_action` returns
   `EpsilonGreedy` / `Softmax` and has its actions chosen inside the step, on the policy stream keyed by
   (`policy_seed`, global lane), so its exploration does not depend on how lanes are sharded or packed
-  (`EpisodeLoop`).  Returns the number of calls made after the first reset."""
+  (`EpisodeLoop`).  An agent with a `replay` attribute that is a `LaneReplay` has its transitions recorded by the
+  step.  Returns the number of calls made after the first reset."""
   loop = EpisodeLoop(agent, environment, num_episodes, policy_seed)
   check_every = max(int(check_every), 1)
   while loop.calls % check_every != 0 or bool(loop.any_left()):
@@ -455,3 +467,130 @@ class HostHalves(HostParts):
     if int(batch) < 2:
       raise ValueError('HostHalves needs at least two lanes')
     super().__init__(bsuite_id, batch, device=device, seed=seed, lane_offset=lane_offset, parts=2, **engine_kwargs)
+
+
+class Transitions(NamedTuple):
+  """A minibatch of `LaneReplay.sample`: `[size, B, ...]` tensors (`.transpose(0, 1)` gives each lane's `[size, ...]`).
+  On a ragged pack `o_tm1` / `o_t` are tuples of per-setting views (`split_observation`).  `ready` (bool [B]): the
+  lanes that had at least `min_size` transitions; the other lanes' entries were not written."""
+  o_tm1: Any
+  a_tm1: Any
+  r_t: Any
+  d_t: Any
+  o_t: Any
+  ready: Any
+
+
+class ReplayBatch:
+  """Caller-owned output tensors of `LaneReplay.sample(size, out=...)` (`LaneReplay.make_batch(size)`)."""
+
+  def __init__(self, replay, size: int):
+    import ctypes  # pylint: disable=import-outside-toplevel
+    from bsuite_b200 import _lib  # pylint: disable=import-outside-toplevel
+    env, torch = replay.environment, replay.environment._torch      # pylint: disable=protected-access
+    self.size = int(size)
+    lead = (self.size, env.batch)
+    self.obs_tm1 = torch.zeros(env._obs_shape_of(lead), dtype=env.obs_dtype, device=env.device)  # pylint: disable=protected-access
+    self.obs = torch.zeros_like(self.obs_tm1)
+    self.actions = torch.zeros(lead, dtype=torch.int32, device=env.device)
+    self.reward = torch.zeros(lead, dtype=replay.transitions.reward.dtype, device=env.device)
+    self.discount = torch.zeros(lead, dtype=torch.float32, device=env.device)
+    self.ready = torch.zeros(env.batch, dtype=torch.uint8, device=env.device)
+    nxt = _lib.Outputs()
+    nxt.observation = self.obs.data_ptr()
+    if self.reward.dtype == torch.float64:
+      nxt.reward_f64 = self.reward.data_ptr()
+    else:
+      nxt.reward = self.reward.data_ptr()
+    nxt.discount = self.discount.data_ptr()
+    self._struct = _lib.Replay(self.size, None, self.obs_tm1.data_ptr(), self.actions.data_ptr(), nxt)
+    self._ctypes = ctypes
+    self._owner = replay
+
+
+class LaneReplay:
+  """One uniform replay ring of `capacity` transitions per lane (baselines/utils/replay.py:24-88 per lane), filled by
+  the budgeted step that produces the transitions (`environment.step(..., replay=self)`, or `run_episodes` with an
+  agent whose `replay` is this) and sampled on the device.
+
+  Storage is the environment's rollout layout with T = capacity: `transitions` (`make_buffers(capacity)`: o_t,
+  r_t, d_t and step_type, [capacity, B, ...]), `obs_tm1` (like transitions.observation), `actions` (int32
+  [capacity, B]) and `num_added` (int64 [B]).  Observations are kept in the environment's `obs_dtype`, so a uint8 or
+  bfloat16 environment's rings are 4x or 2x smaller.  Lane i's k-th transition goes to slot k % capacity.
+
+  Memory: about capacity * B * (2 * observation bytes + 16) bytes.  The reference's replay_capacity = 10 000 needs
+  about 17 GB for catch at B = 4096 in float32 (4.8 GB in uint8), and more than 100 GB for deep_sea's 21 sizes alone
+  in the 468-id packed sweep at 64 lanes per id; the capacity is the caller's choice.  Both observation rings come
+  from torch's default allocator, never from the compressible pool that holds step observations (`obs_memory`).
+
+  `sample(size, min_size)` draws `size` slots per lane uniformly with replacement from the lane's filled slots, on a
+  stateless Philox stream keyed by (`seed`, global lane) at the environment's call index, so sharded, packed and
+  standalone runs draw the same slots (`bsb_replay_sample`)."""
+
+  def __init__(self, environment, capacity: int, seed: int = 0):
+    from bsuite_b200 import _lib  # pylint: disable=import-outside-toplevel
+    torch = environment._torch      # pylint: disable=protected-access
+    capacity = int(capacity)
+    if not 1 <= capacity <= (1 << 31) - 1:
+      raise ValueError(f'capacity must lie in [1, 2^31 - 1], got {capacity}')
+    self.environment, self.capacity, self.seed = environment, capacity, int(seed)
+    B, device = environment.batch, environment.device
+    # make_buffers(capacity)'s layout, with both observation rings from torch's default allocator: a ring of gigabytes
+    # would use up the finite compressible store obs_memory keeps for step observations
+    from bsuite_b200.environment import StepBuffers  # pylint: disable=import-outside-toplevel
+    lead = (capacity, B)
+    obs = torch.empty(environment._obs_shape_of(lead), dtype=environment.obs_dtype, device=device)  # pylint: disable=protected-access
+    step = environment.make_buffers()
+    self.transitions = StepBuffers(observation=obs, reward=torch.empty(lead, dtype=step.reward.dtype, device=device),
+                                   discount=torch.empty(lead, dtype=torch.float32, device=device),
+                                   step_type=torch.empty(lead, dtype=torch.int32, device=device))
+    self.obs_tm1 = torch.empty_like(obs)
+    self.actions = torch.zeros((capacity, B), dtype=torch.int32, device=device)
+    self.num_added = torch.zeros(B, dtype=torch.int64, device=device)
+    self._draw = 0            # samples taken since the last recorded step: keys the index stream
+    nxt = self.transitions.as_outputs()
+    self._ring = _lib.Replay(capacity, self.num_added.data_ptr(), self.obs_tm1.data_ptr(), self.actions.data_ptr(),
+                             _lib.Outputs(nxt.observation, nxt.reward, nxt.reward_f64, nxt.discount, nxt.step_type,
+                                          None))
+
+  @property
+  def size(self):
+    """Transitions held per lane (int64 [B]): min(capacity, num_added)."""
+    return self.num_added.clamp(max=self.capacity)
+
+  @property
+  def fraction_filled(self):
+    """size / capacity per lane (float64 [B])."""
+    return self.size.double() / self.capacity
+
+  def reset(self) -> None:
+    """Empties every lane's ring."""
+    self.num_added.zero_()
+    self._draw = 0
+
+  def make_batch(self, size: int) -> ReplayBatch:
+    """Output tensors for `sample(size, out=...)`."""
+    return ReplayBatch(self, size)
+
+  def sample(self, size: int, min_size: int = 1, out: Optional[ReplayBatch] = None) -> Transitions:
+    """`size` transitions of every lane holding at least max(min_size, 1) of them, drawn uniformly with replacement
+    (replay.py:56-59; a lane below `min_size` is the reference's `if replay.size < min_replay_size: return`): one
+    launch.  Repeated samples between two steps draw different slots."""
+    env = self.environment
+    size = int(size)
+    if out is None:
+      out = ReplayBatch(self, size)
+    elif not isinstance(out, ReplayBatch) or out._owner is not self or out.size != size:   # pylint: disable=protected-access
+      raise ValueError(f'out must be make_batch({size}) of this replay')
+    env._async_work = True      # pylint: disable=protected-access
+    status = env._lib.bsb_replay_sample(env._handle.ptr, out._ctypes.byref(self._ring), size, int(min_size),      # pylint: disable=protected-access
+                                        self.seed % (1 << 64), self._draw, out._ctypes.byref(out._struct),       # pylint: disable=protected-access
+                                        out.ready.data_ptr(), env._stream())      # pylint: disable=protected-access
+    if status:
+      from bsuite_b200 import _lib  # pylint: disable=import-outside-toplevel
+      _lib.check(status)
+    self._draw += 1
+    o_tm1, o_t = out.obs_tm1, out.obs
+    if env.ragged:
+      o_tm1, o_t = env.split_observation(o_tm1), env.split_observation(o_t)
+    return Transitions(o_tm1, out.actions, out.reward, out.discount, o_t, out.ready.view(env._torch.bool))  # pylint: disable=protected-access

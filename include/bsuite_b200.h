@@ -491,6 +491,83 @@ int32_t bsb_step_budgeted_policy(bsb_env* env, const bsb_policy* policy, uint8_t
                                  int64_t* episodes_left, const bsb_outputs* out,
                                  const bsb_outputs* previous, int32_t* actions_out, void* stream);
 
+/*
+ * Per-lane replay rings (baselines/replay.py, one ring per lane, as each
+ * bsuite_id run of the reference owns its own replay).  The layout is the
+ * engine's [T, B, ...] rollout layout with T = capacity: obs_tm1 and
+ * next.observation are [capacity][step_elems] in the handle's obs_dtype (raw
+ * bytes, cast as for bsb_outputs; a ragged pack's settings at the offsets
+ * bsb_ragged_layout reports), action / next.reward / next.reward_f64 /
+ * next.discount / next.step_type are [capacity, B].  Offsets are 64-bit.
+ * next.final_observation is always NULL.  In a batch written by
+ * bsb_replay_sample, capacity is the sample size and num_added is NULL.
+ */
+typedef struct bsb_replay {
+  int64_t capacity;        /* slots per lane, in [1, 2^31 - 1] */
+  int64_t* num_added;      /* int64 [B]: transitions added per lane; NULL in a sample's output */
+  float* obs_tm1;          /* [capacity][step_elems] in the handle's obs_dtype */
+  int32_t* action;         /* int32 [capacity, B] */
+  bsb_outputs next;        /* o_t / r_t / d_t / step_type with a leading capacity axis (scalars nullable) */
+} bsb_replay;
+
+/*
+ * Recorded step: bsb_step_budgeted (actions != NULL) or
+ * bsb_step_budgeted_policy (policy != NULL; exactly one of the two) that also
+ * appends each transition to its lane's ring.  The call equals that call bit
+ * for bit in everything it defines.  In addition every lane that stepped
+ * (mask set and episodes_left > 0 before the call) and whose new step_type
+ * is not FIRST writes slot c = num_added[i] % capacity of its ring, then
+ * num_added[i] += 1 (replay.py:51-54):
+ *   obs_tm1[c]            the observation row copied to `previous`
+ *   action[c, i]          the action used (the caller's action after
+ *                         clamping, or the policy's pick)
+ *   next.reward[c, i]     the new reward, in whichever of float32 / float64
+ *                         the ring carries (cast from out's if out carries the
+ *                         other one); next.discount, next.step_type likewise
+ *   next.observation[c]   the new observation row; on a same-step handle whose
+ *                         new step_type is LAST, the final observation row.
+ * Lanes that only restarted (new FIRST) or sat out write nothing.  The rows
+ * are copied, never re-rendered.  out->step_type is required (it decides
+ * FIRST), and a same-step handle must pass out->final_observation.
+ * Refused (BSB_INVALID_ARGUMENT, before anything moves): whatever the
+ * underlying budgeted or policy step refuses, both or neither of actions and
+ * policy, a NULL replay / num_added / obs_tm1 / action / next.observation or
+ * out->step_type, a ring reward with no reward in `out`, capacity outside
+ * [1, 2^31 - 1], a ring observation buffer that is out's or previous's,
+ * next.final_observation non-NULL, a same-step handle without
+ * out->final_observation.  Every handle bsb_step_budgeted accepts; graph-safe
+ * mode and capture included: a replay reads and writes num_added as it is
+ * then.
+ */
+int32_t bsb_step_budgeted_record(bsb_env* env, const int32_t* actions, const bsb_policy* policy,
+                                 uint8_t* mask, int64_t* episodes_left,
+                                 const bsb_outputs* out, const bsb_outputs* previous,
+                                 int32_t* actions_out, const bsb_replay* replay, void* stream);
+
+/*
+ * Uniform minibatches from every lane's ring, in one launch.  For every lane
+ * i with n = min(capacity, num_added[i]) >= max(min_size, 1), batch slot j
+ * in [0, size) receives ring slot s_j = (lo32(w) * n) >> 32 of lane i --
+ * obs_tm1, action and each of next's fields that both `replay` and `batch`
+ * carry -- where w is word (j & 3) of the Philox4x64-10 block at counter
+ * (c, draw, j >> 2, 4) with key (seed, global lane).  c is the handle's
+ * current call index (bsb_steps_done; in graph-safe mode read on the device,
+ * so a captured sample draws fresh slots at every replay), `draw` tells apart
+ * several samples between two calls, and the global lane is keyed as the
+ * policy stream keys it (in a pack: the lane within its setting), so shards,
+ * packs and standalone handles draw the same slots.  ready[i] (uint8 [B],
+ * nullable) is set to 1 for these lanes and 0 for the others, whose batch
+ * entries are not written (replay.py: `if size < min_replay_size: return`).
+ * The gather moves raw bytes.  Refused (BSB_INVALID_ARGUMENT): size <= 0,
+ * min_size < 0, a NULL replay / num_added / obs_tm1 / action /
+ * next.observation, or batch / obs_tm1 / action / next.observation, a batch
+ * whose capacity != size or whose num_added is non-NULL, a ring capacity out
+ * of range, a batch scalar the ring does not carry.
+ */
+int32_t bsb_replay_sample(bsb_env* env, const bsb_replay* replay, int64_t size, int64_t min_size,
+                          uint64_t seed, uint64_t draw, const bsb_replay* batch, uint8_t* ready,
+                          void* stream);
+
 /* Host mirror of the on-device action sampler: out int32 [T,B] (host). */
 int32_t bsb_random_actions(uint64_t action_seed, uint64_t lane_offset,
                            int64_t batch, int64_t first_step, int64_t num_steps,
@@ -522,7 +599,8 @@ int32_t bsb_read_episode_stats(bsb_env* env, int32_t field, double* dst,
 
 /*
  * CUDA graphs.  bsb_step / bsb_reset / bsb_rollout / the masked calls (bsb_reset_masked / bsb_step_masked /
- * bsb_rollout_masked / bsb_advance_masked / bsb_step_budgeted / bsb_step_budgeted_policy) / bsb_read_* / bsb_sum_* may
+ * bsb_rollout_masked / bsb_advance_masked / bsb_step_budgeted / bsb_step_budgeted_policy / bsb_step_budgeted_record)
+ * / bsb_replay_sample / bsb_read_* / bsb_sum_* may
  * be called on a stream that is being captured.  A graph freezes launch arguments, so the first captured launch moves the handle's step
  * counter (it indexes the on-device action stream and the Logging columns) and its chunk scheduler into device
  * memory, for good: replays and eager calls can then be mixed in any order, and bsb_steps_done / bsb_get_state
