@@ -95,6 +95,12 @@ class Replay(ctypes.Structure):
               ('action', ctypes.c_void_p), ('next', Outputs)]
 
 
+class Sequence(ctypes.Structure):
+  """struct bsb_sequence: per-lane sequence buffers."""
+  _fields_ = [('max_length', ctypes.c_int64), ('length', ctypes.c_void_p), ('ready', ctypes.c_void_p),
+              ('observations', ctypes.c_void_p), ('action', ctypes.c_void_p), ('next', Outputs)]
+
+
 SCORE_MAX_SOURCES = 512      # bsb_score: sources per call
 # enum bsb_score_quantity: the row columns a score reads
 SCORE_QUANTITIES = ('episode', 'total_return', 'total_regret', 'raw_return', 'best_episode', 'total_perfect',
@@ -154,6 +160,10 @@ EXPORTS = {
                                                   ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Outputs),
                                                   ctypes.POINTER(Outputs), ctypes.c_void_p, ctypes.POINTER(Replay),
                                                   ctypes.c_void_p]),
+    'bsb_step_budgeted_sequence': (ctypes.c_int32, [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Policy),
+                                                    ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(Outputs),
+                                                    ctypes.POINTER(Outputs), ctypes.c_void_p, ctypes.POINTER(Sequence),
+                                                    ctypes.c_void_p]),
     'bsb_replay_sample': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(Replay), ctypes.c_int64, ctypes.c_int64,
                                            ctypes.c_uint64, ctypes.c_uint64, ctypes.POINTER(Replay), ctypes.c_void_p,
                                            ctypes.c_void_p]),

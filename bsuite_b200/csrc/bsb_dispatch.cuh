@@ -376,20 +376,17 @@ void host_policy(const bsb_env* e, const LaunchArgs& a, uint8_t* mask, int64_t* 
   host_budgeted<V>(e, chosen, mask, episodes_left, previous);
 }
 
-// bsb_step_budgeted_record on a host handle, as masked_kernel's CALL_RECORD runs it: host_policy (a policy) or
-// host_budgeted (the caller's actions), then every lane that stepped (mask set, budget left before the call) and whose
-// new step type is not FIRST appends its transition to slot num_added % capacity of its ring: o_tm1 from `previous`,
-// o_t from the new observation row (a same-step LAST: the final observation row), as raw bytes.
+// The step of a recorded or sequence step on a host handle (CALL_RECORD's and CALL_SEQUENCE's): host_policy (a
+// policy) or host_budgeted (the caller's actions).  `stepped[i]`: lane i stepped (mask set, budget left before the
+// call); `used[i]`: the action it stepped with.
 template <class V>
-void host_record(const bsb_env* e, const LaunchArgs& a, uint8_t* mask, int64_t* episodes_left,
-                 const bsb_outputs* previous, const bsb_policy* policy, const bsb_replay& r) {
-  typedef typename V::Obs O;
+void host_step_used(const bsb_env* e, const LaunchArgs& a, uint8_t* mask, int64_t* episodes_left,
+                    const bsb_outputs* previous, const bsb_policy* policy, std::vector<uint8_t>& stepped,
+                    std::vector<int32_t>& used) {
   const EnvParams& p = e->p;
   const int64_t B = p.batch;
-  const RaggedTable* ragged = V::kRagged ? reinterpret_cast<const RaggedTable*>(p.pack) : nullptr;
-  const int64_t step_elems = V::kRagged ? ragged->step_elems : B * (int64_t)p.obs_numel;
-  std::vector<uint8_t> stepped((size_t)B, 0);
-  std::vector<int32_t> used((size_t)B, 0);
+  stepped.assign((size_t)B, 0);
+  used.assign((size_t)B, 0);
   for (int64_t lane = 0; lane < B; ++lane) {
     stepped[(size_t)lane] = mask[lane] && episodes_left[lane] > 0;
     if (stepped[(size_t)lane] && !policy) {
@@ -407,6 +404,22 @@ void host_record(const bsb_env* e, const LaunchArgs& a, uint8_t* mask, int64_t* 
   } else {
     host_budgeted<V>(e, a, mask, episodes_left, previous);
   }
+}
+
+// bsb_step_budgeted_record on a host handle, as masked_kernel's CALL_RECORD runs it: host_step_used, then every lane
+// that stepped and whose new step type is not FIRST appends its transition to slot num_added % capacity of its ring:
+// o_tm1 from `previous`, o_t from the new observation row (a same-step LAST: the final observation row), as raw bytes.
+template <class V>
+void host_record(const bsb_env* e, const LaunchArgs& a, uint8_t* mask, int64_t* episodes_left,
+                 const bsb_outputs* previous, const bsb_policy* policy, const bsb_replay& r) {
+  typedef typename V::Obs O;
+  const EnvParams& p = e->p;
+  const int64_t B = p.batch;
+  const RaggedTable* ragged = V::kRagged ? reinterpret_cast<const RaggedTable*>(p.pack) : nullptr;
+  const int64_t step_elems = V::kRagged ? ragged->step_elems : B * (int64_t)p.obs_numel;
+  std::vector<uint8_t> stepped;
+  std::vector<int32_t> used;
+  host_step_used<V>(e, a, mask, episodes_left, previous, policy, stepped, used);
   const O* prev_obs = reinterpret_cast<const O*>(previous->observation);
   const O* obs = reinterpret_cast<const O*>(a.obs);
   const O* fin = reinterpret_cast<const O*>(a.final_obs);
@@ -433,6 +446,54 @@ void host_record(const bsb_env* e, const LaunchArgs& a, uint8_t* mask, int64_t* 
     const bool final_row = V::kSameStep && type == LAST;
     memcpy(ring_tm1 + slot * step_elems + row, prev_obs + row, (size_t)K * sizeof(O));
     memcpy(ring_obs + slot * step_elems + row, (final_row ? fin : obs) + row, (size_t)K * sizeof(O));
+  }
+}
+
+// bsb_step_budgeted_sequence on a host handle, as masked_kernel's CALL_SEQUENCE runs it: host_step_used, then every
+// lane that stepped and whose new step type is not FIRST appends its transition at entry t of its sequence (t = 0
+// after a full sequence or a LAST, with o_tm1 from `previous` at observation slot 0), and every lane's ready flag is
+// written.  Rows move as raw bytes.
+template <class V>
+void host_sequence(const bsb_env* e, const LaunchArgs& a, uint8_t* mask, int64_t* episodes_left,
+                   const bsb_outputs* previous, const bsb_policy* policy, const bsb_sequence& q) {
+  typedef typename V::Obs O;
+  const EnvParams& p = e->p;
+  const int64_t B = p.batch;
+  const RaggedTable* ragged = V::kRagged ? reinterpret_cast<const RaggedTable*>(p.pack) : nullptr;
+  const int64_t step_elems = V::kRagged ? ragged->step_elems : B * (int64_t)p.obs_numel;
+  std::vector<uint8_t> stepped;
+  std::vector<int32_t> used;
+  host_step_used<V>(e, a, mask, episodes_left, previous, policy, stepped, used);
+  const O* prev_obs = reinterpret_cast<const O*>(previous->observation);
+  const O* obs = reinterpret_cast<const O*>(a.obs);
+  const O* fin = reinterpret_cast<const O*>(a.final_obs);
+  O* seq = reinterpret_cast<O*>(q.observations);
+  const int64_t T = q.max_length;
+  for (int64_t lane = 0; lane < B; ++lane) {
+    const int32_t type = a.step_type[lane];
+    if (!stepped[(size_t)lane] || type == FIRST) {
+      q.ready[lane] = 0;
+      continue;
+    }
+    int64_t t = q.length[lane];
+    if ((uint64_t)t >= (uint64_t)T || (t > 0 && q.next.step_type[(t - 1) * B + lane] == LAST)) t = 0;
+    const int64_t at = t * B + lane;
+    q.action[at] = used[(size_t)lane];
+    if (q.next.reward) q.next.reward[at] = a.reward ? a.reward[lane] : (float)a.reward_f64[lane];
+    if (q.next.reward_f64) q.next.reward_f64[at] = a.reward_f64 ? a.reward_f64[lane] : (double)a.reward[lane];
+    q.next.discount[at] = a.discount[lane];
+    q.next.step_type[at] = type;
+    q.length[lane] = t + 1;
+    q.ready[lane] = t + 1 == T || type == LAST ? 1 : 0;
+    int64_t row = lane * (int64_t)p.obs_numel, K = p.obs_numel;
+    if constexpr (V::kRagged) {
+      const RaggedSetting& s = ragged_setting(ragged, lane / ragged->pack.lanes_per_setting);
+      row = s.obs_offset + (lane - s.lane_shift) * (int64_t)s.obs_numel;
+      K = s.obs_numel;
+    }
+    const bool final_row = V::kSameStep && type == LAST;
+    if (t == 0) memcpy(seq + row, prev_obs + row, (size_t)K * sizeof(O));
+    memcpy(seq + (t + 1) * step_elems + row, (final_row ? fin : obs) + row, (size_t)K * sizeof(O));
   }
 }
 
@@ -473,10 +534,12 @@ int run_variant(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoP
 // nothing for the T loop, the action stream or the budgets to do (every masked reset and step) takes CALL_ONE.  A
 // budgeted step (`previous` given: bsb_step_budgeted, whose `mask_out` is the mask) takes CALL_BUDGETED, and one with a
 // `policy` (bsb_step_budgeted_policy: no actions, the picks to a.actions_out) takes CALL_POLICY.  A budgeted step with
-// a `replay` (bsb_step_budgeted_record, actions or a policy) takes CALL_RECORD.
+// a `replay` (bsb_step_budgeted_record, actions or a policy) takes CALL_RECORD, and one with a `sequence`
+// (bsb_step_budgeted_sequence) takes CALL_SEQUENCE.
 template <class V>
 int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* episodes_left, uint8_t* mask_out,
-               const bsb_outputs* previous, const bsb_policy* policy, const bsb_replay* replay, cudaStream_t stream) {
+               const bsb_outputs* previous, const bsb_policy* policy, const bsb_replay* replay,
+               const bsb_sequence* sequence, cudaStream_t stream) {
   constexpr bool kMt = Compiled<V>::kMt;
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
   if (previous && (a.T != 1 || a.mode != MODE_STEP || !a.actions == !policy || (a.actions_out && !policy) ||
@@ -485,15 +548,20 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
                               "clearing its mask");
   if (policy && !previous) return fail(BSB_INTERNAL, "a policy step must be a budgeted step");
   if (replay && (!previous || !a.step_type)) return fail(BSB_INTERNAL, "a recorded step must be a budgeted step with step types");
+  if (sequence && (!previous || !a.step_type || replay))
+    return fail(BSB_INTERNAL, "a sequence step must be a budgeted step with step types and no replay");
   if (e->device < 0) {
-    if (replay) host_record<V>(e, a, mask_out, episodes_left, previous, policy, *replay);
+    if (sequence) host_sequence<V>(e, a, mask_out, episodes_left, previous, policy, *sequence);
+    else if (replay) host_record<V>(e, a, mask_out, episodes_left, previous, policy, *replay);
     else if (policy) host_policy<V>(e, a, mask_out, episodes_left, previous, *policy);
     else if (previous) host_budgeted<V>(e, a, mask_out, episodes_left, previous);
     else run_host<V>(e, a, mask, episodes_left);
     return BSB_OK;
   }
-  RecordArgs m;                          // a MaskArgs for every kind but CALL_RECORD
+  RecordArgs m;                          // a MaskArgs for every kind but CALL_RECORD and CALL_SEQUENCE
   memset(&m, 0, sizeof(m));
+  SequenceArgs sq;                       // CALL_SEQUENCE: m's MaskArgs and the sequence buffers
+  memset(&sq, 0, sizeof(sq));
   m.mask = mask;
   m.noise = e->p.wrapper == BSB_WRAP_REWARD_NOISE ? 1 : 0;
   m.track = e->p.ep != nullptr ? 1 : 0;
@@ -515,6 +583,9 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
     if constexpr (kCall == CALL_RECORD) {
       if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_record_kernel<V, 1>, e->p, la, m); }
       return launch(e, la, g, stream, masked_record_kernel<V, 0>, e->p, la, m);
+    } else if constexpr (kCall == CALL_SEQUENCE) {
+      if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_sequence_kernel<V, 1>, e->p, la, sq); }
+      return launch(e, la, g, stream, masked_sequence_kernel<V, 0>, e->p, la, sq);
     } else {
       const MaskArgs& base = m;
       if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_kernel<V, 1, kCall>, e->p, la, base); }
@@ -550,6 +621,21 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
                      reinterpret_cast<uintptr_t>(replay->next.observation) % 16 == 0 &&
                      ((size_t)e->step_elems * (size_t)e->obs_elem_bytes) % 16 == 0 ? 1 : 0;
       return go(std::integral_constant<int, CALL_RECORD>());
+    }
+    if (sequence) {
+      static_cast<MaskArgs&>(sq) = m;
+      sq.seq_max_length = sequence->max_length;
+      sq.seq_length = sequence->length;
+      sq.seq_ready = sequence->ready;
+      sq.seq_obs = sequence->observations;
+      sq.seq_action = sequence->action;
+      sq.seq_reward = sequence->next.reward;
+      sq.seq_reward_f64 = sequence->next.reward_f64;
+      sq.seq_discount = sequence->next.discount;
+      sq.seq_step_type = sequence->next.step_type;
+      sq.seq_vec_ok = reinterpret_cast<uintptr_t>(sequence->observations) % 16 == 0 &&
+                      ((size_t)e->step_elems * (size_t)e->obs_elem_bytes) % 16 == 0 ? 1 : 0;
+      return go(std::integral_constant<int, CALL_SEQUENCE>());
     }
     if (policy) return go(std::integral_constant<int, CALL_POLICY>());
     return go(std::integral_constant<int, CALL_BUDGETED>());

@@ -86,10 +86,12 @@ template <class T> int env_alloc_t(bsb_env* e, T** out, size_t count, bool snaps
 // `two_phase`: a two-phase host step (mailbox_launch; deep_sea and catch only).  `mask`: a masked call, rollout or
 // host step (`episodes_left`: the budgets, nullable; `mask_out`: a budgeted host step's mask write-back, nullable;
 // `previous`: a budgeted step's previous outputs, nullable; `policy`: a budgeted step's selection rule, nullable;
-// `replay`: the rings a recorded step appends to, nullable).
+// `replay`: the rings a recorded step appends to, nullable; `sequence`: the buffers a sequence step appends to,
+// nullable).
 int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr,
         const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr,
-        const bsb_outputs* previous = nullptr, const bsb_policy* policy = nullptr, const bsb_replay* replay = nullptr) {
+        const bsb_outputs* previous = nullptr, const bsb_policy* policy = nullptr, const bsb_replay* replay = nullptr,
+        const bsb_sequence* sequence = nullptr) {
   DeviceGuard guard(e->device);
   LaunchArgs a = args;
   if (e->device >= 0) {
@@ -98,7 +100,7 @@ int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseA
     if (capture != cudaStreamCaptureStatusNone) e->graph_safe = true;
     if (e->graph_safe) a.clock = e->clock;      // a.step0 == e->steps_done, which no longer moves
   }
-  if (mask) return e->variant->run_masked(e, a, mask, episodes_left, mask_out, previous, policy, replay, stream);
+  if (mask) return e->variant->run_masked(e, a, mask, episodes_left, mask_out, previous, policy, replay, sequence, stream);
   return e->variant->run(e, a, stream, two_phase);
 }
 
@@ -859,12 +861,12 @@ int32_t bsb_step(bsb_env* env, const int32_t* actions, const bsb_outputs* out, v
 // the actions of masked-in lanes only, at every step of a rollout (a host step: of lanes with budget left): an
 // inactive lane's action is never read.  `mask_out`: a budgeted host step's write-back, or a budgeted step's mask;
 // `previous`: a budgeted step's previous outputs; `policy`: the rule that picks a budgeted step's actions; `replay`:
-// the rings a recorded step appends to (run_masked).
+// the rings a recorded step appends to; `sequence`: the buffers a sequence step appends to (run_masked).
 static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask, const bsb_outputs* out, void* stream,
                        int mode, int64_t T = 1, bool rollout = false, uint64_t action_seed = 0,
                        int32_t* actions_out = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr,
                        const bsb_outputs* previous = nullptr, const bsb_policy* policy = nullptr,
-                       const bsb_replay* replay = nullptr) {
+                       const bsb_replay* replay = nullptr, const bsb_sequence* sequence = nullptr) {
   { int crc = check_final_observation(env, out); if (crc != BSB_OK) return crc; }
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
   if (env->device < 0 && mode == MODE_STEP && actions) {
@@ -880,7 +882,7 @@ static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask
   LaunchArgs a = make_args(env, out, mode == MODE_STEP ? actions : nullptr, T, mode);
   a.action_seed = action_seed; a.actions_out = actions_out;
   int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask, episodes_left, mask_out, previous, policy,
-               replay);
+               replay, sequence);
   if (rc == BSB_OK) advance_steps(env, T);
   return rc;
 }
@@ -934,8 +936,8 @@ int32_t bsb_advance_masked(bsb_env* env, int64_t num_steps, uint64_t action_seed
 // One masked step with budgets that first keeps the masked-in lanes' current outputs in `previous`: masked_kernel's
 // CALL_BUDGETED instantiation (run_masked), or host_budgeted on a host handle.  The mask is cleared in place one call
 // after a lane's budget is spent.
-// The refusals bsb_step_budgeted, bsb_step_budgeted_policy and bsb_step_budgeted_record share (`choice`: the actions or
-// the policy).
+// The refusals bsb_step_budgeted, bsb_step_budgeted_policy, bsb_step_budgeted_record and bsb_step_budgeted_sequence
+// share (`choice`: the actions or the policy).
 static int check_budgeted(const bsb_env* env, const void* choice, const uint8_t* mask, const int64_t* episodes_left,
                           const bsb_outputs* out, const bsb_outputs* previous, const std::string& name,
                           const char* what) {
@@ -949,7 +951,7 @@ static int check_budgeted(const bsb_env* env, const void* choice, const uint8_t*
   return check_final_observation(env, previous);
 }
 
-// The refusals of a policy (bsb_step_budgeted_policy, bsb_step_budgeted_record).
+// The refusals of a policy (bsb_step_budgeted_policy, bsb_step_budgeted_record, bsb_step_budgeted_sequence).
 static int check_policy(const bsb_policy* policy, const std::string& name) {
   if (!policy->values) return fail(BSB_INVALID_ARGUMENT, name + " needs the policy's values");
   if (policy->kind != BSB_POLICY_EPSILON_GREEDY && policy->kind != BSB_POLICY_SOFTMAX)
@@ -1017,6 +1019,38 @@ int32_t bsb_step_budgeted_record(bsb_env* env, const int32_t* actions, const bsb
     return fail(BSB_INVALID_ARGUMENT, name + " on a same-step handle needs out->final_observation: it is o_t of a LAST");
   return masked_call(env, actions, mask, out, stream, MODE_STEP, 1, false, 0, actions_out, episodes_left, mask, previous,
                      policy, replay);
+}
+
+// bsb_step_budgeted or bsb_step_budgeted_policy that appends each transition to its lane's sequence buffer:
+// masked_sequence_kernel (CALL_SEQUENCE, run_masked), or host_sequence on a host handle.
+int32_t bsb_step_budgeted_sequence(bsb_env* env, const int32_t* actions, const bsb_policy* policy, uint8_t* mask,
+                                   int64_t* episodes_left, const bsb_outputs* out, const bsb_outputs* previous,
+                                   int32_t* actions_out, const bsb_sequence* sequence, void* stream) {
+  const std::string name = "bsb_step_budgeted_sequence";
+  if (!actions == !policy) return fail(BSB_INVALID_ARGUMENT, name + " takes actions or a policy: exactly one of them");
+  const void* choice = actions ? static_cast<const void*>(actions) : static_cast<const void*>(policy);
+  { int rc = check_budgeted(env, choice, mask, episodes_left, out, previous, name, actions ? "actions" : "a policy"); if (rc != BSB_OK) return rc; }
+  if (policy) { int rc = check_policy(policy, name); if (rc != BSB_OK) return rc; }
+  else if (actions_out) return fail(BSB_INVALID_ARGUMENT, name + ": actions_out reports a policy's picks: pass NULL with actions");
+  const bsb_sequence* q = sequence;
+  if (!q || !q->length || !q->ready || !q->observations || !q->action || !q->next.step_type || !q->next.discount ||
+      (!q->next.reward && !q->next.reward_f64))
+    return fail(BSB_INVALID_ARGUMENT, name + " needs a sequence with length, ready, observations, action and next's "
+                                             "step_type, discount and reward (or reward_f64)");
+  if (q->max_length < 1 || q->max_length > INT32_MAX)
+    return fail(BSB_INVALID_ARGUMENT, name + ": max_length must lie in [1, 2^31 - 1], got " + std::to_string(q->max_length));
+  if (q->next.observation || q->next.final_observation)
+    return fail(BSB_INVALID_ARGUMENT, name + ": a sequence keeps its observations in `observations` (next.observation "
+                                             "and next.final_observation must be NULL)");
+  if (!out->step_type || !out->discount || (!out->reward && !out->reward_f64))
+    return fail(BSB_INVALID_ARGUMENT, name + " needs out's step_type, discount and reward (or reward_f64)");
+  if (q->observations == out->observation || q->observations == previous->observation ||
+      (out->final_observation && q->observations == out->final_observation))
+    return fail(BSB_INVALID_ARGUMENT, name + ": the sequence's observation buffer must not be out's or previous's");
+  if (env->same_step && !out->final_observation)
+    return fail(BSB_INVALID_ARGUMENT, name + " on a same-step handle needs out->final_observation: it is o_t of a LAST");
+  return masked_call(env, actions, mask, out, stream, MODE_STEP, 1, false, 0, actions_out, episodes_left, mask, previous,
+                     policy, nullptr, sequence);
 }
 
 // ----- replay sampling --------------------------------------------------------------------------------------------

@@ -1521,6 +1521,22 @@ struct RecordArgs : MaskArgs {
   int32_t rec_vec_ok;
 };
 
+// The arguments of a CALL_SEQUENCE launch: MaskArgs grown at its end by the lanes' sequence buffers (bsb_sequence),
+// passed to masked_sequence_kernel only, for the reason RecordArgs is.  The action source is RecordArgs's.
+// seq_vec_ok: the observation buffer starts 16-byte aligned and a slot is a whole number of 16-byte words.
+struct SequenceArgs : MaskArgs {
+  int64_t seq_max_length;
+  int64_t* seq_length;
+  uint8_t* seq_ready;
+  float* seq_obs;
+  int32_t* seq_action;
+  float* seq_reward;
+  double* seq_reward_f64;
+  float* seq_discount;
+  int32_t* seq_step_type;
+  int32_t seq_vec_ok;
+};
+
 // What one masked_kernel instantiation runs.  CALL_ROLLOUT: bsb_rollout_masked (T steps, sampled or given actions,
 // budgets, actions_out).  CALL_ONE: a masked reset or step (T = 1, the caller's actions, no budgets).  CALL_HOST:
 // bsb_step_host_masked (T = 1, the caller's actions, optional budgets, the mask write-back, the mailbox signal).
@@ -1530,9 +1546,10 @@ struct RecordArgs : MaskArgs {
 // CALL_POLICY: bsb_step_budgeted_policy (CALL_BUDGETED with each stepping lane's action chosen from its row of the
 // policy's values by select_action, and written to actions_out).  CALL_RECORD: bsb_step_budgeted_record
 // (CALL_BUDGETED or CALL_POLICY, chosen at run time by m.policy_values, with each transition appended to its lane's
-// ring).
+// ring).  CALL_SEQUENCE: bsb_step_budgeted_sequence (CALL_RECORD's step, with each transition appended to its lane's
+// sequence buffer instead of a ring).
 enum CallKind { CALL_ROLLOUT = 0, CALL_ONE = 1, CALL_HOST = 2, CALL_ADVANCE = 3, CALL_BUDGETED = 4, CALL_POLICY = 5,
-                CALL_RECORD = 6 };
+                CALL_RECORD = 6, CALL_SEQUENCE = 7 };
 
 // Writes lane j's observation `val(e)` (element e of K) with the whole warp: 16-byte streaming stores when `vec`
 // (the row starts 16-byte aligned and is a whole number of 16-byte words), else one element per store.
@@ -1669,8 +1686,12 @@ __device__ __forceinline__ void record_lane_rows(const O* src, O* ring, int64_t 
 // stepped and whose new step type is not FIRST appends (o_tm1, a_tm1, r_t, d_t, o_t) to slot num_added % capacity of
 // its ring and counts it.  The rows are copied, never rendered again (rendering draws for some families): o_tm1 from
 // the row the lane copied to `previous`, o_t from the row the warp has just emitted (a same-step LAST: the final
-// observation), after a __syncwarp.  The body (bsb_masked_body.inc) is shared with masked_record_kernel, which runs
-// CALL_RECORD.
+// observation), after a __syncwarp.  kCall == CALL_SEQUENCE: CALL_RECORD's step, after which every such lane appends
+// (a_tm1, r_t, d_t, o_t) at entry t of its sequence buffer, and o_tm1 at observation slot 0 when t == 0 (a new
+// sequence): t is the lane's length, or 0 when the length reached max_length or the entry before it is a LAST (the
+// sequence was closed by an earlier call).  Every lane writes its ready flag: set where the append closed the sequence.
+// The body (bsb_masked_body.inc) is shared with masked_record_kernel and masked_sequence_kernel, which run CALL_RECORD
+// and CALL_SEQUENCE.
 template <class V, int RK, int kCall>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(const EnvParams p, const LaunchArgs a, const MaskArgs m) {
 #include "bsb_masked_body.inc"
@@ -1680,6 +1701,13 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(c
 template <class V, int RK>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_record_kernel(const EnvParams p, const LaunchArgs a, const RecordArgs m) {
   constexpr int kCall = CALL_RECORD;
+#include "bsb_masked_body.inc"
+}
+
+// CALL_SEQUENCE: masked_kernel's body with SequenceArgs.
+template <class V, int RK>
+__global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_sequence_kernel(const EnvParams p, const LaunchArgs a, const SequenceArgs m) {
+  constexpr int kCall = CALL_SEQUENCE;
 #include "bsb_masked_body.inc"
 }
 

@@ -9,7 +9,8 @@ namespace bsb {
 #define BSB_INSTANTIATE(F, O, mode, mt, two_phase) \
   template int run_variant<Variant<F, O, mode> >(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs*); \
   template int run_masked<Variant<F, O, mode> >(bsb_env*, const LaunchArgs&, const uint8_t*, int64_t*, uint8_t*, \
-                                                const bsb_outputs*, const bsb_policy*, const bsb_replay*, cudaStream_t);
+                                                const bsb_outputs*, const bsb_policy*, const bsb_replay*, \
+                                                const bsb_sequence*, cudaStream_t);
 BSB_UNIT(BSB_INSTANTIATE)
 #undef BSB_INSTANTIATE
 }  // namespace bsb

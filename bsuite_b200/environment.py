@@ -464,7 +464,7 @@ class BatchedEnvironment:
     return out.timestep()
 
   def step(self, actions=None, out: Optional[StepBuffers] = None, mask=None, episodes_left=None,
-           previous: Optional[StepBuffers] = None, policy=None, policy_seed: int = 0, replay=None):
+           previous: Optional[StepBuffers] = None, policy=None, policy_seed: int = 0, replay=None, sequence=None):
     """base.Environment.step for every lane (base.py:59-65); actions int [B].
 
     `mask` (bool or uint8 tensor [B] on the environment's device; needs `out`): only the lanes where it is set step;
@@ -490,14 +490,25 @@ class BatchedEnvironment:
     (`bsb_step_budgeted_record`): the call is the same step, bit for bit, and every lane that stepped and whose new
     step type is not FIRST appends (o_tm1, a_tm1, r_t, d_t, o_t) to its own ring in the same launch -- o_tm1 the row
     copied to `previous`, o_t the new row (a same-step LAST: `out.final_observation`, which such an environment's
-    `out` must carry)."""
+    `out` must carry).
+
+    `sequence` (a `rollouts.LaneSequence` of this environment) fills each lane's sequence buffer in a budgeted or
+    policy step (`bsb_step_budgeted_sequence`): the call is the same step, bit for bit, and every lane that stepped and
+    whose new step type is not FIRST appends (a_tm1, r_t, d_t, o_t) to its current sequence, which starts with o_tm1
+    (the row copied to `previous`); `sequence.ready` marks the lanes whose sequence this call closed (full, or ended by
+    a LAST), which the agent reads before the next call.  Not together with `replay`."""
     torch = self._torch
     if replay is not None and episodes_left is None and previous is None:
       raise ValueError('replay= records a budgeted or policy step: it needs mask=, episodes_left= and previous=')
+    if sequence is not None:
+      if replay is not None:
+        raise ValueError('replay= and sequence= record the same transitions two ways: pass one of them')
+      if episodes_left is None or previous is None:
+        raise ValueError('sequence= fills a budgeted or policy step: it needs mask=, episodes_left= and previous=')
     if policy is not None:
-      return self._step_policy(actions, out, mask, episodes_left, previous, policy, policy_seed, replay)
+      return self._step_policy(actions, out, mask, episodes_left, previous, policy, policy_seed, replay, sequence)
     if episodes_left is not None or previous is not None:
-      return self._step_budgeted(actions, out, mask, episodes_left, previous, replay)
+      return self._step_budgeted(actions, out, mask, episodes_left, previous, replay, sequence)
     if mask is not None:
       return self._step_masked(actions, out, mask)
     if not (type(actions) is torch.Tensor and actions.dtype is torch.int32 and actions.dim() == 1
@@ -550,18 +561,34 @@ class BatchedEnvironment:
       raise ValueError('replay belongs to another environment: make it with LaneReplay(this environment, capacity)')
     return replay._ring      # pylint: disable=protected-access
 
-  def _step_budgeted(self, actions, out, mask, episodes_left, previous, replay=None):
-    mask, outputs, prev = self._budgeted_args(out, mask, episodes_left, previous)
-    actions = self._device_actions(actions, (self._batch,))
+  def _step_recorded(self, actions, policy, mask, episodes_left, outputs, prev, chosen, replay, sequence):
+    """bsb_step_budgeted_record (`replay`) or bsb_step_budgeted_sequence (`sequence`): `actions` (a pointer) or
+    `policy` (a bsb_policy) chooses, and `chosen` (a pointer) receives a policy's picks."""
+    args = (self._handle.ptr, actions, None if policy is None else ctypes.byref(policy), mask.data_ptr(),
+            episodes_left.data_ptr(), ctypes.byref(outputs), ctypes.byref(prev), chosen)
     if replay is not None:
       ring = self._ring(replay)
       self._async_work = True
-      status = self._lib.bsb_step_budgeted_record(self._handle.ptr, actions.data_ptr(), None, mask.data_ptr(),
-                                                  episodes_left.data_ptr(), ctypes.byref(outputs), ctypes.byref(prev),
-                                                  None, ctypes.byref(ring), self._stream())
+      status = self._lib.bsb_step_budgeted_record(*args, ctypes.byref(ring), self._stream())
       if status:
         _lib.check(status)
       replay._draw = 0        # pylint: disable=protected-access
+    else:
+      if not isinstance(sequence, rollouts.LaneSequence):
+        raise ValueError(f'sequence must be a rollouts.LaneSequence, got {type(sequence).__name__}')
+      if sequence.environment is not self:
+        raise ValueError('sequence belongs to another environment: make it with LaneSequence(this environment, '
+                         'max_sequence_length)')
+      self._async_work = True
+      status = self._lib.bsb_step_budgeted_sequence(*args, ctypes.byref(sequence._struct), self._stream())  # pylint: disable=protected-access
+      if status:
+        _lib.check(status)
+
+  def _step_budgeted(self, actions, out, mask, episodes_left, previous, replay=None, sequence=None):
+    mask, outputs, prev = self._budgeted_args(out, mask, episodes_left, previous)
+    actions = self._device_actions(actions, (self._batch,))
+    if replay is not None or sequence is not None:
+      self._step_recorded(actions.data_ptr(), None, mask, episodes_left, outputs, prev, None, replay, sequence)
       return out.timestep()
     self._async_work = True
     status = self._lib.bsb_step_budgeted(self._handle.ptr, actions.data_ptr(), mask.data_ptr(), episodes_left.data_ptr(),
@@ -570,7 +597,7 @@ class BatchedEnvironment:
       _lib.check(status)
     return out.timestep()
 
-  def _step_policy(self, actions, out, mask, episodes_left, previous, policy, policy_seed, replay=None):
+  def _step_policy(self, actions, out, mask, episodes_left, previous, policy, policy_seed, replay=None, sequence=None):
     torch = self._torch
     if actions is not None:
       raise ValueError('policy replaces actions: pass one or the other')
@@ -597,15 +624,8 @@ class BatchedEnvironment:
             and chosen.is_contiguous()):
       raise ValueError(f'out.actions must be a contiguous int32 tensor of shape ({self._batch},) on {self._device}')
     spec = _lib.Policy(kind, 0, values.data_ptr(), epsilon, int(policy_seed) % (1 << 64))
-    if replay is not None:
-      ring = self._ring(replay)
-      self._async_work = True
-      status = self._lib.bsb_step_budgeted_record(self._handle.ptr, None, ctypes.byref(spec), mask.data_ptr(),
-                                                  episodes_left.data_ptr(), ctypes.byref(outputs), ctypes.byref(prev),
-                                                  chosen.data_ptr(), ctypes.byref(ring), self._stream())
-      if status:
-        _lib.check(status)
-      replay._draw = 0        # pylint: disable=protected-access
+    if replay is not None or sequence is not None:
+      self._step_recorded(None, spec, mask, episodes_left, outputs, prev, chosen.data_ptr(), replay, sequence)
       return out.timestep()
     self._async_work = True
     status = self._lib.bsb_step_budgeted_policy(self._handle.ptr, ctypes.byref(spec), mask.data_ptr(),

@@ -16,6 +16,9 @@
   * `LaneReplay` -- one replay ring per lane (baselines/utils/replay.py, as each bsuite_id run of the reference owns
     its own), filled by the budgeted step itself (`step(..., replay=...)`) and sampled on the device in one launch;
     `run_episodes` records for an agent that carries one as `agent.replay`.
+  * `LaneSequence` -- one sequence buffer per lane (baselines/utils/sequence.py's `Buffer`, which the reference's
+    actor-critic agents drain when it is full or the episode ends), filled by the budgeted step itself
+    (`step(..., sequence=...)`); `run_episodes` fills it for an agent that carries one as `agent.sequence`.
   * `Trajectory` / `collect` -- the `[T + 1]` observations / `[T]` actions, rewards, discounts layout of
     `bsuite/baselines/utils/sequence.py:26-35`, as device tensors with a lane axis, filled by ONE fused rollout
     (`bsb_rollout`: on-device uniform random actions) instead of T appends.
@@ -125,7 +128,9 @@ class EpisodeLoop:
   `select_action` has its actions chosen inside the step (`step(policy=..., policy_seed=...)`); its `update` receives
   `out.actions`, where a lane that sat out keeps its last pick (0 before its first).  An agent whose `replay`
   attribute is a `LaneReplay` of the environment has every transition recorded into it by the step
-  (`step(..., replay=...)`); its `update` is called as before and need only sample and learn."""
+  (`step(..., replay=...)`); its `update` is called as before and need only sample and learn.  Likewise an agent whose
+  `sequence` attribute is a `LaneSequence` has its sequences filled by the step (`step(..., sequence=...)`); its
+  `update` reads the sequences `sequence.ready` marks.  An agent may carry one of the two, not both."""
 
   def __init__(self, agent, environment, num_episodes: Optional[int] = None, policy_seed: int = 0):
     self.agent, self.environment = agent, environment
@@ -133,10 +138,13 @@ class EpisodeLoop:
     self.policy_seed = int(policy_seed)
     self.left = episode_budget(environment, num_episodes)
     self.mask = self.left > 0
-    replay = getattr(agent, 'replay', None)
+    replay, sequence = getattr(agent, 'replay', None), getattr(agent, 'sequence', None)
     self.replay = replay if isinstance(replay, LaneReplay) else None
+    self.sequence = sequence if isinstance(sequence, LaneSequence) else None
+    if self.replay is not None and self.sequence is not None:
+      raise ValueError('the agent carries a LaneReplay and a LaneSequence: the step fills one of them')
     # a recorded same-step environment keeps the final observations: they are o_t of the LAST transitions
-    final = self.replay is not None and environment.autoreset == 'same_step'
+    final = (self.replay is not None or self.sequence is not None) and environment.autoreset == 'same_step'
     self.out = environment.make_buffers(with_actions=self.uses_policy, final_observation=final)
     self.previous = environment.make_buffers(final_observation=final)
     if self.uses_policy:
@@ -156,12 +164,12 @@ class EpisodeLoop:
       policy = self.agent.select_policy(self.timestep)
       self.timestep = self.environment.step(out=self.out, mask=self.mask, episodes_left=self.left,
                                             previous=self.previous, policy=policy, policy_seed=self.policy_seed,
-                                            replay=self.replay)
+                                            replay=self.replay, sequence=self.sequence)
       actions = self.out.actions
     else:
       actions = self.agent.select_action(self.timestep)
       self.timestep = self.environment.step(actions, out=self.out, mask=self.mask, episodes_left=self.left,
-                                            previous=self.previous, replay=self.replay)
+                                            previous=self.previous, replay=self.replay, sequence=self.sequence)
     self.calls += 1
     self.agent.update(self.previous.timestep(), actions, self.timestep)
 
@@ -180,8 +188,8 @@ def run_episodes(agent, environment, num_episodes: Optional[int] = None, check_e
   running once every `check_every` calls.  An agent with `select_policy(timestep)` instead of `select_action` returns
   `EpsilonGreedy` / `Softmax` and has its actions chosen inside the step, on the policy stream keyed by
   (`policy_seed`, global lane), so its exploration does not depend on how lanes are sharded or packed
-  (`EpisodeLoop`).  An agent with a `replay` attribute that is a `LaneReplay` has its transitions recorded by the
-  step.  Returns the number of calls made after the first reset."""
+  (`EpisodeLoop`).  An agent with a `replay` attribute that is a `LaneReplay`, or a `sequence` attribute that is a
+  `LaneSequence`, has its transitions recorded by the step.  Returns the number of calls made after the first reset."""
   loop = EpisodeLoop(agent, environment, num_episodes, policy_seed)
   check_every = max(int(check_every), 1)
   while loop.calls % check_every != 0 or bool(loop.any_left()):
@@ -594,3 +602,69 @@ class LaneReplay:
     if env.ragged:
       o_tm1, o_t = env.split_observation(o_tm1), env.split_observation(o_t)
     return Transitions(o_tm1, out.actions, out.reward, out.discount, o_t, out.ready.view(env._torch.bool))  # pylint: disable=protected-access
+
+
+class LaneSequence:
+  """One sequence buffer of at most `max_sequence_length` (T) transitions per lane (baselines/utils/sequence.py's
+  `Buffer` per lane), filled by the budgeted step that produces the transitions (`environment.step(...,
+  sequence=self)`, or `run_episodes` with an agent whose `sequence` is this).
+
+  Storage, zero-initialised, in the rollout layout: `observations` [T + 1, B, ...] in the environment's `obs_dtype`,
+  `actions` int32 [T, B], `rewards` [T, B] in the step's reward dtype, `discounts` float32 [T, B], `step_types` int32
+  [T, B], `length` int64 [B] and `ready` bool [B].  Lane i's current sequence is `observations[:length[i] + 1, i]`
+  and the first `length[i]` entries of the others (`valid`); later entries are stale.
+
+  A step appends to every lane that stepped and whose new step type is not FIRST, as `Buffer.append` does; a lane's
+  sequence starts over (drained) at its first append after it was full or ended with a LAST.  `ready` marks the lanes
+  whose sequence the latest call closed (`if full() or last(): drain()` of actor_critic/agent.py), so an agent reads
+  `trajectory()` where `ready` is set, between two calls.  Memory: (T + 1) * B * observation bytes plus 16 T B bytes
+  of scalars.  The observation buffer comes from torch's default allocator, never from the compressible pool that
+  holds step observations (`obs_memory`)."""
+
+  def __init__(self, environment, max_sequence_length: int):
+    from bsuite_b200 import _lib  # pylint: disable=import-outside-toplevel
+    torch = environment._torch      # pylint: disable=protected-access
+    T = int(max_sequence_length)
+    if not 1 <= T <= (1 << 31) - 1:
+      raise ValueError(f'max_sequence_length must lie in [1, 2^31 - 1], got {max_sequence_length}')
+    self.environment, self.max_sequence_length = environment, T
+    B, device = environment.batch, environment.device
+    lead = (T, B)
+    self.observations = torch.zeros(environment._obs_shape_of((T + 1, B)), dtype=environment.obs_dtype,  # pylint: disable=protected-access
+                                    device=device)
+    self.actions = torch.zeros(lead, dtype=torch.int32, device=device)
+    self.rewards = torch.zeros(lead, dtype=environment._reward_dtype, device=device)  # pylint: disable=protected-access
+    self.discounts = torch.zeros(lead, dtype=torch.float32, device=device)
+    self.step_types = torch.zeros(lead, dtype=torch.int32, device=device)
+    self.length = torch.zeros(B, dtype=torch.int64, device=device)
+    self._ready = torch.zeros(B, dtype=torch.uint8, device=device)
+    self.ready = self._ready.view(torch.bool)
+    nxt = _lib.Outputs()
+    if self.rewards.dtype == torch.float64:
+      nxt.reward_f64 = self.rewards.data_ptr()
+    else:
+      nxt.reward = self.rewards.data_ptr()
+    nxt.discount = self.discounts.data_ptr()
+    nxt.step_type = self.step_types.data_ptr()
+    self._struct = _lib.Sequence(T, self.length.data_ptr(), self._ready.data_ptr(), self.observations.data_ptr(),
+                                 self.actions.data_ptr(), nxt)
+
+  @property
+  def valid(self):
+    """bool [T, B]: entry t of lane i belongs to its current sequence (t < length[i])."""
+    torch = self.environment._torch      # pylint: disable=protected-access
+    t = torch.arange(self.max_sequence_length, device=self.length.device).unsqueeze(1)
+    return t < self.length.unsqueeze(0)
+
+  def trajectory(self) -> Trajectory:
+    """The buffers as a `Trajectory` (no copy); on a ragged pack `observations` is a tuple of per-setting views
+    (`split_observation`)."""
+    observations = self.observations
+    if self.environment.ragged:
+      observations = self.environment.split_observation(observations)
+    return Trajectory(observations, self.actions, self.rewards, self.discounts, self.step_types)
+
+  def reset(self) -> None:
+    """Empties every lane's sequence."""
+    self.length.zero_()
+    self._ready.zero_()

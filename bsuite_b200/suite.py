@@ -234,8 +234,9 @@ class SweepBatch:
     device-to-host copy; an environment leaves the rotation once its lanes are done.  The caller's current stream
     waits for all of them before this returns.  Agents may define `select_policy` instead of `select_action`
     (`rollouts.EpisodeLoop`); their policy streams are keyed by (`policy_seed`, lane within the setting), so a pack,
-    a per-id sweep and every shard pick the same actions for the same values.  Returns the calls made after the reset
-    per environment."""
+    a per-id sweep and every shard pick the same actions for the same values.  An agent whose `replay` is a
+    `rollouts.LaneReplay`, or whose `sequence` is a `rollouts.LaneSequence`, has it filled by the step, as in
+    `run_episodes`.  Returns the calls made after the reset per environment."""
     import contextlib  # pylint: disable=import-outside-toplevel
     from bsuite_b200 import rollouts  # pylint: disable=import-outside-toplevel
     torch = self._torch

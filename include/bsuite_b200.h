@@ -568,6 +568,66 @@ int32_t bsb_replay_sample(bsb_env* env, const bsb_replay* replay, int64_t size, 
                           uint64_t seed, uint64_t draw, const bsb_replay* batch, uint8_t* ready,
                           void* stream);
 
+/*
+ * Per-lane sequence buffers (baselines/utils/sequence.py's Buffer, one
+ * window of at most T = max_length transitions per lane, as the reference's
+ * actor_critic and actor_critic_rnn keep one per bsuite_id run).  The layout
+ * is the engine's rollout layout: observations is [T + 1][step_elems] in the
+ * handle's obs_dtype (raw bytes, a ragged pack's settings at the offsets
+ * bsb_ragged_layout reports), action / next.reward / next.reward_f64 /
+ * next.discount / next.step_type are [T, B].  Offsets are 64-bit.  Lane i's
+ * current sequence is observations[0 .. length[i]] and entries
+ * [0, length[i]) of the others; later entries are stale.
+ */
+typedef struct bsb_sequence {
+  int64_t max_length;      /* T, in [1, 2^31 - 1] */
+  int64_t* length;         /* int64 [B]: transitions in the lane's current sequence */
+  uint8_t* ready;          /* uint8 [B]: written for every lane by every call */
+  float* observations;     /* [T + 1][step_elems] in the handle's obs_dtype */
+  int32_t* action;         /* int32 [T, B] */
+  bsb_outputs next;        /* reward or reward_f64, discount, step_type [T, B];
+                              observation and final_observation NULL */
+} bsb_sequence;
+
+/*
+ * Sequence step: bsb_step_budgeted (actions != NULL) or
+ * bsb_step_budgeted_policy (policy != NULL; exactly one of the two) that also
+ * appends each transition to its lane's sequence.  The call equals that call
+ * bit for bit in everything it defines.  In addition every lane i that
+ * stepped (mask set and episodes_left > 0 before the call) and whose new
+ * step_type is not FIRST appends one transition (sequence.py's append):
+ *   t = length[i]; if t == T, or t > 0 and next.step_type[t - 1, i] is LAST,
+ *   the previous sequence was drained: t = 0 (a length outside [0, T) also
+ *   starts over)
+ *   observations[0]       (t == 0 only) the observation row copied to
+ *                         `previous`: o_tm1, what the agent acted on
+ *   observations[t + 1]   the new observation row; on a same-step handle whose
+ *                         new step_type is LAST, the final observation row
+ *   action[t, i]          the action used (the caller's action after
+ *                         clamping, or the policy's pick)
+ *   next.*[t, i]          the new reward (cast as bsb_step_budgeted_record
+ *                         casts it), discount and step_type
+ *   length[i] = t + 1, ready[i] = (t + 1 == T or the new step_type is LAST).
+ * Every other lane gets ready[i] = 0 and nothing else is written, so `ready`
+ * marks exactly the sequences this call closed (sequence.py: `if full() or
+ * last(): drain()`); the drain happens lazily at the lane's next append, so
+ * the closed sequence can be read until the next call.  The rows are copied,
+ * never re-rendered.  State lives in `length` and next.step_type only.
+ * Refused (BSB_INVALID_ARGUMENT, before anything moves): whatever the
+ * underlying budgeted or policy step refuses, both or neither of actions and
+ * policy, actions_out with actions, a NULL sequence / length / ready /
+ * observations / action / next.step_type / next.discount, both rewards
+ * NULL, a sequence reward with no reward in `out`, max_length outside
+ * [1, 2^31 - 1], next.observation or next.final_observation non-NULL, an
+ * observation buffer that is out's or previous's, out->step_type NULL, a
+ * same-step handle without out->final_observation.  Every handle
+ * bsb_step_budgeted accepts; graph-safe mode and capture included.
+ */
+int32_t bsb_step_budgeted_sequence(bsb_env* env, const int32_t* actions, const bsb_policy* policy,
+                                   uint8_t* mask, int64_t* episodes_left,
+                                   const bsb_outputs* out, const bsb_outputs* previous,
+                                   int32_t* actions_out, const bsb_sequence* sequence, void* stream);
+
 /* Host mirror of the on-device action sampler: out int32 [T,B] (host). */
 int32_t bsb_random_actions(uint64_t action_seed, uint64_t lane_offset,
                            int64_t batch, int64_t first_step, int64_t num_steps,
@@ -599,8 +659,8 @@ int32_t bsb_read_episode_stats(bsb_env* env, int32_t field, double* dst,
 
 /*
  * CUDA graphs.  bsb_step / bsb_reset / bsb_rollout / the masked calls (bsb_reset_masked / bsb_step_masked /
- * bsb_rollout_masked / bsb_advance_masked / bsb_step_budgeted / bsb_step_budgeted_policy / bsb_step_budgeted_record)
- * / bsb_replay_sample / bsb_read_* / bsb_sum_* may
+ * bsb_rollout_masked / bsb_advance_masked / bsb_step_budgeted / bsb_step_budgeted_policy / bsb_step_budgeted_record
+ * / bsb_step_budgeted_sequence) / bsb_replay_sample / bsb_read_* / bsb_sum_* may
  * be called on a stream that is being captured.  A graph freezes launch arguments, so the first captured launch moves the handle's step
  * counter (it indexes the on-device action stream and the Logging columns) and its chunk scheduler into device
  * memory, for good: replays and eager calls can then be mixed in any order, and bsb_steps_done / bsb_get_state
