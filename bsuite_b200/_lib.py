@@ -101,6 +101,18 @@ class Sequence(ctypes.Structure):
               ('observations', ctypes.c_void_p), ('action', ctypes.c_void_p), ('next', Outputs)]
 
 
+class EnsemblePolicy(ctypes.Structure):
+  """struct bsb_ensemble_policy: every head's action values and each lane's active head."""
+  _fields_ = [('num_heads', ctypes.c_int32), ('reserved', ctypes.c_int32), ('values', ctypes.c_void_p),
+              ('heads', ctypes.c_void_p), ('epsilon', ctypes.c_double), ('seed', ctypes.c_uint64)]
+
+
+class Bootstrap(ctypes.Structure):
+  """struct bsb_bootstrap: the bootstrap masks and reward noise a sample draws."""
+  _fields_ = [('num_heads', ctypes.c_int32), ('reserved', ctypes.c_int32), ('mask_prob', ctypes.c_double),
+              ('seed', ctypes.c_uint64), ('mask', ctypes.c_void_p), ('noise', ctypes.c_void_p)]
+
+
 SCORE_MAX_SOURCES = 512      # bsb_score: sources per call
 # enum bsb_score_quantity: the row columns a score reads
 SCORE_QUANTITIES = ('episode', 'total_return', 'total_regret', 'raw_return', 'best_episode', 'total_perfect',
@@ -167,6 +179,13 @@ EXPORTS = {
     'bsb_replay_sample': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(Replay), ctypes.c_int64, ctypes.c_int64,
                                            ctypes.c_uint64, ctypes.c_uint64, ctypes.POINTER(Replay), ctypes.c_void_p,
                                            ctypes.c_void_p]),
+    'bsb_step_budgeted_ensemble': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(EnsemblePolicy), ctypes.c_void_p,
+                                                    ctypes.c_void_p, ctypes.POINTER(Outputs), ctypes.POINTER(Outputs),
+                                                    ctypes.c_void_p, ctypes.POINTER(Replay), ctypes.c_void_p]),
+    'bsb_replay_sample_bootstrap': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(Replay), ctypes.c_int64,
+                                                     ctypes.c_int64, ctypes.c_uint64, ctypes.c_uint64,
+                                                     ctypes.POINTER(Replay), ctypes.c_void_p, ctypes.POINTER(Bootstrap),
+                                                     ctypes.c_void_p]),
     'bsb_random_actions': (ctypes.c_int32, [ctypes.c_uint64, ctypes.c_uint64, ctypes.c_int64, ctypes.c_int64,
                                             ctypes.c_int64, ctypes.c_int32, ctypes.c_void_p]),
     'bsb_steps_done': (ctypes.c_int32, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int64)]),

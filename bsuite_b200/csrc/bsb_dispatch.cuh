@@ -497,6 +497,46 @@ void host_sequence(const bsb_env* e, const LaunchArgs& a, uint8_t* mask, int64_t
   }
 }
 
+// bsb_step_budgeted_ensemble on a host handle, as masked_kernel's CALL_ENSEMBLE runs it: every lane that steps (mask
+// set, budget left) reads head h = heads[lane] (clamped into [0, K), raising the invalid-action flag, when outside it)
+// and its row (h, lane) of the values is gathered into a [B, A] policy; host_record (a replay) or host_policy steps
+// with it; then every such lane whose step ended an episode -- its budget counted down -- draws its new head.
+template <class V>
+void host_ensemble(const bsb_env* e, const LaunchArgs& a, uint8_t* mask, int64_t* episodes_left,
+                   const bsb_outputs* previous, const bsb_policy& policy, const bsb_ensemble_policy& ens,
+                   const bsb_replay* replay) {
+  const EnvParams& p = e->p;
+  const int64_t B = p.batch, A = p.num_actions;
+  const RaggedTable* ragged = V::kRagged ? reinterpret_cast<const RaggedTable*>(p.pack) : nullptr;
+  std::vector<float> rows((size_t)(B * A), 0.f);
+  std::vector<int64_t> before(episodes_left, episodes_left + B);
+  std::vector<uint8_t> stepped((size_t)B, 0);
+  for (int64_t lane = 0; lane < B; ++lane) {
+    stepped[(size_t)lane] = mask[lane] && episodes_left[lane] > 0;
+    if (!stepped[(size_t)lane]) continue;
+    int32_t head = ens.heads[lane];
+    if ((uint32_t)head >= (uint32_t)ens.num_heads) {
+      if (e->bad_action_host) *e->bad_action_host = 1;
+      head = head < 0 ? 0 : ens.num_heads - 1;
+    }
+    memcpy(rows.data() + lane * A, ens.values + ((int64_t)head * B + lane) * A, (size_t)A * sizeof(float));
+  }
+  bsb_policy gathered = policy;
+  gathered.values = rows.data();
+  if (replay) host_record<V>(e, a, mask, episodes_left, previous, &gathered, *replay);
+  else host_policy<V>(e, a, mask, episodes_left, previous, gathered);
+  for (int64_t lane = 0; lane < B; ++lane) {
+    if (!stepped[(size_t)lane] || episodes_left[lane] == before[(size_t)lane]) continue;
+    EnvParams lp = p;                     // the lane's setting: its lane_offset keys the stream as the kernel's does
+    if constexpr (V::kRagged) {
+      ragged_setting_params(lp, ragged_setting(ragged, lane / ragged->pack.lanes_per_setting), ragged->mapping_bits);
+    } else if constexpr (V::kPacked) {
+      pack_lane_params(lp, lane);
+    }
+    ens.heads[lane] = ensemble_head(policy.seed, lp.lane_offset + (uint64_t)lane, (uint64_t)a.step0, ens.num_heads);
+  }
+}
+
 // Kernels and host path of variant V, the runner bsb_create stores in the handle.  The bit sources and kernels are
 // those the variant list (BSB_VARIANTS) compiles for V: bsb_create picks no runner for an MT19937 handle whose variant
 // lacks MT19937, and only a variant with two_phase_host_kernel is given `two_phase` (a two-phase host step).
@@ -535,11 +575,12 @@ int run_variant(bsb_env* e, const LaunchArgs& a, cudaStream_t stream, const TwoP
 // budgeted step (`previous` given: bsb_step_budgeted, whose `mask_out` is the mask) takes CALL_BUDGETED, and one with a
 // `policy` (bsb_step_budgeted_policy: no actions, the picks to a.actions_out) takes CALL_POLICY.  A budgeted step with
 // a `replay` (bsb_step_budgeted_record, actions or a policy) takes CALL_RECORD, and one with a `sequence`
-// (bsb_step_budgeted_sequence) takes CALL_SEQUENCE.
+// (bsb_step_budgeted_sequence) takes CALL_SEQUENCE.  An `ensemble` step (bsb_step_budgeted_ensemble: its rule in
+// `policy`, a replay optional) takes CALL_ENSEMBLE.
 template <class V>
 int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* episodes_left, uint8_t* mask_out,
                const bsb_outputs* previous, const bsb_policy* policy, const bsb_replay* replay,
-               const bsb_sequence* sequence, cudaStream_t stream) {
+               const bsb_sequence* sequence, const bsb_ensemble_policy* ensemble, cudaStream_t stream) {
   constexpr bool kMt = Compiled<V>::kMt;
   const bool mt = e->p.rng_kind == BSB_RNG_MT19937;
   if (previous && (a.T != 1 || a.mode != MODE_STEP || !a.actions == !policy || (a.actions_out && !policy) ||
@@ -550,8 +591,11 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
   if (replay && (!previous || !a.step_type)) return fail(BSB_INTERNAL, "a recorded step must be a budgeted step with step types");
   if (sequence && (!previous || !a.step_type || replay))
     return fail(BSB_INTERNAL, "a sequence step must be a budgeted step with step types and no replay");
+  if (ensemble && (!policy || sequence))
+    return fail(BSB_INTERNAL, "an ensemble step must be a policy step with no sequence");
   if (e->device < 0) {
-    if (sequence) host_sequence<V>(e, a, mask_out, episodes_left, previous, policy, *sequence);
+    if (ensemble) host_ensemble<V>(e, a, mask_out, episodes_left, previous, *policy, *ensemble, replay);
+    else if (sequence) host_sequence<V>(e, a, mask_out, episodes_left, previous, policy, *sequence);
     else if (replay) host_record<V>(e, a, mask_out, episodes_left, previous, policy, *replay);
     else if (policy) host_policy<V>(e, a, mask_out, episodes_left, previous, *policy);
     else if (previous) host_budgeted<V>(e, a, mask_out, episodes_left, previous);
@@ -562,6 +606,8 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
   memset(&m, 0, sizeof(m));
   SequenceArgs sq;                       // CALL_SEQUENCE: m's MaskArgs and the sequence buffers
   memset(&sq, 0, sizeof(sq));
+  EnsembleArgs en;                       // CALL_ENSEMBLE: m's RecordArgs and the heads
+  memset(&en, 0, sizeof(en));
   m.mask = mask;
   m.noise = e->p.wrapper == BSB_WRAP_REWARD_NOISE ? 1 : 0;
   m.track = e->p.ep != nullptr ? 1 : 0;
@@ -586,6 +632,9 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
     } else if constexpr (kCall == CALL_SEQUENCE) {
       if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_sequence_kernel<V, 1>, e->p, la, sq); }
       return launch(e, la, g, stream, masked_sequence_kernel<V, 0>, e->p, la, sq);
+    } else if constexpr (kCall == CALL_ENSEMBLE) {
+      if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_ensemble_kernel<V, 1>, e->p, la, en); }
+      return launch(e, la, g, stream, masked_ensemble_kernel<V, 0>, e->p, la, en);
     } else {
       const MaskArgs& base = m;
       if constexpr (kMt) { if (mt) return launch(e, la, g, stream, masked_kernel<V, 1, kCall>, e->p, la, base); }
@@ -620,7 +669,13 @@ int run_masked(bsb_env* e, const LaunchArgs& a, const uint8_t* mask, int64_t* ep
       m.rec_vec_ok = reinterpret_cast<uintptr_t>(replay->obs_tm1) % 16 == 0 &&
                      reinterpret_cast<uintptr_t>(replay->next.observation) % 16 == 0 &&
                      ((size_t)e->step_elems * (size_t)e->obs_elem_bytes) % 16 == 0 ? 1 : 0;
-      return go(std::integral_constant<int, CALL_RECORD>());
+      if (!ensemble) return go(std::integral_constant<int, CALL_RECORD>());
+    }
+    if (ensemble) {
+      static_cast<RecordArgs&>(en) = m;
+      en.ens_heads = ensemble->heads;
+      en.ens_num_heads = ensemble->num_heads;
+      return go(std::integral_constant<int, CALL_ENSEMBLE>());
     }
     if (sequence) {
       static_cast<MaskArgs&>(sq) = m;

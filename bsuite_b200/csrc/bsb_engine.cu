@@ -87,11 +87,11 @@ template <class T> int env_alloc_t(bsb_env* e, T** out, size_t count, bool snaps
 // host step (`episodes_left`: the budgets, nullable; `mask_out`: a budgeted host step's mask write-back, nullable;
 // `previous`: a budgeted step's previous outputs, nullable; `policy`: a budgeted step's selection rule, nullable;
 // `replay`: the rings a recorded step appends to, nullable; `sequence`: the buffers a sequence step appends to,
-// nullable).
+// nullable; `ensemble`: an ensemble step's heads and values, nullable).
 int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseArgs* two_phase = nullptr,
         const uint8_t* mask = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr,
         const bsb_outputs* previous = nullptr, const bsb_policy* policy = nullptr, const bsb_replay* replay = nullptr,
-        const bsb_sequence* sequence = nullptr) {
+        const bsb_sequence* sequence = nullptr, const bsb_ensemble_policy* ensemble = nullptr) {
   DeviceGuard guard(e->device);
   LaunchArgs a = args;
   if (e->device >= 0) {
@@ -100,7 +100,9 @@ int run(bsb_env* e, const LaunchArgs& args, cudaStream_t stream, const TwoPhaseA
     if (capture != cudaStreamCaptureStatusNone) e->graph_safe = true;
     if (e->graph_safe) a.clock = e->clock;      // a.step0 == e->steps_done, which no longer moves
   }
-  if (mask) return e->variant->run_masked(e, a, mask, episodes_left, mask_out, previous, policy, replay, sequence, stream);
+  if (mask)
+    return e->variant->run_masked(e, a, mask, episodes_left, mask_out, previous, policy, replay, sequence, ensemble,
+                                  stream);
   return e->variant->run(e, a, stream, two_phase);
 }
 
@@ -861,12 +863,14 @@ int32_t bsb_step(bsb_env* env, const int32_t* actions, const bsb_outputs* out, v
 // the actions of masked-in lanes only, at every step of a rollout (a host step: of lanes with budget left): an
 // inactive lane's action is never read.  `mask_out`: a budgeted host step's write-back, or a budgeted step's mask;
 // `previous`: a budgeted step's previous outputs; `policy`: the rule that picks a budgeted step's actions; `replay`:
-// the rings a recorded step appends to; `sequence`: the buffers a sequence step appends to (run_masked).
+// the rings a recorded step appends to; `sequence`: the buffers a sequence step appends to; `ensemble`: an ensemble
+// step's heads and values (run_masked).
 static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask, const bsb_outputs* out, void* stream,
                        int mode, int64_t T = 1, bool rollout = false, uint64_t action_seed = 0,
                        int32_t* actions_out = nullptr, int64_t* episodes_left = nullptr, uint8_t* mask_out = nullptr,
                        const bsb_outputs* previous = nullptr, const bsb_policy* policy = nullptr,
-                       const bsb_replay* replay = nullptr, const bsb_sequence* sequence = nullptr) {
+                       const bsb_replay* replay = nullptr, const bsb_sequence* sequence = nullptr,
+                       const bsb_ensemble_policy* ensemble = nullptr) {
   { int crc = check_final_observation(env, out); if (crc != BSB_OK) return crc; }
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
   if (env->device < 0 && mode == MODE_STEP && actions) {
@@ -882,7 +886,7 @@ static int masked_call(bsb_env* env, const int32_t* actions, const uint8_t* mask
   LaunchArgs a = make_args(env, out, mode == MODE_STEP ? actions : nullptr, T, mode);
   a.action_seed = action_seed; a.actions_out = actions_out;
   int rc = run(env, a, static_cast<cudaStream_t>(stream), nullptr, mask, episodes_left, mask_out, previous, policy,
-               replay, sequence);
+               replay, sequence, ensemble);
   if (rc == BSB_OK) advance_steps(env, T);
   return rc;
 }
@@ -998,6 +1002,20 @@ static int check_ring(const bsb_replay* r, const std::string& name, const char* 
   return BSB_OK;
 }
 
+// The refusals of a replay a step appends to (bsb_step_budgeted_record, bsb_step_budgeted_ensemble).
+static int check_record(const bsb_env* env, const bsb_outputs* out, const bsb_outputs* previous, const bsb_replay* replay,
+                        const std::string& name) {
+  { int rc = check_ring(replay, name, "a replay", false); if (rc != BSB_OK) return rc; }
+  if (!out->step_type || !out->discount || (!out->reward && !out->reward_f64))
+    return fail(BSB_INVALID_ARGUMENT, name + " needs out's step_type, discount and reward (or reward_f64)");
+  for (const float* ring : {replay->obs_tm1, replay->next.observation})
+    if (ring == out->observation || ring == previous->observation || (out->final_observation && ring == out->final_observation))
+      return fail(BSB_INVALID_ARGUMENT, name + ": a ring observation buffer must not be out's or previous's");
+  if (env->same_step && !out->final_observation)
+    return fail(BSB_INVALID_ARGUMENT, name + " on a same-step handle needs out->final_observation: it is o_t of a LAST");
+  return BSB_OK;
+}
+
 // bsb_step_budgeted or bsb_step_budgeted_policy that appends each transition to its lane's ring: masked_kernel's
 // CALL_RECORD instantiation (run_masked), or host_record on a host handle.
 int32_t bsb_step_budgeted_record(bsb_env* env, const int32_t* actions, const bsb_policy* policy, uint8_t* mask,
@@ -1009,14 +1027,7 @@ int32_t bsb_step_budgeted_record(bsb_env* env, const int32_t* actions, const bsb
   { int rc = check_budgeted(env, choice, mask, episodes_left, out, previous, name, actions ? "actions" : "a policy"); if (rc != BSB_OK) return rc; }
   if (policy) { int rc = check_policy(policy, name); if (rc != BSB_OK) return rc; }
   else if (actions_out) return fail(BSB_INVALID_ARGUMENT, name + ": actions_out reports a policy's picks: pass NULL with actions");
-  { int rc = check_ring(replay, name, "a replay", false); if (rc != BSB_OK) return rc; }
-  if (!out->step_type || !out->discount || (!out->reward && !out->reward_f64))
-    return fail(BSB_INVALID_ARGUMENT, name + " needs out's step_type, discount and reward (or reward_f64)");
-  for (const float* ring : {replay->obs_tm1, replay->next.observation})
-    if (ring == out->observation || ring == previous->observation || (out->final_observation && ring == out->final_observation))
-      return fail(BSB_INVALID_ARGUMENT, name + ": a ring observation buffer must not be out's or previous's");
-  if (env->same_step && !out->final_observation)
-    return fail(BSB_INVALID_ARGUMENT, name + " on a same-step handle needs out->final_observation: it is o_t of a LAST");
+  { int rc = check_record(env, out, previous, replay, name); if (rc != BSB_OK) return rc; }
   return masked_call(env, actions, mask, out, stream, MODE_STEP, 1, false, 0, actions_out, episodes_left, mask, previous,
                      policy, replay);
 }
@@ -1051,6 +1062,31 @@ int32_t bsb_step_budgeted_sequence(bsb_env* env, const int32_t* actions, const b
     return fail(BSB_INVALID_ARGUMENT, name + " on a same-step handle needs out->final_observation: it is o_t of a LAST");
   return masked_call(env, actions, mask, out, stream, MODE_STEP, 1, false, 0, actions_out, episodes_left, mask, previous,
                      policy, nullptr, sequence);
+}
+
+// bsb_step_budgeted_policy (no replay) or bsb_step_budgeted_record (a replay) with epsilon-greedy over the rows of
+// each lane's active head, which is redrawn when the lane's episode ends: masked_ensemble_kernel (CALL_ENSEMBLE,
+// run_masked), or host_ensemble on a host handle.
+int32_t bsb_step_budgeted_ensemble(bsb_env* env, const bsb_ensemble_policy* policy, uint8_t* mask,
+                                   int64_t* episodes_left, const bsb_outputs* out, const bsb_outputs* previous,
+                                   int32_t* actions_out, const bsb_replay* replay, void* stream) {
+  const std::string name = "bsb_step_budgeted_ensemble";
+  { int rc = check_budgeted(env, policy, mask, episodes_left, out, previous, name, "a policy"); if (rc != BSB_OK) return rc; }
+  if (!policy->values || !policy->heads) return fail(BSB_INVALID_ARGUMENT, name + " needs the policy's values and heads");
+  if (policy->num_heads < 1 || policy->num_heads > 65536)
+    return fail(BSB_INVALID_ARGUMENT, name + ": num_heads must lie in [1, 65536], got " + std::to_string(policy->num_heads));
+  if (policy->reserved != 0) return fail(BSB_INVALID_ARGUMENT, "bsb_ensemble_policy.reserved must be 0");
+  if (!(policy->epsilon >= 0.0 && policy->epsilon <= 1.0))
+    return fail(BSB_INVALID_ARGUMENT, "epsilon must lie in [0, 1], got " + std::to_string(policy->epsilon));
+  if (replay) { int rc = check_record(env, out, previous, replay, name); if (rc != BSB_OK) return rc; }
+  bsb_policy rule;                       // the rule; its values are the rows of the active heads
+  memset(&rule, 0, sizeof(rule));
+  rule.kind = BSB_POLICY_EPSILON_GREEDY;
+  rule.values = policy->values;
+  rule.epsilon = policy->epsilon;
+  rule.seed = policy->seed;
+  return masked_call(env, nullptr, mask, out, stream, MODE_STEP, 1, false, 0, actions_out, episodes_left, mask, previous,
+                     &rule, replay, nullptr, policy);
 }
 
 // ----- replay sampling --------------------------------------------------------------------------------------------
@@ -1141,8 +1177,66 @@ __global__ void __launch_bounds__(256) replay_sample_kernel(const SampleArgs s) 
   }
 }
 
-// bsb_replay_sample on a host handle: the kernel's gather, lane by lane.
-void host_sample(const SampleArgs& s) {
+// What a bootstrap sample adds (bsb_replay_sample_bootstrap): SampleArgs grown at its end, passed to
+// bootstrap_sample_kernel only, so that replay_sample_kernel compiles as it did.  boot_mask / boot_noise: [size, B, K],
+// nullable.
+struct BootstrapArgs : SampleArgs {
+  uint8_t* boot_mask;
+  float* boot_noise;
+  double mask_prob;
+  uint64_t boot_seed;
+  int32_t num_heads;
+};
+
+// The bootstrap draws of sample j of lane i (global lane g), which drew ring slot `slot`: the slot's transition index
+// t (the lane's (t + 1)-th transition; the ring holds its last min(N, capacity) of N), then every head's mask and
+// noise.  `tid`, `threads`: this thread's share of the heads (the kernel's warp, or all of them on the host); a mask
+// thread draws one Philox block for four heads, a noise thread one head.
+BSB_HD void bootstrap_draws(const BootstrapArgs& s, int64_t i, int64_t j, int64_t slot, u64 g, int tid, int threads) {
+  const int64_t N = s.num_added[i];
+  const int64_t t = N - 1 - (N - 1 - slot) % s.capacity;
+  const int64_t base = (j * s.batch + i) * (int64_t)s.num_heads;
+  if (s.boot_mask) {
+    const bool draw = s.mask_prob > 0.0 && s.mask_prob < 1.0;      // else every draw gives mask_prob itself
+    for (int64_t q = tid; 4 * q < s.num_heads; q += threads) {
+      PhiloxBlock b = {0, 0, 0, 0};
+      if (draw) b = bootstrap_mask_block(s.boot_seed, g, (u64)t, (u64)q);
+      for (int64_t k = 4 * q; k < 4 * q + 4 && k < s.num_heads; ++k)
+        s.boot_mask[base + k] = draw ? bootstrap_mask_word(replay_word(b, k), s.mask_prob) : (s.mask_prob >= 1.0 ? 1 : 0);
+    }
+  }
+  if (s.boot_noise)
+    for (int64_t k = tid; k < s.num_heads; k += threads) s.boot_noise[base + k] = bootstrap_noise(s.boot_seed, g, (u64)t, (u64)k);
+}
+
+// replay_sample_kernel with the bootstrap draws of every sample it gathers: one warp per (group of four samples, lane
+// i), the heads' draws spread over the warp's threads.
+__global__ void __launch_bounds__(256) bootstrap_sample_kernel(const BootstrapArgs s) {
+  const int tid = threadIdx.x & 31;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  const int64_t groups = (s.size + 3) / 4, items = groups * s.batch;
+  int64_t c = s.step0;
+  if (s.clock) c += (int64_t)*reinterpret_cast<const volatile unsigned long long*>(s.clock + 16 * (blockIdx.x % CLOCK_GROUPS));
+  for (int64_t item = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); item < items; item += warps) {
+    const int64_t q = item / s.batch, i = item - q * s.batch;
+    int64_t n, row, K;
+    bool ok;
+    sample_lane(s, i, n, ok, row, K);
+    if (q == 0 && tid == 0 && s.ready) s.ready[i] = ok ? 1 : 0;
+    if (!ok) continue;
+    const PhiloxBlock b = sample_block(s, c, i, q);
+    const u64 g = s.lane_offset + (u64)(i % s.lanes_per_setting);
+    for (int64_t j = 4 * q; j < 4 * q + 4 && j < s.size; ++j) {
+      const int64_t slot = replay_slot(replay_word(b, j), n);
+      sample_copy(s, i, j, slot, row, K, tid, 32);
+      bootstrap_draws(s, i, j, slot, g, tid, 32);
+    }
+  }
+}
+
+// bsb_replay_sample on a host handle: the kernel's gather, lane by lane; with `boot`
+// (bsb_replay_sample_bootstrap), bootstrap_sample_kernel's draws too.
+void host_sample(const SampleArgs& s, const BootstrapArgs* boot = nullptr) {
   for (int64_t i = 0; i < s.batch; ++i) {
     int64_t n, row, K;
     bool ok;
@@ -1151,8 +1245,11 @@ void host_sample(const SampleArgs& s) {
     if (!ok) continue;
     for (int64_t q = 0; 4 * q < s.size; ++q) {
       const PhiloxBlock b = sample_block(s, s.step0, i, q);
-      for (int64_t j = 4 * q; j < 4 * q + 4 && j < s.size; ++j)
-        sample_copy(s, i, j, replay_slot(replay_word(b, j), n), row, K, 0, 1);
+      for (int64_t j = 4 * q; j < 4 * q + 4 && j < s.size; ++j) {
+        const int64_t slot = replay_slot(replay_word(b, j), n);
+        sample_copy(s, i, j, slot, row, K, 0, 1);
+        if (boot) bootstrap_draws(*boot, i, j, slot, s.lane_offset + (u64)(i % s.lanes_per_setting), 0, 1);
+      }
     }
   }
 }
@@ -1160,9 +1257,11 @@ void host_sample(const SampleArgs& s) {
 }  // namespace
 }  // namespace bsb
 
-int32_t bsb_replay_sample(bsb_env* env, const bsb_replay* replay, int64_t size, int64_t min_size, uint64_t seed,
-                          uint64_t draw, const bsb_replay* batch, uint8_t* ready, void* stream) {
-  const std::string name = "bsb_replay_sample";
+// bsb_replay_sample (`bootstrap` null: replay_sample_kernel) and bsb_replay_sample_bootstrap
+// (bootstrap_sample_kernel), or host_sample on a host handle.
+static int sample_call(bsb_env* env, const bsb_replay* replay, int64_t size, int64_t min_size, uint64_t seed,
+                       uint64_t draw, const bsb_replay* batch, uint8_t* ready, const bsb_bootstrap* bootstrap,
+                       void* stream, const std::string& name) {
   if (!env) return fail(BSB_INVALID_ARGUMENT, name + " needs a handle");
   if (size <= 0) return fail(BSB_INVALID_ARGUMENT, name + ": size must be positive, got " + std::to_string(size));
   if (min_size < 0) return fail(BSB_INVALID_ARGUMENT, name + ": min_size must not be negative, got " + std::to_string(min_size));
@@ -1174,9 +1273,19 @@ int32_t bsb_replay_sample(bsb_env* env, const bsb_replay* replay, int64_t size, 
   if ((batch->next.reward && !replay->next.reward) || (batch->next.reward_f64 && !replay->next.reward_f64) ||
       (batch->next.discount && !replay->next.discount) || (batch->next.step_type && !replay->next.step_type))
     return fail(BSB_INVALID_ARGUMENT, name + ": the batch asks for a scalar the ring does not carry");
+  if (bootstrap) {
+    if (bootstrap->num_heads < 1 || bootstrap->num_heads > 65536)
+      return fail(BSB_INVALID_ARGUMENT, name + ": num_heads must lie in [1, 65536], got " + std::to_string(bootstrap->num_heads));
+    if (bootstrap->reserved != 0) return fail(BSB_INVALID_ARGUMENT, "bsb_bootstrap.reserved must be 0");
+    if (!(bootstrap->mask_prob >= 0.0 && bootstrap->mask_prob <= 1.0))
+      return fail(BSB_INVALID_ARGUMENT, name + ": mask_prob must lie in [0, 1], got " + std::to_string(bootstrap->mask_prob));
+    if (!bootstrap->mask && !bootstrap->noise)
+      return fail(BSB_INVALID_ARGUMENT, name + " needs the bootstrap's mask or noise buffer (or both)");
+  }
   { int frc = drain_host_steps(env); if (frc != BSB_OK) return frc; }
-  SampleArgs s;
-  memset(&s, 0, sizeof(s));
+  BootstrapArgs boot;                    // s, grown by the bootstrap draws
+  memset(&boot, 0, sizeof(boot));
+  SampleArgs& s = boot;
   s.num_added = replay->num_added;
   s.obs_tm1 = reinterpret_cast<const uint8_t*>(replay->obs_tm1);
   s.obs = reinterpret_cast<const uint8_t*>(replay->next.observation);
@@ -1196,7 +1305,14 @@ int32_t bsb_replay_sample(bsb_env* env, const bsb_replay* replay, int64_t size, 
     if (reinterpret_cast<uintptr_t>(buf) % 16 != 0) s.vec_ok = 0;
   s.seed = seed; s.draw = draw; s.lane_offset = env->p.lane_offset;
   s.step0 = env->steps_done;
-  if (env->device < 0) { host_sample(s); return BSB_OK; }
+  if (bootstrap) {
+    boot.boot_mask = bootstrap->mask;
+    boot.boot_noise = bootstrap->noise;
+    boot.mask_prob = bootstrap->mask_prob;
+    boot.boot_seed = bootstrap->seed;
+    boot.num_heads = bootstrap->num_heads;
+  }
+  if (env->device < 0) { host_sample(s, bootstrap ? &boot : nullptr); return BSB_OK; }
   DeviceGuard guard(env->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
@@ -1207,10 +1323,24 @@ int32_t bsb_replay_sample(bsb_env* env, const bsb_replay* replay, int64_t size, 
   int64_t grid = (warps + 7) / 8;
   const int64_t cap = (int64_t)env->num_sms * 64;
   if (grid > cap) grid = cap;
-  replay_sample_kernel<<<(unsigned)grid, 256, 0, st>>>(s);
+  if (bootstrap) bootstrap_sample_kernel<<<(unsigned)grid, 256, 0, st>>>(boot);
+  else replay_sample_kernel<<<(unsigned)grid, 256, 0, st>>>(s);
   BSB_CUDA(cudaGetLastError());
   g_launches.fetch_add(1, std::memory_order_relaxed);
   return BSB_OK;
+}
+
+int32_t bsb_replay_sample(bsb_env* env, const bsb_replay* replay, int64_t size, int64_t min_size, uint64_t seed,
+                          uint64_t draw, const bsb_replay* batch, uint8_t* ready, void* stream) {
+  return sample_call(env, replay, size, min_size, seed, draw, batch, ready, nullptr, stream, "bsb_replay_sample");
+}
+
+int32_t bsb_replay_sample_bootstrap(bsb_env* env, const bsb_replay* replay, int64_t size, int64_t min_size,
+                                    uint64_t seed, uint64_t draw, const bsb_replay* batch, uint8_t* ready,
+                                    const bsb_bootstrap* bootstrap, void* stream) {
+  const std::string name = "bsb_replay_sample_bootstrap";
+  if (!bootstrap) return fail(BSB_INVALID_ARGUMENT, name + " needs a bootstrap");
+  return sample_call(env, replay, size, min_size, seed, draw, batch, ready, bootstrap, stream, name);
 }
 
 int32_t bsb_random_actions(uint64_t action_seed, uint64_t lane_offset, int64_t batch, int64_t first_step,

@@ -33,17 +33,19 @@ template <class V> int run_variant(bsb_env*, const LaunchArgs&, cudaStream_t, co
 // outputs that receive the masked-in lanes' current entries before the step.  `policy` (bsb_step_budgeted_policy,
 // else null): the rule that chooses a budgeted step's actions.  `replay` (bsb_step_budgeted_record, else null): the
 // lanes' rings a budgeted step appends its transitions to.  `sequence` (bsb_step_budgeted_sequence, else null): the
-// lanes' sequence buffers a budgeted step appends its transitions to.
+// lanes' sequence buffers a budgeted step appends its transitions to.  `ensemble` (bsb_step_budgeted_ensemble, else
+// null): the heads and values of an ensemble step, whose `policy` is then its epsilon-greedy rule.
 template <class V> int run_masked(bsb_env*, const LaunchArgs&, const uint8_t* mask, int64_t* episodes_left,
                                   uint8_t* mask_out, const bsb_outputs* previous, const bsb_policy* policy,
-                                  const bsb_replay* replay, const bsb_sequence* sequence, cudaStream_t);
+                                  const bsb_replay* replay, const bsb_sequence* sequence,
+                                  const bsb_ensemble_policy* ensemble, cudaStream_t);
 // An entry of the variant list, as bsb_create looks it up (bsb_engine.cu).
 struct VariantEntry {
   int family, obs_dtype, mode;
   bool mt, two_phase;
   int (*run)(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs*);
   int (*run_masked)(bsb_env*, const LaunchArgs&, const uint8_t*, int64_t*, uint8_t*, const bsb_outputs*, const bsb_policy*,
-                    const bsb_replay*, const bsb_sequence*, cudaStream_t);
+                    const bsb_replay*, const bsb_sequence*, const bsb_ensemble_policy*, cudaStream_t);
 };
 
 #define BSB_CUDA(expr)                                                                   \

@@ -1537,6 +1537,14 @@ struct SequenceArgs : MaskArgs {
   int32_t seq_vec_ok;
 };
 
+// The arguments of a CALL_ENSEMBLE launch: RecordArgs grown at its end by boot_dqn's ensemble (bsb_ensemble_policy),
+// passed to masked_ensemble_kernel only, for the reason RecordArgs is.  policy_values holds every head's values
+// [K, B, num_actions]; the ring fields are null when the step records nothing (rec_num_added decides, at run time).
+struct EnsembleArgs : RecordArgs {
+  int32_t* ens_heads;
+  int32_t ens_num_heads;
+};
+
 // What one masked_kernel instantiation runs.  CALL_ROLLOUT: bsb_rollout_masked (T steps, sampled or given actions,
 // budgets, actions_out).  CALL_ONE: a masked reset or step (T = 1, the caller's actions, no budgets).  CALL_HOST:
 // bsb_step_host_masked (T = 1, the caller's actions, optional budgets, the mask write-back, the mailbox signal).
@@ -1547,9 +1555,10 @@ struct SequenceArgs : MaskArgs {
 // policy's values by select_action, and written to actions_out).  CALL_RECORD: bsb_step_budgeted_record
 // (CALL_BUDGETED or CALL_POLICY, chosen at run time by m.policy_values, with each transition appended to its lane's
 // ring).  CALL_SEQUENCE: bsb_step_budgeted_sequence (CALL_RECORD's step, with each transition appended to its lane's
-// sequence buffer instead of a ring).
+// sequence buffer instead of a ring).  CALL_ENSEMBLE: bsb_step_budgeted_ensemble (CALL_RECORD's policy step reading
+// the row of the lane's active head, the ring write when a replay is given, then the head redrawn at a LAST).
 enum CallKind { CALL_ROLLOUT = 0, CALL_ONE = 1, CALL_HOST = 2, CALL_ADVANCE = 3, CALL_BUDGETED = 4, CALL_POLICY = 5,
-                CALL_RECORD = 6, CALL_SEQUENCE = 7 };
+                CALL_RECORD = 6, CALL_SEQUENCE = 7, CALL_ENSEMBLE = 8 };
 
 // Writes lane j's observation `val(e)` (element e of K) with the whole warp: 16-byte streaming stores when `vec`
 // (the row starts 16-byte aligned and is a whole number of 16-byte words), else one element per store.
@@ -1690,8 +1699,12 @@ __device__ __forceinline__ void record_lane_rows(const O* src, O* ring, int64_t 
 // (a_tm1, r_t, d_t, o_t) at entry t of its sequence buffer, and o_tm1 at observation slot 0 when t == 0 (a new
 // sequence): t is the lane's length, or 0 when the length reached max_length or the entry before it is a LAST (the
 // sequence was closed by an earlier call).  Every lane writes its ready flag: set where the append closed the sequence.
-// The body (bsb_masked_body.inc) is shared with masked_record_kernel and masked_sequence_kernel, which run CALL_RECORD
-// and CALL_SEQUENCE.
+// kCall == CALL_ENSEMBLE: CALL_RECORD with a policy, where a stepping lane reads head h = ens_heads[lane] (clamped
+// into [0, K) with the invalid-action flag raised when outside it) and selects epsilon-greedily from row (h, lane) of
+// policy_values [K, B, num_actions]; the ring write runs when rec_num_added is set; then a lane that stepped and whose
+// step ended an episode (the LAST that counts its budget down) writes a new head drawn by ensemble_head at the call's
+// step index.  The body (bsb_masked_body.inc) is shared with masked_record_kernel, masked_sequence_kernel and
+// masked_ensemble_kernel, which run CALL_RECORD, CALL_SEQUENCE and CALL_ENSEMBLE.
 template <class V, int RK, int kCall>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_kernel(const EnvParams p, const LaunchArgs a, const MaskArgs m) {
 #include "bsb_masked_body.inc"
@@ -1708,6 +1721,13 @@ __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_record_k
 template <class V, int RK>
 __global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_sequence_kernel(const EnvParams p, const LaunchArgs a, const SequenceArgs m) {
   constexpr int kCall = CALL_SEQUENCE;
+#include "bsb_masked_body.inc"
+}
+
+// CALL_ENSEMBLE: masked_kernel's body with EnsembleArgs.
+template <class V, int RK>
+__global__ void __launch_bounds__(128, BSB_LAUNCH_MIN_BLOCKS(V)) masked_ensemble_kernel(const EnvParams p, const LaunchArgs a, const EnsembleArgs m) {
+  constexpr int kCall = CALL_ENSEMBLE;
 #include "bsb_masked_body.inc"
 }
 

@@ -61,7 +61,8 @@ BSB_HD PhiloxBlock philox4x64_10(u64 c0, u64 c1, u64 c2, u64 c3, u64 k0, u64 k1)
 }
 
 // Stream ids carried in counter word 3.
-enum : u64 { STREAM_ENV = 0, STREAM_WRAPPER = 1, STREAM_ACTIONS = 2, STREAM_POLICY = 3, STREAM_REPLAY = 4 };
+enum : u64 { STREAM_ENV = 0, STREAM_WRAPPER = 1, STREAM_ACTIONS = 2, STREAM_POLICY = 3, STREAM_REPLAY = 4,
+             STREAM_HEAD = 5, STREAM_BOOTSTRAP = 6 };
 
 // On-device uniform random actions (the workload of baselines/random/agent.py:35-37).
 // The action stream of a lane is the Philox stream (key = (action_seed, global lane), counter word 3 =
@@ -171,6 +172,59 @@ BSB_HD u64 replay_word(const PhiloxBlock& b, int64_t j) {
   switch (j & 3) { case 0: return b.v0; case 1: return b.v1; case 2: return b.v2; default: return b.v3; }
 }
 BSB_HD int64_t replay_slot(u64 word, int64_t n) { return (int64_t)(((word & 0xffffffffull) * (u64)n) >> 32); }
+
+// log(x) for x in (0, 1] built from + - * / and frexp / ldexp alone, so the host path and the kernels (compiled with
+// --fmad=false / -ffp-contract=off) compute the same bits, as bsb_exp does.  x = m 2^k with m in [sqrt(1/2), sqrt(2));
+// with f = m - 1 (exact) and s = f / (2 + f), log(m) = f - f^2/2 + s (f^2/2 + R(s^2)), R the minimax series of
+// 2 atanh(s) / s - 2 - 2 s^2 / 3 ... in s^2 to degree 7 (FreeBSD's msun e_log.c coefficients); k ln2 is added in
+// Cody-Waite halves as bsb_exp splits it.  Within one ulp of numpy.log on (0, 1] (DESIGN.md §3, "Ensemble steps and
+// bootstrap samples").  0 gives -inf, anything else outside (0, 1] NaN.
+BSB_HD double bsb_log(double x) {
+  if (!(x > 0.0 && x <= 1.0)) return x == 0.0 ? -INFINITY : NAN;
+  int k;
+  double m = frexp(x, &k);               // m in [1/2, 1)
+  if (m < 0.7071067811865476) { m = m + m; k -= 1; }
+  const double f = m - 1.0;
+  const double s = f / (2.0 + f);
+  const double z = s * s, w = z * z;
+  const double t1 = w * (3.999999999940941908e-01 + w * (2.222219843214978396e-01 + w * 1.531383769920937332e-01));
+  const double t2 = z * (6.666666666666735130e-01 + w * (2.857142874366239149e-01 + w * (1.818357216161805012e-01 +
+                                                                                         w * 1.479819860511658591e-01)));
+  const double R = t2 + t1;
+  const double hfsq = 0.5 * f * f;
+  const double dk = (double)k;
+  return dk * 6.93147180369123816490e-01 - ((hfsq - (s * (hfsq + R) + dk * 1.90821492927058770002e-10)) - f);
+}
+
+// Boot_dqn's per-episode head (bsb_step_budgeted_ensemble): a lane whose step ended an episode at global step s draws
+// head (lo32(w0) * K) >> 32, w0 word 0 of the Philox block at counter (s, 0, 0, STREAM_HEAD) with key (seed, g).
+BSB_HD int32_t ensemble_head(u64 seed, u64 global_lane, u64 step, int32_t num_heads) {
+  const PhiloxBlock b = philox4x64_10(step, 0, 0, STREAM_HEAD, seed, global_lane);
+  return (int32_t)(((b.v0 & 0xffffffffull) * (u64)(u32)num_heads) >> 32);
+}
+
+// Boot_dqn's bootstrap mask and reward noise of transition j (the lane's 0-based count of transitions added before
+// it) of global lane g, head k, key (seed, g) (bsb_replay_sample_bootstrap).  Mask: word k & 3 of the block at counter
+// (j, k >> 2, 0, STREAM_BOOTSTRAP) gives u = (w >> 11) 2^-53, and the mask is u < mask_prob.  Noise: numpy's legacy
+// polar method on the blocks at counter (j, k, 1 + a, STREAM_BOOTSTRAP), attempt a = 0, 1, ...: x, y = 2 u - 1 from
+// words 0 and 1, accepted when 0 < r2 = x^2 + y^2 < 1, z = y sqrt(-2 bsb_log(r2) / r2) (gauss's first variate); 0
+// after 64 rejected attempts (probability below 1e-42).
+BSB_HD uint8_t bootstrap_mask_word(u64 w, double mask_prob) {
+  return (double)(w >> 11) * 1.1102230246251565e-16 < mask_prob ? 1 : 0;      // 2^-53
+}
+BSB_HD PhiloxBlock bootstrap_mask_block(u64 seed, u64 global_lane, u64 j, u64 k4) {
+  return philox4x64_10(j, k4, 0, STREAM_BOOTSTRAP, seed, global_lane);
+}
+BSB_HD float bootstrap_noise(u64 seed, u64 global_lane, u64 j, u64 k) {
+  for (u64 attempt = 0; attempt < 64; ++attempt) {
+    const PhiloxBlock b = philox4x64_10(j, k, 1 + attempt, STREAM_BOOTSTRAP, seed, global_lane);
+    const double x = 2.0 * ((double)(b.v0 >> 11) * 1.1102230246251565e-16) - 1.0;
+    const double y = 2.0 * ((double)(b.v1 >> 11) * 1.1102230246251565e-16) - 1.0;
+    const double r2 = x * x + y * y;
+    if (r2 < 1.0 && r2 != 0.0) return (float)(y * sqrt(-2.0 * bsb_log(r2) / r2));
+  }
+  return 0.0f;
+}
 
 // ---------------------------------------------------------------------------
 // Bit source 1: Philox stream with numpy's buffering semantics.

@@ -10,7 +10,7 @@ namespace bsb {
   template int run_variant<Variant<F, O, mode> >(bsb_env*, const LaunchArgs&, cudaStream_t, const TwoPhaseArgs*); \
   template int run_masked<Variant<F, O, mode> >(bsb_env*, const LaunchArgs&, const uint8_t*, int64_t*, uint8_t*, \
                                                 const bsb_outputs*, const bsb_policy*, const bsb_replay*, \
-                                                const bsb_sequence*, cudaStream_t);
+                                                const bsb_sequence*, const bsb_ensemble_policy*, cudaStream_t);
 BSB_UNIT(BSB_INSTANTIATE)
 #undef BSB_INSTANTIATE
 }  // namespace bsb

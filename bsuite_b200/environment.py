@@ -496,7 +496,13 @@ class BatchedEnvironment:
     policy step (`bsb_step_budgeted_sequence`): the call is the same step, bit for bit, and every lane that stepped and
     whose new step type is not FIRST appends (a_tm1, r_t, d_t, o_t) to its current sequence, which starts with o_tm1
     (the row copied to `previous`); `sequence.ready` marks the lanes whose sequence this call closed (full, or ended by
-    a LAST), which the agent reads before the next call.  Not together with `replay`."""
+    a LAST), which the agent reads before the next call.  Not together with `replay`.
+
+    `policy` may also be `rollouts.EnsembleEpsilonGreedy(values, heads, epsilon)` (boot_dqn; values float32 [K, B,
+    num_actions], heads int32 [B], both contiguous on the device): a policy step (`bsb_step_budgeted_ensemble`),
+    recorded when `replay` is given, that reads each stepping lane's row of its active head `heads[i]` and, where the
+    lane's episode ended in this call, writes a new head drawn on the head stream keyed by (`policy_seed`, global
+    lane).  It equals `EpsilonGreedy` over the gathered rows, bit for bit.  Not together with `sequence`."""
     torch = self._torch
     if replay is not None and episodes_left is None and previous is None:
       raise ValueError('replay= records a budgeted or policy step: it needs mask=, episodes_left= and previous=')
@@ -601,6 +607,8 @@ class BatchedEnvironment:
     torch = self._torch
     if actions is not None:
       raise ValueError('policy replaces actions: pass one or the other')
+    if isinstance(policy, rollouts.EnsembleEpsilonGreedy):
+      return self._step_ensemble(out, mask, episodes_left, previous, policy, policy_seed, replay, sequence)
     if isinstance(policy, rollouts.EpsilonGreedy):
       kind, values, epsilon = _lib.POLICY_EPSILON_GREEDY, policy.values, float(policy.epsilon)
     elif isinstance(policy, rollouts.Softmax):
@@ -633,6 +641,44 @@ class BatchedEnvironment:
                                                 chosen.data_ptr(), self._stream())
     if status:
       _lib.check(status)
+    return out.timestep()
+
+  def _step_ensemble(self, out, mask, episodes_left, previous, policy, policy_seed, replay, sequence):
+    torch = self._torch
+    if sequence is not None:
+      raise ValueError('an EnsembleEpsilonGreedy step records into replay= only: sequence= is not supported with it')
+    if episodes_left is None or previous is None:
+      raise ValueError('a policy step is a budgeted step: it needs episodes_left= and previous=')
+    values, heads = policy.values, policy.heads
+    if not (isinstance(values, torch.Tensor) and values.dtype is torch.float32 and values.dim() == 3
+            and tuple(values.shape[1:]) == (self._batch, self._spec.num_actions) and 1 <= values.shape[0] <= 65536
+            and values.device == self._device and values.is_contiguous()):
+      raise ValueError(f'ensemble values must be a contiguous float32 tensor of shape (K, {self._batch}, '
+                       f'{self._spec.num_actions}) with K in [1, 65536] on {self._device}, got '
+                       f'{getattr(values, "dtype", type(values).__name__)} {tuple(getattr(values, "shape", ()))} on '
+                       f'{getattr(values, "device", None)}')
+    if not (isinstance(heads, torch.Tensor) and heads.dtype is torch.int32 and tuple(heads.shape) == (self._batch,)
+            and heads.device == self._device and heads.is_contiguous()):
+      raise ValueError(f'ensemble heads must be a contiguous int32 tensor of shape ({self._batch},) on {self._device}')
+    if out is not None and out.actions is None:
+      raise ValueError('a policy step writes the chosen actions to out.actions: make out with '
+                       'make_buffers(with_actions=True)')
+    mask, outputs, prev = self._budgeted_args(out, mask, episodes_left, previous)
+    chosen = out.actions
+    if not (chosen.dtype is torch.int32 and tuple(chosen.shape) == (self._batch,) and chosen.device == self._device
+            and chosen.is_contiguous()):
+      raise ValueError(f'out.actions must be a contiguous int32 tensor of shape ({self._batch},) on {self._device}')
+    spec = _lib.EnsemblePolicy(values.shape[0], 0, values.data_ptr(), heads.data_ptr(), float(policy.epsilon),
+                               int(policy_seed) % (1 << 64))
+    ring = None if replay is None else ctypes.byref(self._ring(replay))
+    self._async_work = True
+    status = self._lib.bsb_step_budgeted_ensemble(self._handle.ptr, ctypes.byref(spec), mask.data_ptr(),
+                                                  episodes_left.data_ptr(), ctypes.byref(outputs), ctypes.byref(prev),
+                                                  chosen.data_ptr(), ring, self._stream())
+    if status:
+      _lib.check(status)
+    if replay is not None:
+      replay._draw = 0        # pylint: disable=protected-access
     return out.timestep()
 
   def make_mixed_buffers(self) -> StepBuffers:

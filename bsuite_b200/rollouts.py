@@ -6,7 +6,9 @@
     runs unchanged on the B = 1 face (`DmEnvAdapter`): it only calls `reset()` / `step()`.
   * `RandomAgent` -- `bsuite/baselines/random/agent.py:26-45` with one generator call per step for the whole batch.
   * `EpsilonGreedy` / `Softmax` -- the selection rules of the reference's dqn / boot_dqn and actor_critic agents,
-    which an agent's `select_policy` returns so that the budgeted step picks its actions on the device.
+    which an agent's `select_policy` returns so that the budgeted step picks its actions on the device;
+    `EnsembleEpsilonGreedy` -- boot_dqn's rule over an ensemble, with each lane's active head kept and redrawn at the
+    end of every episode by the step itself.
   * `run_episodes` / `run_random_episodes` -- `experiment.run` to each lane's episode budget, with any agent through
     budgeted steps (one launch per call), or with the random agent's actions sampled on the device through fused
     masked launches that write no per-step output (`advance`); `suite.SweepBatch.run_episodes` and
@@ -15,7 +17,8 @@
     (`step_host(..., mask=..., episodes_left=...)`), on one handle or over part-batches.
   * `LaneReplay` -- one replay ring per lane (baselines/utils/replay.py, as each bsuite_id run of the reference owns
     its own), filled by the budgeted step itself (`step(..., replay=...)`) and sampled on the device in one launch;
-    `run_episodes` records for an agent that carries one as `agent.replay`.
+    `run_episodes` records for an agent that carries one as `agent.replay`.  With a `Bootstrap`, each sample also
+    draws boot_dqn's per-transition bootstrap masks and reward noise.
   * `LaneSequence` -- one sequence buffer per lane (baselines/utils/sequence.py's `Buffer`, which the reference's
     actor-critic agents drain when it is full or the episode ends), filled by the budgeted step itself
     (`step(..., sequence=...)`); `run_episodes` fills it for an agent that carries one as `agent.sequence`.
@@ -40,6 +43,27 @@ class EpsilonGreedy(NamedTuple):
 class Softmax(NamedTuple):
   """A categorical sample over `logits` (baselines/jax/actor_critic/agent.py:102-108): float32 [B, num_actions]."""
   logits: Any
+
+
+class EnsembleEpsilonGreedy(NamedTuple):
+  """Boot_dqn's selection (baselines/jax/boot_dqn/agent.py:146-169): `EpsilonGreedy` over the values of each lane's
+  active ensemble member, which is drawn anew, uniformly, whenever the lane's episode ends.  `values`: float32
+  [K, B, num_actions], contiguous, every head's action values; `heads`: int32 [B], the caller's, zero-filled before a
+  run (the reference starts on member 0) and updated in place by the step."""
+  values: Any
+  heads: Any
+  epsilon: float
+
+
+class Bootstrap(NamedTuple):
+  """Boot_dqn's bootstrap draws for a `LaneReplay` (agent.py:171-185): every transition gets a mask ~
+  Bernoulli(mask_prob) and, with `noise`, a reward noise ~ N(0, 1) per head, drawn when the transition is sampled
+  from a stream keyed by (`seed`, global lane, the transition's index in its lane), so a transition shows the same
+  draws every time it is sampled and the rings store nothing more."""
+  num_heads: int
+  mask_prob: float = 1.0
+  noise: bool = False
+  seed: int = 0
 
 
 class Trajectory(NamedTuple):
@@ -125,7 +149,8 @@ class EpisodeLoop:
   `any_left()` is the device flag "some lane has episodes left".
 
   An agent that defines `select_policy(timestep)` (returning `EpsilonGreedy` or `Softmax`) instead of
-  `select_action` has its actions chosen inside the step (`step(policy=..., policy_seed=...)`); its `update` receives
+  `select_action` has its actions chosen inside the step (`step(policy=..., policy_seed=...)`; an
+  `EnsembleEpsilonGreedy` also has its heads redrawn there); its `update` receives
   `out.actions`, where a lane that sat out keeps its last pick (0 before its first).  An agent whose `replay`
   attribute is a `LaneReplay` of the environment has every transition recorded into it by the step
   (`step(..., replay=...)`); its `update` is called as before and need only sample and learn.  Likewise an agent whose
@@ -489,8 +514,23 @@ class Transitions(NamedTuple):
   ready: Any
 
 
+class BootstrapTransitions(NamedTuple):
+  """A minibatch of `LaneReplay.sample` with a `Bootstrap`: `Transitions` in the reference's order with each
+  transition's bootstrap mask `m_t` (uint8 [size, B, K]) and reward noise `z_t` (float32 [size, B, K], None without
+  noise) before `ready`."""
+  o_tm1: Any
+  a_tm1: Any
+  r_t: Any
+  d_t: Any
+  o_t: Any
+  m_t: Any
+  z_t: Any
+  ready: Any
+
+
 class ReplayBatch:
-  """Caller-owned output tensors of `LaneReplay.sample(size, out=...)` (`LaneReplay.make_batch(size)`)."""
+  """Caller-owned output tensors of `LaneReplay.sample(size, out=...)` (`LaneReplay.make_batch(size)`); with the
+  replay's `Bootstrap`, also `mask` (uint8 [size, B, K]) and `noise` (float32 [size, B, K], or None)."""
 
   def __init__(self, replay, size: int):
     import ctypes  # pylint: disable=import-outside-toplevel
@@ -512,6 +552,15 @@ class ReplayBatch:
       nxt.reward = self.reward.data_ptr()
     nxt.discount = self.discount.data_ptr()
     self._struct = _lib.Replay(self.size, None, self.obs_tm1.data_ptr(), self.actions.data_ptr(), nxt)
+    self.mask = self.noise = self._bootstrap = None
+    boot = replay.bootstrap
+    if boot is not None:
+      draws = (self.size, env.batch, int(boot.num_heads))
+      self.mask = torch.zeros(draws, dtype=torch.uint8, device=env.device)
+      if boot.noise:
+        self.noise = torch.zeros(draws, dtype=torch.float32, device=env.device)
+      self._bootstrap = _lib.Bootstrap(int(boot.num_heads), 0, float(boot.mask_prob), int(boot.seed) % (1 << 64),
+                                       self.mask.data_ptr(), None if self.noise is None else self.noise.data_ptr())
     self._ctypes = ctypes
     self._owner = replay
 
@@ -533,15 +582,24 @@ class LaneReplay:
 
   `sample(size, min_size)` draws `size` slots per lane uniformly with replacement from the lane's filled slots, on a
   stateless Philox stream keyed by (`seed`, global lane) at the environment's call index, so sharded, packed and
-  standalone runs draw the same slots (`bsb_replay_sample`)."""
+  standalone runs draw the same slots (`bsb_replay_sample`).  With `bootstrap` (a `Bootstrap`) it returns
+  `BootstrapTransitions` instead, whose masks and noise the same launch draws (`bsb_replay_sample_bootstrap`)."""
 
-  def __init__(self, environment, capacity: int, seed: int = 0):
+  def __init__(self, environment, capacity: int, seed: int = 0, bootstrap: Optional[Bootstrap] = None):
     from bsuite_b200 import _lib  # pylint: disable=import-outside-toplevel
     torch = environment._torch      # pylint: disable=protected-access
     capacity = int(capacity)
     if not 1 <= capacity <= (1 << 31) - 1:
       raise ValueError(f'capacity must lie in [1, 2^31 - 1], got {capacity}')
+    if bootstrap is not None:
+      if not isinstance(bootstrap, Bootstrap):
+        raise ValueError(f'bootstrap must be a rollouts.Bootstrap, got {type(bootstrap).__name__}')
+      if not 1 <= int(bootstrap.num_heads) <= 65536:
+        raise ValueError(f'bootstrap.num_heads must lie in [1, 65536], got {bootstrap.num_heads}')
+      if not 0.0 <= float(bootstrap.mask_prob) <= 1.0:
+        raise ValueError(f'bootstrap.mask_prob must lie in [0, 1], got {bootstrap.mask_prob}')
     self.environment, self.capacity, self.seed = environment, capacity, int(seed)
+    self.bootstrap = bootstrap
     B, device = environment.batch, environment.device
     # make_buffers(capacity)'s layout, with both observation rings from torch's default allocator: a ring of gigabytes
     # would use up the finite compressible store obs_memory keeps for step observations
@@ -580,10 +638,11 @@ class LaneReplay:
     """Output tensors for `sample(size, out=...)`."""
     return ReplayBatch(self, size)
 
-  def sample(self, size: int, min_size: int = 1, out: Optional[ReplayBatch] = None) -> Transitions:
+  def sample(self, size: int, min_size: int = 1, out: Optional[ReplayBatch] = None):
     """`size` transitions of every lane holding at least max(min_size, 1) of them, drawn uniformly with replacement
     (replay.py:56-59; a lane below `min_size` is the reference's `if replay.size < min_replay_size: return`): one
-    launch.  Repeated samples between two steps draw different slots."""
+    launch.  Repeated samples between two steps draw different slots.  Returns `Transitions`, or with a `Bootstrap`
+    `BootstrapTransitions`."""
     env = self.environment
     size = int(size)
     if out is None:
@@ -591,9 +650,12 @@ class LaneReplay:
     elif not isinstance(out, ReplayBatch) or out._owner is not self or out.size != size:   # pylint: disable=protected-access
       raise ValueError(f'out must be make_batch({size}) of this replay')
     env._async_work = True      # pylint: disable=protected-access
-    status = env._lib.bsb_replay_sample(env._handle.ptr, out._ctypes.byref(self._ring), size, int(min_size),      # pylint: disable=protected-access
-                                        self.seed % (1 << 64), self._draw, out._ctypes.byref(out._struct),       # pylint: disable=protected-access
-                                        out.ready.data_ptr(), env._stream())      # pylint: disable=protected-access
+    args = (env._handle.ptr, out._ctypes.byref(self._ring), size, int(min_size), self.seed % (1 << 64), self._draw,  # pylint: disable=protected-access
+            out._ctypes.byref(out._struct), out.ready.data_ptr())      # pylint: disable=protected-access
+    if self.bootstrap is None:
+      status = env._lib.bsb_replay_sample(*args, env._stream())      # pylint: disable=protected-access
+    else:
+      status = env._lib.bsb_replay_sample_bootstrap(*args, out._ctypes.byref(out._bootstrap), env._stream())  # pylint: disable=protected-access
     if status:
       from bsuite_b200 import _lib  # pylint: disable=import-outside-toplevel
       _lib.check(status)
@@ -601,7 +663,10 @@ class LaneReplay:
     o_tm1, o_t = out.obs_tm1, out.obs
     if env.ragged:
       o_tm1, o_t = env.split_observation(o_tm1), env.split_observation(o_t)
-    return Transitions(o_tm1, out.actions, out.reward, out.discount, o_t, out.ready.view(env._torch.bool))  # pylint: disable=protected-access
+    ready = out.ready.view(env._torch.bool)      # pylint: disable=protected-access
+    if self.bootstrap is not None:
+      return BootstrapTransitions(o_tm1, out.actions, out.reward, out.discount, o_t, out.mask, out.noise, ready)
+    return Transitions(o_tm1, out.actions, out.reward, out.discount, o_t, ready)
 
 
 class LaneSequence:

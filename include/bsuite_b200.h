@@ -628,6 +628,90 @@ int32_t bsb_step_budgeted_sequence(bsb_env* env, const int32_t* actions, const b
                                    const bsb_outputs* out, const bsb_outputs* previous,
                                    int32_t* actions_out, const bsb_sequence* sequence, void* stream);
 
+/*
+ * Ensemble policy (the reference's boot_dqn, baselines/jax/boot_dqn/agent.py:
+ * one ensemble member acts per episode, epsilon-greedily over its Q-values).
+ * values holds every head's action values; heads holds each lane's active
+ * head, which the caller zero-fills before a run (the reference starts on
+ * member 0) and the step redraws when an episode ends.
+ */
+typedef struct bsb_ensemble_policy {
+  int32_t num_heads;     /* K, in [1, 65536] */
+  int32_t reserved;      /* 0 */
+  const float* values;   /* float32 [K, B, num_actions], contiguous: every head's action values */
+  int32_t* heads;        /* int32 [B]: each lane's active head; read, and redrawn at a LAST */
+  double epsilon;        /* in [0, 1] */
+  uint64_t seed;         /* keys the policy stream and the head stream */
+} bsb_ensemble_policy;
+
+/*
+ * Ensemble step.  Let h_i = heads[i] before the call and V the [B, A] rows
+ * values[h_i, i, :].  With replay == NULL the call equals
+ * bsb_step_budgeted_policy with {EPSILON_GREEDY, V, epsilon, seed} bit for
+ * bit (outputs, previous, actions_out, mask, budgets, lane state, streams,
+ * info, Logging columns, log rows, step count); with a replay it equals
+ * bsb_step_budgeted_record with that policy, rings included.  In addition
+ * every lane that stepped (mask set and episodes_left > 0 before the call)
+ * and whose step ended an episode (the LAST that counts its budget down; no
+ * output is read for it) sets heads[i] = (lo32(w0) * K) >> 32 (update(),
+ * agent.py:166-169), w0 being word 0 of the Philox4x64-10 block at counter
+ * (s, 0, 0, 5) with key (seed, global lane): s and the global lane are those
+ * of the policy stream.  Lanes that sit out read no row and keep their head.
+ * A head outside [0, K) raises the invalid-action flag and is clamped for
+ * the row read, as actions are; it is not written back.
+ * Refused (BSB_INVALID_ARGUMENT, before anything moves): whatever
+ * bsb_step_budgeted_policy or bsb_step_budgeted_record refuses, a NULL
+ * policy / values / heads, num_heads outside [1, 65536], a non-zero
+ * `reserved`, epsilon outside [0, 1] or NaN.  values and heads live in the
+ * handle's memory space.  May be captured: a replay reads values, heads,
+ * mask and budgets as they are then.
+ */
+int32_t bsb_step_budgeted_ensemble(bsb_env* env, const bsb_ensemble_policy* policy, uint8_t* mask,
+                                   int64_t* episodes_left, const bsb_outputs* out,
+                                   const bsb_outputs* previous, int32_t* actions_out,
+                                   const bsb_replay* replay, void* stream);
+
+/*
+ * Bootstrap masks and reward noise of boot_dqn's transitions
+ * (agent.py:171-185: m_t ~ Bernoulli(mask_prob)^K, z_t ~ N(0, 1)^K per
+ * transition), drawn when a transition is sampled rather than stored.  Each is
+ * a pure function of (seed, global lane, j), j being the 0-based count of
+ * transitions the lane had added before this one, so a transition keeps its
+ * draws however often it is sampled.  mask and noise are [size, B, K] in the
+ * handle's memory space; either may be NULL, not both.
+ */
+typedef struct bsb_bootstrap {
+  int32_t num_heads;     /* K, in [1, 65536] */
+  int32_t reserved;      /* 0 */
+  double mask_prob;      /* in [0, 1] */
+  uint64_t seed;         /* key of the bootstrap stream */
+  uint8_t* mask;         /* uint8 [size, B, K], nullable */
+  float* noise;          /* float32 [size, B, K], nullable */
+} bsb_bootstrap;
+
+/*
+ * bsb_replay_sample with bootstrap draws: the call equals bsb_replay_sample
+ * bit for bit.  In addition, for every entry (j', i) it writes for a ready
+ * lane, with slot the ring slot it drew, N = num_added[i] and
+ * j = N - 1 - ((N - 1 - slot) mod capacity) the transition's index, and for
+ * every head k, on the Philox4x64-10 blocks with key (bootstrap->seed, global
+ * lane) (the global lane keyed as the sample keys it):
+ *   mask[j', i, k] = ((w >> 11) * 2^-53 < mask_prob), w = word k & 3 of the
+ *     block at counter (j, k >> 2, 0, 6);
+ *   noise[j', i, k] = numpy's legacy polar method on the blocks at counter
+ *     (j, k, 1 + a, 6), a = 0, 1, ...: x = 2 (w0 >> 11) 2^-53 - 1, y likewise
+ *     from w1, accepted when 0 < r2 = x^2 + y^2 < 1, noise = (float)(y *
+ *     sqrt(-2 log(r2) / r2)) with a log the host path and the kernels share;
+ *     0 after 64 rejected attempts (probability below 1e-42).
+ * Entries of other lanes are not written.  Refused (BSB_INVALID_ARGUMENT):
+ * whatever bsb_replay_sample refuses, a NULL bootstrap, num_heads outside
+ * [1, 65536], a non-zero `reserved`, mask_prob outside [0, 1] or NaN, mask
+ * and noise both NULL.  May be captured, as bsb_replay_sample.
+ */
+int32_t bsb_replay_sample_bootstrap(bsb_env* env, const bsb_replay* replay, int64_t size, int64_t min_size,
+                                    uint64_t seed, uint64_t draw, const bsb_replay* batch, uint8_t* ready,
+                                    const bsb_bootstrap* bootstrap, void* stream);
+
 /* Host mirror of the on-device action sampler: out int32 [T,B] (host). */
 int32_t bsb_random_actions(uint64_t action_seed, uint64_t lane_offset,
                            int64_t batch, int64_t first_step, int64_t num_steps,
@@ -660,7 +744,8 @@ int32_t bsb_read_episode_stats(bsb_env* env, int32_t field, double* dst,
 /*
  * CUDA graphs.  bsb_step / bsb_reset / bsb_rollout / the masked calls (bsb_reset_masked / bsb_step_masked /
  * bsb_rollout_masked / bsb_advance_masked / bsb_step_budgeted / bsb_step_budgeted_policy / bsb_step_budgeted_record
- * / bsb_step_budgeted_sequence) / bsb_replay_sample / bsb_read_* / bsb_sum_* may
+ * / bsb_step_budgeted_sequence / bsb_step_budgeted_ensemble) / bsb_replay_sample / bsb_replay_sample_bootstrap /
+ * bsb_read_* / bsb_sum_* may
  * be called on a stream that is being captured.  A graph freezes launch arguments, so the first captured launch moves the handle's step
  * counter (it indexes the on-device action stream and the Logging columns) and its chunk scheduler into device
  * memory, for good: replays and eager calls can then be mixed in any order, and bsb_steps_done / bsb_get_state
